@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""bench.py — entity-steps/s of the B200 six_dof() RK4 path (BASELINE.json metric).
+"""bench.py — entity-steps/s of the six_dof() RK4 path on the H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--worlds M]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--worlds M] [--dump-outputs DIR]
 
 One "step" = one RK4 tick of the hot path over the whole batch of synthetic worlds
 (one body kernel launch, the state streaming HBM -> registers -> HBM).  Workload at
 every N: BASELINE.json configs[1] — the cube-sat single 6DOF body, RK4, dt = 1e-3 —
 batched over the Monte-Carlo world axis (SURVEY §8d C2 "also run M = 2^20.. copies for
-throughput"): 1 body x M worlds per GPU, M = 2^22 (read set 671 MB > 126 MB L2), weak
+throughput"): 1 body x M worlds per GPU, M = 2^22 (read set 671 MB > 50 MB L2), weak
 scaling (per-GPU work fixed, worlds shard with no data-path collective).  The literal
 configs[1] latency chain (1 body, dependent steps) is reported beside it as
 `single_body`.
@@ -23,7 +23,7 @@ e2e       the same metric through the reference-shaped C-ABI call
 verified  the timed executor's final state (256 strided worlds) against the CPU oracle advanced the
           same number of ticks: the timed launches did the work.
 roofline  algorithmic 264 B/entity-step (SURVEY §8d) / mean kernel time vs the measured
-          HBM copy peak (MEASURED_PEAKS.json, else the 6.65 TB/s fallback).
+          HBM copy peak (MEASURED_PEAKS.json, else this run's device-to-device copy probe).
 multi_gpu BASELINE configs[3] (n-body 1024, sharded worlds; one world: replicas vs row shards) and
           configs[4] (falcon9-style Monte-Carlo, 100 000 rollouts over the N GPUs, wall time including
           the end-of-run NCCL gather done inside libb200_sixdof.so).
@@ -31,6 +31,10 @@ cpu_baseline / --impl reference
           the CPU oracle port of the reference arithmetic (oracle/, the reference's
           Rust+JAX+Cranelift stack cannot be built here) on every CPU this process may use,
           one driver call for the whole run (threads created once), >= 1 s timed.
+--dump-outputs DIR
+          after the timed steps, the output columns the timed executor holds (world_pos, world_vel,
+          world_accel, force, inertia) for a fixed, seeded sample of DUMP_WORLDS worlds, as DIR/<name>.npy
+          (float64); the inputs are seeded, so two builds run with the same arguments compare output for output.
 """
 
 from __future__ import annotations
@@ -70,22 +74,29 @@ def synth_world(M: int, seed: int):
     return np.ascontiguousarray(pos), np.ascontiguousarray(vel), np.ascontiguousarray(ine)
 
 
-def measured_peak():
+def measured_peak(copy_probe: float):
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     try:
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return copy_probe, "measured (b200_probe_copy_gbs, this run)"
 
 
-def ncu_traffic(workload_key: str):
-    """dram bytes per launch of the dominant kernel from the committed ncu --set full capture."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(workload_key)
-    except Exception:
-        return None
+DUMP_WORLDS = 1 << 16  # 256 B of outputs per world: 16 MB per dump
+
+
+def dump_outputs(out_dir: str, ex, n_worlds: int) -> None:
+    """Write the timed executor's output columns for a fixed, seeded sample of its worlds as out_dir/<name>.npy."""
+    from elodin_b200.executor import FORCE, INERTIA, WORLD_ACCEL, WORLD_POS, WORLD_VEL
+
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.arange(n_worlds)
+    if n_worlds > DUMP_WORLDS:
+        idx = np.sort(np.random.default_rng(0).choice(n_worlds, DUMP_WORLDS, replace=False))
+    for name, cid in (("world_pos", WORLD_POS), ("world_vel", WORLD_VEL), ("world_accel", WORLD_ACCEL),
+                      ("force", FORCE), ("inertia", INERTIA)):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(ex.download(cid)[idx], dtype=np.float64))
 
 
 class ClockSampler:
@@ -331,21 +342,8 @@ def run_baseline_configs(args, torch, el, stream, local, rank, world_size):
     return out
 
 
-def ensure_built():
-    """Harness step: (re)build the in-tree CUDA library if its sources are newer (make is a no-op otherwise)."""
-    import fcntl
-
-    try:
-        with open(os.path.join(ROOT, "elodin_b200", "csrc", ".build.lock"), "w") as lock:
-            fcntl.flock(lock, fcntl.LOCK_EX)  # ranks of one node take turns; all but the first find it up to date
-            subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "elodin_b200", "csrc")], check=True,
-                           stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-    except Exception:
-        pass  # the import below fails loudly if the library is really missing
-
-
 def run_b200(args):
-    ensure_built()
+    # runs the library the build left in the tree (it may be read-only here): a missing one fails at its first call
     import torch
     import torch.distributed as dist
 
@@ -409,6 +407,8 @@ def run_b200(args):
         t_end = time.perf_counter()
         ms = max_over_ranks(e0.elapsed_time(e1))
         launches = ex.timings()["kernel_launches"] - launches0
+        if args.dump_outputs and rank == 0:  # before the clock replay below advances the state
+            dump_outputs(args.dump_outputs, ex, M)
         window = "timed region"
         if ms * 1e-3 < 0.3:  # `ms` is the max over ranks, so every rank takes the same branch
             # too short for nvidia-smi's 50 ms period: replay the identical loop for ~0.5 s and sample that
@@ -430,7 +430,7 @@ def run_b200(args):
     final_vel = ex.download(WORLD_VEL)[vidx]
     value = world_size * M * K / (ms * 1e-3)
     kernel_ms = ms / K
-    peak, peak_src = measured_peak()
+    peak, peak_src = measured_peak(copy_probe)
     achieved = B_ALG * M / (kernel_ms * 1e-3) / 1e9
 
     if args.kernel_only:
@@ -504,10 +504,8 @@ def run_b200(args):
                 q1.record(stream)
                 torch.cuda.synchronize()
                 t_ms = q0.elapsed_time(q1) / 100
-                tr = ncu_traffic("body_fast_rk4_%s_bytes_per_launch_M%d" % (name, M))
                 eff_out[name] = {"value": M / (t_ms * 1e-3), "unit": UNIT, "bytes_per_entity_step": bytes_per, "us_per_tick": t_ms * 1e3,
                                  "achieved_GBps": bytes_per * M / (t_ms * 1e-3) / 1e9, "frac": bytes_per * M / (t_ms * 1e-3) / 1e9 / peak,
-                                 "traffic": tr, "dram_frac": (tr / (t_ms * 1e-3) / 1e9 / peak) if tr else None,
                                  "touched_bytes_per_entity_step": bytes_per - (B_ALG - B_TOUCHED),
                                  "kernel": "body_fast_spec_kernel<RK4, sig %s, 128 x 3, 2 bodies/thread>" % {"rocket": "THRUST|DRAG", "falcon9": "FRAME|WRENCH", "cube_sat": "WHEELS|J2"}[name]}
                 sx.close()
@@ -608,8 +606,6 @@ def run_b200(args):
     if rank == 0:
         cpu = None
         verified = None
-        traffic = ncu_traffic("body_fast_rk4_bytes_per_launch_M%d" % M)
-        steady = ncu_traffic("body_fast_rk4_steady_bytes_per_launch_M%d" % M)
         if world_size == 1:
             from oracle import oracle as O
 
@@ -628,26 +624,19 @@ def run_b200(args):
             "config": {"workload": "cube-sat 6DOF RK4 dt=1e-3, 1 body x M worlds (BASELINE configs[1] batched over the Monte-Carlo world axis)",
                        "worlds_per_gpu": M, "bodies_per_world": 1, "dt": DT, "integrator": "rk4", "math": "fast (<=1e-12/tick vs exact)",
                        "ticks_per_launch": 1, "parallelism": f"worlds sharded x{world_size}, no data-path collective",
-                       "l2_policy": "inputs larger than L2 (read set %.0f MB per tick > 126 MB)" % (160 * M / 1e6),
+                       "l2_policy": "inputs larger than L2 (read set %.0f MB per tick > 50 MB)" % (160 * M / 1e6),
                        "e2e_ticks_per_call": e2e["ticks_per_call"], "e2e_worlds_per_gpu": args.e2e_worlds},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "algorithmic_bytes_per_entity_step": B_ALG, "kernel": "body_fast_spec_kernel<RK4, sig 0, 128 x 3, 2 bodies/thread>",
                          "kernel_ms": kernel_ms,
-                         "dram_frac": (traffic / (kernel_ms * 1e-3) / 1e9 / peak) if traffic else None,
                          "touched_bytes_per_entity_step": B_TOUCHED,
                          "touched_frac": B_TOUCHED * M / (kernel_ms * 1e-3) / 1e9 / peak,
-                         "traffic_steady": steady, "steady_dram_frac": (steady / (kernel_ms * 1e-3) / 1e9 / peak) if steady else None,
                          "copy_probe_GBps_this_run": copy_probe, "fp64_probe_GFLOPs_this_run": fp64_peak,
-                         "note": "frac counts the algorithmic 264 B/entity-step against the measured copy peak and reads above 1.0 for "
-                                 "two reasons: the kernel touches 240 B of them (the free tick never needs the three Inertia momentum "
+                         "note": "frac counts the algorithmic 264 B/entity-step against the measured copy peak and can read above 1.0 "
+                                 "for two reasons: the kernel touches 240 B of them (the free tick never needs the three Inertia momentum "
                                  "planes), and consecutive launches walk the planes in opposite directions, so the tail of the "
-                                 "previous launch's state is served from the 126 MB L2 (event-timed 152 -> 142 us per tick, "
-                                 "profiles/r02_tune_snake.txt).  traffic = DRAM bytes of one cold-cache launch (ncu --set full); "
-                                 "traffic_steady = DRAM bytes per launch with ncu --cache-control none (profiles/r02_steady_traffic.txt): "
-                                 "the touched 240 B/body and nothing twice — ncu serialises launches, so the L2 saving of the "
-                                 "alternating traversal is not visible to it and steady_dram_frac (traffic_steady / kernel time / "
-                                 "peak) is an upper bound on what DRAM moves in the timed loop"},
+                                 "previous launch's state is served from the 50 MB L2"},
             "e2e": e2e,
             "gpu_launches": int(launches),
             "verified": verified,
@@ -801,7 +790,7 @@ def run_multi_gpu(args, torch, dist, el, stream, local, rank, world_size, barrie
                 "launch and, at 8 worlds, 5.3 rounds of work items quantised to 6"})
     out["nbody_1024_sharded_worlds"] = {
         "config": "BASELINE configs[3]: 1024 bodies, softened all-pairs gravity + 6DOF RK4, dt = 3600 s, 8 worlds per GPU", "scaling": "weak",
-        **small, "saturated_batch": nbody_batch(296, 30, 3)}
+        **small, "saturated_batch": nbody_batch(264, 30, 3)}
     # (b) ONE world on N GPUs: replicas (every GPU integrates the whole world, zero communication) ...
     p1, v1, I1 = nbody_world(1, rng)
     ex = el.B200Exec(N, 1, 3600.0, None, [grav()], "rk4", "fast", device=local)
@@ -899,8 +888,8 @@ def run_multi_gpu(args, torch, dist, el, stream, local, rank, world_size, barrie
                    "nccl_version": int(__import__("elodin_b200")._lib.lib().b200_comm_version()),
                    "bytes_result_per_gpu": int(full.numel() * 8), "bytes_received_per_gpu": int(recv_bytes),
                    "ms_median_of_5": g_ms, "ms_all": gms, "recv_GBps_per_gpu": recv_bytes / (g_ms * 1e-3) / 1e9 if world_size > 1 else None,
-                   "nvlink5_peak_GBps_per_direction": 900.0,
-                   "frac_of_nvlink_peak": recv_bytes / (g_ms * 1e-3) / 1e9 / 900.0 if world_size > 1 else None,
+                   "nvlink4_peak_GBps_per_direction": 450.0,
+                   "frac_of_nvlink_peak": recv_bytes / (g_ms * 1e-3) / 1e9 / 450.0 if world_size > 1 else None,
                    "result_checked": gather_ok}}
     return out
 
@@ -932,6 +921,7 @@ def main():
     ap.add_argument("--mc-steps", type=int, default=1000, help="configs[4]: ticks per rollout (dt = 1e-3)")
     ap.add_argument("--configs", action="store_true", help="also time the other BASELINE.json configs (adds ~1 min)")
     ap.add_argument("--kernel-only", action="store_true", help="profiling aid: only the main timed loop (no e2e / cpu / extras)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the timed executor's outputs after the timed steps as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

@@ -1,9 +1,9 @@
-"""elodin_b200 — B200-native drop-in for the six_dof() hot path of elodin-sys/elodin.
+"""elodin_b200 — GPU-native (H100) drop-in for the six_dof() hot path of elodin-sys/elodin.
 
 The package mirrors the slice of the nox-py ECS surface that path needs (World,
 Body, WorldPos/WorldVel/Force/Inertia columns, six_dof(), World.build()/run(),
 Exec.run()/history()) and routes every tick through libb200_sixdof.so — hand-written
-sm_100a CUDA kernels behind the C ABI in include/b200_sixdof.h.  There is no CPU
+sm_90a CUDA kernels behind the C ABI in include/b200_sixdof.h.  There is no CPU
 implementation here: importing works anywhere, but building an executor without
 the CUDA library or without a GPU raises.
 

@@ -1,4 +1,4 @@
-// sm_100a per-body integrator kernels of the six_dof() hot path (K1/K2/K4/K5 of SURVEY §2.4).
+// sm_90a per-body integrator kernels of the six_dof() hot path (K1/K2/K4/K5 of SURVEY §2.4).
 //
 //   body_exact_kernel       EXACT arithmetic: one thread per body, the whole tick (clear_forces, effectors x4,
 //                           calc_accel x4, stage advance x4, final combine, renormalise) in registers, n_ticks
@@ -129,9 +129,9 @@ template <int INTEG, uint32_t SIG, bool TRAJ, int BLOCK, int MINB, int BPT>
 __global__ void __launch_bounds__(BLOCK, MINB) body_fast_spec_kernel(const __grid_constant__ StepParams P)
 {
     // Odd launches walk the planes from the far end: the tail of the state the previous launch read and wrote last is
-    // still in the 126 MB L2 when this launch starts — read it first, before this launch's own traffic evicts it, and the
-    // rewrite lands on lines that are still dirty instead of costing a second DRAM write (scripts/tune_snake.py: 152.4 ->
-    // 142.1 us per tick at 2^22 bodies; L2 eviction-class hints on top of it measured nothing and cost registers).
+    // still in the 50 MB L2 when this launch starts — read it first, before this launch's own traffic evicts it, and the
+    // rewrite lands on lines that are still dirty instead of costing a second DRAM write (scripts/tune_snake.py A/B-times it
+    // against B200_SNAKE=0).
     const unsigned blk = P.reverse ? gridDim.x - 1u - blockIdx.x : blockIdx.x;
     const uint64_t b0 = ((uint64_t)blk * BLOCK + threadIdx.x) * BPT;
     if (b0 >= P.n_bodies) return;
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) body_fast_spec_kernel(const __gri
 
     // A (WorldPos, WorldVel) sample on every launch of one tick: the pair stores it from here as one 16-byte store per
     // plane — the per-body 8-byte stores inside fast_ticks fill half of every sector, and the other half arrives a whole
-    // tick of arithmetic later (telemetry on every tick: 254 -> see profiles/r02_tune_telemetry.txt)
+    // tick of arithmetic later
     const bool defer_traj = TRAJ && BPT == 2 && both && P.n_ticks == 1 && P.traj_planes == 13;
     Motion a_last[BPT], f_last[BPT];
 #pragma unroll
@@ -468,9 +468,9 @@ static bool planes_16B_aligned(const StepParams &Q, uint32_t sig)
     return (a & 15u) == 0 && (Q.ld & 1u) == 0;
 }
 
-// Default shape, measured on B200 at 2^22 worlds (profiles/r02_tune_spec.md): body pairs (BPT = 2, LDG.E.128) at
-// 128 threads x 3 CTAs/SM (<= 168 registers, no spills) run the free / rocket / falcon9 signatures at 7.2 TB/s of
-// algorithmic bytes; one body per thread at 128 x 4 is 9 % (rocket) to 11 % (falcon9) slower.  Ranges too small to
+// Default shape (scripts/tune_spec.py sweeps the others in a tuning build): body pairs (BPT = 2, LDG.E.128) at
+// 128 threads x 3 CTAs/SM (<= 168 registers) keep every load of the pair in flight under the first body's arithmetic;
+// on the H100 the free / rocket / falcon9 signatures move their touched bytes at the device copy rate.  Ranges too small to
 // fill the machine with pairs, or whose planes are not 16-byte aligned (odd world-range offsets), take one body
 // per thread.
 template <int INTEG, uint32_t SIG, bool TRAJ>
@@ -492,7 +492,7 @@ static void launch_spec(const StepParams &Q, cudaStream_t s)
     default: break;
     }
 #endif
-    constexpr uint64_t kPairMinBodies = 2ull * 128 * 3 * 148; // one full wave of body pairs
+    constexpr uint64_t kPairMinBodies = 2ull * 128 * 3 * kNumSMs; // one full wave of body pairs
     if (vec_ok && Q.n_bodies >= kPairMinBodies) launch_spec_shape<INTEG, SIG, TRAJ, 128, 3, 2>(Q, s);
     else launch_spec_shape<INTEG, SIG, TRAJ, 128, 4, 1>(Q, s);
 }
@@ -575,8 +575,8 @@ cudaError_t launch_body_step(const StepParams &P, int integrator, int math_mode,
         static const int xcfg = env_int("B200_EXACT_CFG", 3);
 #endif
         auto g = [&](int blk) { return (unsigned)((P.n_bodies + blk - 1) / blk); };
-        // default: the kernel compiled for this effector sequence (no interpreter: 5.4e9 vs 4.1e9 entity-steps/s on free
-        // bodies, profiles/r02_tune_misc.md); the interpreter kernel for every other list
+        // default: the kernel compiled for this effector sequence (no run-time interpreter in the tick); the interpreter
+        // kernel for every other list
         if (xcfg == 3) {
             const uint32_t seq = exact_sequence(P);
 #ifdef B200_TUNE
@@ -653,7 +653,7 @@ cudaError_t launch_body_step(const StepParams &P, int integrator, int math_mode,
     if (sig != SIG_GENERIC) done = rk4 ? launch_spec_sig<B200_INTEGRATOR_RK4>(Q, sig, s)
                                        : launch_spec_sig<B200_INTEGRATOR_SEMI_IMPLICIT>(Q, sig, s);
     if (!done) {
-        // 128 threads x 4 CTAs/SM = 16 warps/SM at <= 128 registers (profiles/r01_tuning.md)
+        // 128 threads x 4 CTAs/SM = 16 warps/SM at <= 128 registers
         if (rk4) BODY_FAST(B200_INTEGRATOR_RK4, 128, 4);
         else BODY_FAST(B200_INTEGRATOR_SEMI_IMPLICIT, 128, 4);
     }

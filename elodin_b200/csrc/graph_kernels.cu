@@ -1,4 +1,4 @@
-// sm_100a kernels of GraphQuery.edge_fold gravity (K3 of SURVEY §2.4) and the kernels that fuse it with the
+// sm_90a kernels of GraphQuery.edge_fold gravity (K3 of SURVEY §2.4) and the kernels that fuse it with the
 // body tick (nbody_tick_fused_kernel, small_world_kernel).
 //
 // Why one launch per tick suffices even with body-body coupling: in the reference's RK4
@@ -205,8 +205,8 @@ __global__ void __launch_bounds__(32 * kFastSrc * ((RK4 && SPLIT) ? 3 : 1)) grap
 
 // FAST all-pairs for worlds of N <= TJ bodies, persistent: a CTA keeps ONE world's three stage-position tiles and
 // masses in shared memory (80 KB at TJ = 1024) and folds many sources against them — the round-1 kernel re-staged
-// the world for every 8 sources and its grid (one CTA per 8 sources) quantised badly against the 148 SMs (M = 8:
-// 1024 CTAs on 444 slots = 2.3 waves).  A work item is (SRC sources, one stage slot), one warp each, lanes striding
+// the world for every 8 sources and its grid (one CTA per 8 sources) quantised badly against the SM count (M = 8:
+// 1024 CTAs on 3 x 132 = 396 slots = 2.6 waves).  A work item is (SRC sources, one stage slot), one warp each, lanes striding
 // the targets TGT at a time (SRC x TGT independent chains for the FP64 pipe); with fewer worlds than CTAs a world's
 // sources are split over grid/M CTAs, otherwise a CTA walks whole worlds.  No self test (pair_fold), one third-order
 // rsqrt step: 18 FP64-pipe slots per pair evaluation.
@@ -617,7 +617,7 @@ cudaError_t launch_graph_force(const GraphParams &G, int math_mode, bool dense, 
         else {
             if (gcfg == 1 && G.n_entities <= 1024 && G.n_entities >= 64) {
                 // worlds that fit one shared-memory tile set: persistent world-resident kernel
-                int dev = 0, sms = 148;
+                int dev = 0, sms = (int)kNumSMs;
                 cudaGetDevice(&dev);
                 cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
                 auto launch_world = [&](auto kern, int nt, int minb, int src) -> cudaError_t {
@@ -626,7 +626,7 @@ cudaError_t launch_graph_force(const GraphParams &G, int math_mode, bool dense, 
                     if (G.n_worlds >= slots) grid_w = slots;
                     else {
                         // few worlds: as many CTAs per world as the SMs allow, down to four busy warps per CTA (latency,
-                        // not throughput, is the price of a tick then: profiles/r02_tune_nbody_small.txt)
+                        // not throughput, is the price of a tick then)
                         const unsigned items = (n_src + src - 1) / src * (rk4 ? 3u : 1u), warps = (unsigned)nt / 32u;
                         const unsigned busy = std::min(warps, 4u); // one busy warp per FP64 pipe when there is room to spread
                         const unsigned cpw = std::max(1u, std::min(slots / G.n_worlds, (items + busy - 1) / busy));
@@ -657,7 +657,7 @@ cudaError_t launch_graph_force(const GraphParams &G, int math_mode, bool dense, 
                 default: break;
                 }
 #endif
-                // default shapes by measurement (profiles/r02_tune_world.md): one 512-thread CTA per SM stages each world
+                // default shapes: one 512-thread CTA per SM stages each world
                 // once per SM.  Big batches (>= 8 rounds of four-source items per resident warp) fold four sources per
                 // item — four chains that share every target load: 0.81 of the DFMA issue rate; small batches keep
                 // two sources x two targets so that the item count still divides over the warps (M = 8: 0.55)
@@ -671,7 +671,7 @@ cudaError_t launch_graph_force(const GraphParams &G, int math_mode, bool dense, 
             const unsigned gridf = ((n_src + kFastSrc - 1) / kFastSrc) * G.n_worlds;
             // few CTAs: split the stage slots over warps to fill the machine; many CTAs: keep
             // 3 slots per warp (more ILP per lane, 3 CTAs/SM) — measured on N = 1024, M = 1 / 8
-            const bool split = gcfg == 2 || (gcfg == 1 && gridf < 3u * 148u);
+            const bool split = gcfg == 2 || (gcfg == 1 && gridf < 3u * kNumSMs);
             constexpr size_t smem256 = (3 * 3 + 1) * 256 * sizeof(double), smem1024 = (3 * 3 + 1) * 1024 * sizeof(double);
             if (!rk4) graph_dense_fast_kernel<false, false, 256><<<gridf, dim3(32, kFastSrc, 1), smem256, s>>>(G);
             else if (split) {
@@ -711,9 +711,9 @@ bool nbody_fused_applicable(const GraphParams &G, int math_mode, bool dense)
     static const int fcfg = [] { const char *e = getenv("B200_NBODY_FUSED"); return e ? atoi(e) : 1; }();
     if (fcfg == 0) return false;
     const unsigned gridf = ((G.n_entities + kFastSrc - 1) / kFastSrc) * G.n_worlds;
-    if (gridf < 3u * 148u) return true; // small grids: one launch per tick (pair kernel for 64..1024 bodies, nbody_tick_fused_kernel otherwise)
-    // worlds that fit the persistent kernel's tile set: fused at any batch size (measured: 43.1 -> 41.0 us per tick at 8
-    // worlds of 1024 bodies, identical bits; B200_NBODY_FUSED=2 keeps the two-launch route)
+    if (gridf < 3u * kNumSMs) return true; // small grids: one launch per tick (pair kernel for 64..1024 bodies, nbody_tick_fused_kernel otherwise)
+    // worlds that fit the persistent kernel's tile set: fused at any batch size (one launch per tick instead of two,
+    // identical bits; B200_NBODY_FUSED=2 keeps the two-launch route)
     return fcfg != 2 && G.n_entities >= 64 && G.n_entities <= 1024;
 }
 
@@ -722,13 +722,12 @@ cudaError_t launch_nbody_tick_fused(const GraphParams &G, const StepParams &P, d
     constexpr size_t smem = (3 * 3 + 1) * 1024 * sizeof(double);
     const unsigned gridf = ((G.n_entities + kFastSrc - 1) / kFastSrc) * G.n_worlds;
     // One to three worlds too: a world's (source pair, slot) items spread over as many CTAs as give every warp one item
-    // (scripts/tune_nbody_small.py: 1024 bodies x 1 / 2 / 3 worlds 15.4 / 26.7 / 37.7 -> 14.4 / 16.4 / 20.5 us per tick,
-    // 64 bodies 8.2 -> 6.2, same bits); B200_NBODY_WORLD_MIN=444 restores the small-grid kernel below 444 split-kernel CTAs
+    // (scripts/tune_nbody_small.py compares the routes; same bits); B200_NBODY_WORLD_MIN=396 restores the small-grid kernel below 3 x 132 split-kernel CTAs
     static const unsigned world_min = (unsigned)env_int("B200_NBODY_WORLD_MIN", 0);
     static const unsigned world_rounds = (unsigned)std::max(1, env_int("B200_NBODY_WORLD_ROUNDS", 1));
     if (gridf >= world_min && G.n_entities >= 64 && G.n_entities <= 1024) {
         // the persistent world-resident kernel with the integration fused in (same shapes as launch_graph_force picks)
-        int dev = 0, sms = 148;
+        int dev = 0, sms = (int)kNumSMs;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const unsigned long long items4 = (unsigned long long)((G.n_entities + 3) / 4) * 3u * G.n_worlds;
@@ -739,7 +738,6 @@ cudaError_t launch_nbody_tick_fused(const GraphParams &G, const StepParams &P, d
         else {
             const unsigned items = (G.n_entities + src - 1) / src * 3u;
             // few worlds: spread a world's items over the SMs until a CTA keeps only four warps busy — one per FP64 pipe
-            // (1024 bodies, one world: 14.4 -> 10.3 us per tick; profiles/r02_tune_nbody_small.txt)
             static const unsigned spread = (unsigned)std::max(1, env_int("B200_NBODY_WORLD_SPREAD", 4));
             const unsigned per_cta = world_rounds * std::min(warps, spread);
             grid_w = std::max(1u, std::min(slots / G.n_worlds, (items + per_cta - 1) / per_cta)) * G.n_worlds;
@@ -763,7 +761,7 @@ cudaError_t launch_nbody_tick_fused(const GraphParams &G, const StepParams &P, d
 
 bool small_world_applicable(const GraphParams &G, int math_mode)
 {
-    // measured (profiles/r01_small_world.md): faster than the two-launch route over the whole range a warp can
+    // faster than the two-launch route over the whole range a warp can
     // hold, in both arithmetic modes (N = 3: 53x FAST / 4.4x EXACT; N = 32: 3.6x / 1.35x)
     (void)math_mode;
     static const int cfg = [] { const char *e = getenv("B200_SMALL_WORLD"); return e ? atoi(e) : 1; }();

@@ -1,4 +1,4 @@
-// sm_100a layout kernels (K6 of SURVEY §2.4): host column layout [body][width] <-> device SoA planes,
+// sm_90a layout kernels (K6 of SURVEY §2.4): host column layout [body][width] <-> device SoA planes,
 // and the FP64 throughput probe.
 #include <algorithm>
 
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(256) selftest_div_kernel(uint64_t seed, uint64
 
 cudaError_t launch_selftest_div(uint64_t seed, uint64_t n_groups, unsigned long long *counts, cudaStream_t s)
 {
-    const unsigned blocks = (unsigned)std::min<uint64_t>((n_groups + 255) / 256, 148u * 16u);
+    const unsigned blocks = (unsigned)std::min<uint64_t>((n_groups + 255) / 256, kNumSMs * 16u);
     if (blocks) selftest_div_kernel<<<blocks, 256, 0, s>>>(seed, n_groups, counts);
     return cudaGetLastError();
 }

@@ -2,7 +2,7 @@
 //
 // Replaces CraneliftExec (libs/nox-py/src/cranelift_exec.rs:54-195) on the
 // six_dof() path: owns device-resident SoA columns, maps the reference's host
-// column buffers in and out, and drives the sm_100a kernels.  There is no CPU
+// column buffers in and out, and drives the sm_90a kernels.  There is no CPU
 // fallback anywhere in this file: without a CUDA device every entry point fails
 // with B200_ERR_NO_DEVICE.
 #include <sys/mman.h>

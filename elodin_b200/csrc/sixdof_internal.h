@@ -8,6 +8,10 @@
 
 namespace b200 {
 
+// SMs of the target GPU (H100 SXM): launch-shape thresholds that are fixed at compile time size themselves by it;
+// grids that depend on occupancy query the device instead.
+constexpr unsigned kNumSMs = 132;
+
 // One built-in effector as the kernels see it.  `col` points at the SoA planes
 // of its per-body input column (plane p at col + p*ld), nullptr if none.
 struct EffDev {

@@ -3,8 +3,8 @@
 Reference: `CraneliftExec` / `WorldExec` (libs/nox-py/src/cranelift_exec.rs:13-195,
 libs/nox-py/src/exec.rs:53-94).  Same contract: `invoke_batch(columns, n)` takes
 the host column buffers (one per input ComponentId), integrates n ticks, and
-returns every output column — but the state lives in B200 HBM between calls and
-the ticks run in hand-written sm_100a kernels behind the C ABI
+returns every output column — but the state lives in GPU HBM between calls and
+the ticks run in hand-written sm_90a kernels behind the C ABI
 (include/b200_sixdof.h).  All numerics happen in libb200_sixdof.so.
 """
 

@@ -1,5 +1,5 @@
 /*
- * b200_sixdof.h — C ABI of the B200-native 6DOF rigid-body integrator.
+ * b200_sixdof.h — C ABI of the H100-native 6DOF rigid-body integrator.
  *
  * This library replaces, on the six_dof() hot path only, the executor seam of
  * elodin-sys/elodin's nox-py host:
@@ -288,7 +288,7 @@ uint64_t b200_sixdof_plane_stride(const b200_sixdof *h); /* doubles between plan
 /* ---- multi-GPU (SURVEY §8e).  Worlds shard across GPUs — one handle per GPU, one process (or thread) per
  * handle, no data-path collective — exactly like the reference's one-OS-process-per-world Monte-Carlo driver
  * (libs/monte-carlo/src/lib.rs:2083).  The one exchange is the end-of-run gather of the trajectory ring, over
- * NCCL (NVLink 5 / NVSwitch).  NCCL is bound at run time (dlopen of libnccl.so.2: the copy the host process already
+ * NCCL (NVLink 4 / NVSwitch).  NCCL is bound at run time (dlopen of libnccl.so.2: the copy the host process already
  * loaded, else the system one); b200_comm_available() == 0 means it could not be found. ---- */
 #define B200_COMM_ID_BYTES 128u                      /* sizeof(ncclUniqueId) */
 typedef struct b200_comm b200_comm;                   /* opaque: one NCCL communicator rank */

@@ -4,7 +4,7 @@ here = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "elodin_b2
 src = sys.argv[1]
 flags = [a for a in sys.argv[2:] if a.startswith("-")]
 filt = [a for a in sys.argv[2:] if not a.startswith("-")]
-out = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xptxas", "-v", *flags,
+out = subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xptxas", "-v", *flags,
                       "-c", src, "-o", "/tmp/ptxas_table.o"], cwd=here, capture_output=True, text=True).stderr
 name = None
 rows = []

@@ -1,4 +1,4 @@
-"""Secondary kernels on one B200 (tuning build for the EXACT shapes: make -C elodin_b200/csrc TUNE=1):
+"""Secondary kernels on one GPU (tuning build for the EXACT shapes: make -C elodin_b200/csrc TUNE=1):
   * EXACT body kernel launch shapes (B200_EXACT_CFG re-read per launch in a tuning build), 2^20 worlds
   * n-body 1024: pair kernel at M = 1 / 8 / 64 worlds, FP64-pipe fraction against b200_probe_fp64_gflops
 Prints one JSON row per measurement and writes gpurun_out/tune_misc.json."""
