@@ -157,7 +157,24 @@ __global__ void __launch_bounds__(BLOCK, MINB) body_fast_spec_kernel(const __gri
 #pragma unroll
         for (int k = 0; k < BPT; ++k) I[k].diag = Vec3{0.0, 0.0, 0.0};
     }
-    B200_LDV(P.ine, 6, I[k].m);
+    // The mass-class summary (P.mass_class; the host passes it only to signature-0 launches with a +0 gravity that form
+    // no Force): one byte per warp of pairs, 1 when mass_is_regular holds for all 64 masses of the segment.  Such a warp
+    // integrates with m = 1 — the same bits — and leaves the mass plane in HBM; a warp whose byte is 0 reads the plane
+    // and, when its whole segment lies in this launch, records what it found.
+    uint8_t *const mass_class = SIG == 0u && BPT == 2 ? P.mass_class : nullptr;
+    const bool mass_known = mass_class && mass_class[b0 >> 6] != 0; // warp-uniform
+    if (mass_known) {
+#pragma unroll
+        for (int k = 0; k < BPT; ++k) I[k].m = 1.0;
+    } else {
+        B200_LDV(P.ine, 6, I[k].m);
+        if (mass_class && (b0 | 63u) < P.n_bodies) { // every lane of the warp is live and holds two bodies
+            bool regular = true;
+#pragma unroll
+            for (int k = 0; k < BPT; ++k) regular &= mass_is_regular(I[k].m);
+            if (__all_sync(0xffffffffu, regular) && (threadIdx.x & 31u) == 0) mass_class[b0 >> 6] = 1;
+        }
+    }
 #pragma unroll
     for (int k = 0; k < BPT; ++k) {
         in[k].thrust = 0.0; in[k].cd_rho = in[k].area = 0.0;
@@ -495,6 +512,13 @@ cudaError_t launch_body_step(const StepParams &P, int integrator, int math_mode,
     static const int snake = env_int("B200_SNAKE", 1);
     if (!snake) Q.reverse = 0; // A/B switch: always walk forward
     const uint32_t sig = no_spec ? (uint32_t)SIG_GENERIC : spec_signature(Q);
+    // the mass-class summary stands in for the mass only where its one use is (0 m + 0) rcp_nr(m): signature 0 with a
+    // +0 gravity, no Force (write_fa) and no full trajectory sample (both form m a); the one-body-per-thread kernels
+    // never read it.  B200_MASS_CLASS=0 reads every mass (A/B switch).
+    static const int mass_class = env_int("B200_MASS_CLASS", 1);
+    static const double pos_zero[3] = {0.0, 0.0, 0.0};
+    const bool g_pos_zero = std::memcmp(Q.spec.g, pos_zero, sizeof pos_zero) == 0;
+    if (!mass_class || sig != 0u || !g_pos_zero || Q.write_fa || (Q.traj_every && Q.traj_planes == 25)) Q.mass_class = nullptr;
     bool done = false;
     if (sig != SIG_GENERIC) done = rk4 ? launch_spec_sig<B200_INTEGRATOR_RK4>(Q, sig, s)
                                        : launch_spec_sig<B200_INTEGRATOR_SEMI_IMPLICIT>(Q, sig, s);

@@ -257,6 +257,8 @@ int launch_ticks(b200_sixdof *h, uint64_t w0, uint64_t nw, uint64_t n_ticks, cud
     if (P.traj) P.traj += b0;
     for (uint32_t i = 0; i < P.n_eff; ++i) if (P.eff[i].col) P.eff[i].col += b0;
     P.n_bodies = nb;
+    // the summary's segments must be the launch's warps of pairs: only a range that starts on a segment boundary uses it
+    P.mass_class = (!h->mass_class_off && b0 % 64 == 0) ? h->mass_class + b0 / 64 : nullptr;
     const bool exact = h->desc.math_mode == B200_MATH_EXACT;
     const bool graph = h->graph_eff >= 0;
     const bool egm = h->egm_eff >= 0; // its stage forces are a function of the tick's input state: one launch per tick
@@ -342,6 +344,16 @@ int do_step(b200_sixdof *h, uint64_t n_ticks)
     return B200_OK;
 }
 
+// Forget what the mass-class summary knows about every segment that overlaps bodies [b0, b0 + n): their Inertia is
+// about to be written.  Stream-ordered before that write and after every launch already queued.
+int clear_mass_class(b200_sixdof *h, uint64_t b0, uint64_t n)
+{
+    if (n == 0) return B200_OK;
+    const uint64_t s0 = b0 / 64, s1 = (b0 + n + 63) / 64;
+    CU(h, cudaMemsetAsync(h->mass_class + s0, 0, s1 - s0, h->stream));
+    return B200_OK;
+}
+
 int do_upload(b200_sixdof *h, uint64_t id, const void *src, uint64_t bytes)
 {
     Column *c = h->find(id);
@@ -361,6 +373,7 @@ int do_upload(b200_sixdof *h, uint64_t id, const void *src, uint64_t bytes)
     if (bytes == 0) return B200_OK;
     int rc = ensure_staging(h, bytes);
     if (rc) return rc;
+    if (id == B200_ID_INERTIA && (rc = clear_mass_class(h, 0, h->n_bodies))) return rc;
     CU(h, cudaMemcpyAsync(h->staging, src, bytes, cudaMemcpyDefault, h->stream));
     CU(h, launch_aos_to_soa(h->staging, c->dev, h->n_bodies, c->width, h->ld, h->stream));
     h->timings.kernel_launches++;
@@ -624,6 +637,12 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
                 return bail(fail(B200_ERR_VALUE_SIZE_MISMATCH, "column 0x%016llx declared with two widths", (unsigned long long)e.column_id));
             if ((rc = add_column(h, e.column_id, e.column_width, false))) return bail(rc);
         }
+    {
+        const uint64_t bytes = (h->ld + 63) / 64;
+        if (cudaMalloc(&h->mass_class, bytes) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(mass classes)"));
+        if (cudaMemsetAsync(h->mass_class, 0, bytes, h->stream) != cudaSuccess)
+            return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMemset(mass classes)"));
+    }
     build_id_tables(h);
     // per-effector entity masks: copy now, the caller's arrays are only valid for this call
     h->eff_masks.assign(h->effectors.size(), nullptr);
@@ -684,6 +703,7 @@ void b200_sixdof_destroy(b200_sixdof *h)
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     for (auto &c : h->cols) if (c.dev) cudaFree(c.dev);
+    if (h->mass_class) cudaFree(h->mass_class);
     for (auto m : h->eff_masks) if (m) cudaFree(m);
     for (auto t : h->eff_tables) if (t) cudaFree(t);
     if (h->row_ptr) cudaFree(h->row_ptr);
@@ -791,6 +811,7 @@ static int invoke_small(b200_sixdof *h, const uint8_t *const *in_cols, uint8_t *
         if (!in_cols[i]) continue; // not dirty: the device-resident copy stands
         if (c->global) { int rc = do_upload(h, c->id, in_cols[i], 8); if (rc) return rc; continue; }
         if (!input_is_live(h, c->id)) continue;
+        if (c->id == B200_ID_INERTIA) { int rc = clear_mass_class(h, 0, h->n_bodies); if (rc) return rc; }
         mi.col[mi.n++] = {in_total, c->dev, c->width, 0};
         in_map.push_back({i, in_total * 8});
         in_total += h->n_bodies * c->width;
@@ -958,6 +979,7 @@ static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8
         for (size_t i = 0; i < h->input_ids.size(); ++i) {
             const Column *c = h->find(h->input_ids[i]);
             if (!in_cols[i] || c->global || !input_is_live(h, c->id)) continue;
+            if (c->id == B200_ID_INERTIA) { int rc = clear_mass_class(h, b0, nb); if (rc) return rc; }
             CU(h, launch_aos_to_soa(h->stage_in + in_off[i] + b0 * c->width, c->dev + b0, nb, c->width, h->ld, h->stream));
             h->timings.kernel_launches++;
         }
@@ -1158,6 +1180,7 @@ void *b200_sixdof_device_plane(b200_sixdof *h, uint64_t id, uint32_t plane)
     if (!h) return nullptr;
     Column *c = h->find(id);
     if (!c || c->global || plane >= c->width) return nullptr;
+    if (id == B200_ID_INERTIA) h->mass_class_off = true; // the caller may now write masses the handle never sees
     return c->dev + (uint64_t)plane * h->ld;
 }
 

@@ -50,6 +50,11 @@ struct b200_sixdof {
     bool nbody_fused = false;                       // decided once per handle (whole-batch grid size)
     bool small_world = false;                       // <= 32 bodies per world: whole ticks in one warp, n ticks per launch
     uint32_t max_deg = 0;
+    // one byte per 64-body segment (absolute body index / 64): 1 = every mass of the segment is regular for the FAST
+    // signature-0 tick (body_fast_spec_kernel), 0 = unknown.  Every write of the Inertia planes clears the bytes of the
+    // segments it touches first (clear_mass_class); once a raw Inertia pointer is handed out, it is never used again.
+    uint8_t *mass_class = nullptr;
+    bool mass_class_off = false;
     // staging for AoS <-> SoA
     double *staging = nullptr;
     uint64_t staging_bytes = 0;

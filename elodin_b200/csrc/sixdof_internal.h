@@ -52,6 +52,9 @@ struct StepParams {
     uint64_t tick0;     // global tick count before this launch
     uint32_t ent0;      // entity row of body 0 of this launch (row-sharded single worlds start inside a world)
     uint32_t reverse;   // walk the tiles from the last one down (alternating launches: L2 reuse of the previous launch's tail)
+    // mass-class summary of this launch's bodies (one byte per 64-body segment, segment 0 starting at body 0 of the
+    // launch; see body_fast_spec_kernel), or nullptr where the launch must read every mass
+    uint8_t *mass_class;
     // compile-time-specialised FAST kernels (sixdof_tick.cuh SIG_*): what body_kernels.cu:spec_signature
     // distilled from eff[] — uniform constants and the plane bases of the per-body input columns
     struct Spec {

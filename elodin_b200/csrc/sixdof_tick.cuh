@@ -536,6 +536,15 @@ __device__ __forceinline__ Vec3 lin_accel_fast(const StepParams &P, const Folded
     return Vec3{F.x * inv_m, F.y * inv_m, F.z * inv_m};
 }
 
+// Where the only force is a +0 gravity (signature 0, spec.g == +0 bit for bit) and Force is not formed, lin_accel_fast
+// is (0 m + 0) rcp_nr(m): true when that is +0, as it is for m = 1, so such a tick cannot tell m from 1.  It is -0 for a
+// negative m and NaN for m = +-0, +-inf, NaN and a subnormal m (rcp.approx.ftz flushes it: the Newton steps turn the
+// infinite seed into NaN); DBL_MAX gives +0 (its reciprocal flushes to 0).
+__device__ __forceinline__ bool mass_is_regular(double m)
+{
+    return __double_as_longlong((0.0 * m + 0.0) * fa::rcp_nr(m)) == 0;
+}
+
 // world-frame force this stage's state produced (only materialised when Force is written back)
 __device__ __forceinline__ Motion force_out_fast(const Vec3 &a_lin, const Vec3 &a_ang_body_u, const Quat &q,
                                                  const Inertia &I, const Vec3 &tw)

@@ -281,7 +281,9 @@ uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 int b200_sixdof_set_stream(b200_sixdof *h, void *cuda_stream, int use_own_stream);
 int b200_sixdof_timings(const b200_sixdof *h, b200_timings *out);
 int b200_sixdof_status(const b200_sixdof *h);                  /* sticky status of the handle */
-/* raw device plane pointer (plane p of a column), for zero-copy interop (NCCL gather) */
+/* raw device plane pointer (plane p of a column), for zero-copy interop (NCCL gather).  Asking for an Inertia
+ * plane lets the caller change masses behind the handle's back: from that call on, the handle reads every mass
+ * on every tick (it no longer trusts its per-segment summary of which masses are regular). */
 void *b200_sixdof_device_plane(b200_sixdof *h, uint64_t component_id, uint32_t plane);
 uint64_t b200_sixdof_plane_stride(const b200_sixdof *h); /* doubles between planes */
 
