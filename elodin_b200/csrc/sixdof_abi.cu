@@ -603,6 +603,9 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
         case B200_EFF_GRAVITY_EDGES_NEWTON: case B200_EFF_GRAVITY_EDGES_SOFTENED:
             if (h->graph_eff >= 0) return bail(fail(B200_ERR_UNSUPPORTED, "only one edge_fold gravity effector is supported"));
             if (e.n_edges && (!e.edge_from || !e.edge_to)) return bail(fail(B200_ERR_INVALID_ARGUMENT, "edge arrays are null"));
+            // the fold's members are the sources of its edges: a mask would define a membership the reference lacks
+            if (e.entity_mask)
+                return bail(fail(B200_ERR_UNSUPPORTED, "effector %zu: an edge_fold gravity effector takes no entity mask", i));
             if (d->math_mode == B200_MATH_FAST && i != 0)
                 return bail(fail(B200_ERR_UNSUPPORTED, "FAST math: the edge_fold gravity effector must come first (it overwrites Force)"));
             h->graph_eff = (int)i;

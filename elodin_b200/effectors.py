@@ -253,7 +253,7 @@ class GravityEdges(Effector):
         e.n_edges = len(f)
         e.edge_from = f.ctypes.data
         e.edge_to = t.ctypes.data
-        return e
+        return self._attach_mask(e)  # the library refuses a mask here: pass it on rather than drop it silently
 
 
 def all_pairs_edges(n: int) -> np.ndarray:

@@ -155,7 +155,9 @@ typedef struct b200_effector {
     const uint8_t *entity_mask; /* [n_entities] or NULL: 1 = the effector applies to that entity row.
                                    Mirrors the reference's query join (query.rs:672-710): an @el.map
                                    effector only runs on entities that own every component it reads
-                                   (e.g. drag only on bodies with a `wind` component).  Copied at create. */
+                                   (e.g. drag only on bodies with a `wind` component).  Copied at create.
+                                   GRAVITY_EDGES_* refuse a mask (B200_ERR_UNSUPPORTED): the fold's
+                                   members are the sources of its edges. */
     const double *table0;       /* ABI v3.  GRAVITY_EGM08: C coefficients; copied at create; NULL otherwise  */
     const double *table1;       /*          GRAVITY_EGM08: S coefficients                                     */
     uint64_t table_len;         /*          (L+1)^2                                                            */

@@ -8,21 +8,17 @@ the oracle per body (tests.util.assert_nbody_close).  EXACT stays bit-identical.
 once per process, so their cases run in child processes.
 """
 
-import json
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 import elodin_b200 as el
 from elodin_b200.executor import FORCE, INERTIA, WORLD_ACCEL, WORLD_POS, WORLD_VEL
-from tests.util import assert_nbody_close, assert_route, launched_kernels, nbody_world
+from tests.util import assert_nbody_close, assert_route, launched_kernels, nbody_world, run_child
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DT = 1e-3
 
 # kernel name prefixes (template arguments: RK4 / SPLIT / TJ, and for the world kernel RK4, TJ, threads, min CTAs,
@@ -174,15 +170,7 @@ def _child_run(out_path, cases, attempts=3):
 
 def _run_child(cases, out, setting=None):
     """Run _child_run in a child process (with one B200_* route switch set) and load what it wrote."""
-    env = {k: v for k, v in os.environ.items() if not k.startswith("B200_")}
-    if setting:
-        key, val = setting.split("=")
-        env[key] = val
-    code = "import json, sys; from tests.test_nbody_routes import _child_run; _child_run(sys.argv[1], json.loads(sys.argv[2]))"
-    argv = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code, out, json.dumps(cases)]
-    p = subprocess.run(argv, cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, f"{setting or 'default'} child failed ({p.returncode}):\n{p.stderr[-4000:]}"
-    return np.load(out)
+    return run_child("tests.test_nbody_routes:_child_run", out, cases, setting)
 
 
 def _names(res, k, kernels, what):

@@ -99,19 +99,41 @@ def nbody_pair_scale(pos, ine, k, soft):
     return out
 
 
-def nbody_world(seed, M, N, dt, kick=1e-2, size=1.0, speed=1.0, soft=1e-2):
-    """A softened all-pairs world where a tick's gravity is visible at FAST tolerance: positions in a cube of
-    `size`, linear speeds ~ `speed`, and the gravity constant k scaled so that the median body gets a kick of
+def graph_pair_scale(pos, ine, edges, kind, k, soft):
+    """S_i = sum over body i's out-edges (i, j), with multiplicity, of |a_ij| = k m_j |r_ij| / (|r_ij|^2 + soft)^1.5
+    at the positions `pos` [M, N, 7]; kind "newton" has no softening.  A self-edge contributes 0 (softened: r = 0;
+    Newton divides 0 by 0, which no bound can cover).  Returns [M, N]."""
+    x, m = pos[..., 4:], ine[..., 6]
+    out = np.zeros(m.shape)
+    e = np.asarray(edges, dtype=np.int64).reshape(-1, 2)
+    if len(e) == 0:
+        return out
+    soft = 0.0 if kind == "newton" else soft
+    a, b = e[:, 0], e[:, 1]
+    r = x[:, b] - x[:, a]  # [M, E, 3]
+    d = np.sqrt(np.sum(r * r, -1))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        acc = k * m[:, b] * d / (d * d + soft) ** 1.5
+    acc[:, a == b] = 0.0
+    np.add.at(out, (slice(None), a), acc)
+    return out
+
+
+def nbody_world(seed, M, N, dt, kick=1e-2, size=1.0, speed=1.0, soft=1e-2, edges=None, kind="softened"):
+    """A gravity world where a tick's gravity is visible at FAST tolerance: positions in a cube of `size`, linear
+    speeds ~ `speed`, and the gravity constant k scaled so that the median body with an out-edge gets a kick of
     `kick` * |v| per tick.  A tick moves a body by dt * speed, which must be at least 1e-5 of the cube, so that
-    gravity evaluated at the wrong stage position differs visibly.  Attitude, angular velocity and inertia come
-    from random_world.  Returns (pos, vel, ine, k, soft, S)."""
+    gravity evaluated at the wrong stage position differs visibly.  The graph is all pairs (softened), or the
+    `edges` of `kind` (graph_pair_scale).  Attitude, angular velocity and inertia come from random_world.
+    Returns (pos, vel, ine, k, soft, S)."""
     assert dt * speed >= 1e-5 * size
     pos, vel, ine = random_world(seed, M, N)
     rng = np.random.default_rng(seed + 1)
     pos[..., 4:] = rng.uniform(-size, size, (M, N, 3))
     vel[..., 3:] = rng.normal(0, speed / np.sqrt(3), (M, N, 3))
-    S1 = nbody_pair_scale(pos, ine, 1.0, soft)
-    k = kick * np.median(np.linalg.norm(vel[..., 3:], axis=-1)) / (dt * np.median(S1))
+    S1 = nbody_pair_scale(pos, ine, 1.0, soft) if edges is None else graph_pair_scale(pos, ine, edges, kind, 1.0, soft)
+    live = S1[S1 > 0]
+    k = kick * np.median(np.linalg.norm(vel[..., 3:], axis=-1)) / (dt * np.median(live)) if live.size else 1.0
     return pos, vel, ine, k, soft, k * S1
 
 
@@ -162,7 +184,9 @@ def assert_nbody_close(got, want, start, dt, n_ticks, S, tol=1e-12, what=""):
 # errors a kernel can make independently
 BODY_TERMS = {"gravity": ("g",), "thrust": ("thrust",), "drag": ("drag",), "wrench": ("wrench_force", "wrench_torque"),
               "wrench_world": ("world_force", "world_torque"), "frame": ("central", "coriolis", "centrifugal"),
-              "j2": ("j2_central", "j2"), "wheels": ("wheels",), "egm08": ("egm08",)}
+              "j2": ("j2_central", "j2"), "wheels": ("wheels",), "egm08": ("egm08",),
+              "softened": ("graph",), "newton": ("graph",)}
+GRAPH_KINDS = ("softened", "newton")
 ANGULAR_TERMS = ("wrench_torque", "world_torque", "wheels")
 MU_EARTH, OMEGA_EARTH, J2_EARTH, R_EARTH = 3.986004418e14, (0.0, 0.0, 7.292115e-5), 1.08262668e-3, 6.378e6
 
@@ -187,9 +211,12 @@ def body_effectors(O, spec):
 
 def body_terms(spec):
     """[(effector index, term)] of the terms of `spec` that reach the Force.  The wheel fold overwrites everything
-    accumulated before it, and a drag resets the torque accumulated before it (both as the reference does)."""
+    accumulated before it, and a drag resets the torque accumulated before it (both as the reference does).  The
+    edge-fold gravity overwrites the Force of the bodies with an out-edge; FAST math takes it only first in the list,
+    where nothing precedes it, so it is one more additive term there (lists with it later are compared bit for bit)."""
     terms = []
     for i, (kind, _) in enumerate(spec):
+        assert kind not in GRAPH_KINDS or i == 0, "the edge-fold gravity must be the first effector of a FAST list"
         if kind == "wheels":
             terms = []
         if kind == "drag":
@@ -254,6 +281,9 @@ def body_term_accels(kind, kw, term, pos, vel, ine):
         series = sum((n + 1) * ratio ** n * (np.sum(np.abs(c[n, :n + 1])) + np.sum(np.abs(s[n, :n + 1])))
                      for n in range(L + 1))
         return kw.get("mu", MU_EARTH) / (r * r) * series, zero
+    if term == "graph":  # sum over the body's out-edges of |a_ij| (graph_pair_scale), at the start positions
+        k = kw.get("k2", 1e-3) if kind == "softened" else kw.get("G", 6.6743e-11)
+        return graph_pair_scale(pos, ine, kw["edges"], kind, k, kw.get("soft", 1e-10)), zero
     raise KeyError(term)
 
 
@@ -286,7 +316,7 @@ def body_scales(spec, pos, vel, ine):
     return A, B, C
 
 
-def assert_body_close(got, want, start, dt, n_ticks, scales, tol=1e-12, what=""):
+def assert_body_close(got, want, start, dt, n_ticks, scales, tol=1e-12, what="", check=True):
     """FAST body-kernel parity per body, on what the run changed.
 
     got / want: (WorldPos, WorldVel, WorldAccel, Force) after `n_ticks` ticks of (final) step `dt` from start =
@@ -298,7 +328,8 @@ def assert_body_close(got, want, start, dt, n_ticks, scales, tol=1e-12, what="")
       * stage-4 WorldAccel:            tol A_i + u |a| (linear), tol B_i + u |alpha| (angular)
       * Force:                         m_i (tol A_i) + u |F| (linear), tol C_i + u |tau| (angular; C_i = sum of the
                                        terms' |tau|, i.e. B_i with each component multiplied by its own I_i)
-    The linear and angular parts are separate checks.  Returns {quantity: worst error / bound} (every entry <= 1)."""
+    The linear and angular parts are separate checks.  Returns {quantity: worst error / bound} (every entry <= 1;
+    check=False returns the ratios without asserting, for the self-tests that measure how far a fault lands)."""
     ine = start[2]  # the start state enters through the scales: the differences below are differences of changes
     A, B, C = scales
     T = n_ticks
@@ -324,8 +355,8 @@ def assert_body_close(got, want, start, dt, n_ticks, scales, tol=1e-12, what="")
         ratio = np.divide(err, bound, out=np.where(err > 0, np.inf, 0.0), where=bound > 0)
         i = np.unravel_index(int(np.argmax(ratio)), ratio.shape)
         worst[name] = float(ratio[i])
-        assert ratio[i] <= 1.0, (f"{what} {name}: body (world {i[0]}, entity {i[1]}) error {err[i]:.3e} > bound {bound[i]:.3e} "
-                                 f"({ratio[i]:.3g}x); A_i = {A[i]:.3e}, B_i = {B[i]:.3e}")
+        assert not check or ratio[i] <= 1.0, (f"{what} {name}: body (world {i[0]}, entity {i[1]}) error {err[i]:.3e} > bound "
+                                              f"{bound[i]:.3e} ({ratio[i]:.3g}x); A_i = {A[i]:.3e}, B_i = {B[i]:.3e}")
     return worst
 
 
@@ -413,6 +444,11 @@ def mutate_term(O, spec, index, term, s):
             a = 1.0 - b
         kw["omega"] = tuple(a * om)
         extra = [("frame", {"mu": 0.0, "omega": tuple(b * om)})]
+    elif term == "graph":
+        if kind == "softened":
+            kw["k2"] = kw.get("k2", 1e-3) * s
+        else:
+            kw["G"] = kw.get("G", 6.6743e-11) * s
     else:
         raise KeyError(term)
     spec[index] = (kind, kw)
@@ -459,6 +495,29 @@ def launched_kernels(fn, settle=0.05):
     evs = [e for e in prof.profiler.kineto_results.events() if e.device_type() == DeviceType.CUDA]
     evs.sort(key=lambda e: e.start_ns())
     return out, [_canonical_kernel_name(e.name()) for e in evs]
+
+
+def run_child(target, out, args, setting=None, timeout=900):
+    """Run `target` ("module:function") as function(out, args) in a fresh child process, with every inherited B200_*
+    route switch removed and `setting` ("B200_X=v") set, and load the .npz it wrote to `out`.  The switches are read
+    once per process, and torch.profiler loses launch records of short windows more often once a process has run
+    other CUDA work (seen with torch 2.11 / CUDA 12.8 on an H100), so kernel names are recorded in a fresh child."""
+    import json
+    import os
+    import subprocess
+    import sys
+
+    env = {k: v for k, v in os.environ.items() if not k.startswith("B200_")}
+    if setting:
+        key, val = setting.split("=")
+        env[key] = val
+    module, func = target.split(":")
+    code = f"import json, sys; from {module} import {func}; {func}(sys.argv[1], json.loads(sys.argv[2]))"
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    argv = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code, out, json.dumps(args)]
+    p = subprocess.run(argv, cwd=root, env=env, capture_output=True, text=True, timeout=timeout)
+    assert p.returncode == 0, f"{setting or 'default'} child failed ({p.returncode}):\n{p.stderr[-4000:]}"
+    return np.load(out)
 
 
 # the kernels that advance a tick; layout (AoS <-> SoA) kernels and copies are not part of a route
