@@ -59,7 +59,9 @@ SYMBOLS = [
     "b200_comm_rank", "b200_comm_size", "b200_comm_last_ms", "b200_sixdof_trajectory_gather_bytes",
     "b200_sixdof_trajectory_allgather", "b200_sixdof_step_row_sharded", "b200_probe_pcie_gbs",
     "b200_comm_peer_attach", "b200_comm_peer_attached", "b200_comm_peer_detach", "b200_selftest_shared_divisor", "b200_probe_zero_copy_gbs", "b200_egm08_stream_len", "b200_egm08_stream",
+    "b200_sixdof_trajectory_stats", "b200_sixdof_state_stats", "b200_stats_merge",
 ]
+STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 COMM_ID_BYTES = 128
 
 
@@ -179,6 +181,9 @@ def lib():
     L.b200_sixdof_trajectory_width.restype = C.c_uint32
     L.b200_sixdof_trajectory_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_trajectory_reset.argtypes = [vp]
+    L.b200_sixdof_trajectory_stats.argtypes = [vp, vp, u64]
+    L.b200_sixdof_state_stats.argtypes = [vp, vp, u64]
+    L.b200_stats_merge.argtypes = [C.POINTER(C.c_double), u32, u64, C.POINTER(C.c_double)]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1144,6 +1144,98 @@ int b200_sixdof_trajectory_download(b200_sixdof *h, void *dst, uint64_t bytes)
 
 uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h) { return (h && h->traj) ? h->traj_planes : 0; }
 
+// Ensemble statistics of the planes in S (stats_kernels.cu) into dst, `bytes` already checked.  A device buffer on the
+// handle's GPU takes the table straight from the kernel; any other goes through the staging buffer.
+static int run_world_stats(b200_sixdof *h, StatsParams &S, void *dst, uint64_t bytes)
+{
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (bytes == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    cudaPointerAttributes a{};
+    const bool direct = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
+    (void)cudaGetLastError();
+    const uint64_t scratch = world_stats_scratch_doubles(S);
+    int rc = ensure_staging(h, std::max<uint64_t>((scratch + (direct ? 0 : bytes / 8)) * 8ull, 8));
+    if (rc) return rc;
+    S.out = direct ? (double *)dst : h->staging + scratch;
+    int launches = 0;
+    CU(h, launch_world_stats(S, h->staging, &launches, h->stream));
+    h->timings.kernel_launches += (uint64_t)launches;
+    if (!direct) CU(h, cudaMemcpyAsync(dst, S.out, bytes, cudaMemcpyDefault, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return B200_OK;
+}
+
+int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t n = b200_sixdof_trajectory_len(h);
+    const uint64_t W = h->traj_planes;
+    const uint64_t want = n * h->desc.n_entities * W * 5ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "trajectory statistics are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    StatsParams S{};
+    S.seg[0] = {h->traj, n * W};
+    S.n_segs = 1;
+    S.planes_per_sample = (uint32_t)W;
+    S.n_planes = n * W;
+    S.ld = h->ld;
+    S.n_worlds = h->desc.n_worlds;
+    S.n_entities = h->desc.n_entities;
+    return run_world_stats(h, S, dst, bytes);
+}
+
+int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t want = h->desc.n_entities * 25ull * 5ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "state statistics are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    StatsParams S{};
+    const uint64_t ids[4] = {B200_ID_WORLD_POS, B200_ID_WORLD_VEL, B200_ID_WORLD_ACCEL, B200_ID_FORCE};
+    for (int k = 0; k < 4; ++k) {
+        const Column *c = h->find(ids[k]);
+        S.seg[k] = {c->dev, c->width};
+    }
+    S.n_segs = 4;
+    S.planes_per_sample = 25;
+    S.n_planes = 25;
+    S.ld = h->ld;
+    S.n_worlds = h->desc.n_worlds;
+    S.n_entities = h->desc.n_entities;
+    return run_world_stats(h, S, dst, bytes);
+}
+
+// The cross-rank step of a world-sharded campaign: host-only, no GPU needed (a Rust host merges its ranks' tables
+// without torch).  Parts are folded left to right with the kernels' stats_merge, so the result does not depend on who
+// calls it.
+int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, double *out)
+{
+    if (n_groups && (!out || (n_parts && !parts))) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+    const double nan = std::nan("");
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        StatsGroup acc{0.0, 0.0, 0.0, 0.0, 0.0};
+        for (uint32_t p = 0; p < n_parts; ++p) {
+            const double *q = parts + ((uint64_t)p * n_groups + g) * 5;
+            if (!(q[0] >= 0.0)) return fail(B200_ERR_INVALID_ARGUMENT, "part %u, group %llu: count %g is not a count", p,
+                                             (unsigned long long)g, q[0]);
+            stats_merge(acc, StatsGroup{q[0], q[1], q[2], q[3], q[4]});
+        }
+        double *o = out + g * 5;
+        const bool any = acc.n > 0.0;
+        o[0] = acc.n;
+        o[1] = any ? acc.mean : nan;
+        o[2] = any ? acc.m2 : nan;
+        o[3] = any ? acc.mn : nan;
+        o[4] = any ? acc.mx : nan;
+    }
+    return B200_OK;
+}
+
 int b200_sixdof_trajectory_reset(b200_sixdof *h)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");

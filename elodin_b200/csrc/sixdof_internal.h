@@ -136,4 +136,47 @@ cudaError_t launch_multi_transpose(const MultiColumns &mc, uint64_t n_bodies, ui
 cudaError_t launch_probe_fp64(double *out, int iters, int blocks, cudaStream_t s);
 cudaError_t launch_selftest_div(uint64_t seed, uint64_t n_groups, unsigned long long *counts, cudaStream_t s);
 
+// Ensemble statistics over the world axis (stats_kernels.cu).  One group = (count, mean, m2 = sum (x - mean)^2, min,
+// max) over the finite values of a set of worlds; while count = 0 the other fields are mean = m2 = 0, min = +inf,
+// max = -inf (a finished table writes NaN there instead).
+struct StatsGroup {
+    double n, mean, m2, mn, mx;
+};
+
+// a := a (+) b, Chan et al.'s pairwise update.  Every merge of partial groups, on the device and in b200_stats_merge,
+// goes through this function.  A group with count 0 is the identity, whatever its other fields hold.
+__host__ __device__ inline void stats_merge(StatsGroup &a, const StatsGroup &b)
+{
+    if (b.n == 0.0) return;
+    if (a.n == 0.0) { a = b; return; }
+    const double n = a.n + b.n;
+    const double d = b.mean - a.mean;
+    a.mean = a.mean + d * b.n / n;
+    a.m2 = a.m2 + b.m2 + d * d * a.n * b.n / n;
+    a.mn = fmin(a.mn, b.mn);
+    a.mx = fmax(a.mx, b.mx);
+    a.n = n;
+}
+
+// Planes to reduce: segment s holds n_planes planes at base + k*ld (k < n_planes); plane i of the launch is plane i of
+// the concatenated segments.  Group (plane i, entity e) goes to out[((i / W) * n_entities + e) * W + i % W][5],
+// W = planes_per_sample.  Only bodies b = w * n_entities + e with w < n_worlds are read (never the padding to ld).
+struct StatsParams {
+    struct Seg {
+        const double *base;
+        uint64_t n_planes;
+    } seg[4];
+    uint32_t n_segs;
+    uint32_t planes_per_sample;
+    uint64_t n_planes;
+    uint64_t ld;
+    uint64_t n_worlds;
+    uint64_t n_entities;
+    double *out;
+};
+// f64 of device scratch the reduction needs for this shape (0: one pass, no scratch)
+uint64_t world_stats_scratch_doubles(const StatsParams &S);
+// one or two launches on s (written to *launches); `scratch` holds world_stats_scratch_doubles(S) f64
+cudaError_t launch_world_stats(const StatsParams &S, double *scratch, int *launches, cudaStream_t s);
+
 } // namespace b200

@@ -229,6 +229,29 @@ class B200Exec:
     def trajectory_reset(self) -> None:
         _lib.check(self._L.b200_sixdof_trajectory_reset(self._h))
 
+    # ---- ensemble statistics (reductions over the world axis, on the device) ------------------------------------
+    def trajectory_stats(self, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """The ring's samples reduced over the worlds: [samples, n_entities, width, 5] with the fields (count, mean,
+        m2 = sum (x - mean)^2, min, max) over the finite values (count = 0: NaN in the other four)."""
+        shape = (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13), _lib.STATS_FIELDS)
+        if out is None:
+            out = np.empty(shape)
+        elif out.shape != shape or out.dtype != np.float64 or not out.flags.c_contiguous:
+            raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, f"trajectory statistics are {shape} f64, got {out.shape} {out.dtype}")
+        _lib.check(self._L.b200_sixdof_trajectory_stats(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    def trajectory_stats_to_ptr(self, ptr: int, nbytes: int) -> None:
+        """trajectory_stats() into a raw host or device pointer (e.g. a torch CUDA tensor's data_ptr())."""
+        _lib.check(self._L.b200_sixdof_trajectory_stats(self._h, C.c_void_p(ptr), nbytes))
+
+    def state_stats(self) -> np.ndarray:
+        """The current state reduced over the worlds: [n_entities, 25, 5] — world_pos[7], world_vel[6],
+        world_accel[6], force[6] (the B200_TRAJ_FULL sample layout), fields as trajectory_stats()."""
+        out = np.empty((self.n_entities, 25, _lib.STATS_FIELDS))
+        _lib.check(self._L.b200_sixdof_state_stats(self._h, out.ctypes.data, out.nbytes))
+        return out
+
     # ---- plumbing ---------------------------------------------------------------
     def set_stream(self, cuda_stream: Optional[int]) -> None:
         """Run on a caller-owned cudaStream_t (0 = the legacy default stream, which is what
@@ -252,6 +275,24 @@ class B200Exec:
     @property
     def plane_stride(self) -> int:
         return int(self._L.b200_sixdof_plane_stride(self._h))
+
+
+def merge_stats(tables: Sequence[np.ndarray]) -> np.ndarray:
+    """Merge statistics tables of the same shape [..., 5] (e.g. one per rank of a world-sharded campaign, or per
+    handle) left to right, in list order, with b200_stats_merge: the table of the union of their worlds."""
+    parts = [np.asarray(t, dtype=np.float64) for t in tables]
+    if not parts:
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, "merge_stats needs at least one table")
+    shape = parts[0].shape
+    if shape[-1:] != (_lib.STATS_FIELDS,) or any(p.shape != shape for p in parts):
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH,
+                                  f"statistics tables must share one shape [..., 5], got {[p.shape for p in parts]}")
+    stacked = np.ascontiguousarray(np.stack(parts))
+    out = np.empty(shape)
+    dp = C.POINTER(C.c_double)
+    _lib.check(_lib.lib().b200_stats_merge(stacked.ctypes.data_as(dp), len(parts), out.size // _lib.STATS_FIELDS,
+                                            out.ctypes.data_as(dp)))
+    return out
 
 
 def math_nan() -> float:

@@ -49,6 +49,25 @@ def gather_worlds(local, n_worlds: int, group=None):
     return torch.cat([o[:s] for o, s in zip(out, sizes)], 0)
 
 
+def gather_ensemble(table, group=None) -> np.ndarray:
+    """Ensemble statistics of a world-sharded campaign: every rank passes the table of its own worlds ([..., 5] from
+    `B200Exec.trajectory_stats` / `state_stats`, numpy or torch), the tables are all-gathered and merged in rank order
+    with `merge_stats` (b200_stats_merge) on the host.  Every rank gets the same bits.  The tables are small (5 f64
+    per group): a CUDA copy for NCCL groups, host memory for gloo."""
+    import torch
+    import torch.distributed as dist
+
+    from .executor import merge_stats
+
+    local = table.detach().to("cpu", torch.float64) if isinstance(table, torch.Tensor) else torch.from_numpy(
+        np.ascontiguousarray(table, dtype=np.float64))
+    dev = "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+    local = local.to(dev).contiguous()
+    parts = [torch.empty_like(local) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(parts, local, group=group)
+    return merge_stats([p.cpu().numpy() for p in parts])
+
+
 def total_entity_steps(local_entity_steps: int, group=None) -> int:
     import torch
     import torch.distributed as dist

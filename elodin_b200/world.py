@@ -435,14 +435,19 @@ class World:
               telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
               max_ticks: Optional[int] = None, optimize: bool = False, db_path: Optional[str] = None,
               backend: str = "b200", math: str = "exact", n_worlds: int = 1, device: int = -1,
-              world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None) -> "Exec":
+              world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
+              ensemble: bool = False, ensemble_ring: Optional[int] = None) -> "Exec":
+        """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
+        the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
+        between two reductions (default: as many as fit in 256 MiB, at least one)."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
                 f"unknown backend '{backend}': this package only provides 'b200' (no cranelift / jax fallback)")
         if backend == "b200-fast":
             math = "fast"
-        return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident)
+        return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
+                    ensemble, ensemble_ring)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -493,6 +498,11 @@ class World:
         return ex
 
 
+# the Body columns six_dof() writes, as planes of a B200_TRAJ_FULL sample (and of a state_stats table)
+_SAMPLED = {"world_pos": (0, 7), "world_vel": (7, 13), "world_accel": (13, 19), "force": (19, 25)}
+_ENSEMBLE_RING_BYTES = 256 << 20  # device memory of the ensemble mode's trajectory ring
+
+
 class _Row(np.ndarray):
     def to_numpy(self):
         return np.asarray(self)
@@ -511,7 +521,8 @@ class Exec:
 
     def __init__(self, world: World, system: System, simulation_rate: float, telemetry_rate: Optional[float],
                  max_ticks: Optional[int], math: str, n_worlds: int, device: int,
-                 world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None):
+                 world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
+                 ensemble: bool = False, ensemble_ring: Optional[int] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -572,10 +583,17 @@ class Exec:
         # ring, read back in one transfer per `_ring_cap` cycles instead of one PCIe round trip per cycle.
         # Results are identical to the invoke_batch path (same kernels, same tick boundaries).
         n_bodies = len(bodies) * self.n_worlds
+        self._ensemble = bool(ensemble)
         if resident is None:
             resident = os.environ.get("B200_RESIDENT", "1") != "0" and 0 < n_bodies <= 65536
         self._ring_cap = 0
-        if resident and n_bodies:
+        if self._ensemble:
+            # Ensemble mode: the state never leaves the device between the initial upload and the end of run();
+            # each ring-full of telemetry samples is reduced over the worlds in place, then the ring is reset.
+            ld = (n_bodies + 127) // 128 * 128
+            cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max(25 * ld * 8, 1)
+            self._ring_cap = int(max(1, min(4096, cap)))
+        elif resident and n_bodies:
             ld = (n_bodies + 127) // 128 * 128
             self._ring_cap = int(max(1, min(4096, (64 << 20) // (25 * ld * 8))))
         # ticks of one invoke_batch stay in registers up to 32 at a time (no effect on results)
@@ -590,7 +608,14 @@ class Exec:
         self._db = None
         self._history: Dict[int, List[np.ndarray]] = {cid: [] for cid in self.world.columns}
         self._globals_hist: List[tuple] = []
-        self._record()
+        self._ens_rows: List[np.ndarray] = []  # ensemble mode: blocks of rows [k, n_entities, 25, 5]
+        if self._ensemble:
+            self._history = {}
+            self._upload_inputs()
+            self._ens_rows.append(self.backend.state_stats()[None])  # row 0: the initial state
+            self._globals_hist.append((self.tick, self.sim_time_step))
+        else:
+            self._record()
 
     # -- data plumbing -------------------------------------------------------------
     def _record(self) -> None:
@@ -648,13 +673,10 @@ class Exec:
                     raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, "value size mismatch")
                 np.copyto(col.buffer, buf)
 
-    def _run_resident(self, cycles: int) -> None:
-        """`cycles` whole telemetry cycles without leaving the device: upload the host columns once, step,
-        read the recorded samples back per ring-full, leave the final state in the host columns."""
+    def _upload_inputs(self) -> None:
+        """Every input column of the host world -> the device (the state the next ticks start from)."""
         be = self.backend
-        tpt = self.ticks_per_telemetry
         tick_id, dt_id = component_id("tick"), component_id("simulation_time_step")
-        t0 = time.perf_counter()
         for cid in be.input_ids:
             if cid == tick_id:
                 be.upload(cid, np.array([self.tick], dtype=np.uint64))
@@ -666,6 +688,92 @@ class Exec:
                 be.upload(cid, expanded)
             else:
                 be.upload(cid, self.world.columns[cid].buffer)
+
+    def _add_ensemble_rows(self, rows: np.ndarray, tpt: int) -> None:
+        """rows [k, n_entities, 25, 5]: k telemetry rows, `tpt` ticks apart, the last one at the current tick."""
+        k = rows.shape[0]
+        self._ens_rows.append(rows)
+        self._globals_hist.extend((self.tick - (k - 1 - i) * tpt, self.sim_time_step) for i in range(k))
+
+    def _run_ensemble(self, ticks: int, is_canceled, pre_step, post_step) -> None:
+        """Ensemble mode: one row of world-axis statistics per telemetry cycle, reduced on the device from the
+        trajectory ring.  Runs without host callbacks stay on the device for the whole call (upload once, one
+        reduction per ring-full); the others go one cycle at a time through invoke_batch, as the default mode does,
+        and record their rows the same way.  The final state of every world is in the host columns on return."""
+        be = self.backend
+        tpt = self.ticks_per_telemetry
+        remaining = int(ticks)
+        host_cb = bool(self.pre_systems or self.post_systems or pre_step or post_step)
+        if not host_cb and is_canceled is None:
+            self._upload_inputs()
+            whole = remaining // tpt
+            while whole > 0:
+                c = min(whole, self._ring_cap)
+                t0 = time.perf_counter()
+                be.trajectory_reset()
+                be.step(c * tpt)
+                rows = be.trajectory_stats()                          # [c, n_entities, 25, 5]
+                self.tick += c * tpt
+                self._add_ensemble_rows(rows, tpt)
+                ms = (time.perf_counter() - t0) * 1e3
+                self._prof["execute_buffers"] += [ms / c] * c
+                for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
+                    self._prof[k_dst] += [0.0] * c                    # not separable on this path
+                whole -= c
+            remaining %= tpt
+            if remaining:                                             # a last, partial cycle
+                t0 = time.perf_counter()
+                be.step(remaining)
+                self.tick += remaining
+                self._add_ensemble_rows(be.state_stats()[None], tpt)
+                self._prof["execute_buffers"].append((time.perf_counter() - t0) * 1e3)
+                for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
+                    self._prof[k_dst].append(0.0)
+            for name in _SAMPLED:                                     # the final state, once
+                col = self.world.columns[component_id(name)]
+                be.download(col.component.id, out=col.buffer)
+            return
+        while remaining > 0:
+            n = min(tpt, remaining)
+            per_call = 1 if host_cb else n
+            done = 0
+            be.trajectory_reset()
+            while done < n:
+                ctx = StepContext(self)
+                if pre_step:
+                    pre_step(self.tick, ctx)
+                for s in self.pre_systems:
+                    s.fn(ctx)
+                t_inv = time.perf_counter()
+                self._invoke(per_call)                                # host columns stay current
+                self._prof["execute_buffers"].append((time.perf_counter() - t_inv) * 1e3 * (n / per_call))
+                tm = be.timings()
+                for k_src, k_dst in (("h2d_upload_ms", "h2d_upload"), ("kernel_invoke_ms", "kernel_invoke"), ("d2h_download_ms", "d2h_download")):
+                    self._prof[k_dst].append(tm[k_src])
+                for s in self.post_systems:
+                    s.fn(ctx)
+                if post_step:
+                    post_step(self.tick, ctx)
+                done += per_call
+            t_hist = time.perf_counter()
+            self._add_ensemble_rows(be.trajectory_stats() if n == tpt else be.state_stats()[None], tpt)
+            self._prof["add_to_history"].append((time.perf_counter() - t_hist) * 1e3)
+            remaining -= n
+            if is_canceled is not None and is_canceled():
+                break
+
+    def _no_rows(self, what: str):
+        raise _lib.B200Error(_lib.ERR_UNSUPPORTED,
+                             f"{what}: this Exec was built with ensemble=True and records statistics over the worlds, "
+                             "not per-world rows; read them with Exec.ensemble('<entity>.<component>')")
+
+    def _run_resident(self, cycles: int) -> None:
+        """`cycles` whole telemetry cycles without leaving the device: upload the host columns once, step,
+        read the recorded samples back per ring-full, leave the final state in the host columns."""
+        be = self.backend
+        tpt = self.ticks_per_telemetry
+        t0 = time.perf_counter()
+        self._upload_inputs()
         upload_ms = (time.perf_counter() - t0) * 1e3
         body_cols = [(component_id("world_pos"), 0, 7), (component_id("world_vel"), 7, 13),
                      (component_id("world_accel"), 13, 19), (component_id("force"), 19, 25)]
@@ -702,6 +810,9 @@ class Exec:
         """exec.rs:111-173: `while remaining > 0 { exec.run(); commit_world_head }` — one
         invoke_batch of ticks_per_telemetry ticks per cycle, a history row per cycle.  Runs without host
         callbacks take the device-resident route for their whole cycles (same rows, one transfer)."""
+        if self._ensemble:
+            self._run_ensemble(ticks, is_canceled, pre_step, post_step)
+            return self
         remaining = int(ticks)
         host_cb = bool(self.pre_systems or self.post_systems or pre_step or post_step)
         if self._ring_cap and not host_cb and is_canceled is None and remaining >= self.ticks_per_telemetry:
@@ -741,6 +852,8 @@ class Exec:
     def history(self, names: Union[str, Sequence[str]]):
         """`exec.history("e1.world_pos")` -> {name: rows[T, width]} (world 0; use
         `history_worlds` for the batch).  The reference returns a polars frame."""
+        if self._ensemble:
+            self._no_rows("history()")
         if isinstance(names, str):
             names = [names]
         out = {}
@@ -765,6 +878,8 @@ class Exec:
         `close_db()` finishes the directory."""
         from . import db_sink
 
+        if self._ensemble:
+            self._no_rows("attach_db()")
         if getattr(self, "_db", None) is not None:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "a database is already attached")
         self._db = (db_sink.LiveDbWriter(self, path, world=world) if start_timestamp_us is None
@@ -780,15 +895,43 @@ class Exec:
         reference's `init_db` + `commit_world_head_unified` leave on disk for `elodin-db export` / the editor."""
         from . import db_sink
 
+        if self._ensemble:
+            self._no_rows("write_db()")
         if start_timestamp_us is None:
             return db_sink.write_db(self, path, world=world)
         return db_sink.write_db(self, path, start_timestamp_us, world)
 
     def history_worlds(self, pair: str) -> np.ndarray:
+        if self._ensemble:
+            self._no_rows("history_worlds()")
         ent, comp = pair.rsplit(".", 1)
         col = self.world.columns[component_id(comp)]
         row = col.row_of(self.world.entity_by_name(ent))
         return np.stack([h[:, row] for h in self._history[col.component.id]])
+
+    def ensemble(self, pair: str) -> Dict[str, np.ndarray]:
+        """`exec.ensemble("rocket.world_pos")` -> {"count", "mean", "std", "min", "max"}, each [rows, width]: one row
+        per telemetry cycle (row 0 = the initial state), taken over the worlds whose value is finite; count = the
+        number of such worlds (a diverged world is missing from it), std = sqrt(m2 / count) (numpy's ddof=0), NaN
+        where no world is finite.  Needs World.build(..., ensemble=True); the sampled components are world_pos,
+        world_vel, world_accel and force."""
+        if not self._ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "ensemble(): build the Exec with World.build(..., ensemble=True)")
+        ent, comp = pair.rsplit(".", 1)
+        span = _SAMPLED.get(comp)
+        if span is None:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                      f"component not found: {pair} (ensemble statistics cover {', '.join(_SAMPLED)})")
+        col = self.world.columns[component_id(comp)]
+        ent_id = self.world.entity_by_name(ent)
+        if ent_id not in col.entity_ids:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
+        t = np.concatenate(self._ens_rows)[:, col.row_of(ent_id), span[0]:span[1], :]  # [rows, width, 5]
+        count = np.ascontiguousarray(t[..., 0])
+        with np.errstate(invalid="ignore", divide="ignore"):
+            std = np.sqrt(t[..., 2] / count)
+        return {"count": count, "mean": np.ascontiguousarray(t[..., 1]), "std": std,
+                "min": np.ascontiguousarray(t[..., 3]), "max": np.ascontiguousarray(t[..., 4])}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

@@ -275,6 +275,28 @@ uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h);
 int b200_sixdof_trajectory_download(b200_sixdof *h, void *dst, uint64_t bytes);
 int b200_sixdof_trajectory_reset(b200_sixdof *h);
 
+/* ---- ensemble statistics: the world axis reduced on the device, so that a Monte-Carlo campaign records dispersion
+ * over time without moving every world's state to the host.  A group is 5 f64 over the worlds of one sampled value of
+ * one entity:  count  = worlds whose value is finite (a double, exact up to 2^53),
+ *              mean, m2 = sum (x - mean)^2, min, max  over those finite values only  (std = sqrt(m2 / count));
+ * a group with count = 0 holds NaN in the other four.  A non-finite world is therefore never averaged in: a diverged
+ * run shows up as a missing count.  Partial groups are merged with Chan et al.'s pairwise update in a fixed order (no
+ * atomics): the same input gives the same bits on every call, and a sample's bits do not depend on how many other
+ * samples are reduced with it.  Both device entries run on the handle's stream, return once dst is filled (like
+ * b200_sixdof_trajectory_download), count their launches in timings.kernel_launches, and take host or device dst;
+ * `bytes` must match exactly (else B200_ERR_VALUE_SIZE_MISMATCH). ---- */
+#define B200_STATS_FIELDS 5u  /* count, mean, m2 = sum (x - mean)^2, min, max  over the finite values of the worlds */
+/* the samples now in the trajectory ring, reduced over the world axis:
+ * dst = [trajectory_len][n_entities][trajectory_width][5] f64.  An empty ring takes bytes = 0 and launches nothing. */
+int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* the current device state: world_pos, world_vel, world_accel, force (the 25-component B200_TRAJ_FULL sample layout):
+ * dst = [n_entities][25][5] f64 */
+int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* host-only: merge n_parts tables of n_groups stat groups each ([n_parts][n_groups][5]), left to right in part order,
+ * into out[n_groups][5] — the cross-rank step of a world-sharded campaign (ranks exchange their tables over any channel;
+ * every rank that merges the same tables in the same order gets the same bits).  Needs no GPU. */
+int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, double *out);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
