@@ -22,7 +22,7 @@ from .effectors import (DragQuadratic, GravityConst, GravityEGM08, GravityEdges,
 from .executor import B200Exec, device_count, merge_stats, pinned_empty, pinned_free
 from .world import (Annotated, Archetype, Body, Component, ComponentType, Edge, EntityId, Exec, Force, HostSystem,
                     Inertia, Integrator, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
-                    SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, World, WorldAccel,
+                    SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, Threshold, World, WorldAccel,
                     WorldPos, WorldVel, dataclass, host_system, quantised_time_step, six_dof, ticks_per_telemetry)
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -60,8 +60,12 @@ SYMBOLS = [
     "b200_sixdof_trajectory_allgather", "b200_sixdof_step_row_sharded", "b200_probe_pcie_gbs",
     "b200_comm_peer_attach", "b200_comm_peer_attached", "b200_comm_peer_detach", "b200_selftest_shared_divisor", "b200_probe_zero_copy_gbs", "b200_egm08_stream_len", "b200_egm08_stream",
     "b200_sixdof_trajectory_stats", "b200_sixdof_state_stats", "b200_stats_merge",
+    "b200_sixdof_summary_begin", "b200_sixdof_summary_add_state", "b200_sixdof_summary_add_trajectory",
+    "b200_sixdof_extrema_download", "b200_sixdof_thresholds_download",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
+EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
+MAX_THRESHOLDS = 8
 COMM_ID_BYTES = 128
 
 
@@ -112,6 +116,15 @@ class Timings(C.Structure):
         ("invoke_wall_ms", C.c_double),
         ("kernel_launches", C.c_uint64),
         ("ticks", C.c_uint64),
+    ]
+
+
+class Threshold(C.Structure):
+    _fields_ = [
+        ("entity", C.c_uint64),
+        ("plane", C.c_uint32),
+        ("above", C.c_int32),
+        ("value", C.c_double),
     ]
 
 
@@ -184,6 +197,11 @@ def lib():
     L.b200_sixdof_trajectory_stats.argtypes = [vp, vp, u64]
     L.b200_sixdof_state_stats.argtypes = [vp, vp, u64]
     L.b200_stats_merge.argtypes = [C.POINTER(C.c_double), u32, u64, C.POINTER(C.c_double)]
+    L.b200_sixdof_summary_begin.argtypes = [vp, u32, C.POINTER(Threshold), u32]
+    L.b200_sixdof_summary_add_state.argtypes = [vp]
+    L.b200_sixdof_summary_add_trajectory.argtypes = [vp]
+    L.b200_sixdof_extrema_download.argtypes = [vp, vp, u64]
+    L.b200_sixdof_thresholds_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -720,6 +720,8 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->stage_in) cudaFree(h->stage_in);
     if (h->stage_out) cudaFree(h->stage_out);
     if (h->traj) cudaFree(h->traj);
+    if (h->sum_ext) cudaFree(h->sum_ext);
+    if (h->sum_thr) cudaFree(h->sum_thr);
     for (auto &e : h->chunk_in) if (e) cudaEventDestroy(e);
     for (auto &e : h->chunk_out) if (e) cudaEventDestroy(e);
     if (h->host_pack) cudaFreeHost(h->host_pack);
@@ -1233,6 +1235,168 @@ int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, d
         o[3] = any ? acc.mn : nan;
         o[4] = any ? acc.mx : nan;
     }
+    return B200_OK;
+}
+
+// The fold parameters of the handle's summary accumulators; the caller fills in the rows.
+static SummaryParams summary_params(const b200_sixdof *h)
+{
+    SummaryParams S{};
+    S.ld = h->ld;
+    S.n_bodies = h->n_bodies;
+    S.n_entities = (uint32_t)h->desc.n_entities;
+    S.n_thr = (uint32_t)h->sum_thr_list.size();
+    S.ext = h->sum_extrema ? h->sum_ext : nullptr;
+    S.thr = S.n_thr ? h->sum_thr : nullptr;
+    for (uint32_t i = 0; i < S.n_thr; ++i) {
+        const b200_threshold &t = h->sum_thr_list[i];
+        S.t[i] = {(uint32_t)t.entity, t.plane, t.above ? 1 : 0, 0u, t.value};
+    }
+    uint32_t seen = 0;
+    for (uint32_t p = 0; p < 25; ++p) {
+        bool used = h->sum_extrema;
+        for (uint32_t i = 0; i < S.n_thr; ++i) used = used || S.t[i].plane == p;
+        if (used && !((seen >> p) & 1u)) {
+            seen |= 1u << p;
+            S.planes[S.n_planes++] = (uint8_t)p;
+        }
+    }
+    return S;
+}
+
+static int summary_ready(b200_sixdof *h, const char *what)
+{
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (!h->sum_begun) return fail(B200_ERR_INVALID_ARGUMENT, "%s: call b200_sixdof_summary_begin first", what);
+    return B200_OK;
+}
+
+static int run_summary_fold(b200_sixdof *h, const SummaryParams &S)
+{
+    int launches = 0;
+    CU(h, launch_summary_fold(S, &launches, h->stream));
+    h->timings.kernel_launches += (uint64_t)launches;
+    return B200_OK;
+}
+
+int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_threshold *t, uint32_t n_thresholds)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (n_thresholds > B200_MAX_THRESHOLDS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u thresholds: at most %u", n_thresholds, B200_MAX_THRESHOLDS);
+    if (!extrema && n_thresholds == 0) return fail(B200_ERR_INVALID_ARGUMENT, "summary_begin: neither extrema nor thresholds");
+    if (n_thresholds && !t) return fail(B200_ERR_INVALID_ARGUMENT, "null thresholds");
+    for (uint32_t i = 0; i < n_thresholds; ++i) {
+        if (t[i].entity >= h->desc.n_entities)
+            return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: entity row %llu, the world has %llu", i,
+                        (unsigned long long)t[i].entity, (unsigned long long)h->desc.n_entities);
+        if (t[i].plane >= 25) return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: plane %u, a row has 25", i, t[i].plane);
+        if (std::isnan(t[i].value)) return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: the bound is NaN", i);
+    }
+    h->sum_begun = false;
+    if (extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 125ull * h->ld * 8ull));
+    const uint64_t thr_bytes = h->desc.n_worlds * n_thresholds * 26ull * 8ull;
+    if (thr_bytes > h->sum_thr_bytes) {
+        if (h->sum_thr) CU(h, cudaFree(h->sum_thr));
+        h->sum_thr = nullptr;
+        h->sum_thr_bytes = 0;
+        CU(h, cudaMalloc(&h->sum_thr, thr_bytes));
+        h->sum_thr_bytes = thr_bytes;
+    }
+    h->sum_extrema = extrema != 0;
+    h->sum_thr_list.assign(t, t + n_thresholds);
+    int launches = 0;
+    CU(h, launch_summary_clear(summary_params(h), &launches, h->stream));
+    h->timings.kernel_launches += (uint64_t)launches;
+    h->sum_begun = true;
+    return B200_OK;
+}
+
+int b200_sixdof_summary_add_state(b200_sixdof *h)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "summary_add_state");
+    if (rc) return rc;
+    SummaryParams S = summary_params(h);
+    const uint64_t ids[4] = {B200_ID_WORLD_POS, B200_ID_WORLD_VEL, B200_ID_WORLD_ACCEL, B200_ID_FORCE};
+    uint32_t p = 0;
+    for (uint64_t id : ids) {
+        const Column *c = h->find(id);
+        for (uint32_t j = 0; j < c->width; ++j) S.row[p++] = c->dev + j * h->ld;
+    }
+    S.n_rows = 1;
+    S.tick0 = h->tick;
+    return run_summary_fold(h, S);
+}
+
+int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "summary_add_trajectory");
+    if (rc) return rc;
+    if (!h->traj || h->traj_planes != 25)
+        return fail(B200_ERR_INVALID_ARGUMENT, "summary_add_trajectory needs a B200_TRAJ_FULL trajectory ring");
+    SummaryParams S = summary_params(h);
+    for (uint32_t p = 0; p < 25; ++p) S.row[p] = h->traj + p * h->ld;
+    S.row_stride = 25ull * h->ld;
+    S.n_rows = b200_sixdof_trajectory_len(h);
+    // sample k was recorded when the ticks since the reset reached (k + 1) * every (sixdof_tick.cuh traj slots)
+    S.tick_step = h->desc.trajectory_every;
+    S.tick0 = h->tick - h->ticks_done + S.tick_step;
+    return run_summary_fold(h, S);
+}
+
+// dst on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer in
+// chunks of 256 MB.
+int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "extrema_download");
+    if (rc) return rc;
+    if (!h->sum_extrema) return fail(B200_ERR_INVALID_ARGUMENT, "extrema_download: summary_begin had no extrema");
+    const uint64_t per_body = 125ull * 8ull;
+    const uint64_t want = h->n_bodies * per_body;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "extrema are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    if (want == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    cudaPointerAttributes a{};
+    const bool direct = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
+    (void)cudaGetLastError();
+    const uint64_t chunk = direct ? h->n_bodies : std::max<uint64_t>(1, std::min<uint64_t>(h->n_bodies, (256ull << 20) / per_body));
+    if (!direct && (rc = ensure_staging(h, chunk * per_body))) return rc;
+    for (uint64_t b0 = 0; b0 < h->n_bodies; b0 += chunk) {
+        const uint64_t nb = std::min(chunk, h->n_bodies - b0);
+        double *out = direct ? (double *)dst : h->staging;
+        CU(h, launch_extrema_table(h->sum_ext, h->ld, b0, nb, out, h->stream));
+        h->timings.kernel_launches++;
+        if (!direct) CU(h, cudaMemcpyAsync((char *)dst + b0 * per_body, out, nb * per_body, cudaMemcpyDefault, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream)); // the staging buffer is reused by the next chunk
+    }
+    return B200_OK;
+}
+
+int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "thresholds_download");
+    if (rc) return rc;
+    if (h->sum_thr_list.empty()) return fail(B200_ERR_INVALID_ARGUMENT, "thresholds_download: summary_begin had no thresholds");
+    const uint64_t want = h->desc.n_worlds * h->sum_thr_list.size() * 26ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "threshold events are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    if (want == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    CU(h, cudaMemcpyAsync(dst, h->sum_thr, want, cudaMemcpyDefault, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
 }
 

@@ -61,6 +61,13 @@ struct b200_sixdof {
     // trajectory
     double *traj = nullptr;
     uint32_t traj_planes = 13;   // 25 with B200_TRAJ_FULL
+    // run summaries (b200_sixdof_summary_*): device accumulators, allocated on first use, kept across begins
+    bool sum_begun = false;
+    bool sum_extrema = false;
+    std::vector<b200_threshold> sum_thr_list;
+    double *sum_ext = nullptr;       // 125 planes of ld (SummaryParams::ext)
+    double *sum_thr = nullptr;       // [n_worlds][thresholds][26] (SummaryParams::thr)
+    uint64_t sum_thr_bytes = 0;
     // plumbing
     cudaStream_t stream = nullptr;
     bool own_stream = true;

@@ -179,4 +179,37 @@ uint64_t world_stats_scratch_doubles(const StatsParams &S);
 // one or two launches on s (written to *launches); `scratch` holds world_stats_scratch_doubles(S) f64
 cudaError_t launch_world_stats(const StatsParams &S, double *scratch, int *launches, cudaStream_t s);
 
+// Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
+// row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.
+//   ext: extrema accumulators, plane p * 5 + f of ld doubles (f = min, max, min_tick, max_tick, first_nonfinite_tick),
+//        i.e. body b's 125 values read in plane order are its row of the public table; nullptr = no extrema.
+//   thr: the public threshold table itself, [n_worlds][n_thr][26] f64 (tick, 25 planes); nullptr = no thresholds.
+// Ticks are stored as f64 (exact below 2^53), -1 = none; every accumulator has one owning thread per fold.
+// A fold reads only the planes listed in planes[0 .. n_planes): all 25 with extrema, else the thresholds' planes.
+struct SummaryParams {
+    const double *row[25];
+    uint64_t row_stride;
+    uint64_t n_rows;
+    uint64_t tick0, tick_step;
+    uint64_t ld, n_bodies;
+    uint32_t n_entities;
+    uint32_t n_thr;
+    double *ext;
+    double *thr;
+    uint32_t n_planes;
+    uint8_t planes[25];
+    struct Thr {
+        uint32_t entity, plane;
+        int32_t above;
+        uint32_t pad;
+        double value;
+    } t[B200_MAX_THRESHOLDS];
+};
+// the accumulators of S (ext and / or thr) set to "nothing seen yet"; launches written to *launches (0 or 1)
+cudaError_t launch_summary_clear(const SummaryParams &S, int *launches, cudaStream_t s);
+// fold S's rows into the accumulators; launches written to *launches (0 when there are no rows, else 1)
+cudaError_t launch_summary_fold(const SummaryParams &S, int *launches, cudaStream_t s);
+// extrema accumulators of bodies [b0, b0 + nb) -> out[nb][125] (the public table's rows)
+cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint64_t b0, uint64_t nb, double *out, cudaStream_t s);
+
 } // namespace b200

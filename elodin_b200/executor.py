@@ -252,6 +252,40 @@ class B200Exec:
         _lib.check(self._L.b200_sixdof_state_stats(self._h, out.ctypes.data, out.nbytes))
         return out
 
+    # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
+    def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
+        """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
+        up to 8 (entity row, plane 0..24, above, value) tuples, each firing on value > bound (above) or < bound."""
+        ts = list(thresholds)
+        arr = (_lib.Threshold * max(len(ts), 1))()
+        for i, (entity, plane, above, value) in enumerate(ts):
+            arr[i] = _lib.Threshold(int(entity), int(plane), 1 if above else 0, float(value))
+        _lib.check(self._L.b200_sixdof_summary_begin(self._h, 1 if extrema else 0, arr, len(ts)))
+        self._n_thresholds = len(ts)
+
+    def summary_add_state(self) -> None:
+        """Fold the current device state as one row at the current tick."""
+        _lib.check(self._L.b200_sixdof_summary_add_state(self._h))
+
+    def summary_add_trajectory(self) -> None:
+        """Fold every sample now in the (trajectory_full) ring, each at the tick it was recorded."""
+        _lib.check(self._L.b200_sixdof_summary_add_trajectory(self._h))
+
+    def extrema(self) -> np.ndarray:
+        """[n_worlds, n_entities, 25, 5]: (min, max, min_tick, max_tick, first_nonfinite_tick) of every plane of the
+        B200_TRAJ_FULL row layout over the rows folded; min / max over the finite values (NaN if none), ticks -1 where
+        they never applied."""
+        out = np.empty((self.n_worlds, self.n_entities, 25, _lib.EXTREMA_FIELDS))
+        _lib.check(self._L.b200_sixdof_extrema_download(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    def thresholds(self) -> np.ndarray:
+        """[n_worlds, n_thresholds, 26]: the tick of each threshold's first firing row (-1 = never), then the
+        entity's 25 planes at that row (NaN if it never fired)."""
+        out = np.empty((self.n_worlds, getattr(self, "_n_thresholds", 0), 26))
+        _lib.check(self._L.b200_sixdof_thresholds_download(self._h, out.ctypes.data, out.nbytes))
+        return out
+
     # ---- plumbing ---------------------------------------------------------------
     def set_stream(self, cuda_stream: Optional[int]) -> None:
         """Run on a caller-owned cudaStream_t (0 = the legacy default stream, which is what

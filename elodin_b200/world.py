@@ -436,10 +436,13 @@ class World:
               max_ticks: Optional[int] = None, optimize: bool = False, db_path: Optional[str] = None,
               backend: str = "b200", math: str = "exact", n_worlds: int = 1, device: int = -1,
               world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
-              ensemble: bool = False, ensemble_ring: Optional[int] = None) -> "Exec":
+              ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
+              thresholds: Optional[Sequence["Threshold"]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
-        between two reductions (default: as many as fit in 256 MiB, at least one)."""
+        between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
+        also keeps every world's extrema over its telemetry rows (`Exec.extrema`) and `thresholds` (up to 8
+        `Threshold`s) every world's first threshold events (`Exec.threshold`), both on the device."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -447,7 +450,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring)
+                    ensemble, ensemble_ring, extrema, thresholds)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -503,6 +506,40 @@ _SAMPLED = {"world_pos": (0, 7), "world_vel": (7, 13), "world_accel": (13, 19), 
 _ENSEMBLE_RING_BYTES = 256 << 20  # device memory of the ensemble mode's trajectory ring
 
 
+def _sampled_span(pair: str, what: str):
+    """`<entity>.<component>` -> (entity, (first, end) plane of the component in a 25-plane row)."""
+    ent, _, comp = pair.rpartition(".")
+    span = _SAMPLED.get(comp)
+    if not ent or span is None:
+        raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                  f"component not found: {pair} ({what} cover {', '.join(_SAMPLED)})")
+    return ent, span
+
+
+class Threshold:
+    """A per-world event for `World.build(..., ensemble=True, thresholds=[...])`: the first telemetry row at which
+    component `index` of `pair` ("<entity>.<component>": world_pos, world_vel, world_accel or force) is strictly
+    below `below`, or strictly above `above` (exactly one of the two).  It is a first-time condition, not a crossing:
+    row 0 (the initial state) is checked too, so a world that starts beyond the bound fires at its initial tick.
+    NaN never fires."""
+
+    def __init__(self, pair: str, index: int, below: Optional[float] = None, above: Optional[float] = None):
+        if (below is None) == (above is None):
+            raise ValueError(f"Threshold({pair!r}, {index!r}): give exactly one of below= and above=")
+        value = float(above if below is None else below)
+        if np.isnan(value):
+            raise ValueError(f"Threshold({pair!r}, {index!r}): the bound is NaN, it would never fire")
+        self.entity, span = _sampled_span(pair, "thresholds")
+        width = span[1] - span[0]
+        if isinstance(index, bool) or not isinstance(index, (int, np.integer)) or not 0 <= index < width:
+            raise ValueError(f"Threshold({pair!r}, {index!r}): index must be an integer in [0, {width})")
+        self.pair, self.index, self.above, self.value = pair, int(index), below is None, value
+        self.plane = span[0] + self.index  # in the 25-plane row layout
+
+    def __repr__(self) -> str:
+        return f"Threshold({self.pair!r}, {self.index}, {'above' if self.above else 'below'}={self.value!r})"
+
+
 class _Row(np.ndarray):
     def to_numpy(self):
         return np.asarray(self)
@@ -522,7 +559,8 @@ class Exec:
     def __init__(self, world: World, system: System, simulation_rate: float, telemetry_rate: Optional[float],
                  max_ticks: Optional[int], math: str, n_worlds: int, device: int,
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
-                 ensemble: bool = False, ensemble_ring: Optional[int] = None):
+                 ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
+                 thresholds: Optional[Sequence[Threshold]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -558,6 +596,24 @@ class Exec:
             col = world.columns.get(component_id(cname))
             if col is None or col.entity_ids != bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {cname}")
+        # run summaries: checked here, before any device call
+        self._extrema = bool(extrema)
+        self._thresholds = list(thresholds or [])
+        if (self._extrema or self._thresholds) and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "extrema and thresholds need World.build(..., ensemble=True)")
+        if len(self._thresholds) > _lib.MAX_THRESHOLDS:
+            raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
+        self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
+        for t in self._thresholds:
+            if not isinstance(t, Threshold):
+                raise TypeError(f"thresholds take el.Threshold objects, got {t!r}")
+            try:
+                ent = world.entity_by_name(t.entity)
+            except _lib.B200ValueError:
+                ent = None
+            if ent not in bodies:
+                raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
+            self._threshold_rows.append((bodies.index(ent), t.plane, t.above, t.value))
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
         # a body-row-expanded copy of the column for the device; no members / foreign order -> error.
@@ -609,10 +665,14 @@ class Exec:
         self._history: Dict[int, List[np.ndarray]] = {cid: [] for cid in self.world.columns}
         self._globals_hist: List[tuple] = []
         self._ens_rows: List[np.ndarray] = []  # ensemble mode: blocks of rows [k, n_entities, 25, 5]
+        self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
+        if self._extrema or self._thresholds:
+            self.backend.summary_begin(self._extrema, self._threshold_rows)
         if self._ensemble:
             self._history = {}
             self._upload_inputs()
             self._ens_rows.append(self.backend.state_stats()[None])  # row 0: the initial state
+            self._fold_summary(ring=False)
             self._globals_hist.append((self.tick, self.sim_time_step))
         else:
             self._record()
@@ -689,6 +749,12 @@ class Exec:
             else:
                 be.upload(cid, self.world.columns[cid].buffer)
 
+    def _fold_summary(self, ring: bool) -> None:
+        """Run summaries: fold the ring's samples (ring=True) or the current state as one row, on the device."""
+        if self._extrema or self._thresholds:
+            (self.backend.summary_add_trajectory if ring else self.backend.summary_add_state)()
+            self._summary_tables.clear()
+
     def _add_ensemble_rows(self, rows: np.ndarray, tpt: int) -> None:
         """rows [k, n_entities, 25, 5]: k telemetry rows, `tpt` ticks apart, the last one at the current tick."""
         k = rows.shape[0]
@@ -713,6 +779,7 @@ class Exec:
                 be.trajectory_reset()
                 be.step(c * tpt)
                 rows = be.trajectory_stats()                          # [c, n_entities, 25, 5]
+                self._fold_summary(ring=True)
                 self.tick += c * tpt
                 self._add_ensemble_rows(rows, tpt)
                 ms = (time.perf_counter() - t0) * 1e3
@@ -726,6 +793,7 @@ class Exec:
                 be.step(remaining)
                 self.tick += remaining
                 self._add_ensemble_rows(be.state_stats()[None], tpt)
+                self._fold_summary(ring=False)
                 self._prof["execute_buffers"].append((time.perf_counter() - t0) * 1e3)
                 for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
                     self._prof[k_dst].append(0.0)
@@ -757,6 +825,7 @@ class Exec:
                 done += per_call
             t_hist = time.perf_counter()
             self._add_ensemble_rows(be.trajectory_stats() if n == tpt else be.state_stats()[None], tpt)
+            self._fold_summary(ring=n == tpt)
             self._prof["add_to_history"].append((time.perf_counter() - t_hist) * 1e3)
             remaining -= n
             if is_canceled is not None and is_canceled():
@@ -917,21 +986,59 @@ class Exec:
         world_vel, world_accel and force."""
         if not self._ensemble:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "ensemble(): build the Exec with World.build(..., ensemble=True)")
-        ent, comp = pair.rsplit(".", 1)
-        span = _SAMPLED.get(comp)
-        if span is None:
-            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
-                                      f"component not found: {pair} (ensemble statistics cover {', '.join(_SAMPLED)})")
-        col = self.world.columns[component_id(comp)]
-        ent_id = self.world.entity_by_name(ent)
-        if ent_id not in col.entity_ids:
-            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
-        t = np.concatenate(self._ens_rows)[:, col.row_of(ent_id), span[0]:span[1], :]  # [rows, width, 5]
+        row, span = self._sampled_row(pair, "ensemble statistics")
+        t = np.concatenate(self._ens_rows)[:, row, span[0]:span[1], :]  # [rows, width, 5]
         count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
             std = np.sqrt(t[..., 2] / count)
         return {"count": count, "mean": np.ascontiguousarray(t[..., 1]), "std": std,
                 "min": np.ascontiguousarray(t[..., 3]), "max": np.ascontiguousarray(t[..., 4])}
+
+    def _sampled_row(self, pair: str, what: str):
+        """`<entity>.<component>` -> (Body row of the entity, plane span of the component in a 25-plane row)."""
+        ent, span = _sampled_span(pair, what)
+        ent_id = self.world.entity_by_name(ent)
+        col = self.world.columns[component_id("world_pos")]
+        if ent_id not in col.entity_ids:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
+        return col.row_of(ent_id), span
+
+    def _summary_table(self, name: str) -> np.ndarray:
+        """The backend's extrema / thresholds table, downloaded once per fold."""
+        if name not in self._summary_tables:
+            self._summary_tables[name] = getattr(self.backend, name)()
+        return self._summary_tables[name]
+
+    def extrema(self, pair: str) -> Dict[str, np.ndarray]:
+        """`exec.extrema("rocket.world_pos")` -> {"min", "max", "min_tick", "max_tick", "first_nonfinite_tick"}, each
+        [n_worlds, width], over every telemetry row of each world (row 0 = the initial state): min / max over the
+        finite values (NaN if none), the tick of the row that holds them (the earliest on ties) and the tick of the first
+        NaN / inf row; ticks are int64, -1 where they never applied.  Needs World.build(..., ensemble=True,
+        extrema=True)."""
+        if not self._extrema:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "extrema(): build the Exec with World.build(..., ensemble=True, extrema=True)")
+        row, span = self._sampled_row(pair, "extrema")
+        t = self._summary_table("extrema")[:, row, span[0]:span[1], :]  # [n_worlds, width, 5]
+        out = {k: np.ascontiguousarray(t[..., f]) for f, k in enumerate(("min", "max"))}
+        for f, k in enumerate(("min_tick", "max_tick", "first_nonfinite_tick"), start=2):
+            out[k] = t[..., f].astype(np.int64)
+        return out
+
+    def threshold(self, i: int) -> Dict[str, np.ndarray]:
+        """`exec.threshold(i)` -> {"tick": int64 [n_worlds], "world_pos": [n_worlds, 7], "world_vel", "world_accel",
+        "force"}: for threshold i of World.build(..., thresholds=[...]), the tick of each world's first telemetry row
+        that meets it (-1 = never) and the entity's state at that row (NaN where it never fired)."""
+        if not self._thresholds:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "threshold(): build the Exec with World.build(..., ensemble=True, thresholds=[...])")
+        if not 0 <= i < len(self._thresholds):
+            raise IndexError(f"threshold {i}: this Exec has {len(self._thresholds)}")
+        t = self._summary_table("thresholds")[:, i, :]  # [n_worlds, 26]
+        out = {"tick": t[:, 0].astype(np.int64)}
+        for name, (lo, hi) in _SAMPLED.items():
+            out[name] = np.ascontiguousarray(t[:, 1 + lo:1 + hi])
+        return out
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

@@ -297,6 +297,49 @@ int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes);
  * every rank that merges the same tables in the same order gets the same bits).  Needs no GPU. */
 int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, double *out);
 
+/* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
+ * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the
+ * B200_TRAJ_FULL layout (world_pos[7], world_vel[6], world_accel[6], force[6]: planes 0..24) at one tick.
+ * Extrema, per (world, entity, plane), 5 f64:
+ *   min, max              over the rows whose value is finite (NaN while there is none),
+ *   min_tick, max_tick    tick of the row that holds min / max; among equal values the earliest tick wins,
+ *   first_nonfinite_tick  tick of the first row whose value is NaN or +-inf;
+ * a tick field is -1 where it never applied.
+ * Thresholds, per (world, threshold), 26 f64: the tick of the first row where the value of (entity, plane) is strictly
+ * below (above = 0) or above (above != 0) `value` (NaN never fires), then the entity's 25 planes at that row; tick -1
+ * and NaN planes while it has not fired.  This is a first-time condition, not a crossing: a world that starts beyond
+ * the bound fires at its first row.
+ * Every comparison is strict and ties go to the smaller tick, so folding the same rows in any grouping or order, or
+ * folding a row twice, gives the same bits; no field involves arithmetic.  Ticks have the resolution of the rows folded
+ * (telemetry rows, not ticks).  Every entry runs on the handle's stream and leaves the sticky status alone on success;
+ * each one called before b200_sixdof_summary_begin fails with B200_ERR_INVALID_ARGUMENT. ---- */
+#define B200_EXTREMA_FIELDS 5u   /* min, max, min_tick, max_tick, first_nonfinite_tick */
+#define B200_MAX_THRESHOLDS 8u
+typedef struct b200_threshold {
+    uint64_t entity;  /* entity row within a world (< n_entities)                  */
+    uint32_t plane;   /* 0..24 in the B200_TRAJ_FULL row layout, e.g. 6 = world_pos z */
+    int32_t  above;   /* 0: fires on value < bound; otherwise on value > bound         */
+    double   value;   /* the bound (not NaN)                                           */
+} b200_threshold;
+/* Start (or start over): extrema != 0 keeps the extrema table; t[0 .. n_thresholds) are copied.  Allocates the device
+ * accumulators on first use (extrema: 1000 B per body; thresholds: 208 B per world and threshold) and clears them.
+ * B200_ERR_INVALID_ARGUMENT: entity >= n_entities, plane >= 25, a NaN bound, n_thresholds > B200_MAX_THRESHOLDS, or
+ * neither extrema nor thresholds. */
+int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_threshold *t, uint32_t n_thresholds);
+/* fold the current device state as one row at the current tick (b200_sixdof_tick_count) */
+int b200_sixdof_summary_add_state(b200_sixdof *h);
+/* fold the b200_sixdof_trajectory_len samples now in the ring (B200_TRAJ_FULL only, else B200_ERR_INVALID_ARGUMENT);
+ * sample k is the row at tick (tick_count - T) + (k + 1) * trajectory_every, T = ticks stepped since the last
+ * b200_sixdof_trajectory_reset (or create) by b200_sixdof_step and b200_sixdof_invoke_batch together.  An empty ring
+ * launches nothing. */
+int b200_sixdof_summary_add_trajectory(b200_sixdof *h);
+/* dst = [n_worlds][n_entities][25][5] f64; refused when begin had no extrema */
+int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes);
+/* dst = [n_worlds][n_thresholds][26] f64: tick, then the 25 planes; refused when begin had no thresholds */
+int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes);
+/* Both downloads take host or device dst, return once it is filled, need `bytes` to match exactly (else
+ * B200_ERR_VALUE_SIZE_MISMATCH) and count their launches in timings.kernel_launches, as the statistics entries do. */
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
