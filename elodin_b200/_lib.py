@@ -62,10 +62,12 @@ SYMBOLS = [
     "b200_sixdof_trajectory_stats", "b200_sixdof_state_stats", "b200_stats_merge",
     "b200_sixdof_summary_begin", "b200_sixdof_summary_add_state", "b200_sixdof_summary_add_trajectory",
     "b200_sixdof_extrema_download", "b200_sixdof_thresholds_download",
+    "b200_sixdof_trajectory_quantiles", "b200_sixdof_state_quantiles", "b200_sixdof_quantile_reads",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
 MAX_THRESHOLDS = 8
+MAX_QUANTILES = 16  # levels per quantile call
 COMM_ID_BYTES = 128
 
 
@@ -202,6 +204,10 @@ def lib():
     L.b200_sixdof_summary_add_trajectory.argtypes = [vp]
     L.b200_sixdof_extrema_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_thresholds_download.argtypes = [vp, vp, u64]
+    L.b200_sixdof_trajectory_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_state_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_quantile_reads.argtypes = [vp]
+    L.b200_sixdof_quantile_reads.restype = C.c_double
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1,0 +1,603 @@
+// Ensemble quantiles over the world axis: for every (plane, entity) group and every level q, numpy's default
+// ("linear") quantile of the finite values of all worlds (include/b200_sixdof.h b200_sixdof_trajectory_quantiles /
+// _state_quantiles).  The result is two order statistics and a fixed lerp, so it needs no floating-point reduction:
+// it is exact, and independent of the launch shape and of the order of any atomic.
+//
+// Values are ordered by the IEEE totalOrder key (key(-0) < key(+0); NaN and +-inf are dropped before).  Two routes,
+// chosen from n_worlds alone:
+//  - small groups (n_worlds <= kSmallMax): a warp (n_worlds <= 256) or a block per group loads the group's finite keys
+//    into shared memory, sorts them (bitonic) and reads off the ranks.  One read of the planes, one launch, no scratch.
+//  - large groups: a radix select on the key with a fixed launch sequence, pass 0 and passes 1..kLevels:
+//      pass 0   per group: finite count n and min / max key (integer atomics)
+//      plan     every rank a level needs is in [kmin, kmax]
+//      pass k   per group, one histogram of kBins bins over the key ranges that still hold a rank too large to finish
+//               (each range gets kBins / 2^ceil(log2 ranges) bins, equal-width in key space); a range small enough is
+//               instead copied to scratch ("compacted") in the same pass
+//      plan     each rank moves to its bin: a range of one key is finished, a range of <= kBucketCap keys is compacted
+//               by the next pass, the others are refined by the next pass
+//      finish   per group, each compacted range is sorted in shared memory and its ranks read off
+//    A range of 2^64 keys takes at most 14 + 6 * 9 = 68 bits of refinement in passes 1..7 (kBins = 2^14 bins for one
+//    range, at least 2^9 for up to 32), so every rank is finished after pass kLevels = 7: at most 8 reads of the planes
+//    on any data.  On continuous data pass 1 leaves buckets of a few thousand keys, so the planes are read 3 times
+//    (count, histogram, compaction).  A pass reads nothing of a group whose ranks are all finished.
+//    Scratch per group: kBins u32 + kGroupCap u64 keys + the plan (QGroup), about 198 KB.  The groups run in slices of
+//    at most kSliceGroups (whole planes, or entity ranges of one plane when a plane has more entities), the same launch
+//    sequence per slice, so the scratch stays under kScratchCap = 256 MiB whatever the ring or entity count.
+// Counts and keys are integers, so the order in which atomics land changes no result.
+#include <algorithm>
+#include <cfloat>
+#include <cub/block/block_scan.cuh>
+
+#include "sixdof_internal.h"
+
+namespace b200 {
+namespace {
+
+constexpr unsigned kSmallMax = 8192;   // largest n_worlds sorted in shared memory (64 KB of keys)
+constexpr unsigned kWarpMax = 256;     // up to this n_worlds a warp sorts a group, eight groups per block
+constexpr unsigned kBins = 1u << 14;   // histogram bins per group and pass (64 KB of u32, in shared memory when E = 1)
+constexpr unsigned kBinBits = 14;
+constexpr unsigned kBucketCap = 8192;  // a range of at most this many keys is compacted and sorted in shared memory
+constexpr unsigned kGroupCap = 16384;  // compacted keys per group
+constexpr int kLevels = 7;             // histogram passes after pass 0
+constexpr unsigned kSlots = 2 * B200_MAX_QUANTILES;
+constexpr unsigned kPassThreads = 256;
+constexpr unsigned kPlanThreads = 1024;
+
+enum : uint32_t { kDone = 0, kRefine = 1, kCompact = 2, kCompacted = 3, kUnused = 4 };
+
+// one rank a level needs: x_(rank) is the key in [lo, hi] of rank rr among the group's keys in that range
+struct QSlot {
+    unsigned long long lo, hi;
+    uint32_t rr, count, state, owner;  // owner: the first slot of the same range (shares its bins / compaction)
+    uint32_t bin0, shift, cofs, fill;  // refine: bins [bin0, bin0 + (hi - lo) >> shift]; compact: area[cofs ..]
+};
+
+struct QGroup {
+    unsigned long long kmin, kmax;
+    uint32_t n, todo, used;         // todo: the next pass has work here; used: compacted keys
+    uint32_t n_act, n_refine;       // the next pass's ranges (refine or compact owners): slot[act[0 .. n_act)]
+    uint8_t act[kSlots];
+    QSlot slot[kSlots];
+};
+
+// A slice of the groups the fixed launch sequence runs on: planes [i0, i0 + ni) x entities [e0, e0 + ne); local group
+// g = (i - i0) * ne + (e - e0).  Slices keep the scratch under kScratchCap whatever the ring or entity count.
+struct Slice {
+    uint64_t i0, ni, e0, ne;
+};
+
+struct Layout {
+    uint64_t G;                   // groups of the slice
+    unsigned long long *reads;    // reads of the planes, summed over the groups of every slice of the call
+    QGroup *grp;                  // [G]
+    uint32_t *hist;               // [G][kBins]
+    unsigned long long *area;     // [G][kGroupCap]
+};
+
+__device__ __forceinline__ unsigned long long order_key(double x)
+{
+    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double key_value(unsigned long long k)
+{
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+__device__ __forceinline__ bool finite(double x) { return fabs(x) <= DBL_MAX; }
+
+__device__ inline const double *plane_of(const QuantileParams &S, uint64_t i)
+{
+    const double *p = nullptr;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; ++k) {
+        if (!p && k < S.n_segs) {
+            if (i < S.seg[k].n_planes) p = S.seg[k].base + i * S.ld;
+            else i -= S.seg[k].n_planes;
+        }
+    }
+    return p;
+}
+
+__device__ __forceinline__ double *out_of(const QuantileParams &S, uint64_t i, uint64_t e)
+{
+    const uint64_t W = S.planes_per_sample;
+    return S.out + (((i / W) * S.n_entities + e) * W + i % W) * S.n_q;
+}
+
+// numpy's linear quantile of the n sorted keys, rank -> key given by `at`
+template <class At>
+__device__ double quantile_of(uint32_t n, double q, At at)
+{
+    if (n == 0) return __longlong_as_double(0x7ff8000000000000ll);
+    const double h = __dmul_rn((double)(n - 1), q);
+    if (h >= (double)(n - 1)) return key_value(at(n - 1));
+    const uint32_t i = (uint32_t)floor(h);
+    const double t = __dsub_rn(h, (double)i);
+    const double a = key_value(at(i)), b = key_value(at(i + 1));
+    const double d = __dsub_rn(b, a);
+    return t >= 0.5 ? __dsub_rn(b, __dmul_rn(d, __dsub_rn(1.0, t))) : __dadd_rn(a, __dmul_rn(d, t));
+}
+
+// ranks (i, i + 1) of level l, or (n - 1, unused) when h >= n - 1
+__device__ inline void ranks_of(uint32_t n, double q, uint32_t &r0, uint32_t &r1, bool &two)
+{
+    const double h = __dmul_rn((double)(n - 1), q);
+    two = h < (double)(n - 1);
+    r0 = two ? (uint32_t)floor(h) : n - 1;
+    r1 = r0 + 1;
+}
+
+// ascending bitonic sort of a[0, P) (P a power of two) by `team` threads; sync() is the team barrier
+template <class Sync>
+__device__ void bitonic(unsigned long long *a, uint32_t P, uint32_t tid, uint32_t team, Sync sync)
+{
+    for (uint32_t k = 2; k <= P; k <<= 1) {
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t t = tid; t < P / 2; t += team) {
+                const uint32_t i = 2 * j * (t / j) + t % j, l = i + j;
+                const unsigned long long x = a[i], y = a[l];
+                if ((x > y) == ((i & k) == 0)) { a[i] = y; a[l] = x; }
+            }
+            sync();
+        }
+    }
+}
+
+__device__ __forceinline__ uint32_t pow2_at_least(uint32_t n)
+{
+    return n <= 1 ? 1 : 1u << (32 - __clz(n - 1));
+}
+
+// ---- small groups ---------------------------------------------------------------------------------------------------
+
+// load the finite keys of group (i, e) into a[], pad to a power of two with ~0 (above every finite key), sort
+template <class Sync>
+__device__ uint32_t load_sort(const QuantileParams &S, uint64_t i, uint64_t e, unsigned long long *a, uint32_t *cnt,
+                              uint32_t tid, uint32_t team, Sync sync)
+{
+    if (tid == 0) *cnt = 0;
+    sync();
+    const double *p = plane_of(S, i) + e;
+    for (uint64_t w = tid; w < S.n_worlds; w += team) {
+        const double x = p[w * S.n_entities];
+        if (finite(x)) a[atomicAdd(cnt, 1u)] = order_key(x);
+    }
+    sync();
+    const uint32_t n = *cnt, P = pow2_at_least(n);
+    for (uint32_t k = n + tid; k < P; k += team) a[k] = ~0ull;
+    sync();
+    bitonic(a, P, tid, team, sync);
+    return n;
+}
+
+// a warp per group, eight groups per block (n_worlds <= kWarpMax)
+__global__ void __launch_bounds__(256) quantile_warp_kernel(QuantileParams S)
+{
+    __shared__ unsigned long long keys[8][kWarpMax];
+    __shared__ uint32_t cnt[8];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint64_t G = S.n_planes * S.n_entities;
+    for (uint64_t g = blockIdx.x * 8ull + wid; g < G; g += gridDim.x * 8ull) {
+        const uint64_t i = g / S.n_entities, e = g % S.n_entities;
+        const uint32_t n = load_sort(S, i, e, keys[wid], &cnt[wid], lane, 32, []() { __syncwarp(); });
+        double *o = out_of(S, i, e);
+        for (uint32_t l = lane; l < S.n_q; l += 32)
+            o[l] = quantile_of(n, S.q[l], [&](uint32_t r) { return keys[wid][r]; });
+        __syncwarp();
+    }
+}
+
+// a block per group (kWarpMax < n_worlds <= kSmallMax); dynamic shared memory: pow2(n_worlds) keys
+__global__ void __launch_bounds__(512) quantile_block_kernel(QuantileParams S)
+{
+    extern __shared__ unsigned long long keys[];
+    __shared__ uint32_t cnt;
+    const uint64_t G = S.n_planes * S.n_entities;
+    for (uint64_t g = blockIdx.x; g < G; g += gridDim.x) {
+        const uint64_t i = g / S.n_entities, e = g % S.n_entities;
+        const uint32_t n = load_sort(S, i, e, keys, &cnt, threadIdx.x, blockDim.x, []() { __syncthreads(); });
+        double *o = out_of(S, i, e);
+        for (uint32_t l = threadIdx.x; l < S.n_q; l += blockDim.x)
+            o[l] = quantile_of(n, S.q[l], [&](uint32_t r) { return keys[r]; });
+        __syncthreads();
+    }
+}
+
+// ---- large groups ---------------------------------------------------------------------------------------------------
+
+// Thread mapping of the passes (as in stats_kernels.cu): a task is (plane, world chunk, tile of Et entities); thread t
+// takes entity t % Et of the tile and every J-th world of the chunk, so a warp reads consecutive doubles.
+struct PassShape {
+    uint64_t Et, J, T, Wc, C;
+};
+
+inline PassShape pass_shape(uint64_t n_worlds, uint64_t E, uint64_t n_planes)
+{
+    PassShape s;
+    s.Et = E <= kPassThreads ? E : kPassThreads;
+    s.J = E <= kPassThreads ? kPassThreads / E : 1;
+    s.T = (E + s.Et - 1) / s.Et;
+    // about 4 blocks per SM in all, at least 4096 values per thread-lane group (a block's histogram flush is amortised)
+    const uint64_t want = std::max<uint64_t>(1, 4ull * kNumSMs / std::max<uint64_t>(1, n_planes * s.T));
+    uint64_t per = (n_worlds + want * s.J - 1) / (want * s.J);
+    per = std::max<uint64_t>(per, 16);
+    s.Wc = per * s.J;
+    s.C = (n_worlds + s.Wc - 1) / s.Wc;
+    return s;
+}
+
+// pass 0: finite count and min / max key per group
+__global__ void __launch_bounds__(kPassThreads) quantile_count_kernel(QuantileParams S, Slice sl, PassShape sp, Layout L)
+{
+    const uint64_t E = S.n_entities;
+    const unsigned t = threadIdx.x, el = t % (unsigned)sp.Et, j = t / (unsigned)sp.Et;
+    const uint64_t n_tasks = sl.ni * sp.C * sp.T;
+    for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
+        const uint64_t tile = task % sp.T, c = (task / sp.T) % sp.C, il = task / (sp.T * sp.C);
+        const uint64_t e = tile * sp.Et + el;  // within the slice
+        uint32_t n = 0;
+        unsigned long long mn = ~0ull, mx = 0;
+        const bool live = j < sp.J && e < sl.ne;
+        if (live) {
+            const double *p = plane_of(S, sl.i0 + il) + sl.e0 + e;
+            const uint64_t w1 = min((c + 1) * sp.Wc, S.n_worlds);
+            for (uint64_t w = c * sp.Wc + j; w < w1; w += sp.J) {
+                const double x = p[w * E];
+                if (finite(x)) {
+                    const unsigned long long k = order_key(x);
+                    ++n;
+                    mn = min(mn, k);
+                    mx = max(mx, k);
+                }
+            }
+        }
+        if (sl.ne == 1) {  // one group per block: reduce the warp first
+            for (int o = 16; o > 0; o >>= 1) {
+                n += __shfl_xor_sync(0xffffffffu, n, o);
+                mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+                mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            }
+            if ((t & 31) != 0) n = 0;
+        }
+        if (live && n) {
+            QGroup &G = L.grp[il * sl.ne + e];
+            atomicAdd(&G.n, n);
+            atomicMin(&G.kmin, mn);
+            atomicMax(&G.kmax, mx);
+        }
+    }
+}
+
+// pass k >= 1: histogram of the refined ranges, copy of the compacted ones
+__global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantileParams S, Slice sl, PassShape sp, Layout L)
+{
+    extern __shared__ uint32_t sh_hist[];  // kBins counters when ne == 1 (one group per block), else unused
+    __shared__ unsigned long long sh_lo[kSlots], sh_hi[kSlots];  // ne == 1: the group's active ranges
+    __shared__ uint32_t sh_bin0[kSlots], sh_shift[kSlots], sh_slot[kSlots];
+    const uint64_t E = S.n_entities;
+    const bool shared_hist = sl.ne == 1;
+    const unsigned t = threadIdx.x, el = t % (unsigned)sp.Et, j = t / (unsigned)sp.Et;
+    const uint64_t n_tasks = sl.ni * sp.C * sp.T;
+    for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
+        const uint64_t tile = task % sp.T, c = (task / sp.T) % sp.C, il = task / (sp.T * sp.C);
+        const uint64_t e = tile * sp.Et + el;  // within the slice
+        const bool live = j < sp.J && e < sl.ne;
+        const uint64_t g = il * sl.ne + (live ? e : 0);
+        QGroup &G = L.grp[g];
+        if (shared_hist) {
+            if (!G.todo) continue;  // the whole block is this group: uniform
+            for (uint32_t b = t; b < kBins; b += blockDim.x) sh_hist[b] = 0;
+            if (t < G.n_act) {
+                const QSlot &q = G.slot[G.act[t]];
+                sh_lo[t] = q.lo;
+                sh_hi[t] = q.hi;
+                sh_bin0[t] = q.state == kRefine ? q.bin0 : ~0u;  // ~0: compact
+                sh_shift[t] = q.shift;
+                sh_slot[t] = G.act[t];
+            }
+            __syncthreads();
+        }
+        if (live && G.todo) {
+            uint32_t *hist = L.hist + g * kBins;
+            unsigned long long *area = L.area + g * kGroupCap;
+            const double *p = plane_of(S, sl.i0 + il) + sl.e0 + e;
+            const uint64_t w1 = min((c + 1) * sp.Wc, S.n_worlds);
+            const unsigned long long kmin = G.kmin, kmax = G.kmax;
+            const uint32_t n_act = G.n_act;
+            for (uint64_t w = c * sp.Wc + j; w < w1; w += sp.J) {
+                const double x = p[w * E];
+                if (!finite(x)) continue;
+                const unsigned long long k = order_key(x);
+                if (k < kmin || k > kmax) continue;
+                for (uint32_t r = 0; r < n_act; ++r) {
+                    if (shared_hist) {
+                        if (k < sh_lo[r] || k > sh_hi[r]) continue;
+                        if (sh_bin0[r] != ~0u) atomicAdd(&sh_hist[sh_bin0[r] + (uint32_t)((k - sh_lo[r]) >> sh_shift[r])], 1u);
+                        else area[G.slot[sh_slot[r]].cofs + atomicAdd(&G.slot[sh_slot[r]].fill, 1u)] = k;
+                        break;
+                    }
+                    QSlot &q = G.slot[G.act[r]];
+                    if (k < q.lo || k > q.hi) continue;
+                    if (q.state == kRefine) atomicAdd(&hist[q.bin0 + (uint32_t)((k - q.lo) >> q.shift)], 1u);
+                    else area[q.cofs + atomicAdd(&q.fill, 1u)] = k;
+                    break;
+                }
+            }
+        }
+        if (shared_hist) {
+            __syncthreads();
+            uint32_t *hist = L.hist + g * kBins;
+            for (uint32_t b = t; b < kBins; b += blockDim.x)
+                if (sh_hist[b]) atomicAdd(&hist[b], sh_hist[b]);
+            __syncthreads();
+        }
+    }
+}
+
+__device__ __forceinline__ uint32_t bit_len(unsigned long long x) { return 64 - __clzll(x); }
+
+// Plan after pass `level`: one block per group.  Moves each refined rank into its bin, then (thread 0) groups the ranks
+// into ranges and decides what the next pass does with each; clears the histogram for the next pass.
+__global__ void __launch_bounds__(kPlanThreads) quantile_plan_kernel(QuantileParams S, Layout L, int level)
+{
+    using Scan = cub::BlockScan<uint32_t, kPlanThreads>;
+    __shared__ typename Scan::TempStorage scan_tmp;
+    __shared__ bool dirty;  // the histogram holds counts: the pass before this plan refined a range (or fresh scratch)
+    extern __shared__ uint32_t bins[];  // kBins: the counts of the range being scanned
+    constexpr uint32_t kItems = kBins / kPlanThreads;
+    QGroup &G = L.grp[blockIdx.x];
+    uint32_t *hist = L.hist + (uint64_t)blockIdx.x * kBins;
+    const uint32_t t = threadIdx.x;
+    if (t == 0) dirty = level == 0 || (G.todo && G.n_refine);
+    if (level == 0) {
+        if (t == 0) {
+            for (uint32_t s = 0; s < kSlots; ++s) {
+                QSlot &q = G.slot[s];
+                q = QSlot{G.kmin, G.kmax, 0, G.n, kUnused, s, 0, 0, 0, 0};
+                if (G.n == 0 || s / 2 >= S.n_q) continue;
+                uint32_t r0, r1;
+                bool two;
+                ranks_of(G.n, S.q[s / 2], r0, r1, two);
+                if (s % 2 == 1 && !two) continue;
+                q.rr = s % 2 ? r1 : r0;
+                q.state = kRefine;
+            }
+        }
+    } else {
+        __shared__ QSlot moved[kSlots];  // the new range of each refined rank, applied once every bin is scanned
+        __shared__ uint32_t hit[kSlots];
+        if (t < kSlots) hit[t] = 0;
+        for (uint32_t a = 0; a < kSlots; ++a) {  // each refined range: exclusive scan of its bins, ranks into bins
+            const QSlot o = G.slot[a];
+            if (o.owner != a || o.state != kRefine) continue;  // uniform over the block
+            const uint32_t nb = (uint32_t)((o.hi - o.lo) >> o.shift) + 1;
+            uint32_t sum = 0;
+            for (uint32_t k = 0; k < kItems; ++k) {
+                const uint32_t b = t * kItems + k;
+                bins[b] = b < nb ? hist[o.bin0 + b] : 0;
+                sum += bins[b];
+            }
+            uint32_t base;
+            Scan(scan_tmp).ExclusiveSum(sum, base);  // keys of the range below this thread's bins
+            __syncthreads();
+            for (uint32_t s = a; s < kSlots; ++s) {
+                const QSlot q = G.slot[s];
+                if (q.owner != a || q.state != kRefine || q.rr < base || q.rr >= base + sum) continue;
+                uint32_t below = base, k = 0;
+                while (q.rr >= below + bins[t * kItems + k]) below += bins[t * kItems + k++];
+                const unsigned long long lo = o.lo + ((unsigned long long)(t * kItems + k) << o.shift);
+                const unsigned long long span = o.shift ? (1ull << o.shift) - 1 : 0;
+                QSlot m = q;
+                m.lo = lo;
+                m.hi = min(o.hi, lo + span);
+                m.count = bins[t * kItems + k];
+                m.rr = q.rr - below;
+                moved[s] = m;
+                hit[s] = 1;
+            }
+            __syncthreads();
+        }
+        if (t < kSlots && hit[t]) {
+            G.slot[t] = moved[t];
+            G.slot[t].state = 5;  // moved: regrouped below
+        }
+    }
+    __syncthreads();
+    if (t == 0) {
+        const bool last = level == kLevels;
+        uint32_t n_refine = 0;
+        for (uint32_t s = 0; s < kSlots; ++s) {
+            QSlot &q = G.slot[s];
+            if (q.state == kCompact) q.state = kCompacted;  // the pass that just ran copied it
+            if (q.state != 5 && q.state != kRefine) continue;
+            q.state = kRefine;
+            q.owner = s;
+            for (uint32_t r = 0; r < s; ++r) {
+                const QSlot &o = G.slot[r];
+                if (o.owner == r && (o.state == kRefine || o.state == kCompact || o.state == kDone) && o.lo == q.lo && o.hi == q.hi) {
+                    q.owner = r;
+                    q.state = o.state;
+                    break;
+                }
+            }
+            if (q.owner != s) continue;
+            if (q.lo == q.hi) {
+                q.state = kDone;
+            } else if (!last && q.count <= kBucketCap && G.used + q.count <= kGroupCap) {
+                q.state = kCompact;
+                q.cofs = G.used;
+                q.fill = 0;
+                G.used += q.count;
+            } else {
+                ++n_refine;
+            }
+        }
+        const uint32_t per = kBins / pow2_at_least(n_refine), bits = kBinBits - (31 - __clz(kBins / per));
+        uint32_t k = 0, n_act = 0;
+        for (uint32_t s = 0; s < kSlots; ++s) {
+            QSlot &q = G.slot[s];
+            if (q.owner != s) continue;
+            if (q.state == kRefine) {
+                const uint32_t len = bit_len(q.hi - q.lo);
+                q.shift = len > bits ? len - bits : 0;
+                q.bin0 = k++ * per;
+            }
+            if (q.state == kRefine || q.state == kCompact) G.act[n_act++] = (uint8_t)s;
+        }
+        G.n_act = n_act;
+        G.n_refine = n_refine;
+        const uint32_t todo = n_act > 0;
+        G.todo = todo;
+        atomicAdd(L.reads, (unsigned long long)(todo + (level == 0)));  // level 0: pass 0 read the group too
+    }
+    __syncthreads();
+    if (dirty)
+        for (uint32_t b = t; b < kBins; b += blockDim.x) hist[b] = 0;
+}
+
+// finish: one block per group sorts each compacted range in shared memory, then writes the group's quantiles
+__global__ void __launch_bounds__(kPlanThreads) quantile_finish_kernel(QuantileParams S, Slice sl, Layout L)
+{
+    extern __shared__ unsigned long long keys[];  // kBucketCap
+    __shared__ unsigned long long rank_key[kSlots];
+    QGroup &G = L.grp[blockIdx.x];
+    const unsigned long long *area = L.area + (uint64_t)blockIdx.x * kGroupCap;
+    const uint32_t t = threadIdx.x;
+    if (t < kSlots) rank_key[t] = G.slot[t].lo;  // a finished range holds one key
+    __syncthreads();
+    for (uint32_t a = 0; a < kSlots; ++a) {
+        const QSlot &o = G.slot[a];
+        if (o.owner != a || o.state != kCompacted) continue;
+        const uint32_t n = o.count, P = pow2_at_least(n);
+        for (uint32_t k = t; k < P; k += blockDim.x) keys[k] = k < n ? area[o.cofs + k] : ~0ull;
+        __syncthreads();
+        bitonic(keys, P, t, blockDim.x, []() { __syncthreads(); });
+        if (t < kSlots && G.slot[t].owner == a) rank_key[t] = keys[G.slot[t].rr];
+        __syncthreads();
+    }
+    double *out = out_of(S, sl.i0 + blockIdx.x / sl.ne, sl.e0 + blockIdx.x % sl.ne);
+    for (uint32_t l = t; l < S.n_q; l += blockDim.x) {
+        // slot 2l holds rank i (or n - 1), slot 2l + 1 rank i + 1: map the two ranks quantile_of asks for onto them
+        uint32_t r0 = 0, r1 = 0;
+        bool two = false;
+        if (G.n) ranks_of(G.n, S.q[l], r0, r1, two);
+        out[l] = quantile_of(G.n, S.q[l], [&](uint32_t r) { return rank_key[2 * l + (r == r0 ? 0 : 1)]; });
+    }
+}
+
+constexpr uint64_t kScratchCap = 256ull << 20;  // device scratch of a large-group call, whatever the ring holds
+constexpr uint64_t kGroupBytes = (sizeof(QGroup) + 7) / 8 * 8 + kBins * 4ull + kGroupCap * 8ull;
+constexpr uint64_t kSliceGroups = (kScratchCap - 256) / kGroupBytes;  // about 1350 groups per slice
+
+inline Layout layout_of(uint64_t G, void *scratch)
+{
+    Layout L;
+    L.G = G;
+    char *p = (char *)scratch;
+    L.reads = (unsigned long long *)p;
+    p += 256;
+    L.grp = (QGroup *)p;
+    p += G * ((sizeof(QGroup) + 7) / 8 * 8);
+    L.hist = (uint32_t *)p;
+    p += G * kBins * sizeof(uint32_t);
+    L.area = (unsigned long long *)p;
+    return L;
+}
+
+__global__ void quantile_init_kernel(Layout L, bool first)
+{
+    if (first && blockIdx.x == 0 && threadIdx.x == 0) *L.reads = 0;
+    for (uint64_t g = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; g < L.G; g += (uint64_t)gridDim.x * blockDim.x) {
+        L.grp[g].kmin = ~0ull;
+        L.grp[g].kmax = 0;
+        L.grp[g].n = 0;
+        L.grp[g].todo = 0;
+        L.grp[g].used = 0;
+        L.grp[g].n_act = 0;
+        L.grp[g].n_refine = 0;
+    }
+}
+
+// groups per slice along each axis: whole planes while a plane's entities fit, else entity ranges of one plane
+inline Slice slice_shape(const QuantileParams &S)
+{
+    if (S.n_entities <= kSliceGroups) return Slice{0, std::max<uint64_t>(1, kSliceGroups / S.n_entities), 0, S.n_entities};
+    return Slice{0, 1, 0, kSliceGroups};
+}
+
+} // namespace
+
+bool quantile_large(const QuantileParams &S) { return S.n_worlds > kSmallMax; }
+
+uint64_t quantile_scratch_bytes(const QuantileParams &S)
+{
+    if (S.n_planes == 0 || S.n_worlds == 0 || S.n_entities == 0 || !quantile_large(S)) return 0;
+    const Slice sh = slice_shape(S);
+    const uint64_t G = std::min(sh.ni, S.n_planes) * sh.ne;
+    return 256 + G * kGroupBytes;
+}
+
+cudaError_t launch_quantiles(const QuantileParams &S, void *scratch, int *launches, unsigned long long *reads,
+                             cudaStream_t s)
+{
+    *launches = 0;
+    if (S.n_planes == 0 || S.n_worlds == 0 || S.n_entities == 0) return cudaSuccess;
+    const uint64_t G = S.n_planes * S.n_entities;
+    const uint64_t cap = 64ull * kNumSMs * 8;
+    if (!quantile_large(S)) {
+        if (S.n_worlds <= kWarpMax) {
+            quantile_warp_kernel<<<(unsigned)std::min((G + 7) / 8, cap), 256, 0, s>>>(S);
+        } else {
+            uint32_t P = 1;
+            while (P < S.n_worlds) P <<= 1;
+            const size_t smem = P * 8ull;
+            cudaError_t e = cudaFuncSetAttribute(quantile_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return e;
+            quantile_block_kernel<<<(unsigned)std::min(G, cap), 512, smem, s>>>(S);
+        }
+        *launches = 1;
+        return cudaGetLastError();
+    }
+    cudaError_t e = cudaFuncSetAttribute(quantile_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(quantile_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(quantile_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBucketCap * 8));
+    if (e != cudaSuccess) return e;
+    const Slice sh = slice_shape(S);
+    const Layout L0 = layout_of(0, scratch);
+    bool first = true;
+    // The same fixed sequence on every slice (one slice unless the groups need more than kScratchCap of scratch);
+    // each plan clears the histograms it leaves for the next pass, so the scratch needs no clearing in between.
+    for (uint64_t i0 = 0; i0 < S.n_planes; i0 += sh.ni) {
+        for (uint64_t e0 = 0; e0 < S.n_entities; e0 += sh.ne) {
+            const Slice sl{i0, std::min(sh.ni, S.n_planes - i0), e0, std::min(sh.ne, S.n_entities - e0)};
+            const uint64_t Gs = sl.ni * sl.ne;
+            const Layout L = layout_of(Gs, scratch);
+            const PassShape sp = pass_shape(S.n_worlds, sl.ne, sl.ni);
+            const unsigned grid = (unsigned)std::min(sl.ni * sp.C * sp.T, cap);
+            const size_t hist_smem = sl.ne == 1 ? kBins * 4ull : 0;
+            quantile_init_kernel<<<(unsigned)std::min((Gs + 255) / 256, cap), 256, 0, s>>>(L, first);
+            quantile_count_kernel<<<grid, kPassThreads, 0, s>>>(S, sl, sp, L);
+            quantile_plan_kernel<<<(unsigned)Gs, kPlanThreads, kBins * 4, s>>>(S, L, 0);
+            *launches += 3;
+            for (int level = 1; level <= kLevels; ++level) {
+                quantile_pass_kernel<<<grid, kPassThreads, hist_smem, s>>>(S, sl, sp, L);
+                quantile_plan_kernel<<<(unsigned)Gs, kPlanThreads, kBins * 4, s>>>(S, L, level);
+                *launches += 2;
+            }
+            quantile_finish_kernel<<<(unsigned)Gs, kPlanThreads, kBucketCap * 8, s>>>(S, sl, L);
+            *launches += 1;
+            first = false;
+        }
+    }
+    e = cudaGetLastError();
+    // the reads counter, 8 bytes, lands before the caller's stream synchronise
+    if (e == cudaSuccess) e = cudaMemcpyAsync(reads, L0.reads, sizeof *reads, cudaMemcpyDeviceToHost, s);
+    return e;
+}
+
+} // namespace b200

@@ -1146,9 +1146,12 @@ int b200_sixdof_trajectory_download(b200_sixdof *h, void *dst, uint64_t bytes)
 
 uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h) { return (h && h->traj) ? h->traj_planes : 0; }
 
-// Ensemble statistics of the planes in S (stats_kernels.cu) into dst, `bytes` already checked.  A device buffer on the
-// handle's GPU takes the table straight from the kernel; any other goes through the staging buffer.
-static int run_world_stats(b200_sixdof *h, StatsParams &S, void *dst, uint64_t bytes)
+// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu) into dst, `bytes` already checked.  A device
+// buffer on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer, after
+// the `scratch` bytes the reduction needs.  launch(out, scratch, &launches) enqueues the reduction on the handle's stream.
+extern "C++" {
+template <class Launch>
+static int run_world_reduction(b200_sixdof *h, uint64_t scratch, void *dst, uint64_t bytes, Launch launch)
 {
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (bytes == 0) return B200_OK;
@@ -1156,28 +1159,32 @@ static int run_world_stats(b200_sixdof *h, StatsParams &S, void *dst, uint64_t b
     cudaPointerAttributes a{};
     const bool direct = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
     (void)cudaGetLastError();
-    const uint64_t scratch = world_stats_scratch_doubles(S);
-    int rc = ensure_staging(h, std::max<uint64_t>((scratch + (direct ? 0 : bytes / 8)) * 8ull, 8));
+    scratch = (scratch + 7) / 8 * 8;
+    int rc = ensure_staging(h, std::max<uint64_t>(scratch + (direct ? 0 : bytes), 8));
     if (rc) return rc;
-    S.out = direct ? (double *)dst : h->staging + scratch;
+    double *out = direct ? (double *)dst : (double *)((char *)h->staging + scratch);
     int launches = 0;
-    CU(h, launch_world_stats(S, h->staging, &launches, h->stream));
+    CU(h, launch(out, (void *)h->staging, &launches));
     h->timings.kernel_launches += (uint64_t)launches;
-    if (!direct) CU(h, cudaMemcpyAsync(dst, S.out, bytes, cudaMemcpyDefault, h->stream));
+    if (!direct) CU(h, cudaMemcpyAsync(dst, out, bytes, cudaMemcpyDefault, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
 }
+}
 
-int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+static int run_world_stats(b200_sixdof *h, StatsParams &S, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
+    return run_world_reduction(h, world_stats_scratch_doubles(S) * 8ull, dst, bytes, [&](double *out, void *scratch, int *n) {
+        S.out = out;
+        return launch_world_stats(S, (double *)scratch, n, h->stream);
+    });
+}
+
+// the planes of the samples now in the trajectory ring, and of the current state (the B200_TRAJ_FULL layout)
+static StatsParams trajectory_planes(const b200_sixdof *h)
+{
     const uint64_t n = b200_sixdof_trajectory_len(h);
     const uint64_t W = h->traj_planes;
-    const uint64_t want = n * h->desc.n_entities * W * 5ull * 8ull;
-    if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "trajectory statistics are %llu bytes, got %llu", (unsigned long long)want,
-                    (unsigned long long)bytes);
     StatsParams S{};
     S.seg[0] = {h->traj, n * W};
     S.n_segs = 1;
@@ -1186,17 +1193,11 @@ int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
     S.ld = h->ld;
     S.n_worlds = h->desc.n_worlds;
     S.n_entities = h->desc.n_entities;
-    return run_world_stats(h, S, dst, bytes);
+    return S;
 }
 
-int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+static StatsParams state_planes(const b200_sixdof *h)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    const uint64_t want = h->desc.n_entities * 25ull * 5ull * 8ull;
-    if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "state statistics are %llu bytes, got %llu", (unsigned long long)want,
-                    (unsigned long long)bytes);
     StatsParams S{};
     const uint64_t ids[4] = {B200_ID_WORLD_POS, B200_ID_WORLD_VEL, B200_ID_WORLD_ACCEL, B200_ID_FORCE};
     for (int k = 0; k < 4; ++k) {
@@ -1209,8 +1210,79 @@ int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
     S.ld = h->ld;
     S.n_worlds = h->desc.n_worlds;
     S.n_entities = h->desc.n_entities;
+    return S;
+}
+
+int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t n = b200_sixdof_trajectory_len(h);
+    const uint64_t W = h->traj_planes;
+    const uint64_t want = n * h->desc.n_entities * W * 5ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "trajectory statistics are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    StatsParams S = trajectory_planes(h);
     return run_world_stats(h, S, dst, bytes);
 }
+
+int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t want = h->desc.n_entities * 25ull * 5ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "state statistics are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    StatsParams S = state_planes(h);
+    return run_world_stats(h, S, dst, bytes);
+}
+
+// Quantiles of the planes in P over the worlds (quantile_kernels.cu) into dst: levels checked, then `bytes`.
+static int run_quantiles(b200_sixdof *h, const StatsParams &P, const double *q, uint32_t n_q, void *dst, uint64_t bytes,
+                         uint64_t want, const char *what)
+{
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (n_q == 0 || n_q > B200_MAX_QUANTILES)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u quantile levels: 1 to %u", n_q, B200_MAX_QUANTILES);
+    if (!q) return fail(B200_ERR_INVALID_ARGUMENT, "null quantile levels");
+    for (uint32_t l = 0; l < n_q; ++l)
+        if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s quantiles are %llu bytes, got %llu", what, (unsigned long long)want,
+                    (unsigned long long)bytes);
+    QuantileParams S{};
+    static_cast<StatsParams &>(S) = P;
+    S.n_q = n_q;
+    for (uint32_t l = 0; l < n_q; ++l) S.q[l] = q[l];
+    const uint64_t groups = S.n_planes * S.n_entities;
+    h->quantile_read_sum = groups;  // the small-group route reads every group once
+    int rc = run_world_reduction(h, quantile_scratch_bytes(S), dst, bytes, [&](double *out, void *scratch, int *n) {
+        S.out = out;
+        return launch_quantiles(S, scratch, n, &h->quantile_read_sum, h->stream);
+    });
+    h->quantile_reads = rc == B200_OK && bytes && groups ? (double)h->quantile_read_sum / (double)groups : 0.0;
+    return rc;
+}
+
+int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const StatsParams P = trajectory_planes(h);
+    return run_quantiles(h, P, q, n_q, dst, bytes, P.n_planes * P.n_entities * n_q * 8ull, "trajectory");
+}
+
+int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const StatsParams P = state_planes(h);
+    return run_quantiles(h, P, q, n_q, dst, bytes, P.n_entities * 25ull * n_q * 8ull, "state");
+}
+
+double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
 // The cross-rank step of a world-sharded campaign: host-only, no GPU needed (a Rust host merges its ranks' tables
 // without torch).  Parts are folded left to right with the kernels' stats_merge, so the result does not depend on who

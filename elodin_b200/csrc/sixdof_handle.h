@@ -58,6 +58,8 @@ struct b200_sixdof {
     // staging for AoS <-> SoA
     double *staging = nullptr;
     uint64_t staging_bytes = 0;
+    double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
+    unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
     // trajectory
     double *traj = nullptr;
     uint32_t traj_planes = 13;   // 25 with B200_TRAJ_FULL

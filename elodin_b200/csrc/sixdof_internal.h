@@ -179,6 +179,20 @@ uint64_t world_stats_scratch_doubles(const StatsParams &S);
 // one or two launches on s (written to *launches); `scratch` holds world_stats_scratch_doubles(S) f64
 cudaError_t launch_world_stats(const StatsParams &S, double *scratch, int *launches, cudaStream_t s);
 
+// Ensemble quantiles over the world axis (quantile_kernels.cu): the planes of a StatsParams, and n_q levels.  Group
+// (plane i, entity e) goes to out[((i / W) * n_entities + e) * W + i % W][n_q].
+struct QuantileParams : StatsParams {
+    uint32_t n_q;
+    double q[B200_MAX_QUANTILES];
+};
+// bytes of device scratch the call needs: 0 below the large-group size (one pass, no scratch), else at most 256 MiB
+uint64_t quantile_scratch_bytes(const QuantileParams &S);
+// a fixed launch sequence per slice of groups (written to *launches); `scratch` holds quantile_scratch_bytes(S).  On
+// the large-group route *reads (host memory) receives, once the stream reaches it, the reads of the planes summed
+// over the groups; it is left alone on the small-group route (one read).
+cudaError_t launch_quantiles(const QuantileParams &S, void *scratch, int *launches, unsigned long long *reads,
+                             cudaStream_t s);
+
 // Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
 // row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.
 //   ext: extrema accumulators, plane p * 5 + f of ld doubles (f = min, max, min_tick, max_tick, first_nonfinite_tick),

@@ -252,6 +252,35 @@ class B200Exec:
         _lib.check(self._L.b200_sixdof_state_stats(self._h, out.ctypes.data, out.nbytes))
         return out
 
+    # ---- ensemble quantiles (order statistics over the world axis, on the device) -------------------------------
+    @staticmethod
+    def _levels(q) -> np.ndarray:
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
+
+    def trajectory_quantiles(self, q, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
+        """The ring's samples: numpy's linear quantile over the finite values of the worlds at each level of `q`,
+        [samples, n_entities, width, n_q] (NaN where no world is finite).  With `out_ptr` (a host or device pointer,
+        e.g. a torch CUDA tensor's data_ptr()) the table is written there and nothing is returned."""
+        lv = self._levels(q)
+        shape = (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13), lv.size)
+        out = None if out_ptr is not None else np.empty(shape)
+        ptr = out_ptr if out is None else out.ctypes.data
+        _lib.check(self._L.b200_sixdof_trajectory_quantiles(self._h, lv.ctypes.data_as(C.POINTER(C.c_double)), lv.size,
+                                                            C.c_void_p(ptr), int(np.prod(shape)) * 8))
+        return out
+
+    def state_quantiles(self, q) -> np.ndarray:
+        """The current state: quantiles over the worlds, [n_entities, 25, n_q] in the B200_TRAJ_FULL plane layout."""
+        lv = self._levels(q)
+        out = np.empty((self.n_entities, 25, lv.size))
+        _lib.check(self._L.b200_sixdof_state_quantiles(self._h, lv.ctypes.data_as(C.POINTER(C.c_double)), lv.size,
+                                                       out.ctypes.data, out.nbytes))
+        return out
+
+    def quantile_reads(self) -> float:
+        """Reads of the reduced planes the last quantile call made, averaged over its groups."""
+        return float(self._L.b200_sixdof_quantile_reads(self._h))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =

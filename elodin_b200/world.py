@@ -437,12 +437,13 @@ class World:
               backend: str = "b200", math: str = "exact", n_worlds: int = 1, device: int = -1,
               world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
-              thresholds: Optional[Sequence["Threshold"]] = None) -> "Exec":
+              thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
         also keeps every world's extrema over its telemetry rows (`Exec.extrema`) and `thresholds` (up to 8
-        `Threshold`s) every world's first threshold events (`Exec.threshold`), both on the device."""
+        `Threshold`s) every world's first threshold events (`Exec.threshold`), both on the device; `quantiles` (1 to 16
+        levels in [0, 1]) also records numpy's linear quantiles over the worlds for every row (`Exec.quantiles`)."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -450,7 +451,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -516,6 +517,22 @@ def _sampled_span(pair: str, what: str):
     return ent, span
 
 
+def _quantile_levels(levels) -> np.ndarray:
+    """World.build(..., quantiles=...): 1 to MAX_QUANTILES real levels in [0, 1], order and duplicates kept."""
+    if isinstance(levels, (str, bytes)) or not isinstance(levels, Sequence) and not isinstance(levels, np.ndarray):
+        raise TypeError(f"quantiles take a sequence of levels in [0, 1], got {levels!r}")
+    out = []
+    for q in levels:
+        if isinstance(q, (bool, np.bool_)) or not isinstance(q, (int, float, np.integer, np.floating)):
+            raise TypeError(f"quantile level {q!r}: a real number in [0, 1]")
+        if not 0.0 <= float(q) <= 1.0:  # NaN fails this too
+            raise ValueError(f"quantile level {q!r}: not in [0, 1]")
+        out.append(float(q))
+    if not 1 <= len(out) <= _lib.MAX_QUANTILES:
+        raise ValueError(f"{len(out)} quantile levels: 1 to {_lib.MAX_QUANTILES}")
+    return np.array(out)
+
+
 class Threshold:
     """A per-world event for `World.build(..., ensemble=True, thresholds=[...])`: the first telemetry row at which
     component `index` of `pair` ("<entity>.<component>": world_pos, world_vel, world_accel or force) is strictly
@@ -560,7 +577,7 @@ class Exec:
                  max_ticks: Optional[int], math: str, n_worlds: int, device: int,
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
-                 thresholds: Optional[Sequence[Threshold]] = None):
+                 thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -614,6 +631,10 @@ class Exec:
             if ent not in bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
             self._threshold_rows.append((bodies.index(ent), t.plane, t.above, t.value))
+        # quantiles: the mode first (as for extrema and thresholds), then the levels
+        if quantiles is not None and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "quantiles need World.build(..., ensemble=True)")
+        self._quantiles = None if quantiles is None else _quantile_levels(quantiles)
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
         # a body-row-expanded copy of the column for the device; no members / foreign order -> error.
@@ -665,13 +686,14 @@ class Exec:
         self._history: Dict[int, List[np.ndarray]] = {cid: [] for cid in self.world.columns}
         self._globals_hist: List[tuple] = []
         self._ens_rows: List[np.ndarray] = []  # ensemble mode: blocks of rows [k, n_entities, 25, 5]
+        self._ens_q: List[np.ndarray] = []     # and, with quantiles=, blocks of rows [k, n_entities, 25, n_q]
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._extrema or self._thresholds:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
         if self._ensemble:
             self._history = {}
             self._upload_inputs()
-            self._ens_rows.append(self.backend.state_stats()[None])  # row 0: the initial state
+            self._ens_rows.append(self._reduce_rows(ring=False))  # row 0: the initial state
             self._fold_summary(ring=False)
             self._globals_hist.append((self.tick, self.sim_time_step))
         else:
@@ -755,6 +777,14 @@ class Exec:
             (self.backend.summary_add_trajectory if ring else self.backend.summary_add_state)()
             self._summary_tables.clear()
 
+    def _reduce_rows(self, ring: bool) -> np.ndarray:
+        """Ensemble rows of the ring's samples (ring=True) or of the current state: the statistics, returned, and the
+        quantiles when the Exec records them, kept in _ens_q."""
+        be = self.backend
+        if self._quantiles is not None:
+            self._ens_q.append(be.trajectory_quantiles(self._quantiles) if ring else be.state_quantiles(self._quantiles)[None])
+        return be.trajectory_stats() if ring else be.state_stats()[None]
+
     def _add_ensemble_rows(self, rows: np.ndarray, tpt: int) -> None:
         """rows [k, n_entities, 25, 5]: k telemetry rows, `tpt` ticks apart, the last one at the current tick."""
         k = rows.shape[0]
@@ -778,7 +808,7 @@ class Exec:
                 t0 = time.perf_counter()
                 be.trajectory_reset()
                 be.step(c * tpt)
-                rows = be.trajectory_stats()                          # [c, n_entities, 25, 5]
+                rows = self._reduce_rows(ring=True)                   # [c, n_entities, 25, 5]
                 self._fold_summary(ring=True)
                 self.tick += c * tpt
                 self._add_ensemble_rows(rows, tpt)
@@ -792,7 +822,7 @@ class Exec:
                 t0 = time.perf_counter()
                 be.step(remaining)
                 self.tick += remaining
-                self._add_ensemble_rows(be.state_stats()[None], tpt)
+                self._add_ensemble_rows(self._reduce_rows(ring=False), tpt)
                 self._fold_summary(ring=False)
                 self._prof["execute_buffers"].append((time.perf_counter() - t0) * 1e3)
                 for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
@@ -824,7 +854,7 @@ class Exec:
                     post_step(self.tick, ctx)
                 done += per_call
             t_hist = time.perf_counter()
-            self._add_ensemble_rows(be.trajectory_stats() if n == tpt else be.state_stats()[None], tpt)
+            self._add_ensemble_rows(self._reduce_rows(ring=n == tpt), tpt)
             self._fold_summary(ring=n == tpt)
             self._prof["add_to_history"].append((time.perf_counter() - t_hist) * 1e3)
             remaining -= n
@@ -993,6 +1023,18 @@ class Exec:
             std = np.sqrt(t[..., 2] / count)
         return {"count": count, "mean": np.ascontiguousarray(t[..., 1]), "std": std,
                 "min": np.ascontiguousarray(t[..., 3]), "max": np.ascontiguousarray(t[..., 4])}
+
+    def quantiles(self, pair: str) -> np.ndarray:
+        """`exec.quantiles("rocket.world_pos")` -> [rows, n_q, width] f64: for every telemetry row (row 0 = the initial
+        state) numpy's linear quantile over the worlds whose value is finite, at each level of World.build(...,
+        quantiles=...) in the order given -- the layout of np.quantile(rows_k, q, axis=0) stacked over rows.  NaN where no
+        world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates."""
+        if self._quantiles is None:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "quantiles(): build the Exec with World.build(..., ensemble=True, quantiles=[...])")
+        row, span = self._sampled_row(pair, "ensemble quantiles")
+        t = np.concatenate(self._ens_q)[:, row, span[0]:span[1], :]  # [rows, width, n_q]
+        return np.ascontiguousarray(t.transpose(0, 2, 1))
 
     def _sampled_row(self, pair: str, what: str):
         """`<entity>.<component>` -> (Body row of the entity, plane span of the component in a 25-plane row)."""

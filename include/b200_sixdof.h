@@ -297,6 +297,35 @@ int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes);
  * every rank that merges the same tables in the same order gets the same bits).  Needs no GPU. */
 int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, double *out);
 
+/* ---- ensemble quantiles: per-row percentile envelopes over the worlds, on the device.  For one group (one sampled
+ * value of one entity) take the n worlds whose value is finite (NaN and +-inf are dropped, as in the statistics) and
+ * order them by IEEE totalOrder (so -0 < +0): x_(0) <= ... <= x_(n-1).  For a level q in [0, 1]:
+ *   n == 0         -> NaN
+ *   h = (n - 1) * q            one correctly rounded f64 multiply
+ *   h >= n - 1     -> x_(n-1)
+ *   else i = floor(h), t = h - i, a = x_(i), b = x_(i+1), d = b - a;  t >= 0.5 -> b - d * (1 - t),  else a + d * t
+ * with correctly rounded, uncontracted f64 operations in both math modes.  This is numpy's default ("linear")
+ * np.quantile(x[np.isfinite(x)], q) operation for operation; the two can differ only in the sign of a zero, where numpy's
+ * partition leaves -0 and +0 in arbitrary order.  A result is two order statistics and that lerp, so it is exact and
+ * does not depend on the algorithm, the launch shape or the order of atomics.
+ * Route: up to 8192 worlds each group is sorted in shared memory (one read of the planes, no scratch); above that, a
+ * radix select reads the planes at most 8 times on any data (3 on continuous data).  It needs about 198 KB of device
+ * scratch per group and runs the groups in slices of about 1350 (a fixed launch sequence per slice), so the scratch,
+ * which lives in the handle's staging buffer, is at most 256 MiB whatever the ring or entity count.  Quantile tables do NOT merge across
+ * ranks (unlike b200_stats_merge): a world-sharded campaign gets one table per rank.
+ * Both entries return the handle's sticky status if it has failed; they take 1 .. B200_MAX_QUANTILES levels
+ * q[0 .. n_q) (any order, duplicates allowed; NaN or outside [0, 1]: B200_ERR_INVALID_ARGUMENT), run on the handle's
+ * stream, return once dst is filled, take host or device dst, count their launches in timings.kernel_launches (1 below
+ * 8192 worlds, else 18 per slice) and need `bytes` to match exactly (else B200_ERR_VALUE_SIZE_MISMATCH). ---- */
+#define B200_MAX_QUANTILES 16u
+/* the ring's samples: dst = [trajectory_len][n_entities][trajectory_width][n_q] f64.  An empty ring takes bytes = 0 and
+ * launches nothing. */
+int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* the current world_pos, world_vel, world_accel, force planes: dst = [n_entities][25][n_q] f64 */
+int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* reads of the reduced planes the last quantile call made, averaged over its groups (1 on the shared-memory route) */
+double b200_sixdof_quantile_reads(const b200_sixdof *h);
+
 /* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
  * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the
  * B200_TRAJ_FULL layout (world_pos[7], world_vel[6], world_accel[6], force[6]: planes 0..24) at one tick.
