@@ -80,20 +80,30 @@ __global__ void __launch_bounds__(256) probe_fp64_kernel(double *out, int iters)
 }
 
 // ================================================================== launchers
+//
+// A tile holds kTile rows of (width | 1) doubles: a column wider than 23 (an 8-wheel torque column is 24, a full
+// trajectory sample 25) needs more than the 48 KB of dynamic shared memory a kernel gets without opting in, so every
+// launcher raises its kernel's limit first (once per kernel, device and size).
 
 cudaError_t launch_aos_to_soa(const double *aos, double *soa, uint64_t n_bodies, uint32_t width, uint64_t ld, cudaStream_t s)
 {
     if (n_bodies == 0) return cudaSuccess;
+    const size_t smem = (size_t)kTile * (width | 1u) * sizeof(double);
+    const cudaError_t e = ensure_dynamic_smem(aos_to_soa_kernel, smem);
+    if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)((n_bodies + kTile - 1) / kTile);
-    aos_to_soa_kernel<<<grid, kTile, kTile * (width | 1u) * sizeof(double), s>>>(aos, soa, n_bodies, width, ld);
+    aos_to_soa_kernel<<<grid, kTile, smem, s>>>(aos, soa, n_bodies, width, ld);
     return cudaGetLastError();
 }
 
 cudaError_t launch_soa_to_aos(const double *soa, double *aos, uint64_t n_bodies, uint32_t width, uint64_t ld, cudaStream_t s)
 {
     if (n_bodies == 0) return cudaSuccess;
+    const size_t smem = (size_t)kTile * (width | 1u) * sizeof(double);
+    const cudaError_t e = ensure_dynamic_smem(soa_to_aos_kernel, smem);
+    if (e != cudaSuccess) return e;
     const dim3 grid((unsigned)((n_bodies + kTile - 1) / kTile), 1);
-    soa_to_aos_kernel<<<grid, kTile, kTile * (width | 1u) * sizeof(double), s>>>(soa, aos, n_bodies, width, ld);
+    soa_to_aos_kernel<<<grid, kTile, smem, s>>>(soa, aos, n_bodies, width, ld);
     return cudaGetLastError();
 }
 
@@ -117,8 +127,11 @@ cudaError_t launch_multi_transpose(const MultiColumns &mc, uint64_t n_bodies, ui
     if (n_bodies == 0 || mc.n == 0) return cudaSuccess;
     uint32_t wmax = 1;
     for (uint32_t i = 0; i < mc.n; ++i) wmax = std::max(wmax, mc.col[i].width);
+    const size_t smem = (size_t)kTile * (wmax | 1u) * sizeof(double);
+    const cudaError_t e = ensure_dynamic_smem(multi_transpose_kernel, smem);
+    if (e != cudaSuccess) return e;
     const dim3 grid((unsigned)((n_bodies + kTile - 1) / kTile), mc.n);
-    multi_transpose_kernel<<<grid, kTile, kTile * (wmax | 1u) * sizeof(double), s>>>(mc, n_bodies, ld, to_soa ? 1 : 0);
+    multi_transpose_kernel<<<grid, kTile, smem, s>>>(mc, n_bodies, ld, to_soa ? 1 : 0);
     return cudaGetLastError();
 }
 

@@ -97,6 +97,19 @@ __device__ __forceinline__ Vec3 grav_slot(const GravReg &g, int slot) { return s
 
 // python/elodin/j2.py:5-29 in the operation order of oracle/sixdof_oracle.c:eff_gravity_j2.  Out of line: its pow()
 // (the reference's `norm**6.0` is a float-exponent lax.pow) would otherwise cost every EXACT kernel registers.
+// norm**6.0 of j2.py, correctly rounded but for results within ~2^-100 of a rounding boundary: x^2, x^4 and x^6 as
+// double-double products (FMA error terms), rounded once.  pow() is not correctly rounded and the GPU's and the
+// host's libm round differently, so the oracle (oracle/sixdof_oracle.c:pow6) runs this same operation sequence.
+static __device__ __forceinline__ double pow6_exact(double x)
+{
+    const double s = __dmul_rn(x, x), se = __fma_rn(x, x, -s);
+    const double q = __dmul_rn(s, s), qe = __dadd_rn(__fma_rn(s, s, -q), __dmul_rn(__dmul_rn(2.0, s), se));
+    const double p = __dmul_rn(q, s);
+    if (!isfinite(p)) return p;
+    const double pe = __dadd_rn(__fma_rn(q, s, -p), __dadd_rn(__dmul_rn(q, se), __dmul_rn(qe, s)));
+    return __dadd_rn(p, pe);
+}
+
 static __device__ __noinline__ Vec3 j2_field_exact(double mu, double J2, double r_ref, Vec3 r, double m)
 {
     using namespace ex;
@@ -105,7 +118,7 @@ static __device__ __noinline__ Vec3 j2_field_exact(double mu, double J2, double 
     const double n3 = mul(mul(norm, norm), norm);
     const double c0 = mul(-mu, m);
     const double n2 = mul(norm, norm), n4 = mul(n2, n2), n5 = mul(norm, n4);
-    const double n6 = pow(norm, 6.0);
+    const double n6 = pow6_exact(norm);
     const double kz = div(mul(3.0, r.z), n5);
     const double kr = sub(div(3.0, mul(2.0, n4)), div(mul(15.0, mul(r.z, r.z)), mul(2.0, n6)));
     const double c1 = mul(mul(c0, J2), mul(r_ref, r_ref));

@@ -235,9 +235,23 @@ static void eff_torque_body_fold(const orc_effector *e, const double *col, const
     for (int k = 0; k < 6; ++k) F[k] = acc[k];
 }
 
+/* x^6, correctly rounded but for results within ~2^-100 of a rounding boundary: x^2, x^4 and x^6 as double-double
+ * products (FMA error terms), rounded once.  pow() is not correctly rounded, and libm implementations (the host's, the
+ * GPU's) round differently; the EXACT kernel (sixdof_tick.cuh:pow6_exact) runs this same operation sequence. */
+static double pow6(double x)
+{
+    const double s = x * x, se = fma(x, x, -s);
+    const double q = s * s, qe = fma(s, s, -q) + (2.0 * s) * se;
+    const double p = q * s;
+    if (!isfinite(p)) return p;
+    const double pe = fma(q, s, -p) + ((q * se) + (qe * s));
+    return p + pe;
+}
+
 /* libs/nox-py/python/elodin/j2.py:5-29 (J2.compute_field), applied as `force + SpatialForce(linear=field)`.
  * p = [mu, J2, r_ref].  Integer powers follow lax.integer_pow's square-and-multiply (x**5 = x * (x^2)^2,
- * x**4 = (x^2)^2); `norm**6.0` has a float exponent and lowers to pow().  Parity unpinned: no golden uses J2. */
+ * x**4 = (x^2)^2); `norm**6.0` has a float exponent and lowers to pow(), evaluated here correctly rounded (pow6).
+ * Parity unpinned: no golden uses J2. */
 static void eff_gravity_j2(const orc_effector *e, const double pos[7], const double inertia[7], double F[6])
 {
     const double mu = e->p[0], J2 = e->p[1], r_ref = e->p[2];
@@ -248,7 +262,7 @@ static void eff_gravity_j2(const orc_effector *e, const double pos[7], const dou
     const double n3 = (norm * norm) * norm;
     const double c0 = (-mu) * m;
     const double n2 = norm * norm, n4 = n2 * n2, n5 = norm * n4;
-    const double n6 = pow(norm, 6.0);
+    const double n6 = pow6(norm);
     const double kz = (3.0 * z) / n5;
     const double kr = 3.0 / (2.0 * n4) - (15.0 * (z * z)) / (2.0 * n6);
     const double c1 = ((c0 * J2) * (r_ref * r_ref));
