@@ -63,11 +63,13 @@ SYMBOLS = [
     "b200_sixdof_summary_begin", "b200_sixdof_summary_add_state", "b200_sixdof_summary_add_trajectory",
     "b200_sixdof_extrema_download", "b200_sixdof_thresholds_download",
     "b200_sixdof_trajectory_quantiles", "b200_sixdof_state_quantiles", "b200_sixdof_quantile_reads",
+    "b200_sixdof_trajectory_covariance", "b200_sixdof_state_covariance", "b200_covariance_merge",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
 MAX_THRESHOLDS = 8
 MAX_QUANTILES = 16  # levels per quantile call
+MAX_COV_PLANES = 25  # planes per covariance selection
 COMM_ID_BYTES = 128
 
 
@@ -208,6 +210,9 @@ def lib():
     L.b200_sixdof_state_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
     L.b200_sixdof_quantile_reads.argtypes = [vp]
     L.b200_sixdof_quantile_reads.restype = C.c_double
+    L.b200_sixdof_trajectory_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_state_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_covariance_merge.argtypes = [C.POINTER(C.c_double), u32, u64, u32, C.POINTER(C.c_double)]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1284,6 +1284,85 @@ int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, v
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
+// Covariance of the selection `planes` (each < width) of every sample in P over the worlds (cov_kernels.cu) into dst:
+// the selection checked, then `bytes`.
+static int run_covariance(b200_sixdof *h, const StatsParams &P, uint32_t width, const uint32_t *planes, uint32_t n_p,
+                          void *dst, uint64_t bytes, const char *what)
+{
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (n_p == 0 || n_p > B200_MAX_COV_PLANES)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u covariance planes: 1 to %u", n_p, B200_MAX_COV_PLANES);
+    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null covariance planes");
+    uint32_t seen = 0;
+    for (uint32_t k = 0; k < n_p; ++k) {
+        if (planes[k] >= width)
+            return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u is %u: the %s has %u planes", k, planes[k], what, width);
+        if (seen & (1u << planes[k])) return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u listed twice", planes[k]);
+        seen |= 1u << planes[k];
+    }
+    const uint64_t n_s = P.planes_per_sample ? P.n_planes / P.planes_per_sample : 0;
+    const uint64_t want = n_s * P.n_entities * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s covariance is %llu bytes, got %llu", what, (unsigned long long)want,
+                    (unsigned long long)bytes);
+    CovParams S{};
+    static_cast<StatsParams &>(S) = P;
+    S.n_p = n_p;
+    for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
+    return run_world_reduction(h, cov_scratch_bytes(S), dst, bytes, [&](double *out, void *scratch, int *n) {
+        S.out = out;
+        return launch_covariance(S, scratch, n, h->stream);
+    });
+}
+
+int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const StatsParams P = trajectory_planes(h);
+    return run_covariance(h, P, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    return run_covariance(h, state_planes(h), 25, planes, n_p, dst, bytes, "state");
+}
+
+// Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.
+int b200_covariance_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, uint32_t n_p, double *out)
+{
+    if (n_p == 0 || n_p > B200_MAX_COV_PLANES)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u covariance planes: 1 to %u", n_p, B200_MAX_COV_PLANES);
+    if (n_groups && (!out || (n_parts && !parts))) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
+    const uint64_t R = 1 + n_p + (uint64_t)n_p * n_p;
+    for (uint32_t k = 0; k < n_parts; ++k)
+        for (uint64_t g = 0; g < n_groups; ++g) {
+            const double n = parts[((uint64_t)k * n_groups + g) * R];
+            if (!(n >= 0.0))
+                return fail(B200_ERR_INVALID_ARGUMENT, "part %u, group %llu: count %g is not a count", k, (unsigned long long)g, n);
+        }
+    const double nan = std::nan("");
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        double *o = out + g * R;
+        for (uint32_t a = 0; a < n_p; ++a)
+            for (uint32_t b = a; b < n_p; ++b) {
+                CovEntry acc{0.0, 0.0, 0.0, 0.0};
+                for (uint32_t k = 0; k < n_parts; ++k) {
+                    const double *q = parts + ((uint64_t)k * n_groups + g) * R;
+                    cov_merge(acc, CovEntry{q[0], q[1 + a], q[1 + b], q[1 + n_p + a * n_p + b]});
+                }
+                const bool any = acc.n > 0.0;
+                if (a == 0 && b == 0) o[0] = acc.n;
+                if (a == b) o[1 + a] = any ? acc.ma : nan;
+                o[1 + n_p + a * n_p + b] = any ? acc.m : nan;
+                o[1 + n_p + b * n_p + a] = any ? acc.m : nan;
+            }
+    }
+    return B200_OK;
+}
+
 // The cross-rank step of a world-sharded campaign: host-only, no GPU needed (a Rust host merges its ranks' tables
 // without torch).  Parts are folded left to right with the kernels' stats_merge, so the result does not depend on who
 // calls it.

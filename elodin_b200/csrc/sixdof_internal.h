@@ -174,6 +174,19 @@ struct StatsParams {
     uint64_t n_entities;
     double *out;
 };
+// plane i (< n_planes) of the concatenated segments
+__device__ inline const double *stats_plane(const StatsParams &S, uint64_t i)
+{
+    const double *p = nullptr;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; ++k) { // constant indices: the segment table stays in the parameter space
+        if (!p && k < S.n_segs) {
+            if (i < S.seg[k].n_planes) p = S.seg[k].base + i * S.ld;
+            else i -= S.seg[k].n_planes;
+        }
+    }
+    return p; // i < n_planes: always set
+}
 // f64 of device scratch the reduction needs for this shape (0: one pass, no scratch)
 uint64_t world_stats_scratch_doubles(const StatsParams &S);
 // one or two launches on s (written to *launches); `scratch` holds world_stats_scratch_doubles(S) f64
@@ -192,6 +205,38 @@ uint64_t quantile_scratch_bytes(const QuantileParams &S);
 // over the groups; it is left alone on the small-group route (one read).
 cudaError_t launch_quantiles(const QuantileParams &S, void *scratch, int *launches, unsigned long long *reads,
                              cudaStream_t s);
+
+// Ensemble covariance over the world axis (cov_kernels.cu).  One entry (a, b) of a group over a set of worlds: the
+// count n, the means of planes a and b, and the co-moment m = sum (x_a - mean_a)(x_b - mean_b); while n = 0 the other
+// fields are unread.
+struct CovEntry {
+    double n, ma, mb, m;
+};
+
+// x := x (+) y, the covariance form of Chan et al.'s pairwise update.  Every merge of partial records, on the device and
+// in b200_covariance_merge, goes through this function.  Swapping a and b swaps ma / mb and leaves m's bits alone.
+__host__ __device__ inline void cov_merge(CovEntry &x, const CovEntry &y)
+{
+    if (y.n == 0.0) return;
+    if (x.n == 0.0) { x = y; return; }
+    const double n = x.n + y.n;
+    const double da = y.ma - x.ma, db = y.mb - x.mb;
+    x.ma = x.ma + da * y.n / n;
+    x.mb = x.mb + db * y.n / n;
+    x.m = x.m + y.m + da * db * x.n * y.n / n;
+    x.n = n;
+}
+
+// The samples of a StatsParams (n_planes / planes_per_sample of them) and a selection of n_p distinct planes of a
+// sample.  Group (sample s, entity e) goes to out[(s * n_entities + e) * (1 + n_p + n_p^2)]: n, mean[n_p], M[n_p][n_p].
+struct CovParams : StatsParams {
+    uint32_t n_p;
+    uint32_t planes[B200_MAX_COV_PLANES];
+};
+// bytes of device scratch the call needs (0: one chunk, no scratch); at most 256 MiB
+uint64_t cov_scratch_bytes(const CovParams &S);
+// one chunk launch, and a merge launch when the worlds take more than one chunk, per slice of groups (*launches)
+cudaError_t launch_covariance(const CovParams &S, void *scratch, int *launches, cudaStream_t s);
 
 // Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
 // row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.

@@ -41,19 +41,6 @@ inline Shape stats_shape(uint64_t n_worlds, uint64_t E)
     return s;
 }
 
-__device__ inline const double *plane_of(const StatsParams &S, uint64_t i)
-{
-    const double *p = nullptr;
-#pragma unroll
-    for (uint32_t k = 0; k < 4; ++k) { // constant indices: the segment table stays in the parameter space
-        if (!p && k < S.n_segs) {
-            if (i < S.seg[k].n_planes) p = S.seg[k].base + i * S.ld;
-            else i -= S.seg[k].n_planes;
-        }
-    }
-    return p; // i < n_planes: always set
-}
-
 __device__ inline void write_final(const StatsParams &S, uint64_t i, uint64_t e, const StatsGroup &g)
 {
     const uint64_t W = S.planes_per_sample;
@@ -112,7 +99,7 @@ __global__ void __launch_bounds__(kStatsThreads, 4) world_stats_chunk_kernel(Sta
         const uint64_t w1 = min(w0 + sp.Wc, S.n_worlds);
         Shifted acc;
         if (j < sp.J && e < E) {
-            const double *p = plane_of(S, i) + e;
+            const double *p = stats_plane(S, i) + e;
             const uint64_t step = sp.J * E;
             uint64_t w = w0 + j;
             for (; w + 3 * sp.J < w1; w += 4 * sp.J) { // four loads in flight before the first is used

@@ -281,6 +281,31 @@ class B200Exec:
         """Reads of the reduced planes the last quantile call made, averaged over its groups."""
         return float(self._L.b200_sixdof_quantile_reads(self._h))
 
+    # ---- ensemble covariance (co-moments of a plane selection over the world axis, on the device) --------------
+    @staticmethod
+    def _selection(planes) -> np.ndarray:
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(planes, dtype=np.uint32)).ravel())
+
+    def trajectory_covariance(self, planes, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
+        """The ring's samples: for the planes `planes` of the 25-plane sample layout, [samples, n_entities, 1 + p + p*p]
+        records (n, mean[p], M[p][p] = co-moments) over the worlds whose p selected values are all finite (NaN after
+        n where n = 0).  With `out_ptr` (a host or device pointer) the table is written there and nothing is returned."""
+        sel = self._selection(planes)
+        shape = (self.trajectory_len(), self.n_entities, 1 + sel.size + sel.size * sel.size)
+        out = None if out_ptr is not None else np.empty(shape)
+        ptr = out_ptr if out is None else out.ctypes.data
+        _lib.check(self._L.b200_sixdof_trajectory_covariance(self._h, sel.ctypes.data_as(C.POINTER(C.c_uint32)), sel.size,
+                                                             C.c_void_p(ptr), int(np.prod(shape)) * 8))
+        return out
+
+    def state_covariance(self, planes) -> np.ndarray:
+        """The current state: [n_entities, 1 + p + p*p] records as trajectory_covariance()."""
+        sel = self._selection(planes)
+        out = np.empty((self.n_entities, 1 + sel.size + sel.size * sel.size))
+        _lib.check(self._L.b200_sixdof_state_covariance(self._h, sel.ctypes.data_as(C.POINTER(C.c_uint32)), sel.size,
+                                                        out.ctypes.data, out.nbytes))
+        return out
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
@@ -355,6 +380,26 @@ def merge_stats(tables: Sequence[np.ndarray]) -> np.ndarray:
     dp = C.POINTER(C.c_double)
     _lib.check(_lib.lib().b200_stats_merge(stacked.ctypes.data_as(dp), len(parts), out.size // _lib.STATS_FIELDS,
                                             out.ctypes.data_as(dp)))
+    return out
+
+
+def merge_covariance(tables: Sequence[np.ndarray]) -> np.ndarray:
+    """Merge covariance tables of the same shape [..., 1 + p + p*p] (e.g. one per rank of a world-sharded campaign, or
+    per handle) left to right, in list order, with b200_covariance_merge: the table of the union of their worlds."""
+    parts = [np.asarray(t, dtype=np.float64) for t in tables]
+    if not parts:
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, "merge_covariance needs at least one table")
+    shape = parts[0].shape
+    rec = shape[-1] if shape else 0
+    p = math.isqrt(max(rec - 1, 0))  # p^2 <= p^2 + p < (p + 1)^2
+    if rec < 3 or p * p + p + 1 != rec or any(t.shape != shape for t in parts):
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH,
+                                  f"covariance tables must share one shape [..., 1 + p + p*p], got {[t.shape for t in parts]}")
+    stacked = np.ascontiguousarray(np.stack(parts))
+    out = np.empty(shape)
+    dp = C.POINTER(C.c_double)
+    _lib.check(_lib.lib().b200_covariance_merge(stacked.ctypes.data_as(dp), len(parts), out.size // rec, p,
+                                                 out.ctypes.data_as(dp)))
     return out
 
 

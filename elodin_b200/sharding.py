@@ -49,15 +49,10 @@ def gather_worlds(local, n_worlds: int, group=None):
     return torch.cat([o[:s] for o, s in zip(out, sizes)], 0)
 
 
-def gather_ensemble(table, group=None) -> np.ndarray:
-    """Ensemble statistics of a world-sharded campaign: every rank passes the table of its own worlds ([..., 5] from
-    `B200Exec.trajectory_stats` / `state_stats`, numpy or torch), the tables are all-gathered and merged in rank order
-    with `merge_stats` (b200_stats_merge) on the host.  Every rank gets the same bits.  The tables are small (5 f64
-    per group): a CUDA copy for NCCL groups, host memory for gloo."""
+def _all_gather_tables(table, group) -> List[np.ndarray]:
+    """Every rank's host table, in rank order: a CUDA copy for NCCL groups, host memory for gloo."""
     import torch
     import torch.distributed as dist
-
-    from .executor import merge_stats
 
     local = table.detach().to("cpu", torch.float64) if isinstance(table, torch.Tensor) else torch.from_numpy(
         np.ascontiguousarray(table, dtype=np.float64))
@@ -65,7 +60,27 @@ def gather_ensemble(table, group=None) -> np.ndarray:
     local = local.to(dev).contiguous()
     parts = [torch.empty_like(local) for _ in range(dist.get_world_size(group))]
     dist.all_gather(parts, local, group=group)
-    return merge_stats([p.cpu().numpy() for p in parts])
+    return [p.cpu().numpy() for p in parts]
+
+
+def gather_ensemble(table, group=None) -> np.ndarray:
+    """Ensemble statistics of a world-sharded campaign: every rank passes the table of its own worlds ([..., 5] from
+    `B200Exec.trajectory_stats` / `state_stats`, numpy or torch), the tables are all-gathered and merged in rank order
+    with `merge_stats` (b200_stats_merge) on the host.  Every rank gets the same bits.  The tables are small (5 f64
+    per group)."""
+    from .executor import merge_stats
+
+    return merge_stats(_all_gather_tables(table, group))
+
+
+def gather_covariance(table, group=None) -> np.ndarray:
+    """Ensemble covariance of a world-sharded campaign: every rank passes the table of its own worlds ([..., 1 + p + p*p]
+    from `B200Exec.trajectory_covariance` / `state_covariance`, numpy or torch, the same selection on every rank), the
+    tables are all-gathered and merged in rank order with `merge_covariance` (b200_covariance_merge) on the host.  Every
+    rank gets the same bits."""
+    from .executor import merge_covariance
+
+    return merge_covariance(_all_gather_tables(table, group))
 
 
 def total_entity_steps(local_entity_steps: int, group=None) -> int:

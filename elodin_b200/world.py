@@ -437,13 +437,17 @@ class World:
               backend: str = "b200", math: str = "exact", n_worlds: int = 1, device: int = -1,
               world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
-              thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None) -> "Exec":
+              thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
+              covariance: Optional[Sequence] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
         also keeps every world's extrema over its telemetry rows (`Exec.extrema`) and `thresholds` (up to 8
         `Threshold`s) every world's first threshold events (`Exec.threshold`), both on the device; `quantiles` (1 to 16
-        levels in [0, 1]) also records numpy's linear quantiles over the worlds for every row (`Exec.quantiles`)."""
+        levels in [0, 1]) also records numpy's linear quantiles over the worlds for every row (`Exec.quantiles`), and
+        `covariance` the covariance over the worlds of a selection of components for every row and entity
+        (`Exec.covariance`): items are a component name ("world_pos": all its planes) or (component, indices), e.g.
+        covariance=[("world_pos", (4, 5, 6)), ("world_vel", (3, 4, 5))], at most 25 distinct planes."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -451,7 +455,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds, quantiles)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -533,6 +537,37 @@ def _quantile_levels(levels) -> np.ndarray:
     return np.array(out)
 
 
+def _covariance_planes(spec):
+    """World.build(..., covariance=...) -> (planes of the 25-plane row layout, labels), selection order kept."""
+    if isinstance(spec, (str, bytes)) or not isinstance(spec, Sequence):
+        raise TypeError(f"covariance takes a sequence of components or (component, indices) pairs, got {spec!r}")
+    planes, labels = [], []
+    for item in spec:
+        if isinstance(item, str):
+            comp, idx = item, None
+        elif isinstance(item, (tuple, list)) and len(item) == 2:
+            comp, idx = item
+        else:
+            comp, idx = None, None
+        if not isinstance(comp, str):
+            raise TypeError(f"covariance item {item!r}: a component name or a (component, indices) pair")
+        span = _SAMPLED.get(comp)
+        if span is None:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                      f"component not found: {comp} (ensemble covariance covers {', '.join(_SAMPLED)})")
+        width = span[1] - span[0]
+        for i in range(width) if idx is None else idx:
+            if isinstance(i, (bool, np.bool_)) or not isinstance(i, (int, np.integer)) or not 0 <= i < width:
+                raise ValueError(f"covariance item {item!r}: index {i!r} is not an integer in [0, {width})")
+            if span[0] + int(i) in planes:
+                raise ValueError(f"covariance selects {comp}[{int(i)}] twice")
+            planes.append(span[0] + int(i))
+            labels.append(f"{comp}[{int(i)}]")
+    if not 1 <= len(planes) <= _lib.MAX_COV_PLANES:
+        raise ValueError(f"covariance selects {len(planes)} planes: 1 to {_lib.MAX_COV_PLANES}")
+    return planes, labels
+
+
 class Threshold:
     """A per-world event for `World.build(..., ensemble=True, thresholds=[...])`: the first telemetry row at which
     component `index` of `pair` ("<entity>.<component>": world_pos, world_vel, world_accel or force) is strictly
@@ -577,7 +612,8 @@ class Exec:
                  max_ticks: Optional[int], math: str, n_worlds: int, device: int,
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
-                 thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None):
+                 thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
+                 covariance: Optional[Sequence] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -635,6 +671,10 @@ class Exec:
         if quantiles is not None and not ensemble:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "quantiles need World.build(..., ensemble=True)")
         self._quantiles = None if quantiles is None else _quantile_levels(quantiles)
+        # covariance: the mode first, then the selection
+        if covariance is not None and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "covariance needs World.build(..., ensemble=True)")
+        self._cov_planes, self._cov_labels = (None, None) if covariance is None else _covariance_planes(covariance)
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
         # a body-row-expanded copy of the column for the device; no members / foreign order -> error.
@@ -687,6 +727,7 @@ class Exec:
         self._globals_hist: List[tuple] = []
         self._ens_rows: List[np.ndarray] = []  # ensemble mode: blocks of rows [k, n_entities, 25, 5]
         self._ens_q: List[np.ndarray] = []     # and, with quantiles=, blocks of rows [k, n_entities, 25, n_q]
+        self._ens_cov: List[np.ndarray] = []   # and, with covariance=, blocks of rows [k, n_entities, 1 + p + p*p]
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._extrema or self._thresholds:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
@@ -779,10 +820,12 @@ class Exec:
 
     def _reduce_rows(self, ring: bool) -> np.ndarray:
         """Ensemble rows of the ring's samples (ring=True) or of the current state: the statistics, returned, and the
-        quantiles when the Exec records them, kept in _ens_q."""
+        quantiles and covariance when the Exec records them, kept in _ens_q and _ens_cov."""
         be = self.backend
         if self._quantiles is not None:
             self._ens_q.append(be.trajectory_quantiles(self._quantiles) if ring else be.state_quantiles(self._quantiles)[None])
+        if self._cov_planes is not None:
+            self._ens_cov.append(be.trajectory_covariance(self._cov_planes) if ring else be.state_covariance(self._cov_planes)[None])
         return be.trajectory_stats() if ring else be.state_stats()[None]
 
     def _add_ensemble_rows(self, rows: np.ndarray, tpt: int) -> None:
@@ -1035,6 +1078,23 @@ class Exec:
         row, span = self._sampled_row(pair, "ensemble quantiles")
         t = np.concatenate(self._ens_q)[:, row, span[0]:span[1], :]  # [rows, width, n_q]
         return np.ascontiguousarray(t.transpose(0, 2, 1))
+
+    def covariance(self, entity: str) -> Dict[str, object]:
+        """`exec.covariance("rocket")` -> {"count" [rows], "mean" [rows, p], "cov" [rows, p, p], "planes" [p] labels such
+        as "world_pos[4]"}: for every telemetry row (row 0 = the initial state) the covariance over the worlds of the
+        selection of World.build(..., covariance=...), in its order.  Only worlds whose p selected values are all
+        finite count (listwise deletion, unlike Exec.ensemble, which counts per component); cov = co-moments / count
+        (numpy's ddof=0, as Exec.ensemble's std), exactly symmetric, NaN where count = 0."""
+        if self._cov_planes is None:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "covariance(): build the Exec with World.build(..., ensemble=True, covariance=[...])")
+        row, _ = self._sampled_row(f"{entity}.world_pos", "ensemble covariance")
+        p = len(self._cov_planes)
+        t = np.concatenate(self._ens_cov)[:, row, :]  # [rows, 1 + p + p*p]
+        count = np.ascontiguousarray(t[:, 0])
+        with np.errstate(invalid="ignore", divide="ignore"):
+            cov = t[:, 1 + p:].reshape(-1, p, p) / count[:, None, None]
+        return {"count": count, "mean": np.ascontiguousarray(t[:, 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
 
     def _sampled_row(self, pair: str, what: str):
         """`<entity>.<component>` -> (Body row of the entity, plane span of the component in a 25-plane row)."""

@@ -326,6 +326,35 @@ int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, v
 /* reads of the reduced planes the last quantile call made, averaged over its groups (1 on the shared-memory route) */
 double b200_sixdof_quantile_reads(const b200_sixdof *h);
 
+/* ---- ensemble covariance: the joint spread of chosen components over the worlds, on the device.  A selection is
+ * planes[0 .. n_p) of the B200_TRAJ_FULL sample layout (world_pos 0-6, world_vel 7-12, world_accel 13-18, force 19-24),
+ * 1 <= n_p <= B200_MAX_COV_PLANES, distinct, in the caller's order.  A group is one (sample, entity), and its record is
+ * 1 + n_p + n_p^2 f64:
+ *   n           the worlds whose n_p selected values are ALL finite (listwise deletion: unlike the statistics, which
+ *               count per plane, a world with one NaN / +-inf among the selected values is left out of every entry;
+ *               non-finite values in planes that are not selected exclude nothing),
+ *   mean[n_p]   over those worlds,
+ *   M[n_p][n_p] the co-moments sum (x_a - mean_a)(x_b - mean_b), row-major, M[b][a] the same bits as M[a][b]
+ *               (covariance = M / n, numpy's ddof = 0);
+ * a group with n = 0 holds NaN after n.  Chunks of worlds are summed shifted by the chunk's first complete world and
+ * merged with Chan et al.'s update in a fixed order (no atomics); the chunking depends on (n_worlds, n_entities) alone,
+ * so the same input gives the same bits on every call, a sample's bits do not depend on the ring, and an entry (a, b)
+ * has the same bits in any selection that holds both planes and has the same complete worlds.  Device scratch (in the
+ * handle's staging buffer) stays under 256 MiB: large calls run their groups in slices, which changes no bits.
+ * Both entries return the handle's sticky status if it has failed, then B200_ERR_INVALID_ARGUMENT for an empty or too
+ * long selection, a duplicate plane or a plane >= the width (b200_sixdof_trajectory_width for the ring, 25 for the
+ * state), then B200_ERR_VALUE_SIZE_MISMATCH unless `bytes` matches exactly.  They run on the handle's stream, return once
+ * dst (host or device) is filled and count their launches in timings.kernel_launches. ---- */
+#define B200_MAX_COV_PLANES 25u
+/* the ring's samples: dst = [trajectory_len][n_entities][1 + n_p + n_p^2] f64.  An empty ring takes bytes = 0. */
+int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* the current world_pos, world_vel, world_accel, force planes: dst = [n_entities][1 + n_p + n_p^2] f64 */
+int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* host-only: merge n_parts tables of n_groups records each ([n_parts][n_groups][1 + n_p + n_p^2]) left to right, in
+ * part order, into out[n_groups][1 + n_p + n_p^2], with the update the kernels use (M[a][b] is read from a <= b).
+ * A negative or NaN count is B200_ERR_INVALID_ARGUMENT.  Needs no GPU. */
+int b200_covariance_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, uint32_t n_p, double *out);
+
 /* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
  * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the
  * B200_TRAJ_FULL layout (world_pos[7], world_vel[6], world_accel[6], force[6]: planes 0..24) at one tick.
