@@ -1146,9 +1146,20 @@ int b200_sixdof_trajectory_download(b200_sixdof *h, void *dst, uint64_t bytes)
 
 uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h) { return (h && h->traj) ? h->traj_planes : 0; }
 
-// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu) into dst, `bytes` already checked.  A device
-// buffer on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer, after
-// the `scratch` bytes the reduction needs.  launch(out, scratch, &launches) enqueues the reduction on the handle's stream.
+// dst is device memory on the handle's GPU, which a kernel can write directly; any other destination goes through the
+// staging buffer.
+static bool device_destination(const b200_sixdof *h, const void *dst)
+{
+    cudaPointerAttributes a{};
+    const bool device = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
+    (void)cudaGetLastError();
+    return device;
+}
+
+// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu) into dst, `bytes` already
+// checked.  A device destination takes the table straight from the kernel; any other gets it through the staging
+// buffer, after the `scratch` bytes the reduction needs.  launch(out, scratch, &launches) enqueues the reduction on the
+// handle's stream.
 extern "C++" {
 template <class Launch>
 static int run_world_reduction(b200_sixdof *h, uint64_t scratch, void *dst, uint64_t bytes, Launch launch)
@@ -1156,9 +1167,7 @@ static int run_world_reduction(b200_sixdof *h, uint64_t scratch, void *dst, uint
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (bytes == 0) return B200_OK;
     if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
-    cudaPointerAttributes a{};
-    const bool direct = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
-    (void)cudaGetLastError();
+    const bool direct = device_destination(h, dst);
     scratch = (scratch + 7) / 8 * 8;
     int rc = ensure_staging(h, std::max<uint64_t>(scratch + (direct ? 0 : bytes), 8));
     if (rc) return rc;
@@ -1172,15 +1181,8 @@ static int run_world_reduction(b200_sixdof *h, uint64_t scratch, void *dst, uint
 }
 }
 
-static int run_world_stats(b200_sixdof *h, StatsParams &S, void *dst, uint64_t bytes)
-{
-    return run_world_reduction(h, world_stats_scratch_doubles(S) * 8ull, dst, bytes, [&](double *out, void *scratch, int *n) {
-        S.out = out;
-        return launch_world_stats(S, (double *)scratch, n, h->stream);
-    });
-}
-
-// the planes of the samples now in the trajectory ring, and of the current state (the B200_TRAJ_FULL layout)
+// The sampled planes (the B200_TRAJ_FULL layout: world_pos 0-6, world_vel 7-12, world_accel 13-18, force 19-24) of the
+// samples now in the trajectory ring, and of the current state.  Every reduction and run summary reads them from here.
 static StatsParams trajectory_planes(const b200_sixdof *h)
 {
     const uint64_t n = b200_sixdof_trajectory_len(h);
@@ -1213,47 +1215,54 @@ static StatsParams state_planes(const b200_sixdof *h)
     return S;
 }
 
-int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+// The reduction entries below run over one of these; `what` names it in error messages.
+using PlaneSource = StatsParams (*)(const b200_sixdof *);
+
+// Statistics of the planes over the worlds (stats_kernels.cu) into dst: `bytes` checked, then the handle's status.
+static int run_world_stats(b200_sixdof *h, PlaneSource source, void *dst, uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     CU(h, cudaSetDevice(h->device));
-    const uint64_t n = b200_sixdof_trajectory_len(h);
-    const uint64_t W = h->traj_planes;
-    const uint64_t want = n * h->desc.n_entities * W * 5ull * 8ull;
+    StatsParams S = source(h);
+    const uint64_t want = S.n_planes * S.n_entities * 5ull * 8ull;
     if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "trajectory statistics are %llu bytes, got %llu", (unsigned long long)want,
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s statistics are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    StatsParams S = trajectory_planes(h);
-    return run_world_stats(h, S, dst, bytes);
+    return run_world_reduction(h, world_stats_scratch_doubles(S) * 8ull, dst, bytes, [&](double *out, void *scratch, int *n) {
+        S.out = out;
+        return launch_world_stats(S, (double *)scratch, n, h->stream);
+    });
+}
+
+int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return run_world_stats(h, trajectory_planes, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    const uint64_t want = h->desc.n_entities * 25ull * 5ull * 8ull;
-    if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "state statistics are %llu bytes, got %llu", (unsigned long long)want,
-                    (unsigned long long)bytes);
-    StatsParams S = state_planes(h);
-    return run_world_stats(h, S, dst, bytes);
+    return run_world_stats(h, state_planes, dst, bytes, "state");
 }
 
-// Quantiles of the planes in P over the worlds (quantile_kernels.cu) into dst: levels checked, then `bytes`.
-static int run_quantiles(b200_sixdof *h, const StatsParams &P, const double *q, uint32_t n_q, void *dst, uint64_t bytes,
-                         uint64_t want, const char *what)
+// Quantiles of the planes over the worlds (quantile_kernels.cu) into dst: the handle's status checked, then the levels,
+// then `bytes`.
+static int run_quantiles(b200_sixdof *h, PlaneSource source, const double *q, uint32_t n_q, void *dst, uint64_t bytes,
+                         const char *what)
 {
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    QuantileParams S{};
+    static_cast<StatsParams &>(S) = source(h);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_q == 0 || n_q > B200_MAX_QUANTILES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u quantile levels: 1 to %u", n_q, B200_MAX_QUANTILES);
     if (!q) return fail(B200_ERR_INVALID_ARGUMENT, "null quantile levels");
     for (uint32_t l = 0; l < n_q; ++l)
         if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
+    const uint64_t want = S.n_planes * S.n_entities * n_q * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s quantiles are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    QuantileParams S{};
-    static_cast<StatsParams &>(S) = P;
     S.n_q = n_q;
     for (uint32_t l = 0; l < n_q; ++l) S.q[l] = q[l];
     const uint64_t groups = S.n_planes * S.n_entities;
@@ -1268,27 +1277,25 @@ static int run_quantiles(b200_sixdof *h, const StatsParams &P, const double *q, 
 
 int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    const StatsParams P = trajectory_planes(h);
-    return run_quantiles(h, P, q, n_q, dst, bytes, P.n_planes * P.n_entities * n_q * 8ull, "trajectory");
+    return run_quantiles(h, trajectory_planes, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    const StatsParams P = state_planes(h);
-    return run_quantiles(h, P, q, n_q, dst, bytes, P.n_entities * 25ull * n_q * 8ull, "state");
+    return run_quantiles(h, state_planes, q, n_q, dst, bytes, "state");
 }
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
-// Covariance of the selection `planes` (each < width) of every sample in P over the worlds (cov_kernels.cu) into dst:
-// the selection checked, then `bytes`.
-static int run_covariance(b200_sixdof *h, const StatsParams &P, uint32_t width, const uint32_t *planes, uint32_t n_p,
+// Covariance of the selection `planes` (each < width) of every sample over the worlds (cov_kernels.cu) into dst: the
+// handle's status checked, then the selection, then `bytes`.
+static int run_covariance(b200_sixdof *h, PlaneSource source, uint32_t width, const uint32_t *planes, uint32_t n_p,
                           void *dst, uint64_t bytes, const char *what)
 {
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    CovParams S{};
+    static_cast<StatsParams &>(S) = source(h);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_p == 0 || n_p > B200_MAX_COV_PLANES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u covariance planes: 1 to %u", n_p, B200_MAX_COV_PLANES);
@@ -1300,13 +1307,11 @@ static int run_covariance(b200_sixdof *h, const StatsParams &P, uint32_t width, 
         if (seen & (1u << planes[k])) return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u listed twice", planes[k]);
         seen |= 1u << planes[k];
     }
-    const uint64_t n_s = P.planes_per_sample ? P.n_planes / P.planes_per_sample : 0;
-    const uint64_t want = n_s * P.n_entities * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
+    const uint64_t n_s = S.planes_per_sample ? S.n_planes / S.planes_per_sample : 0;
+    const uint64_t want = n_s * S.n_entities * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s covariance is %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    CovParams S{};
-    static_cast<StatsParams &>(S) = P;
     S.n_p = n_p;
     for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
     return run_world_reduction(h, cov_scratch_bytes(S), dst, bytes, [&](double *out, void *scratch, int *n) {
@@ -1315,19 +1320,15 @@ static int run_covariance(b200_sixdof *h, const StatsParams &P, uint32_t width, 
     });
 }
 
+// The ring's width, not its planes per sample: a handle without a ring refuses every plane.
 int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    const StatsParams P = trajectory_planes(h);
-    return run_covariance(h, P, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes, "trajectory");
+    return run_covariance(h, trajectory_planes, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    CU(h, cudaSetDevice(h->device));
-    return run_covariance(h, state_planes(h), 25, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, state_planes, 25, planes, n_p, dst, bytes, "state");
 }
 
 // Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.
@@ -1389,7 +1390,7 @@ int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, d
     return B200_OK;
 }
 
-// The fold parameters of the handle's summary accumulators; the caller fills in the rows.
+// The fold parameters of the handle's summary accumulators; run_summary_fold fills in the rows.
 static SummaryParams summary_params(const b200_sixdof *h)
 {
     SummaryParams S{};
@@ -1422,8 +1423,18 @@ static int summary_ready(b200_sixdof *h, const char *what)
     return B200_OK;
 }
 
-static int run_summary_fold(b200_sixdof *h, const SummaryParams &S)
+// Fold the samples of P as rows, sample k at tick tick0 + k * tick_step: row[p] is plane p of sample 0, and each sample
+// starts planes_per_sample planes after the one before it.
+static int run_summary_fold(b200_sixdof *h, const StatsParams &P, uint64_t tick0, uint64_t tick_step)
 {
+    SummaryParams S = summary_params(h);
+    uint32_t p = 0;
+    for (uint32_t k = 0; k < P.n_segs; ++k)
+        for (uint64_t j = 0; j < P.seg[k].n_planes && p < 25; ++j) S.row[p++] = P.seg[k].base + j * P.ld;
+    S.row_stride = P.planes_per_sample * P.ld;
+    S.n_rows = P.n_planes / P.planes_per_sample;
+    S.tick0 = tick0;
+    S.tick_step = tick_step;
     int launches = 0;
     CU(h, launch_summary_fold(S, &launches, h->stream));
     h->timings.kernel_launches += (uint64_t)launches;
@@ -1471,16 +1482,7 @@ int b200_sixdof_summary_add_state(b200_sixdof *h)
     CU(h, cudaSetDevice(h->device));
     int rc = summary_ready(h, "summary_add_state");
     if (rc) return rc;
-    SummaryParams S = summary_params(h);
-    const uint64_t ids[4] = {B200_ID_WORLD_POS, B200_ID_WORLD_VEL, B200_ID_WORLD_ACCEL, B200_ID_FORCE};
-    uint32_t p = 0;
-    for (uint64_t id : ids) {
-        const Column *c = h->find(id);
-        for (uint32_t j = 0; j < c->width; ++j) S.row[p++] = c->dev + j * h->ld;
-    }
-    S.n_rows = 1;
-    S.tick0 = h->tick;
-    return run_summary_fold(h, S);
+    return run_summary_fold(h, state_planes(h), h->tick, 0);
 }
 
 int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
@@ -1491,14 +1493,9 @@ int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
     if (rc) return rc;
     if (!h->traj || h->traj_planes != 25)
         return fail(B200_ERR_INVALID_ARGUMENT, "summary_add_trajectory needs a B200_TRAJ_FULL trajectory ring");
-    SummaryParams S = summary_params(h);
-    for (uint32_t p = 0; p < 25; ++p) S.row[p] = h->traj + p * h->ld;
-    S.row_stride = 25ull * h->ld;
-    S.n_rows = b200_sixdof_trajectory_len(h);
     // sample k was recorded when the ticks since the reset reached (k + 1) * every (sixdof_tick.cuh traj slots)
-    S.tick_step = h->desc.trajectory_every;
-    S.tick0 = h->tick - h->ticks_done + S.tick_step;
-    return run_summary_fold(h, S);
+    const uint64_t every = h->desc.trajectory_every;
+    return run_summary_fold(h, trajectory_planes(h), h->tick - h->ticks_done + every, every);
 }
 
 // dst on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer in
@@ -1517,9 +1514,7 @@ int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
                     (unsigned long long)bytes);
     if (want == 0) return B200_OK;
     if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
-    cudaPointerAttributes a{};
-    const bool direct = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
-    (void)cudaGetLastError();
+    const bool direct = device_destination(h, dst);
     const uint64_t chunk = direct ? h->n_bodies : std::max<uint64_t>(1, std::min<uint64_t>(h->n_bodies, (256ull << 20) / per_body));
     if (!direct && (rc = ensure_staging(h, chunk * per_body))) return rc;
     for (uint64_t b0 = 0; b0 < h->n_bodies; b0 += chunk) {

@@ -215,11 +215,18 @@ class B200Exec:
         """13 = (world_pos[7], world_vel[6]); 25 with trajectory_full: + (world_accel[6], force[6])."""
         return int(self._L.b200_sixdof_trajectory_width(self._h))
 
+    def _planes(self, ring: bool) -> tuple:
+        """The planes a reduction reads, as table axes: [samples, n_entities, width] for the ring's samples,
+        [n_entities, 25] for the current state."""
+        if ring:
+            return (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13))
+        return (self.n_entities, 25)
+
     def trajectory(self) -> np.ndarray:
         """[samples, n_worlds, n_entities, width] — see trajectory_width()."""
         self.sync()
-        n = self.trajectory_len()
-        out = np.empty((n, self.n_worlds, self.n_entities, max(self.trajectory_width(), 13)))
+        n, _, width = self._planes(ring=True)
+        out = np.empty((n, self.n_worlds, self.n_entities, width))
         _lib.check(self._L.b200_sixdof_trajectory_download(self._h, out.ctypes.data, out.nbytes))
         return out
 
@@ -230,52 +237,54 @@ class B200Exec:
         _lib.check(self._L.b200_sixdof_trajectory_reset(self._h))
 
     # ---- ensemble statistics (reductions over the world axis, on the device) ------------------------------------
+    def _reduce(self, kind: str, ring: bool, args: tuple, shape, out_ptr: Optional[int] = None,
+                nbytes: Optional[int] = None) -> Optional[np.ndarray]:
+        """b200_sixdof_{trajectory|state}_{kind}(h, *args, dst, bytes): into `out_ptr` (`nbytes`, by default those of
+        `shape`), returning nothing, or into a new [shape] f64 array, returned."""
+        fn = getattr(self._L, f"b200_sixdof_{'trajectory' if ring else 'state'}_{kind}")
+        out = None if out_ptr is not None else np.empty(shape)
+        ptr = out_ptr if out is None else out.ctypes.data
+        _lib.check(fn(self._h, *args, C.c_void_p(ptr), int(np.prod(shape)) * 8 if nbytes is None else nbytes))
+        return out
+
     def trajectory_stats(self, out: Optional[np.ndarray] = None) -> np.ndarray:
         """The ring's samples reduced over the worlds: [samples, n_entities, width, 5] with the fields (count, mean,
         m2 = sum (x - mean)^2, min, max) over the finite values (count = 0: NaN in the other four)."""
-        shape = (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13), _lib.STATS_FIELDS)
+        shape = self._planes(ring=True) + (_lib.STATS_FIELDS,)
         if out is None:
-            out = np.empty(shape)
-        elif out.shape != shape or out.dtype != np.float64 or not out.flags.c_contiguous:
+            return self._reduce("stats", True, (), shape)
+        if out.shape != shape or out.dtype != np.float64 or not out.flags.c_contiguous:
             raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, f"trajectory statistics are {shape} f64, got {out.shape} {out.dtype}")
-        _lib.check(self._L.b200_sixdof_trajectory_stats(self._h, out.ctypes.data, out.nbytes))
+        self._reduce("stats", True, (), shape, out.ctypes.data)
         return out
 
     def trajectory_stats_to_ptr(self, ptr: int, nbytes: int) -> None:
         """trajectory_stats() into a raw host or device pointer (e.g. a torch CUDA tensor's data_ptr())."""
-        _lib.check(self._L.b200_sixdof_trajectory_stats(self._h, C.c_void_p(ptr), nbytes))
+        self._reduce("stats", True, (), None, ptr, nbytes)
 
     def state_stats(self) -> np.ndarray:
         """The current state reduced over the worlds: [n_entities, 25, 5] — world_pos[7], world_vel[6],
         world_accel[6], force[6] (the B200_TRAJ_FULL sample layout), fields as trajectory_stats()."""
-        out = np.empty((self.n_entities, 25, _lib.STATS_FIELDS))
-        _lib.check(self._L.b200_sixdof_state_stats(self._h, out.ctypes.data, out.nbytes))
-        return out
+        return self._reduce("stats", False, (), self._planes(ring=False) + (_lib.STATS_FIELDS,))
 
     # ---- ensemble quantiles (order statistics over the world axis, on the device) -------------------------------
     @staticmethod
-    def _levels(q) -> np.ndarray:
-        return np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
+    def _levels(q) -> tuple:
+        """q -> the (levels, n_q) arguments of the quantile entries."""
+        lv = np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
+        return lv.ctypes.data_as(C.POINTER(C.c_double)), lv.size  # the pointer keeps lv alive
 
     def trajectory_quantiles(self, q, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
         """The ring's samples: numpy's linear quantile over the finite values of the worlds at each level of `q`,
         [samples, n_entities, width, n_q] (NaN where no world is finite).  With `out_ptr` (a host or device pointer,
         e.g. a torch CUDA tensor's data_ptr()) the table is written there and nothing is returned."""
         lv = self._levels(q)
-        shape = (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13), lv.size)
-        out = None if out_ptr is not None else np.empty(shape)
-        ptr = out_ptr if out is None else out.ctypes.data
-        _lib.check(self._L.b200_sixdof_trajectory_quantiles(self._h, lv.ctypes.data_as(C.POINTER(C.c_double)), lv.size,
-                                                            C.c_void_p(ptr), int(np.prod(shape)) * 8))
-        return out
+        return self._reduce("quantiles", True, lv, self._planes(ring=True) + (lv[1],), out_ptr)
 
     def state_quantiles(self, q) -> np.ndarray:
         """The current state: quantiles over the worlds, [n_entities, 25, n_q] in the B200_TRAJ_FULL plane layout."""
         lv = self._levels(q)
-        out = np.empty((self.n_entities, 25, lv.size))
-        _lib.check(self._L.b200_sixdof_state_quantiles(self._h, lv.ctypes.data_as(C.POINTER(C.c_double)), lv.size,
-                                                       out.ctypes.data, out.nbytes))
-        return out
+        return self._reduce("quantiles", False, lv, self._planes(ring=False) + (lv[1],))
 
     def quantile_reads(self) -> float:
         """Reads of the reduced planes the last quantile call made, averaged over its groups."""
@@ -283,28 +292,22 @@ class B200Exec:
 
     # ---- ensemble covariance (co-moments of a plane selection over the world axis, on the device) --------------
     @staticmethod
-    def _selection(planes) -> np.ndarray:
-        return np.ascontiguousarray(np.atleast_1d(np.asarray(planes, dtype=np.uint32)).ravel())
+    def _selection(planes) -> tuple:
+        """planes -> the (planes, n_p) arguments of the covariance entries."""
+        sel = np.ascontiguousarray(np.atleast_1d(np.asarray(planes, dtype=np.uint32)).ravel())
+        return sel.ctypes.data_as(C.POINTER(C.c_uint32)), sel.size  # the pointer keeps sel alive
 
     def trajectory_covariance(self, planes, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
         """The ring's samples: for the planes `planes` of the 25-plane sample layout, [samples, n_entities, 1 + p + p*p]
         records (n, mean[p], M[p][p] = co-moments) over the worlds whose p selected values are all finite (NaN after
         n where n = 0).  With `out_ptr` (a host or device pointer) the table is written there and nothing is returned."""
         sel = self._selection(planes)
-        shape = (self.trajectory_len(), self.n_entities, 1 + sel.size + sel.size * sel.size)
-        out = None if out_ptr is not None else np.empty(shape)
-        ptr = out_ptr if out is None else out.ctypes.data
-        _lib.check(self._L.b200_sixdof_trajectory_covariance(self._h, sel.ctypes.data_as(C.POINTER(C.c_uint32)), sel.size,
-                                                             C.c_void_p(ptr), int(np.prod(shape)) * 8))
-        return out
+        return self._reduce("covariance", True, sel, self._planes(ring=True)[:-1] + (1 + sel[1] + sel[1] ** 2,), out_ptr)
 
     def state_covariance(self, planes) -> np.ndarray:
         """The current state: [n_entities, 1 + p + p*p] records as trajectory_covariance()."""
         sel = self._selection(planes)
-        out = np.empty((self.n_entities, 1 + sel.size + sel.size * sel.size))
-        _lib.check(self._L.b200_sixdof_state_covariance(self._h, sel.ctypes.data_as(C.POINTER(C.c_uint32)), sel.size,
-                                                        out.ctypes.data, out.nbytes))
-        return out
+        return self._reduce("covariance", False, sel, self._planes(ring=False)[:-1] + (1 + sel[1] + sel[1] ** 2,))
 
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
@@ -365,20 +368,26 @@ class B200Exec:
         return int(self._L.b200_sixdof_plane_stride(self._h))
 
 
+def _stack(tables: Sequence[np.ndarray], merge: str, layout: str, record_ok) -> np.ndarray:
+    """The tables to `merge` as one contiguous f64 array [n_tables, ...]: at least one, all of one shape [..., layout]
+    whose record width (the last axis) passes `record_ok`; B200ValueError otherwise."""
+    parts = [np.asarray(t, dtype=np.float64) for t in tables]
+    if not parts:
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, f"{merge} needs at least one table")
+    shape = parts[0].shape
+    if not (shape and record_ok(shape[-1])) or any(p.shape != shape for p in parts):
+        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH,
+                                  f"{merge}: the tables must share one shape [..., {layout}], got {[p.shape for p in parts]}")
+    return np.ascontiguousarray(np.stack(parts))
+
+
 def merge_stats(tables: Sequence[np.ndarray]) -> np.ndarray:
     """Merge statistics tables of the same shape [..., 5] (e.g. one per rank of a world-sharded campaign, or per
     handle) left to right, in list order, with b200_stats_merge: the table of the union of their worlds."""
-    parts = [np.asarray(t, dtype=np.float64) for t in tables]
-    if not parts:
-        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, "merge_stats needs at least one table")
-    shape = parts[0].shape
-    if shape[-1:] != (_lib.STATS_FIELDS,) or any(p.shape != shape for p in parts):
-        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH,
-                                  f"statistics tables must share one shape [..., 5], got {[p.shape for p in parts]}")
-    stacked = np.ascontiguousarray(np.stack(parts))
-    out = np.empty(shape)
+    stacked = _stack(tables, "merge_stats", "5", lambda rec: rec == _lib.STATS_FIELDS)
+    out = np.empty(stacked.shape[1:])
     dp = C.POINTER(C.c_double)
-    _lib.check(_lib.lib().b200_stats_merge(stacked.ctypes.data_as(dp), len(parts), out.size // _lib.STATS_FIELDS,
+    _lib.check(_lib.lib().b200_stats_merge(stacked.ctypes.data_as(dp), len(stacked), out.size // _lib.STATS_FIELDS,
                                             out.ctypes.data_as(dp)))
     return out
 
@@ -386,19 +395,12 @@ def merge_stats(tables: Sequence[np.ndarray]) -> np.ndarray:
 def merge_covariance(tables: Sequence[np.ndarray]) -> np.ndarray:
     """Merge covariance tables of the same shape [..., 1 + p + p*p] (e.g. one per rank of a world-sharded campaign, or
     per handle) left to right, in list order, with b200_covariance_merge: the table of the union of their worlds."""
-    parts = [np.asarray(t, dtype=np.float64) for t in tables]
-    if not parts:
-        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH, "merge_covariance needs at least one table")
-    shape = parts[0].shape
-    rec = shape[-1] if shape else 0
-    p = math.isqrt(max(rec - 1, 0))  # p^2 <= p^2 + p < (p + 1)^2
-    if rec < 3 or p * p + p + 1 != rec or any(t.shape != shape for t in parts):
-        raise _lib.B200ValueError(_lib.ERR_VALUE_SIZE_MISMATCH,
-                                  f"covariance tables must share one shape [..., 1 + p + p*p], got {[t.shape for t in parts]}")
-    stacked = np.ascontiguousarray(np.stack(parts))
-    out = np.empty(shape)
+    p = lambda rec: math.isqrt(max(rec - 1, 0))  # p^2 <= p^2 + p < (p + 1)^2
+    stacked = _stack(tables, "merge_covariance", "1 + p + p*p", lambda rec: rec >= 3 and p(rec) ** 2 + p(rec) + 1 == rec)
+    out = np.empty(stacked.shape[1:])
+    rec = out.shape[-1]
     dp = C.POINTER(C.c_double)
-    _lib.check(_lib.lib().b200_covariance_merge(stacked.ctypes.data_as(dp), len(parts), out.size // rec, p,
+    _lib.check(_lib.lib().b200_covariance_merge(stacked.ctypes.data_as(dp), len(stacked), out.size // rec, p(rec),
                                                  out.ctypes.data_as(dp)))
     return out
 

@@ -521,6 +521,15 @@ def _sampled_span(pair: str, what: str):
     return ent, span
 
 
+def _sampled_plane(span, index, where: str) -> int:
+    """Plane `index` of the component at `span` (from _SAMPLED) in a 25-plane row; ValueError, prefixed by `where`, for an
+    index that is not an integer in [0, width)."""
+    width = span[1] - span[0]
+    if isinstance(index, (bool, np.bool_)) or not isinstance(index, (int, np.integer)) or not 0 <= index < width:
+        raise ValueError(f"{where}: index {index!r} is not an integer in [0, {width})")
+    return span[0] + int(index)
+
+
 def _quantile_levels(levels) -> np.ndarray:
     """World.build(..., quantiles=...): 1 to MAX_QUANTILES real levels in [0, 1], order and duplicates kept."""
     if isinstance(levels, (str, bytes)) or not isinstance(levels, Sequence) and not isinstance(levels, np.ndarray):
@@ -555,13 +564,11 @@ def _covariance_planes(spec):
         if span is None:
             raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
                                       f"component not found: {comp} (ensemble covariance covers {', '.join(_SAMPLED)})")
-        width = span[1] - span[0]
-        for i in range(width) if idx is None else idx:
-            if isinstance(i, (bool, np.bool_)) or not isinstance(i, (int, np.integer)) or not 0 <= i < width:
-                raise ValueError(f"covariance item {item!r}: index {i!r} is not an integer in [0, {width})")
-            if span[0] + int(i) in planes:
+        for i in range(span[1] - span[0]) if idx is None else idx:
+            plane = _sampled_plane(span, i, f"covariance item {item!r}")
+            if plane in planes:
                 raise ValueError(f"covariance selects {comp}[{int(i)}] twice")
-            planes.append(span[0] + int(i))
+            planes.append(plane)
             labels.append(f"{comp}[{int(i)}]")
     if not 1 <= len(planes) <= _lib.MAX_COV_PLANES:
         raise ValueError(f"covariance selects {len(planes)} planes: 1 to {_lib.MAX_COV_PLANES}")
@@ -582,11 +589,8 @@ class Threshold:
         if np.isnan(value):
             raise ValueError(f"Threshold({pair!r}, {index!r}): the bound is NaN, it would never fire")
         self.entity, span = _sampled_span(pair, "thresholds")
-        width = span[1] - span[0]
-        if isinstance(index, bool) or not isinstance(index, (int, np.integer)) or not 0 <= index < width:
-            raise ValueError(f"Threshold({pair!r}, {index!r}): index must be an integer in [0, {width})")
+        self.plane = _sampled_plane(span, index, f"Threshold({pair!r}, {index!r})")  # in the 25-plane row layout
         self.pair, self.index, self.above, self.value = pair, int(index), below is None, value
-        self.plane = span[0] + self.index  # in the 25-plane row layout
 
     def __repr__(self) -> str:
         return f"Threshold({self.pair!r}, {self.index}, {'above' if self.above else 'below'}={self.value!r})"
@@ -649,11 +653,13 @@ class Exec:
             col = world.columns.get(component_id(cname))
             if col is None or col.entity_ids != bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {cname}")
-        # run summaries: checked here, before any device call
+        # ensemble-mode options: checked here, before any device call, the mode before any option's own values
         self._extrema = bool(extrema)
         self._thresholds = list(thresholds or [])
-        if (self._extrema or self._thresholds) and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "extrema and thresholds need World.build(..., ensemble=True)")
+        given = [name for name, on in (("extrema", self._extrema), ("thresholds", self._thresholds),
+                                       ("quantiles", quantiles is not None), ("covariance", covariance is not None)) if on]
+        if given and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{', '.join(given)}: need World.build(..., ensemble=True)")
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
         self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
@@ -667,14 +673,15 @@ class Exec:
             if ent not in bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
             self._threshold_rows.append((bodies.index(ent), t.plane, t.above, t.value))
-        # quantiles: the mode first (as for extrema and thresholds), then the levels
-        if quantiles is not None and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "quantiles need World.build(..., ensemble=True)")
-        self._quantiles = None if quantiles is None else _quantile_levels(quantiles)
-        # covariance: the mode first, then the selection
-        if covariance is not None and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "covariance needs World.build(..., ensemble=True)")
-        self._cov_planes, self._cov_labels = (None, None) if covariance is None else _covariance_planes(covariance)
+        # ensemble rows, per kind of table: the arguments of B200Exec.trajectory_<kind> / state_<kind>, and the blocks
+        # of rows recorded so far ([k, n_entities, ...] each)
+        self._ens_args: Dict[str, tuple] = {"stats": ()} if ensemble else {}
+        if quantiles is not None:
+            self._ens_args["quantiles"] = (_quantile_levels(quantiles),)
+        if covariance is not None:
+            planes, self._cov_labels = _covariance_planes(covariance)
+            self._ens_args["covariance"] = (planes,)
+        self._ens_rows: Dict[str, List[np.ndarray]] = {kind: [] for kind in self._ens_args}
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
         # a body-row-expanded copy of the column for the device; no members / foreign order -> error.
@@ -725,18 +732,13 @@ class Exec:
         self._db = None
         self._history: Dict[int, List[np.ndarray]] = {cid: [] for cid in self.world.columns}
         self._globals_hist: List[tuple] = []
-        self._ens_rows: List[np.ndarray] = []  # ensemble mode: blocks of rows [k, n_entities, 25, 5]
-        self._ens_q: List[np.ndarray] = []     # and, with quantiles=, blocks of rows [k, n_entities, 25, n_q]
-        self._ens_cov: List[np.ndarray] = []   # and, with covariance=, blocks of rows [k, n_entities, 1 + p + p*p]
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._extrema or self._thresholds:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
         if self._ensemble:
             self._history = {}
             self._upload_inputs()
-            self._ens_rows.append(self._reduce_rows(ring=False))  # row 0: the initial state
-            self._fold_summary(ring=False)
-            self._globals_hist.append((self.tick, self.sim_time_step))
+            self._add_ensemble_rows(ring=False)  # row 0: the initial state
         else:
             self._record()
 
@@ -812,26 +814,18 @@ class Exec:
             else:
                 be.upload(cid, self.world.columns[cid].buffer)
 
-    def _fold_summary(self, ring: bool) -> None:
-        """Run summaries: fold the ring's samples (ring=True) or the current state as one row, on the device."""
-        if self._extrema or self._thresholds:
-            (self.backend.summary_add_trajectory if ring else self.backend.summary_add_state)()
-            self._summary_tables.clear()
-
-    def _reduce_rows(self, ring: bool) -> np.ndarray:
-        """Ensemble rows of the ring's samples (ring=True) or of the current state: the statistics, returned, and the
-        quantiles and covariance when the Exec records them, kept in _ens_q and _ens_cov."""
+    def _add_ensemble_rows(self, ring: bool) -> None:
+        """Record one batch of ensemble rows, on the device: the ring's samples (ring=True; ticks_per_telemetry ticks
+        apart, the last one at the current tick) or the current state as one row.  Reduces every table this Exec
+        records, folds the run summaries and appends the rows' globals."""
         be = self.backend
-        if self._quantiles is not None:
-            self._ens_q.append(be.trajectory_quantiles(self._quantiles) if ring else be.state_quantiles(self._quantiles)[None])
-        if self._cov_planes is not None:
-            self._ens_cov.append(be.trajectory_covariance(self._cov_planes) if ring else be.state_covariance(self._cov_planes)[None])
-        return be.trajectory_stats() if ring else be.state_stats()[None]
-
-    def _add_ensemble_rows(self, rows: np.ndarray, tpt: int) -> None:
-        """rows [k, n_entities, 25, 5]: k telemetry rows, `tpt` ticks apart, the last one at the current tick."""
-        k = rows.shape[0]
-        self._ens_rows.append(rows)
+        for kind, args in self._ens_args.items():
+            rows = getattr(be, f"trajectory_{kind}")(*args) if ring else getattr(be, f"state_{kind}")(*args)[None]
+            self._ens_rows[kind].append(rows)
+        if self._extrema or self._thresholds:
+            (be.summary_add_trajectory if ring else be.summary_add_state)()
+            self._summary_tables.clear()
+        k, tpt = rows.shape[0], self.ticks_per_telemetry
         self._globals_hist.extend((self.tick - (k - 1 - i) * tpt, self.sim_time_step) for i in range(k))
 
     def _run_ensemble(self, ticks: int, is_canceled, pre_step, post_step) -> None:
@@ -851,10 +845,8 @@ class Exec:
                 t0 = time.perf_counter()
                 be.trajectory_reset()
                 be.step(c * tpt)
-                rows = self._reduce_rows(ring=True)                   # [c, n_entities, 25, 5]
-                self._fold_summary(ring=True)
                 self.tick += c * tpt
-                self._add_ensemble_rows(rows, tpt)
+                self._add_ensemble_rows(ring=True)                    # c rows
                 ms = (time.perf_counter() - t0) * 1e3
                 self._prof["execute_buffers"] += [ms / c] * c
                 for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
@@ -865,8 +857,7 @@ class Exec:
                 t0 = time.perf_counter()
                 be.step(remaining)
                 self.tick += remaining
-                self._add_ensemble_rows(self._reduce_rows(ring=False), tpt)
-                self._fold_summary(ring=False)
+                self._add_ensemble_rows(ring=False)
                 self._prof["execute_buffers"].append((time.perf_counter() - t0) * 1e3)
                 for k_dst in ("add_to_history", "h2d_upload", "kernel_invoke", "d2h_download"):
                     self._prof[k_dst].append(0.0)
@@ -897,8 +888,7 @@ class Exec:
                     post_step(self.tick, ctx)
                 done += per_call
             t_hist = time.perf_counter()
-            self._add_ensemble_rows(self._reduce_rows(ring=n == tpt), tpt)
-            self._fold_summary(ring=n == tpt)
+            self._add_ensemble_rows(ring=n == tpt)
             self._prof["add_to_history"].append((time.perf_counter() - t_hist) * 1e3)
             remaining -= n
             if is_canceled is not None and is_canceled():
@@ -917,8 +907,7 @@ class Exec:
         t0 = time.perf_counter()
         self._upload_inputs()
         upload_ms = (time.perf_counter() - t0) * 1e3
-        body_cols = [(component_id("world_pos"), 0, 7), (component_id("world_vel"), 7, 13),
-                     (component_id("world_accel"), 13, 19), (component_id("force"), 19, 25)]
+        body_cols = [(component_id(name), lo, hi) for name, (lo, hi) in _SAMPLED.items()]
         sampled = {cid for cid, _, _ in body_cols}
         while cycles > 0:
             c = min(cycles, self._ring_cap)
@@ -1057,10 +1046,7 @@ class Exec:
         number of such worlds (a diverged world is missing from it), std = sqrt(m2 / count) (numpy's ddof=0), NaN
         where no world is finite.  Needs World.build(..., ensemble=True); the sampled components are world_pos,
         world_vel, world_accel and force."""
-        if not self._ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "ensemble(): build the Exec with World.build(..., ensemble=True)")
-        row, span = self._sampled_row(pair, "ensemble statistics")
-        t = np.concatenate(self._ens_rows)[:, row, span[0]:span[1], :]  # [rows, width, 5]
+        t = self._ensemble_rows("stats", pair, "ensemble statistics", "ensemble()", "")  # [rows, width, 5]
         count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
             std = np.sqrt(t[..., 2] / count)
@@ -1072,11 +1058,7 @@ class Exec:
         state) numpy's linear quantile over the worlds whose value is finite, at each level of World.build(...,
         quantiles=...) in the order given -- the layout of np.quantile(rows_k, q, axis=0) stacked over rows.  NaN where no
         world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates."""
-        if self._quantiles is None:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "quantiles(): build the Exec with World.build(..., ensemble=True, quantiles=[...])")
-        row, span = self._sampled_row(pair, "ensemble quantiles")
-        t = np.concatenate(self._ens_q)[:, row, span[0]:span[1], :]  # [rows, width, n_q]
+        t = self._ensemble_rows("quantiles", pair, "ensemble quantiles", "quantiles()", ", quantiles=[...]")  # [rows, width, n_q]
         return np.ascontiguousarray(t.transpose(0, 2, 1))
 
     def covariance(self, entity: str) -> Dict[str, object]:
@@ -1085,16 +1067,22 @@ class Exec:
         selection of World.build(..., covariance=...), in its order.  Only worlds whose p selected values are all
         finite count (listwise deletion, unlike Exec.ensemble, which counts per component); cov = co-moments / count
         (numpy's ddof=0, as Exec.ensemble's std), exactly symmetric, NaN where count = 0."""
-        if self._cov_planes is None:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "covariance(): build the Exec with World.build(..., ensemble=True, covariance=[...])")
-        row, _ = self._sampled_row(f"{entity}.world_pos", "ensemble covariance")
-        p = len(self._cov_planes)
-        t = np.concatenate(self._ens_cov)[:, row, :]  # [rows, 1 + p + p*p]
+        t = self._ensemble_rows("covariance", f"{entity}.world_pos", "ensemble covariance", "covariance()",
+                                ", covariance=[...]", per_plane=False)  # [rows, 1 + p + p*p]
+        p = len(self._cov_labels)
         count = np.ascontiguousarray(t[:, 0])
         with np.errstate(invalid="ignore", divide="ignore"):
             cov = t[:, 1 + p:].reshape(-1, p, p) / count[:, None, None]
         return {"count": count, "mean": np.ascontiguousarray(t[:, 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
+
+    def _ensemble_rows(self, kind: str, pair: str, what: str, method: str, option: str, per_plane: bool = True):
+        """The recorded rows of table `kind` for the entity of `pair`, sliced to the planes of its component when the
+        table is `per_plane`; refused (ERR_INVALID_ARGUMENT) by `method` if this Exec was not built with `option`."""
+        if kind not in self._ens_rows:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{method}: build the Exec with World.build(..., ensemble=True{option})")
+        row, (lo, hi) = self._sampled_row(pair, what)
+        t = np.concatenate(self._ens_rows[kind])[:, row]
+        return t[:, lo:hi] if per_plane else t
 
     def _sampled_row(self, pair: str, what: str):
         """`<entity>.<component>` -> (Body row of the entity, plane span of the component in a 25-plane row)."""

@@ -9,15 +9,14 @@ test_bounds_are_sensitive shows the one-pass sum(xy) - sum(x) sum(y) / n formula
 
 import ctypes
 import math
-import os
-import socket
 
 import numpy as np
 import pytest
 
 import elodin_b200 as el
 from elodin_b200 import _lib
-from elodin_b200 import world as world_mod
+from tests.ensemble_util import (FREE, ROCKET, handle, need_gpu, no_device, rocket_world, run_gloo,  # noqa: F401
+                                 sampled_state, split, two_body_world)
 
 EPS = np.finfo(np.float64).eps
 NAN = float("nan")
@@ -82,11 +81,6 @@ def symmetric_bits(t, p):
     return M.tobytes() == np.swapaxes(M, -1, -2).copy().tobytes()
 
 
-def _split(rng, n, k):
-    cuts = np.sort(rng.integers(0, n + 1, size=k - 1))
-    return np.split(np.arange(n), cuts)
-
-
 def _empty(groups, p):
     return np.tile(np.concatenate([[0.0], np.full(p + p * p, NAN)]), (groups, 1))
 
@@ -104,7 +98,7 @@ def test_merge_matches_exact_sums(seed):
     x = np.empty((n, 2, p))
     x[:, 0] = 3.0 + z[:, 0] @ np.array([[2.0, 0, 0, 0], [1.0, 1.0, 0, 0], [0, 0.5, 3.0, 0], [0, 0, -1.0, 0.1]])
     x[:, 1] = 7.0e5 + rng.exponential(1.0, (n, p)) * [1.0, 1e3, 1e-3, 5.0]
-    parts = _split(rng, n, k)
+    parts = split(rng, n, k)
     parts.insert(1, parts[0][:0])                                       # an empty part in the middle
     tables = [ref_table(x[idx], range(p)) if len(idx) else _empty(2, p) for idx in parts]
     got = el.merge_covariance(tables)
@@ -131,7 +125,7 @@ def test_bounds_are_sensitive():
     z = rng.normal(size=(n, 2))
     x = np.stack([6.4e6 + 6.4 * z[:, 0], -6.4e6 + 6.4 * (0.9 * z[:, 0] + math.sqrt(1 - 0.81) * z[:, 1])], 1)
     assert 0.9e6 <= abs(np.mean(x[:, 0])) / np.std(x[:, 0]) <= 1.1e6 and abs(np.corrcoef(x.T)[0, 1] - 0.9) < 0.01
-    parts = _split(rng, n, 9)
+    parts = split(rng, n, 9)
     want = ref_table(x, (0, 1))
     got = el.merge_covariance([ref_table(x[idx], (0, 1)) for idx in parts])
     check_table(got, want, scales(x, (0, 1)), "merge")
@@ -149,7 +143,7 @@ def test_non_finite_rows_are_dropped_listwise():
     x[[3, 17, 500], 0, [0, 1, 3]] = [np.nan, np.inf, -np.inf]          # one bad value per row: the whole row goes
     x[:, 1, 2] = np.nan                                                 # no complete world in group 1
     x[::2, 2, 0] = np.inf
-    parts = _split(rng, 1000, 5)
+    parts = split(rng, 1000, 5)
     tables = [ref_table(x[idx], range(4)) if len(idx) else _empty(3, 4) for idx in parts]
     got = el.merge_covariance(tables)
     assert list(got[:, 0]) == [997.0, 0.0, 500.0]
@@ -179,68 +173,28 @@ def test_merge_refusals():
     assert el.merge_covariance([np.zeros((1, 3))]).shape == (1, 3)      # p = 1
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _rank_table(rank):
     rng = np.random.default_rng(100 + rank)
     x = 1.0e4 * (rank + 1) + rng.normal(0.0, 3.0, (300 + 37 * rank, 4, 3))
     return ref_table(x, (2, 0, 1))
 
 
-def _gather_worker(rank, ws, port, q):
-    import torch.distributed as dist
-
+def _gather_worker(rank, ws):
     from elodin_b200.sharding import gather_covariance
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=ws)
-    q.put((rank, gather_covariance(_rank_table(rank))))
-    dist.barrier()
-    dist.destroy_process_group()
+    return gather_covariance(_rank_table(rank))
 
 
 def test_gather_covariance_two_gloo_ranks():
-    import torch.multiprocessing as mp
-
     ws = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_gather_worker, args=(r, ws, port, q)) for r in range(ws)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=120) for _ in range(ws))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = run_gloo(_gather_worker, ws)
     want = el.merge_covariance([_rank_table(r) for r in range(ws)])
     assert got[0].shape == (4, 13)
     assert got[0].tobytes() == want.tobytes() and got[1].tobytes() == want.tobytes()
 
 
-def _two_body_world():
-    w = el.World()
-    w.spawn(el.Body(world_pos=el.SpatialTransform(linear=np.array([0.0, 0.0, 1.0]))), name="rocket")
-    w.spawn(el.Body(), name="ball")
-    return w
-
-
-@pytest.fixture
-def no_device(monkeypatch):
-    def boom(*a, **k):
-        raise AssertionError("validation must finish before the handle is created")
-    monkeypatch.setattr(world_mod, "B200Exec", boom)
-
-
 def test_build_validates_covariance_before_the_device(no_device):
-    w, sys_ = _two_body_world(), el.six_dof()
+    w, sys_ = two_body_world(), el.six_dof()
     for bad in (["world_pos"], ["inertia"], []):                         # the mode is checked before the selection
         with pytest.raises(_lib.B200Error, match="ensemble=True") as e:
             w.build(sys_, covariance=bad)
@@ -275,36 +229,9 @@ def test_covariance_symbols_are_exported():
 # --------------------------------------------------------------------------- GPU
 
 
-def _gpu():
-    if el.device_count() < 1:
-        pytest.skip("needs a CUDA device")
-
-
-ROCKET, FREE = "rocket", "free"
 SHAPES = [(1, 1), (7, 3), ((1 << 16) + 3, 1), (5, 1024), (100, 300)]
 ALL = tuple(range(25))
 SELECTIONS = {1: (6,), 3: (4, 5, 6), 13: tuple(range(12, -1, -1)), 25: (24,) + tuple(range(24))}
-
-
-def _handle(kind, M, N, math_mode, width=25, capacity=3, seed=0, state=None):
-    from tests.util import near_world
-
-    pos, vel, ine, cols, dt = near_world(seed, M, N) if state is None else state
-    effs, up = [], {}
-    if kind == ROCKET:
-        effs = [el.GravityConst((0.0, 0.0, -9.81)), el.ThrustBody((-1.0, 0.0, 0.0), "thrust"),
-                el.DragQuadratic(0.6125, 0.0025, "wind")]
-        up = {"thrust": cols["thrust"], "wind": cols["wind"]}
-    ex = el.B200Exec(N, M, dt, None, effs, "rk4", math_mode, trajectory_every=1, trajectory_capacity=capacity,
-                     trajectory_full=width == 25)
-    ex.set_state(pos, vel, ine, **up)
-    return ex, (pos, vel, ine, cols, dt)
-
-
-def _state(ex):
-    from elodin_b200.executor import FORCE, WORLD_ACCEL, WORLD_POS, WORLD_VEL
-
-    return np.concatenate([ex.download(c) for c in (WORLD_POS, WORLD_VEL, WORLD_ACCEL, FORCE)], axis=-1)  # [M, N, 25]
 
 
 @pytest.mark.gpu
@@ -313,9 +240,9 @@ def _state(ex):
 @pytest.mark.parametrize("width", [13, 25])
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")
 def test_trajectory_covariance_matches_the_ring(shape, width, kind, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
-    with _handle(kind, M, N, math_mode, width=width, capacity=2)[0] as ex:
+    with handle(kind, M, N, math_mode, width=width, capacity=2)[0] as ex:
         ex.step(2)
         traj = np.moveaxis(ex.trajectory(), 1, 0)                       # [M, S, N, W]
         for p, sel in SELECTIONS.items():
@@ -333,13 +260,13 @@ def test_trajectory_covariance_matches_the_ring(shape, width, kind, math_mode):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_diagonal_matches_the_statistics_and_permutations_permute_bits(shape):
-    _gpu()
+    need_gpu()
     M, N = shape
-    with _handle(ROCKET, M, N, "fast", capacity=1)[0] as ex:
+    with handle(ROCKET, M, N, "fast", capacity=1)[0] as ex:
         ex.step(2)
         full = ex.state_covariance(ALL)
         stats = ex.state_stats()                                        # [N, 25, 5], every world finite
-        state = _state(ex)
+        state = sampled_state(ex)
         rng = np.random.default_rng(5)
         perm = rng.permutation(25)
         permuted = ex.state_covariance(perm)
@@ -364,7 +291,7 @@ def test_diagonal_matches_the_statistics_and_permutations_permute_bits(shape):
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_non_finite_worlds_are_dropped_listwise(shape, math_mode):
-    _gpu()
+    need_gpu()
     from tests.util import near_world
 
     M, N = shape
@@ -374,9 +301,9 @@ def test_non_finite_worlds_are_dropped_listwise(shape, math_mode):
     pos[M - 2, 0, 5] = -np.inf                                          # selected
     pos[M - 1, 0, 0] = np.nan                                           # not selected: excludes nothing
     sel = (4, 5, 6, 10)
-    with _handle(FREE, M, N, math_mode, capacity=1, state=(pos, vel, ine, cols, dt))[0] as ex:
+    with handle(FREE, M, N, math_mode, capacity=1, state=(pos, vel, ine, cols, dt))[0] as ex:
         got = ex.state_covariance(sel)
-        state = _state(ex)
+        state = sampled_state(ex)
         sub = ex.state_covariance((6, 11))                              # the bad worlds are in neither plane
     if N == 1:
         assert got[0, 0] == M - 3
@@ -385,7 +312,7 @@ def test_non_finite_worlds_are_dropped_listwise(shape, math_mode):
     assert np.all(sub[:, 0] == M)
     check_table(got, ref_table(state, sel), scales(state, sel), f"{shape} listwise")
     check_table(sub, ref_table(state, (6, 11)), scales(state, (6, 11)), f"{shape} unselected")
-    with _handle(FREE, M, N, math_mode, capacity=1,
+    with handle(FREE, M, N, math_mode, capacity=1,
                  state=(np.full_like(pos, np.nan), vel, ine, cols, dt))[0] as ex:
         empty = ex.state_covariance((4, 10))
     assert np.all(empty[:, 0] == 0) and np.all(np.isnan(empty[:, 1:]))
@@ -395,7 +322,7 @@ def test_non_finite_worlds_are_dropped_listwise(shape, math_mode):
 @pytest.mark.parametrize("shape", [((1 << 16) + 3, 1), (7, 3), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_orbital_offsets_keep_the_bound(shape):
     """|mean| / sigma = 1e6 with correlation 0.9 between x and y, where sum(xy) - sum(x) sum(y) / n breaks the bound."""
-    _gpu()
+    need_gpu()
     from tests.util import near_world
 
     M, N = shape
@@ -407,9 +334,9 @@ def test_orbital_offsets_keep_the_bound(shape):
     pos[..., 6] = 2.2e6 + 6.4 * z[..., 2]
     vel[..., 3:] = 7.6e3 + rng.normal(0.0, 7.6e-3, (M, N, 3))
     sel = (4, 5, 6, 10, 11, 12)
-    with _handle(FREE, M, N, "fast", capacity=1, state=(pos, vel, ine, cols, dt))[0] as ex:
+    with handle(FREE, M, N, "fast", capacity=1, state=(pos, vel, ine, cols, dt))[0] as ex:
         got = ex.state_covariance(sel)
-        state = _state(ex)
+        state = sampled_state(ex)
     want = ref_table(state, sel)
     check_table(got, want, scales(state, sel), f"orbital {shape}")
     if M > 1000:
@@ -425,11 +352,11 @@ def test_orbital_offsets_keep_the_bound(shape):
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (5, 1024), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_a_sample_has_the_same_bits_in_any_ring(shape):
     """At (1<<16)+3 x 1 the 128-sample call at p = 25 needs two scratch slices (a slice holds 98 groups there)."""
-    _gpu()
+    need_gpu()
     M, N = shape
     S = 128 if M > 1000 and N == 1 else 64
-    big, state = _handle(ROCKET, M, N, "fast", capacity=S)
-    one, _ = _handle(ROCKET, M, N, "fast", capacity=1, state=state)
+    big, state = handle(ROCKET, M, N, "fast", capacity=S)
+    one, _ = handle(ROCKET, M, N, "fast", capacity=1, state=state)
     sel = SELECTIONS[25]
     with big, one:
         big.step(S)
@@ -452,13 +379,13 @@ def test_a_sample_has_the_same_bits_in_any_ring(shape):
 
 @pytest.mark.gpu
 def test_refusals_and_device_destinations():
-    _gpu()
+    need_gpu()
     import torch
 
     L = _lib.lib()
     M, N = 20000, 2
     up = ctypes.POINTER(ctypes.c_uint32)
-    with _handle(ROCKET, M, N, "exact", width=13, capacity=2)[0] as ex:
+    with handle(ROCKET, M, N, "exact", width=13, capacity=2)[0] as ex:
         ex.step(2)
         good = ex.trajectory_covariance((4, 5, 6, 10))
         for sel in ([], list(range(14)), [4, 5, 4], [13], [24]):        # a 13-plane ring has no accel / force
@@ -487,7 +414,7 @@ def test_refusals_and_device_destinations():
 
 @pytest.mark.gpu
 def test_two_handles_merged_match_one():
-    _gpu()
+    need_gpu()
     from tests.util import near_world
 
     M, N = 20_001, 2
@@ -496,9 +423,9 @@ def test_two_handles_merged_match_one():
     part = lambda a, lo, hi: np.ascontiguousarray(a[lo:hi])
     sub = lambda lo, hi: (part(pos, lo, hi), part(vel, lo, hi), part(ine, lo, hi),
                           {k: part(v, lo, hi) for k, v in cols.items()}, dt)
-    whole, _ = _handle(ROCKET, M, N, "fast", state=(pos, vel, ine, cols, dt))
-    a, _ = _handle(ROCKET, half, N, "fast", state=sub(0, half))
-    b, _ = _handle(ROCKET, M - half, N, "fast", state=sub(half, M))
+    whole, _ = handle(ROCKET, M, N, "fast", capacity=3, state=(pos, vel, ine, cols, dt))
+    a, _ = handle(ROCKET, half, N, "fast", capacity=3, state=sub(0, half))
+    b, _ = handle(ROCKET, M - half, N, "fast", capacity=3, state=sub(half, M))
     sel = SELECTIONS[13]
     with whole, a, b:
         for ex in (whole, a, b):
@@ -511,36 +438,12 @@ def test_two_handles_merged_match_one():
     check_table(want, ref_table(traj, sel), scales(traj, sel), "one handle")
 
 
-def _rocket_world(n_worlds, seed=4):
-    rng = np.random.default_rng(seed)
-    Thrust = el.Annotated[np.ndarray, el.Component("thrust", el.ComponentType.F64)]
-    Wind = el.Annotated[np.ndarray, el.Component("wind", el.ComponentType(el.PrimitiveType.F64, (3,)))]
-
-    @el.dataclass
-    class Rocket(el.Archetype):
-        thrust: Thrust
-        wind: Wind
-
-    w = el.World()
-    w.spawn([el.Body(world_pos=el.SpatialTransform(angular=el.Quaternion.from_euler([0.0, np.radians(70.0), 0.0]),
-                                                   linear=np.array([0.0, 0.0, 1.0])),
-                     inertia=el.SpatialInertia(3.0, np.array([0.1, 1.0, 1.0]))),
-             Rocket(np.array([88.426]), np.zeros(3))], name="rocket")
-    w.spawn(el.Body(world_vel=el.SpatialMotion(linear=[1.0, 2.0, 0.0])), name="ball")
-    effs = el.GravityConst((0.0, 0.0, -9.81)) | el.ThrustBody((-1.0, 0.0, 0.0), "thrust") | el.DragQuadratic(0.6125, 0.0025, "wind")
-    params = {"thrust": 88.426 * rng.uniform(0.8, 1.2, (n_worlds, 1, 1)),
-              "wind": np.concatenate([rng.normal(0, 2, (n_worlds, 1, 1)), np.zeros((n_worlds, 1, 2))], -1),
-              "inertia": np.tile(np.array([0.1, 1.0, 1.0, 0, 0, 0, 3.0]), (n_worlds, 2, 1))}
-    params["inertia"][:, 0, 6] = rng.uniform(2.5, 3.5, n_worlds)
-    return w, el.six_dof(sys=effs), params
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 def test_exec_covariance_against_the_default_mode(math_mode):
-    _gpu()
+    need_gpu()
     M, ticks = 300, 23
-    w, sys_, params = _rocket_world(M)
+    w, sys_, params = rocket_world(M)
     kw = dict(simulation_rate=120.0, telemetry_rate=24.0, math=math_mode, n_worlds=M, world_params=params)
     ref = w.build(sys_, **kw)
     ref.run(ticks)

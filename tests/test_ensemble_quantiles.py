@@ -10,11 +10,10 @@ import numpy as np
 import pytest
 
 import elodin_b200 as el
-import elodin_b200.world as world_mod
 from elodin_b200 import _lib
+from tests.ensemble_util import SAMPLED, need_gpu, no_device, rocket_world, sampled_state, two_body_world  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SAMPLED = {"world_pos": (0, 7), "world_vel": (7, 13), "world_accel": (13, 19), "force": (19, 25)}
 LEVELS = (0.0, 1e-3, 1 / 3, 0.5, 0.9, 0.999, 1.0)
 DBL_MAX = np.finfo(np.float64).max
 
@@ -108,22 +107,8 @@ def test_reference_is_rank_sensitive_on_the_test_data():
     assert sensitive(_degenerate(20000), LEVELS, frac=0.3)
 
 
-def _two_body_world():
-    w = el.World()
-    w.spawn(el.Body(world_pos=el.SpatialTransform(linear=np.array([0.0, 0.0, 1.0]))), name="rocket")
-    w.spawn(el.Body(), name="ball")
-    return w
-
-
-@pytest.fixture
-def no_device(monkeypatch):
-    def boom(*a, **k):
-        raise AssertionError("validation must finish before the handle is created")
-    monkeypatch.setattr(world_mod, "B200Exec", boom)
-
-
 def test_build_validates_quantiles_before_the_device(no_device):
-    w, sys_ = _two_body_world(), el.six_dof()
+    w, sys_ = two_body_world(), el.six_dof()
     for bad in ((0.5,), [float("nan")], []):                             # the mode is checked before the levels
         with pytest.raises(_lib.B200Error, match="ensemble=True") as e:
             w.build(sys_, quantiles=bad)
@@ -159,17 +144,6 @@ def test_quantile_symbols_and_constant_match_the_header(tmp_path):
 # --------------------------------------------------------------------------- GPU
 
 
-def _gpu():
-    if el.device_count() < 1:
-        pytest.skip("needs a CUDA device")
-
-
-def _state(ex):
-    from elodin_b200.executor import FORCE, WORLD_ACCEL, WORLD_POS, WORLD_VEL
-
-    return np.concatenate([ex.download(c) for c in (WORLD_POS, WORLD_VEL, WORLD_ACCEL, FORCE)], axis=-1)  # [M, N, 25]
-
-
 def _handle(M, N, math_mode, capacity, rocket, full, seed=0):
     from tests.util import near_world
 
@@ -189,7 +163,7 @@ SHAPES = [(1, 1), (7, 3), ((1 << 16) + 3, 1), (5, 1024), (100, 300), ((1 << 20) 
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")
 def test_ring_and_state_quantiles_equal_the_reference(shape, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
     q = LEVELS
     huge = M > 1 << 20                                                  # one sample of one set: the reference sorts
@@ -203,7 +177,7 @@ def test_ring_and_state_quantiles_equal_the_reference(shape, math_mode):
             assert ex.trajectory_quantiles(q).tobytes() == got.tobytes()
             assert same_bits(got, ref_quantiles(np.moveaxis(traj, 1, 0), q)), (rocket, full)
             st = ex.state_quantiles(q)
-            assert same_bits(st, ref_quantiles(_state(ex), q)), (rocket, full)
+            assert same_bits(st, ref_quantiles(sampled_state(ex), q)), (rocket, full)
             if M >= 100:
                 assert sensitive(np.moveaxis(traj, 1, 0)[:, 0, :, :7], q, frac=0.5)
 
@@ -235,12 +209,12 @@ def _degenerate(M, seed=3):
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("M", [1000, 20000, (1 << 18) + 1])
 def test_degenerate_data_equals_the_reference(M, math_mode):
-    _gpu()
+    need_gpu()
     x = _degenerate(M)[:, None, :]                                       # [M, 1, 25]
     ine = np.tile(np.array([1.0, 1.0, 1.0, 0, 0, 0, 1.0]), (M, 1, 1))
     with el.B200Exec(1, M, 0.01, None, [], "rk4", math_mode) as ex:
         ex.set_state(x[..., :7], x[..., 7:13], ine, accel=x[..., 13:19], force=x[..., 19:25])
-        st = _state(ex)
+        st = sampled_state(ex)
         assert same_bits(st, x)
         got = ex.state_quantiles(LEVELS)
         assert ex.quantile_reads() <= 8
@@ -252,7 +226,7 @@ def test_degenerate_data_equals_the_reference(M, math_mode):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(100, 3), (10000, 1)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_ring_size_changes_neither_bytes_nor_launch_count(shape):
-    _gpu()
+    need_gpu()
     M, N = shape
     q = (0.01, 0.5, 0.99)
     big = _handle(M, N, "fast", 64, True, False)
@@ -277,7 +251,7 @@ def test_groups_beyond_one_scratch_slice(math_mode):
     """More groups than one slice of scratch holds: 9000 worlds x 64 samples x 25 planes = 1600 groups (a slice holds
     about 1350), and 9000 worlds x 60 entities x 25 planes in the state.  The slices run the same launch sequence each
     and give the same bytes as the reference."""
-    _gpu()
+    need_gpu()
     M, S = 9000, 64
     q = (0.01, 0.5, 0.99)
     with _handle(M, 1, math_mode, S, True, True) as ex:
@@ -298,12 +272,12 @@ def test_groups_beyond_one_scratch_slice(math_mode):
         n0 = ex.timings()["kernel_launches"]
         got = ex.state_quantiles(q)
         assert ex.timings()["kernel_launches"] - n0 == 2 * per_slice
-        assert same_bits(got, ref_quantiles(_state(ex), q))
+        assert same_bits(got, ref_quantiles(sampled_state(ex), q))
 
 
 @pytest.mark.gpu
 def test_refusals_leave_the_handle_usable_and_device_destinations_match():
-    _gpu()
+    need_gpu()
     import torch
 
     L = _lib.lib()
@@ -334,38 +308,14 @@ def test_refusals_leave_the_handle_usable_and_device_destinations_match():
         assert ex.timings()["kernel_launches"] == n0
 
 
-def _rocket_world(n_worlds, seed=4):
-    rng = np.random.default_rng(seed)
-    Thrust = el.Annotated[np.ndarray, el.Component("thrust", el.ComponentType.F64)]
-    Wind = el.Annotated[np.ndarray, el.Component("wind", el.ComponentType(el.PrimitiveType.F64, (3,)))]
-
-    @el.dataclass
-    class Rocket(el.Archetype):
-        thrust: Thrust
-        wind: Wind
-
-    w = el.World()
-    w.spawn([el.Body(world_pos=el.SpatialTransform(angular=el.Quaternion.from_euler([0.0, np.radians(70.0), 0.0]),
-                                                   linear=np.array([0.0, 0.0, 1.0])),
-                     inertia=el.SpatialInertia(3.0, np.array([0.1, 1.0, 1.0]))),
-             Rocket(np.array([88.426]), np.zeros(3))], name="rocket")
-    w.spawn(el.Body(world_vel=el.SpatialMotion(linear=[1.0, 2.0, 0.0])), name="ball")
-    effs = el.GravityConst((0.0, 0.0, -9.81)) | el.ThrustBody((-1.0, 0.0, 0.0), "thrust") | el.DragQuadratic(0.6125, 0.0025, "wind")
-    params = {"thrust": 88.426 * rng.uniform(0.8, 1.2, (n_worlds, 1, 1)),
-              "wind": np.concatenate([rng.normal(0, 2, (n_worlds, 1, 1)), np.zeros((n_worlds, 1, 2))], -1),
-              "inertia": np.tile(np.array([0.1, 1.0, 1.0, 0, 0, 0, 3.0]), (n_worlds, 2, 1))}
-    params["inertia"][:, 0, 6] = rng.uniform(2.5, 3.5, n_worlds)
-    return w, el.six_dof(sys=effs), params
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("M", [300, 9000])
 def test_exec_quantiles_against_the_default_mode(M, math_mode):
-    _gpu()
+    need_gpu()
     ticks = 23
     q = (0.01, 0.5, 0.99, 0.5)
-    w, sys_, params = _rocket_world(M)
+    w, sys_, params = rocket_world(M)
     kw = dict(simulation_rate=120.0, telemetry_rate=24.0, math=math_mode, n_worlds=M, world_params=params)
     ref = w.build(sys_, **kw)
     ref.run(ticks)

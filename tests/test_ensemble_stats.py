@@ -8,14 +8,13 @@ matters only for groups whose worlds agree to the last bits).  test_bounds_are_s
 E[x^2] - E[x]^2 formula violates the std bound on data with |mean| / std = 1e6, where the library must keep it."""
 
 import math
-import os
-import socket
 
 import numpy as np
 import pytest
 
 import elodin_b200 as el
 from elodin_b200 import _lib
+from tests.ensemble_util import FREE, ROCKET, handle, need_gpu, rocket_world, run_gloo, sampled_state, split
 
 EPS = np.finfo(np.float64).eps
 NAN = float("nan")
@@ -74,19 +73,13 @@ def finite_scale(x):
 # --------------------------------------------------------------------------- CPU: b200_stats_merge
 
 
-def _split(rng, n, k):
-    """k parts of n values (empty parts included) in random sizes."""
-    cuts = np.sort(rng.integers(0, n + 1, size=k - 1))
-    return np.split(np.arange(n), cuts)
-
-
 @pytest.mark.parametrize("seed", range(6))
 def test_merge_matches_exact_sums(seed):
     rng = np.random.default_rng(seed)
     n = int(rng.integers(10_000, 1_000_001)) if seed < 5 else 1_000_000
     k = int(rng.integers(1, 17))
     groups = np.stack([rng.normal(3.0, 2.0, n), rng.uniform(-1e3, 5e3, n), 7.0e5 + rng.exponential(1.0, n)], axis=1)
-    parts = _split(rng, n, k)
+    parts = split(rng, n, k)
     if k > 2:
         parts.insert(1, parts[0][:0])  # an empty part in the middle
     tables = [ref_table(groups[idx]) if len(idx) else np.tile([0.0, NAN, NAN, NAN, NAN], (3, 1)) for idx in parts]
@@ -104,7 +97,7 @@ def test_bounds_are_sensitive():
     n = 200_000
     x = 6.4e6 + rng.normal(0.0, 6.4, n)
     assert 0.9e6 <= abs(np.mean(x)) / np.std(x) <= 1.1e6
-    parts = _split(rng, n, 9)
+    parts = split(rng, n, 9)
     tables = [ref_table(x[idx][:, None]) for idx in parts]
     want = ref_table(x[:, None])
     got = el.merge_stats(tables)
@@ -120,7 +113,7 @@ def test_non_finite_worlds_are_excluded_and_counted():
     x[[3, 17, 500], 0] = [np.nan, np.inf, -np.inf]
     x[:, 2] = np.nan  # nothing finite in this group
     x[::2, 3] = np.inf
-    parts = _split(rng, 1000, 5)
+    parts = split(rng, 1000, 5)
     tables = [ref_table(x[idx]) if len(idx) else np.tile([0.0, NAN, NAN, NAN, NAN], (4, 1)) for idx in parts]
     got = el.merge_stats(tables)
     want = ref_table(x)
@@ -138,47 +131,21 @@ def test_merge_rejects_bad_tables():
         el.merge_stats([np.full((2, 5), -1.0)])  # a negative count
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _rank_table(rank):
     rng = np.random.default_rng(100 + rank)
     x = 1.0e4 * (rank + 1) + rng.normal(0.0, 3.0, (500 + 37 * rank, 6, 4))
     return ref_table(x)
 
 
-def _gather_worker(rank, ws, port, q):
-    import torch.distributed as dist
-
+def _gather_worker(rank, ws):
     from elodin_b200.sharding import gather_ensemble
 
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=ws)
-    q.put((rank, gather_ensemble(_rank_table(rank))))
-    dist.barrier()
-    dist.destroy_process_group()
+    return gather_ensemble(_rank_table(rank))
 
 
 def test_gather_ensemble_two_gloo_ranks():
-    import torch.multiprocessing as mp
-
     ws = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_gather_worker, args=(r, ws, port, q)) for r in range(ws)]
-    for p in procs:
-        p.start()
-    got = dict(q.get(timeout=120) for _ in range(ws))
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = run_gloo(_gather_worker, ws)
     want = el.merge_stats([_rank_table(r) for r in range(ws)])  # rank order
     assert got[0].shape == (6, 4, 5)
     assert got[0].tobytes() == want.tobytes() and got[1].tobytes() == want.tobytes()
@@ -187,31 +154,7 @@ def test_gather_ensemble_two_gloo_ranks():
 # --------------------------------------------------------------------------- GPU
 
 
-def _gpu():
-    if el.device_count() < 1:
-        pytest.skip("needs a CUDA device")
-
-
-ROCKET = "rocket"
-FREE = "free"
 SHAPES = [(1, 1), (7, 3), ((1 << 16) + 3, 1), (5, 1024), (100, 300)]
-
-
-def _handle(kind, M, N, math_mode, width=25, every=1, capacity=4, seed=0, state=None):
-    """A handle with a trajectory ring and a random initial state; returns (handle, (pos, vel, ine, columns))."""
-    from tests.util import near_world
-
-    pos, vel, ine, cols, dt = near_world(seed, M, N) if state is None else state
-    effs = []
-    up = {}
-    if kind == ROCKET:
-        effs = [el.GravityConst((0.0, 0.0, -9.81)), el.ThrustBody((-1.0, 0.0, 0.0), "thrust"),
-                el.DragQuadratic(0.6125, 0.0025, "wind")]
-        up = {"thrust": cols["thrust"], "wind": cols["wind"]}
-    ex = el.B200Exec(N, M, dt, None, effs, "rk4", math_mode, trajectory_every=every, trajectory_capacity=capacity,
-                     trajectory_full=width == 25)
-    ex.set_state(pos, vel, ine, **up)
-    return ex, (pos, vel, ine, cols, dt)
 
 
 def _ring_ref(traj):
@@ -220,21 +163,15 @@ def _ring_ref(traj):
     return ref_table(x), finite_scale(x)
 
 
-def _state(ex):
-    from elodin_b200.executor import FORCE, WORLD_ACCEL, WORLD_POS, WORLD_VEL
-
-    return np.concatenate([ex.download(c) for c in (WORLD_POS, WORLD_VEL, WORLD_ACCEL, FORCE)], axis=-1)  # [M, N, 25]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("kind", [FREE, ROCKET])
 @pytest.mark.parametrize("width", [13, 25])
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")
 def test_trajectory_stats_match_the_ring(shape, width, kind, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
-    with _handle(kind, M, N, math_mode, width=width, capacity=3)[0] as ex:
+    with handle(kind, M, N, math_mode, width=width, capacity=3)[0] as ex:
         ex.step(3)
         traj = ex.trajectory()
         got = ex.trajectory_stats()
@@ -251,12 +188,12 @@ def test_trajectory_stats_match_the_ring(shape, width, kind, math_mode):
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")
 def test_state_stats_match_the_columns(shape, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
-    with _handle(ROCKET, M, N, math_mode, capacity=1)[0] as ex:
+    with handle(ROCKET, M, N, math_mode, capacity=1)[0] as ex:
         ex.step(2)
         got = ex.state_stats()
-        cols = _state(ex)
+        cols = sampled_state(ex)
     assert got.shape == (N, 25, 5)
     check_table(got, ref_table(cols), finite_scale(cols), f"{shape} {math_mode}")
 
@@ -266,7 +203,7 @@ def test_state_stats_match_the_columns(shape, math_mode):
 def test_state_stats_keep_the_bounds_at_orbital_offsets(shape):
     """The kernel on |mean| / std = 1e6 data (orbital positions, metre-level dispersion), where E[x^2] - E[x]^2
     breaks the std bound."""
-    _gpu()
+    need_gpu()
     M, N = shape
     rng = np.random.default_rng(11)
     from tests.util import near_world
@@ -274,9 +211,9 @@ def test_state_stats_keep_the_bounds_at_orbital_offsets(shape):
     pos, vel, ine, cols, dt = near_world(5, M, N)
     pos[..., 4:] = np.array([6.4e6, -3.1e6, 2.2e6]) + rng.normal(0.0, 6.4, (M, N, 3))
     vel[..., 3:] = 7.6e3 + rng.normal(0.0, 7.6e-3, (M, N, 3))
-    with _handle(FREE, M, N, "fast", state=(pos, vel, ine, cols, dt))[0] as ex:
+    with handle(FREE, M, N, "fast", state=(pos, vel, ine, cols, dt))[0] as ex:
         got = ex.state_stats()
-        state = _state(ex)
+        state = sampled_state(ex)
     check_table(got, ref_table(state), finite_scale(state), f"orbital {shape}")
     if M > 1000:
         x = state[:, 0, 4]
@@ -289,7 +226,7 @@ def test_state_stats_keep_the_bounds_at_orbital_offsets(shape):
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_non_finite_worlds_are_dropped_from_the_count(shape, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
     from tests.util import near_world
 
@@ -298,9 +235,9 @@ def test_non_finite_worlds_are_dropped_from_the_count(shape, math_mode):
     pos[bad[0], 0, 4] = np.nan
     vel[bad[1], N - 1, 3] = np.inf
     pos[bad[2], 0, 5] = -np.inf
-    with _handle(ROCKET, M, N, math_mode, capacity=2, state=(pos, vel, ine, cols, dt))[0] as ex:
+    with handle(ROCKET, M, N, math_mode, capacity=2, state=(pos, vel, ine, cols, dt))[0] as ex:
         s0 = ex.state_stats()
-        state0 = _state(ex)
+        state0 = sampled_state(ex)
         ex.step(2)
         traj = ex.trajectory()
         got = ex.trajectory_stats()
@@ -314,11 +251,11 @@ def test_non_finite_worlds_are_dropped_from_the_count(shape, math_mode):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (5, 1024), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_a_sample_has_the_same_bits_in_any_ring(shape):
-    _gpu()
+    need_gpu()
     M, N = shape
     S = 64 if M * N < 100_000 else 8
-    big, state = _handle(ROCKET, M, N, "fast", capacity=S)
-    one, _ = _handle(ROCKET, M, N, "fast", capacity=1, state=state)
+    big, state = handle(ROCKET, M, N, "fast", capacity=S)
+    one, _ = handle(ROCKET, M, N, "fast", capacity=1, state=state)
     with big, one:
         big.step(S)
         many = big.trajectory_stats()
@@ -333,7 +270,7 @@ def test_a_sample_has_the_same_bits_in_any_ring(shape):
 
 @pytest.mark.gpu
 def test_two_handles_merged_match_one():
-    _gpu()
+    need_gpu()
     from tests.util import near_world
 
     M, N = 20_001, 2
@@ -342,9 +279,9 @@ def test_two_handles_merged_match_one():
     part = lambda a, lo, hi: np.ascontiguousarray(a[lo:hi])
     sub = lambda lo, hi: (part(pos, lo, hi), part(vel, lo, hi), part(ine, lo, hi),
                           {k: part(v, lo, hi) for k, v in cols.items()}, dt)
-    whole, _ = _handle(ROCKET, M, N, "fast", capacity=3, state=(pos, vel, ine, cols, dt))
-    a, _ = _handle(ROCKET, half, N, "fast", capacity=3, state=sub(0, half))
-    b, _ = _handle(ROCKET, M - half, N, "fast", capacity=3, state=sub(half, M))
+    whole, _ = handle(ROCKET, M, N, "fast", capacity=3, state=(pos, vel, ine, cols, dt))
+    a, _ = handle(ROCKET, half, N, "fast", capacity=3, state=sub(0, half))
+    b, _ = handle(ROCKET, M - half, N, "fast", capacity=3, state=sub(half, M))
     with whole, a, b:
         for ex in (whole, a, b):
             ex.step(3)
@@ -354,36 +291,12 @@ def test_two_handles_merged_match_one():
     check_table(got, want, _ring_ref(traj)[1], "two handles")
 
 
-def _rocket_world(n_worlds, seed=4):
-    rng = np.random.default_rng(seed)
-    Thrust = el.Annotated[np.ndarray, el.Component("thrust", el.ComponentType.F64)]
-    Wind = el.Annotated[np.ndarray, el.Component("wind", el.ComponentType(el.PrimitiveType.F64, (3,)))]
-
-    @el.dataclass
-    class Rocket(el.Archetype):
-        thrust: Thrust
-        wind: Wind
-
-    w = el.World()
-    w.spawn([el.Body(world_pos=el.SpatialTransform(angular=el.Quaternion.from_euler([0.0, np.radians(70.0), 0.0]),
-                                                   linear=np.array([0.0, 0.0, 1.0])),
-                     inertia=el.SpatialInertia(3.0, np.array([0.1, 1.0, 1.0]))),
-             Rocket(np.array([88.426]), np.zeros(3))], name="rocket")
-    w.spawn(el.Body(world_vel=el.SpatialMotion(linear=[1.0, 2.0, 0.0])), name="ball")
-    effs = el.GravityConst((0.0, 0.0, -9.81)) | el.ThrustBody((-1.0, 0.0, 0.0), "thrust") | el.DragQuadratic(0.6125, 0.0025, "wind")
-    params = {"thrust": 88.426 * rng.uniform(0.8, 1.2, (n_worlds, 1, 1)),
-              "wind": np.concatenate([rng.normal(0, 2, (n_worlds, 1, 1)), np.zeros((n_worlds, 1, 2))], -1),
-              "inertia": np.tile(np.array([0.1, 1.0, 1.0, 0, 0, 0, 3.0]), (n_worlds, 2, 1))}
-    params["inertia"][:, 0, 6] = rng.uniform(2.5, 3.5, n_worlds)
-    return w, el.six_dof(sys=effs), params
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 def test_exec_ensemble_mode_against_the_default_mode(math_mode):
-    _gpu()
+    need_gpu()
     M, ticks = 300, 23
-    w, sys_, params = _rocket_world(M)
+    w, sys_, params = rocket_world(M)
     kw = dict(simulation_rate=120.0, telemetry_rate=24.0, math=math_mode, n_worlds=M, world_params=params)
     ref = w.build(sys_, **kw)
     ref.run(ticks)

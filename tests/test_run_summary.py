@@ -10,11 +10,10 @@ import numpy as np
 import pytest
 
 import elodin_b200 as el
-import elodin_b200.world as world_mod
 from elodin_b200 import _lib
+from tests.ensemble_util import SAMPLED, need_gpu, no_device, rocket_world, sampled_state, two_body_world  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SAMPLED = {"world_pos": (0, 7), "world_vel": (7, 13), "world_accel": (13, 19), "force": (19, 25)}
 
 
 # --------------------------------------------------------------------------- numpy references
@@ -65,21 +64,6 @@ def same(a, b):
 # --------------------------------------------------------------------------- CPU: validation before any device call
 
 
-def _two_body_world():
-    w = el.World()
-    w.spawn(el.Body(world_pos=el.SpatialTransform(linear=np.array([0.0, 0.0, 1.0]))), name="rocket")
-    w.spawn(el.Body(), name="ball")
-    return w
-
-
-@pytest.fixture
-def no_device(monkeypatch):
-    """Fail the test if World.build reaches the device (the handle is created through world.B200Exec)."""
-    def boom(*a, **k):
-        raise AssertionError("validation must finish before the handle is created")
-    monkeypatch.setattr(world_mod, "B200Exec", boom)
-
-
 def test_threshold_validates_its_arguments():
     t = el.Threshold("ball.world_pos", 6, below=0.0)
     assert (t.plane, t.above, t.value) == (6, False, 0.0)
@@ -103,7 +87,7 @@ def test_threshold_validates_its_arguments():
 
 
 def test_build_validates_summaries_before_the_device(no_device):
-    w = _two_body_world()
+    w = two_body_world()
     sys_ = el.six_dof()
     with pytest.raises(_lib.B200ValueError, match="nosuch.world_pos") as e:
         w.build(sys_, ensemble=True, thresholds=[el.Threshold("nosuch.world_pos", 6, below=0.0)])
@@ -160,37 +144,6 @@ def test_references_pick_the_earliest_tick_and_skip_non_finite_rows():
 # --------------------------------------------------------------------------- GPU
 
 
-def _gpu():
-    if el.device_count() < 1:
-        pytest.skip("needs a CUDA device")
-
-
-def _rocket_world(n_worlds, seed=4):
-    """The rocket + ball world of the ensemble statistics tests: a thrusting rocket at z = 1 and a ball at the origin,
-    both under gravity, per-world thrust, wind and mass."""
-    rng = np.random.default_rng(seed)
-    Thrust = el.Annotated[np.ndarray, el.Component("thrust", el.ComponentType.F64)]
-    Wind = el.Annotated[np.ndarray, el.Component("wind", el.ComponentType(el.PrimitiveType.F64, (3,)))]
-
-    @el.dataclass
-    class Rocket(el.Archetype):
-        thrust: Thrust
-        wind: Wind
-
-    w = el.World()
-    w.spawn([el.Body(world_pos=el.SpatialTransform(angular=el.Quaternion.from_euler([0.0, np.radians(70.0), 0.0]),
-                                                   linear=np.array([0.0, 0.0, 1.0])),
-                     inertia=el.SpatialInertia(3.0, np.array([0.1, 1.0, 1.0]))),
-             Rocket(np.array([88.426]), np.zeros(3))], name="rocket")
-    w.spawn(el.Body(world_vel=el.SpatialMotion(linear=[1.0, 2.0, 0.0])), name="ball")
-    effs = el.GravityConst((0.0, 0.0, -9.81)) | el.ThrustBody((-1.0, 0.0, 0.0), "thrust") | el.DragQuadratic(0.6125, 0.0025, "wind")
-    params = {"thrust": 88.426 * rng.uniform(0.8, 1.2, (n_worlds, 1, 1)),
-              "wind": np.concatenate([rng.normal(0, 2, (n_worlds, 1, 1)), np.zeros((n_worlds, 1, 2))], -1),
-              "inertia": np.tile(np.array([0.1, 1.0, 1.0, 0, 0, 0, 3.0]), (n_worlds, 2, 1))}
-    params["inertia"][:, 0, 6] = rng.uniform(2.5, 3.5, n_worlds)
-    return w, el.six_dof(sys=effs), params
-
-
 def _rows(ref, entities):
     """[R, M, N, 25] from a default-mode run's history."""
     return np.stack([np.concatenate([ref.history_worlds(f"{e}.{c}") for c in SAMPLED], -1) for e in entities], 2)
@@ -201,9 +154,9 @@ def _rows(ref, entities):
 def test_exec_summaries_against_the_default_mode(math_mode):
     """Extrema and threshold events of every ensemble route equal numpy on the default mode's history_worlds rows,
     bit for bit, and switching them on changes no ensemble row and no final state."""
-    _gpu()
+    need_gpu()
     M, ticks = 300, 23
-    w, sys_, params = _rocket_world(M)
+    w, sys_, params = rocket_world(M)
     kw = dict(simulation_rate=120.0, telemetry_rate=24.0, math=math_mode, n_worlds=M, world_params=params)
     ref = w.build(sys_, **kw)
     ref.run(ticks)
@@ -275,12 +228,6 @@ def _handle(M, N, math_mode, capacity, full=True, seed=0, state=None):
     return ex, (pos, vel, ine, cols, dt)
 
 
-def _state(ex):
-    from elodin_b200.executor import FORCE, WORLD_ACCEL, WORLD_POS, WORLD_VEL
-
-    return np.concatenate([ex.download(c) for c in (WORLD_POS, WORLD_VEL, WORLD_ACCEL, FORCE)], axis=-1)  # [M, N, 25]
-
-
 def _spec(N, rows):
     """Thresholds: two whose bound lies between rows 3 and 4 of one world (so that world fires mid-run), one at the
     median of row 0 (half the worlds fire at row 0), one that never fires and one that fires at row 0 everywhere."""
@@ -296,12 +243,12 @@ def _spec(N, rows):
 @pytest.mark.parametrize("math_mode", ["exact", "fast"])
 @pytest.mark.parametrize("shape", [(7, 3), ((1 << 16) + 3, 1), (100, 300)], ids=lambda s: f"{s[0]}x{s[1]}")
 def test_one_fold_equals_single_sample_folds_and_refolding_changes_nothing(shape, math_mode):
-    _gpu()
+    need_gpu()
     M, N = shape
     S = 7
     probe, state = _handle(M, N, math_mode, capacity=S)                 # the rows, for the bounds and the reference
     with probe:
-        row0 = _state(probe)
+        row0 = sampled_state(probe)
         probe.step(S)
         rows = np.concatenate([row0[None], probe.trajectory()])          # [S + 1, M, N, 25]
     spec = _spec(N, rows)
@@ -342,7 +289,7 @@ def test_one_fold_equals_single_sample_folds_and_refolding_changes_nothing(shape
 def test_non_finite_rows_are_reported_and_skipped(shape, math_mode):
     """Free bodies: a NaN / inf put into a world's position stays in its plane, so first_nonfinite_tick is 0 exactly
     there and -1 everywhere else, and min / max come from the finite rows alone."""
-    _gpu()
+    need_gpu()
     from tests.util import near_world
 
     M, N = shape
@@ -355,7 +302,7 @@ def test_non_finite_rows_are_reported_and_skipped(shape, math_mode):
                      trajectory_full=True) as ex:
         ex.set_state(pos, vel, ine)
         ex.summary_begin(True, [(0, 4, True, -1e300)])                   # every finite x fires at row 0
-        row0 = _state(ex)
+        row0 = sampled_state(ex)
         ex.summary_add_state()
         ex.step(S)
         traj = ex.trajectory()
@@ -376,7 +323,7 @@ def test_non_finite_rows_are_reported_and_skipped(shape, math_mode):
 
 @pytest.mark.gpu
 def test_refusals_leave_the_handle_usable():
-    _gpu()
+    need_gpu()
     L = _lib.lib()
     M, N = 9, 2
     thin, _ = _handle(M, N, "fast", capacity=2, full=False)

@@ -1,15 +1,11 @@
 """The N>1 host logic on CPU: 2 ranks over gloo (127.0.0.1), no GPU needed."""
 
-import os
-import socket
-
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 from elodin_b200.sharding import gather_worlds, shard_sizes, shard_worlds, total_entity_steps
+from tests.ensemble_util import run_gloo
 
 
 def test_shard_ranges_cover_exactly():
@@ -24,43 +20,21 @@ def test_shard_ranges_cover_exactly():
         shard_worlds(10, 2, 2)
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, ws, port, n_worlds, q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=ws)
+def _worker(rank, ws, n_worlds):
     w0, w1 = shard_worlds(n_worlds, rank, ws)
     # each rank "integrates" its own worlds: the global world id is recoverable from the data
     local = torch.arange(w0, w1, dtype=torch.float64).reshape(-1, 1, 1).repeat(1, 2, 13)
     full = gather_worlds(local, n_worlds)
     steps = total_entity_steps((w1 - w0) * 2 * 10)
-    q.put((rank, full.numpy(), steps))
-    dist.barrier()
-    dist.destroy_process_group()
+    return full.numpy(), steps
 
 
 @pytest.mark.parametrize("n_worlds", [11, 12])  # ragged (6 + 5) and equal shards (flat all-gather path)
 def test_two_rank_gather_and_counters(n_worlds):
     ws = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, ws, port, n_worlds, q)) for r in range(ws)]
-    for p in procs:
-        p.start()
-    got = [q.get(timeout=120) for _ in range(ws)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    got = run_gloo(_worker, ws, n_worlds)
     want = np.arange(n_worlds, dtype=np.float64).reshape(-1, 1, 1).repeat(2, 1).repeat(13, 2)
-    for rank, full, steps in got:
+    for rank, (full, steps) in enumerate(got):
         assert full.shape == (n_worlds, 2, 13)
         assert np.array_equal(full, want), rank  # global world order, no holes, no duplicates
         assert steps == n_worlds * 2 * 10
