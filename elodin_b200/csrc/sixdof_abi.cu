@@ -53,14 +53,7 @@ int cuda_fail(b200_sixdof *h, cudaError_t e, const char *what)
                 cudaGetErrorString(e));
 }
 
-int ensure_staging(b200_sixdof *h, uint64_t bytes)
-{
-    if (h->staging_bytes >= bytes) return B200_OK;
-    if (h->staging) { CU(h, cudaFree(h->staging)); h->staging = nullptr; h->staging_bytes = 0; }
-    CU(h, cudaMalloc(&h->staging, bytes));
-    h->staging_bytes = bytes;
-    return B200_OK;
-}
+int ensure_staging(b200_sixdof *h, uint64_t bytes) { return grow_device(h, &h->staging, &h->staging_bytes, bytes); }
 
 } // namespace b200
 
@@ -202,8 +195,9 @@ int build_graph(b200_sixdof *h, const b200_effector &e)
 
 namespace b200 {
 
-void fill_step_params(b200_sixdof *h, StepParams &P)
+StepParams range_step_params(b200_sixdof *h, uint64_t b0, uint64_t nb)
 {
+    StepParams P;
     std::memset(&P, 0, sizeof P);
     P.pos = h->find(B200_ID_WORLD_POS)->dev;
     P.vel = h->find(B200_ID_WORLD_VEL)->dev;
@@ -214,7 +208,7 @@ void fill_step_params(b200_sixdof *h, StepParams &P)
     P.has_edge = h->has_edge;
     P.aforce = h->aforce;
     P.ld = h->ld;
-    P.n_bodies = h->n_bodies;
+    P.n_bodies = nb;
     P.n_entities = (uint32_t)h->desc.n_entities;
     P.n_eff = (uint32_t)h->effectors.size();
     P.dt_stage = h->sim_time_step;
@@ -234,11 +228,42 @@ void fill_step_params(b200_sixdof *h, StepParams &P)
         P.eff[i].mask = i < h->eff_masks.size() ? h->eff_masks[i] : nullptr;
         P.eff[i].table = i < h->eff_tables.size() ? h->eff_tables[i] : nullptr;
     }
+    P.pos += b0; P.vel += b0; P.acc += b0; P.frc += b0; P.ine += b0;
+    if (P.gforce) P.gforce += b0;
+    if (P.aforce) P.aforce += b0;
+    if (P.traj) P.traj += b0;
+    for (uint32_t i = 0; i < P.n_eff; ++i) if (P.eff[i].col) P.eff[i].col += b0;
+    return P;
+}
+
+GraphParams graph_params(const b200_sixdof *h, const StepParams &P, uint64_t n_worlds)
+{
+    const b200_effector &e = h->effectors[h->graph_eff];
+    GraphParams G{};
+    G.pos = P.pos; G.vel = P.vel; G.ine = P.ine;
+    G.gforce = const_cast<double *>(P.gforce); // the planes the fold writes are the ones the body step then reads
+    G.ld = h->ld; G.n_entities = P.n_entities; G.n_worlds = (uint32_t)n_worlds;
+    G.dt_stage = P.dt_stage; G.kind = e.kind; G.integrator = h->desc.integrator;
+    G.p0 = e.p[0]; G.p1 = e.p[1]; G.row_ptr = h->row_ptr; G.col_idx = h->col_idx; G.max_deg = h->max_deg;
+    return G;
 }
 
 } // namespace b200
 
 namespace {
+
+// The EGM08 stage-force launch over the planes of P (one per tick, before the body launch that adds its forces).
+EgmParams egm_params(const b200_sixdof *h, const StepParams &P)
+{
+    const b200_effector &e = h->effectors[h->egm_eff];
+    EgmParams E{};
+    E.pos = P.pos; E.vel = P.vel; E.ine = P.ine;
+    E.aforce = const_cast<double *>(P.aforce); // written here, read by the body step
+    E.table = h->eff_tables[h->egm_eff]; E.mask = h->eff_masks[h->egm_eff];
+    E.ld = h->ld; E.n_bodies = P.n_bodies; E.n_entities = P.n_entities; E.ent0 = P.ent0;
+    E.L = (uint32_t)e.p[2]; E.integrator = h->desc.integrator; E.mu = e.p[0]; E.r_ref = e.p[1]; E.dt_stage = P.dt_stage;
+    return E;
+}
 
 // Integrate n_ticks ticks of the worlds [w0, w0+nw) on `stream`.  Worlds are independent, so a
 // world range can run to completion before the next one starts (used by the pipelined
@@ -248,15 +273,7 @@ int launch_ticks(b200_sixdof *h, uint64_t w0, uint64_t nw, uint64_t n_ticks, cud
     const uint64_t N = h->desc.n_entities;
     const uint64_t b0 = w0 * N, nb = nw * N;
     if (n_ticks == 0 || nb == 0) return B200_OK;
-    StepParams P;
-    fill_step_params(h, P);
-    // shift every per-body plane base to the range start; rows inside a world keep their index
-    P.pos += b0; P.vel += b0; P.acc += b0; P.frc += b0; P.ine += b0;
-    if (P.gforce) P.gforce += b0;
-    if (P.aforce) P.aforce += b0;
-    if (P.traj) P.traj += b0;
-    for (uint32_t i = 0; i < P.n_eff; ++i) if (P.eff[i].col) P.eff[i].col += b0;
-    P.n_bodies = nb;
+    StepParams P = range_step_params(h, b0, nb);
     // the summary's segments must be the launch's warps of pairs: only a range that starts on a segment boundary uses it
     P.mass_class = (!h->mass_class_off && b0 % 64 == 0) ? h->mass_class + b0 / 64 : nullptr;
     const bool exact = h->desc.math_mode == B200_MATH_EXACT;
@@ -268,22 +285,11 @@ int launch_ticks(b200_sixdof *h, uint64_t w0, uint64_t nw, uint64_t n_ticks, cud
     while (left) {
         const uint64_t n = std::min(left, fuse);
         if (egm) {
-            const b200_effector &ge = h->effectors[h->egm_eff];
-            EgmParams E{};
-            E.pos = P.pos; E.vel = P.vel; E.ine = P.ine; E.aforce = h->aforce + b0;
-            E.table = h->eff_tables[h->egm_eff]; E.mask = h->eff_masks[h->egm_eff];
-            E.ld = h->ld; E.n_bodies = nb; E.n_entities = P.n_entities; E.ent0 = 0;
-            E.L = (uint32_t)ge.p[2]; E.integrator = h->desc.integrator; E.mu = ge.p[0]; E.r_ref = ge.p[1]; E.dt_stage = P.dt_stage;
-            CU(h, launch_egm08_force(E, (int)h->desc.math_mode, stream));
+            CU(h, launch_egm08_force(egm_params(h, P), (int)h->desc.math_mode, stream));
             h->timings.kernel_launches++;
         }
         if (graph) {
-            const b200_effector &e = h->effectors[h->graph_eff];
-            GraphParams G{};
-            G.pos = P.pos; G.vel = P.vel; G.ine = P.ine; G.gforce = h->gforce + b0;
-            G.ld = h->ld; G.n_entities = P.n_entities; G.n_worlds = (uint32_t)nw;
-            G.dt_stage = P.dt_stage; G.kind = e.kind; G.integrator = h->desc.integrator;
-            G.p0 = e.p[0]; G.p1 = e.p[1]; G.row_ptr = h->row_ptr; G.col_idx = h->col_idx; G.max_deg = h->max_deg;
+            const GraphParams G = graph_params(h, P, nw); // of the planes live now: the fused route swaps them every tick
             if (h->small_world) {
                 // gravity through warp shuffles + integration, n ticks in one launch, state in registers
                 P.n_ticks = (uint32_t)n;
@@ -338,9 +344,7 @@ int do_step(b200_sixdof *h, uint64_t n_ticks)
     int rc = launch_ticks(h, 0, h->desc.n_worlds, n_ticks, h->stream);
     if (rc) return rc;
     commit_ping_pong(h, n_ticks);
-    h->ticks_done += n_ticks;
-    h->tick += n_ticks;
-    h->timings.ticks += n_ticks;
+    advance_ticks(h, n_ticks);
     return B200_OK;
 }
 
@@ -527,6 +531,10 @@ void b200_host_free(void *p)
     cudaFreeHost(p);
 }
 
+// Everything of b200_sixdof_create that needs the handle: the stream and events, the effectors' validation, every
+// device allocation.  On failure the caller destroys the handle, which frees whatever was allocated by then.
+static int init_handle(b200_sixdof *h, const b200_sixdof_desc *d);
+
 int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
 {
     if (!d || !out) return fail(B200_ERR_INVALID_ARGUMENT, "null descriptor / out pointer");
@@ -563,13 +571,18 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
     h->ld = round_up(std::max<uint64_t>(h->n_bodies, 1), 128); // whole 128-body tiles inside every plane
     h->sim_time_step = d->sim_time_step;
 
+    const int rc = init_handle(h, d);
+    if (rc) { b200_sixdof_destroy(h); return rc; }
+    *out = h;
+    return B200_OK;
+}
+
+static int init_handle(b200_sixdof *h, const b200_sixdof_desc *d)
+{
     int rc = B200_OK;
-    auto bail = [&](int code) { b200_sixdof_destroy(h); return code; };
-    if (cudaSetDevice(dev) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaSetDevice"));
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess)
-        return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaStreamCreate"));
-    for (auto &e : h->ev)
-        if (cudaEventCreate(&e) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaEventCreate"));
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    for (auto &e : h->ev) CU(h, cudaEventCreate(&e));
 
     // validate effectors
     int n_drag = 0, n_frame = 0;
@@ -586,65 +599,64 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
             want_w = 0;
             const double Ld = e.p[2];
             if (!(Ld >= 0.0) || Ld > 128.0 || Ld != std::floor(Ld))
-                return bail(fail(B200_ERR_INVALID_ARGUMENT, "effector %zu: EGM08 max_degree must be an integer in 0..128 (got %g)", i, Ld));
+                return fail(B200_ERR_INVALID_ARGUMENT, "effector %zu: EGM08 max_degree must be an integer in 0..128 (got %g)", i, Ld);
             const uint64_t n = (uint64_t)Ld + 1;
             if (!e.table0 || !e.table1 || e.table_len != n * n)
-                return bail(fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: EGM08 needs C and S tables of (L+1)^2 = %llu f64 (got %llu)", i,
-                                 (unsigned long long)(n * n), (unsigned long long)e.table_len));
-            if (h->egm_eff >= 0) return bail(fail(B200_ERR_UNSUPPORTED, "only one EGM08 gravity effector is supported"));
+                return fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: EGM08 needs C and S tables of (L+1)^2 = %llu f64 (got %llu)", i,
+                            (unsigned long long)(n * n), (unsigned long long)e.table_len);
+            if (h->egm_eff >= 0) return fail(B200_ERR_UNSUPPORTED, "only one EGM08 gravity effector is supported");
             h->egm_eff = (int)i;
             break;
         }
         case B200_EFF_TORQUE_BODY_FOLD:
             want_w = e.column_width; // 3 per wheel
             if (e.column_width == 0 || e.column_width % 3 != 0 || e.column_width > 24)
-                return bail(fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: a wheel-torque column holds 3 f64 per wheel, 1..8 wheels (got width %u)", i, e.column_width));
+                return fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: a wheel-torque column holds 3 f64 per wheel, 1..8 wheels (got width %u)", i, e.column_width);
             break;
         case B200_EFF_GRAVITY_EDGES_NEWTON: case B200_EFF_GRAVITY_EDGES_SOFTENED:
-            if (h->graph_eff >= 0) return bail(fail(B200_ERR_UNSUPPORTED, "only one edge_fold gravity effector is supported"));
-            if (e.n_edges && (!e.edge_from || !e.edge_to)) return bail(fail(B200_ERR_INVALID_ARGUMENT, "edge arrays are null"));
+            if (h->graph_eff >= 0) return fail(B200_ERR_UNSUPPORTED, "only one edge_fold gravity effector is supported");
+            if (e.n_edges && (!e.edge_from || !e.edge_to)) return fail(B200_ERR_INVALID_ARGUMENT, "edge arrays are null");
             // the fold's members are the sources of its edges: a mask would define a membership the reference lacks
             if (e.entity_mask)
-                return bail(fail(B200_ERR_UNSUPPORTED, "effector %zu: an edge_fold gravity effector takes no entity mask", i));
+                return fail(B200_ERR_UNSUPPORTED, "effector %zu: an edge_fold gravity effector takes no entity mask", i);
             if (d->math_mode == B200_MATH_FAST && i != 0)
-                return bail(fail(B200_ERR_UNSUPPORTED, "FAST math: the edge_fold gravity effector must come first (it overwrites Force)"));
+                return fail(B200_ERR_UNSUPPORTED, "FAST math: the edge_fold gravity effector must come first (it overwrites Force)");
             h->graph_eff = (int)i;
             break;
         default:
-            return bail(fail(B200_ERR_UNSUPPORTED, "effector kind %u is not built in (no CPU fallback, no JIT)", e.kind));
+            return fail(B200_ERR_UNSUPPORTED, "effector kind %u is not built in (no CPU fallback, no JIT)", e.kind);
         }
         if (e.kind == B200_EFF_GRAVITY_FRAME) ++n_frame;
         if (e.column_id) {
             if (e.column_width != want_w && !(e.kind == B200_EFF_DRAG_QUADRATIC && e.column_width == 5))
-                return bail(fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: column width %u, kind %u needs %u", i, e.column_width, e.kind, want_w));
+                return fail(B200_ERR_VALUE_SIZE_MISMATCH, "effector %zu: column width %u, kind %u needs %u", i, e.column_width, e.kind, want_w);
         } else if (e.kind == B200_EFF_THRUST_BODY || e.kind == B200_EFF_WRENCH_BODY || e.kind == B200_EFF_WRENCH_WORLD ||
                    e.kind == B200_EFF_TORQUE_BODY_FOLD) {
-            return bail(fail(B200_ERR_INVALID_ARGUMENT, "effector %zu (kind %u) needs an input column", i, e.kind));
+            return fail(B200_ERR_INVALID_ARGUMENT, "effector %zu (kind %u) needs an input column", i, e.kind);
         }
     }
     if (d->math_mode == B200_MATH_FAST && (n_drag > 1 || n_frame > 1))
-        return bail(fail(B200_ERR_UNSUPPORTED, "FAST math supports at most one drag and one frame effector"));
+        return fail(B200_ERR_UNSUPPORTED, "FAST math supports at most one drag and one frame effector");
 
     // columns
-    if ((rc = add_column(h, B200_ID_TICK, 1, true))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_SIMULATION_TIME_STEP, 1, true))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_WORLD_POS, 7, false))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_WORLD_VEL, 6, false))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_WORLD_ACCEL, 6, false))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_FORCE, 6, false))) return bail(rc);
-    if ((rc = add_column(h, B200_ID_INERTIA, 7, false))) return bail(rc);
+    if ((rc = add_column(h, B200_ID_TICK, 1, true))) return rc;
+    if ((rc = add_column(h, B200_ID_SIMULATION_TIME_STEP, 1, true))) return rc;
+    if ((rc = add_column(h, B200_ID_WORLD_POS, 7, false))) return rc;
+    if ((rc = add_column(h, B200_ID_WORLD_VEL, 6, false))) return rc;
+    if ((rc = add_column(h, B200_ID_WORLD_ACCEL, 6, false))) return rc;
+    if ((rc = add_column(h, B200_ID_FORCE, 6, false))) return rc;
+    if ((rc = add_column(h, B200_ID_INERTIA, 7, false))) return rc;
     for (auto &e : h->effectors)
         if (e.column_id) {
             const Column *c = h->find(e.column_id);
             if (c && c->width != e.column_width)
-                return bail(fail(B200_ERR_VALUE_SIZE_MISMATCH, "column 0x%016llx declared with two widths", (unsigned long long)e.column_id));
-            if ((rc = add_column(h, e.column_id, e.column_width, false))) return bail(rc);
+                return fail(B200_ERR_VALUE_SIZE_MISMATCH, "column 0x%016llx declared with two widths", (unsigned long long)e.column_id);
+            if ((rc = add_column(h, e.column_id, e.column_width, false))) return rc;
         }
     {
         const uint64_t bytes = (h->ld + 63) / 64;
-        if (cudaMalloc(&h->mass_class, bytes) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(mass classes)"));
-        if (cudaMemsetAsync(h->mass_class, 0, bytes, h->stream) != cudaSuccess)
-            return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMemset(mass classes)"));
+        CU(h, cudaMalloc(&h->mass_class, bytes));
+        CU(h, cudaMemsetAsync(h->mass_class, 0, bytes, h->stream));
     }
     build_id_tables(h);
     // per-effector entity masks: copy now, the caller's arrays are only valid for this call
@@ -652,10 +664,8 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
     for (size_t i = 0; i < h->effectors.size(); ++i) {
         b200_effector &e = h->effectors[i];
         if (e.entity_mask && d->n_entities) {
-            if (cudaMalloc(&h->eff_masks[i], d->n_entities) != cudaSuccess)
-                return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(entity mask)"));
-            if (cudaMemcpy(h->eff_masks[i], e.entity_mask, d->n_entities, cudaMemcpyHostToDevice) != cudaSuccess)
-                return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMemcpy(entity mask)"));
+            CU(h, cudaMalloc(&h->eff_masks[i], d->n_entities));
+            CU(h, cudaMemcpy(h->eff_masks[i], e.entity_mask, d->n_entities, cudaMemcpyHostToDevice));
         }
         e.entity_mask = nullptr;
     }
@@ -666,36 +676,29 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
         b200_effector &e = h->effectors[i];
         if (e.kind == B200_EFF_GRAVITY_EGM08) {
             const std::vector<double> t = egm08_tables((int)e.p[2], e.table0, e.table1);
-            if (cudaMalloc(&h->eff_tables[i], t.size() * sizeof(double)) != cudaSuccess)
-                return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(EGM08 tables)"));
-            if (cudaMemcpy(h->eff_tables[i], t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
-                return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMemcpy(EGM08 tables)"));
+            CU(h, cudaMalloc(&h->eff_tables[i], t.size() * sizeof(double)));
+            CU(h, cudaMemcpy(h->eff_tables[i], t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice));
         }
         e.table0 = e.table1 = nullptr;
     }
     if (h->graph_eff >= 0) {
         // copy the edge arrays' content now: the caller's pointers are only valid for this call
-        if ((rc = build_graph(h, h->effectors[h->graph_eff]))) return bail(rc);
-        {
-            GraphParams G{};
-            G.n_entities = (uint32_t)d->n_entities; G.n_worlds = (uint32_t)d->n_worlds; G.integrator = d->integrator;
-            // (an EGM08 effector needs its stage-force launch before every body launch: the generic two-launch route)
-            h->small_world = h->egm_eff < 0 && small_world_applicable(G, (int)d->math_mode);
-            h->nbody_fused = h->egm_eff < 0 && !h->small_world && h->pos_alt && nbody_fused_applicable(G, (int)d->math_mode, h->graph_dense);
-        }
+        if ((rc = build_graph(h, h->effectors[h->graph_eff]))) return rc;
+        const GraphParams G = graph_params(h, range_step_params(h, 0, h->n_bodies), d->n_worlds);
+        // (an EGM08 effector needs its stage-force launch before every body launch: the generic two-launch route)
+        h->small_world = h->egm_eff < 0 && small_world_applicable(G, (int)d->math_mode);
+        h->nbody_fused = h->egm_eff < 0 && !h->small_world && h->pos_alt && nbody_fused_applicable(G, (int)d->math_mode, h->graph_dense);
         h->effectors[h->graph_eff].edge_from = h->effectors[h->graph_eff].edge_to = nullptr;
     }
     if (h->egm_eff >= 0) {
-        if (cudaMalloc(&h->aforce, 9ull * h->ld * 8ull) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(EGM08 stage forces)"));
-        if (cudaMemset(h->aforce, 0, 9ull * h->ld * 8ull) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMemset(EGM08 stage forces)"));
+        CU(h, cudaMalloc(&h->aforce, 9ull * h->ld * 8ull));
+        CU(h, cudaMemset(h->aforce, 0, 9ull * h->ld * 8ull));
     }
     if (d->trajectory_every && d->trajectory_capacity) {
         h->traj_planes = (d->trajectory_flags & B200_TRAJ_FULL) ? 25u : 13u;
-        if (cudaMalloc(&h->traj, d->trajectory_capacity * (uint64_t)h->traj_planes * h->ld * 8ull) != cudaSuccess)
-            return bail(cuda_fail(nullptr, cudaGetLastError(), "cudaMalloc(trajectory)"));
+        CU(h, cudaMalloc(&h->traj, d->trajectory_capacity * (uint64_t)h->traj_planes * h->ld * 8ull));
     }
-    if (cudaStreamSynchronize(h->stream) != cudaSuccess) return bail(cuda_fail(nullptr, cudaGetLastError(), "create sync"));
-    *out = h;
+    CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
 }
 
@@ -803,86 +806,124 @@ static bool output_is_pass_through(uint64_t id)
            id != B200_ID_TICK && id != B200_ID_SIMULATION_TIME_STEP;
 }
 
+// What one b200_sixdof_invoke_batch call does with each caller column, decided once.  A NULL in_cols[i] means "not
+// dirty" (World::dirty_components, world.rs:43,249-252): the device-resident copy of that column stands.  A NULL
+// out_cols[j] means the caller does not read that column after this batch.
+struct BatchPlan {
+    enum Role {
+        ABSENT = 0,   // NULL buffer
+        GLOBAL,       // one of the two host-resident scalars
+        DEAD,         // an input the ticks never read (input_is_live): present, not uploaded
+        UPLOAD,       // an input that crosses PCIe
+        DOWNLOAD,     // an output that crosses PCIe
+        PASS_THROUGH  // an output the ticks never write (output_is_pass_through): filled from the input of the same column
+    };
+    struct Col {
+        Role role;
+        Column *col;
+        const uint8_t *src; // inputs: the caller's buffer.  PASS_THROUGH: the caller's input buffer of the same column, NULL =
+                            // that input is not dirty (the device column is the value: downloaded after the ticks)
+        uint8_t *dst;       // outputs: the caller's buffer
+        uint64_t offset;    // UPLOAD / DOWNLOAD: doubles from the start of the packed / staged block of its direction
+        bool device;        // non-global columns: the caller's buffer (PASS_THROUGH: either of the two) is device memory
+    };
+    // in input_ids / output_ids order; entries past the handle's columns stay ABSENT
+    Col in[B200_MAX_EFFECTORS + 7], out[B200_MAX_EFFECTORS + 7];
+    uint64_t in_total, out_total; // doubles of the UPLOAD / DOWNLOAD columns
+    bool device_buffers;          // some present non-global caller buffer is device memory
+};
+
+static BatchPlan plan_batch(b200_sixdof *h, const uint8_t *const *in_cols, uint8_t *const *out_cols)
+{
+    BatchPlan p{};
+    for (size_t i = 0; i < h->input_ids.size(); ++i) {
+        BatchPlan::Col &c = p.in[i];
+        c.col = h->find(h->input_ids[i]);
+        c.src = in_cols[i];
+        if (!c.src) continue;
+        if (c.col->global) { c.role = BatchPlan::GLOBAL; continue; }
+        c.device = is_device_pointer(c.src);
+        c.role = input_is_live(h, c.col->id) ? BatchPlan::UPLOAD : BatchPlan::DEAD;
+        if (c.role == BatchPlan::UPLOAD) { c.offset = p.in_total; p.in_total += h->n_bodies * c.col->width; }
+        p.device_buffers = p.device_buffers || c.device;
+    }
+    for (size_t i = 0; i < h->output_ids.size(); ++i) {
+        BatchPlan::Col &c = p.out[i];
+        c.col = h->find(h->output_ids[i]);
+        c.dst = out_cols[i];
+        if (!c.dst) continue;
+        if (c.col->global) { c.role = BatchPlan::GLOBAL; continue; }
+        c.device = is_device_pointer(c.dst);
+        p.device_buffers = p.device_buffers || c.device;
+        if (!output_is_pass_through(c.col->id)) {
+            c.role = BatchPlan::DOWNLOAD;
+            c.offset = p.out_total;
+            p.out_total += h->n_bodies * c.col->width;
+            continue;
+        }
+        c.role = BatchPlan::PASS_THROUGH;
+        for (const BatchPlan::Col &in : p.in)
+            if (in.col == c.col && in.src) { c.src = in.src; c.device = c.device || in.device; }
+    }
+    return p;
+}
+
 // Small batches (interactive single-vehicle sims: the reference's everyday case) are bound by the
 // number of driver calls, not by bytes: pack every live input column into one pinned block, ONE
 // host->device copy, ONE layout launch for all columns, the ticks, ONE layout launch, ONE copy back.
-static int invoke_small(b200_sixdof *h, const uint8_t *const *in_cols, uint8_t *const *out_cols, uint64_t n_ticks)
+static int invoke_small(b200_sixdof *h, const BatchPlan &plan, uint64_t n_ticks)
 {
     MultiColumns mi{}, mo{};
-    uint64_t in_total = 0, out_total = 0;
-    std::vector<std::pair<size_t, uint64_t>> in_map, out_map; // (column index, byte offset in the packed block)
-    for (size_t i = 0; i < h->input_ids.size(); ++i) {
-        Column *c = h->find(h->input_ids[i]);
-        if (!in_cols[i]) continue; // not dirty: the device-resident copy stands
-        if (c->global) { int rc = do_upload(h, c->id, in_cols[i], 8); if (rc) return rc; continue; }
-        if (!input_is_live(h, c->id)) continue;
-        if (c->id == B200_ID_INERTIA) { int rc = clear_mass_class(h, 0, h->n_bodies); if (rc) return rc; }
-        mi.col[mi.n++] = {in_total, c->dev, c->width, 0};
-        in_map.push_back({i, in_total * 8});
-        in_total += h->n_bodies * c->width;
+    int rc;
+    for (const BatchPlan::Col &c : plan.in) {
+        if (c.role == BatchPlan::GLOBAL && (rc = do_upload(h, c.col->id, c.src, 8))) return rc;
+        if (c.role != BatchPlan::UPLOAD) continue;
+        if (c.col->id == B200_ID_INERTIA && (rc = clear_mass_class(h, 0, h->n_bodies))) return rc;
+        mi.col[mi.n++] = {c.offset, c.col->dev, c.col->width, 0};
     }
-    for (size_t i = 0; i < h->output_ids.size(); ++i) {
-        Column *c = h->find(h->output_ids[i]);
-        if (!out_cols[i] || c->global || output_is_pass_through(c->id)) continue;
-        mo.col[mo.n++] = {out_total, c->dev, c->width, 0};
-        out_map.push_back({i, out_total * 8});
-        out_total += h->n_bodies * c->width;
-    }
-    const uint64_t need = std::max(in_total, out_total) * 8;
+    const uint64_t need = std::max(plan.in_total, plan.out_total) * 8;
     if (h->host_pack_bytes < need) {
         if (h->host_pack) cudaFreeHost(h->host_pack);
         h->host_pack = nullptr; h->host_pack_bytes = 0;
         CU(h, cudaHostAlloc((void **)&h->host_pack, std::max<uint64_t>(need, 4096), cudaHostAllocDefault));
         h->host_pack_bytes = std::max<uint64_t>(need, 4096);
     }
-    int rc = ensure_staging(h, std::max<uint64_t>(need, 8));
-    if (rc) return rc;
-    for (auto &m : in_map) {
-        const Column *c = h->find(h->input_ids[m.first]);
-        std::memcpy(h->host_pack + m.second, in_cols[m.first], h->n_bodies * c->width * 8);
-    }
+    if ((rc = ensure_staging(h, std::max<uint64_t>(need, 8)))) return rc;
+    for (const BatchPlan::Col &c : plan.in)
+        if (c.role == BatchPlan::UPLOAD) std::memcpy(h->host_pack + c.offset * 8, c.src, column_bytes(h, *c.col));
     mi.packed = mo.packed = h->staging;
-    if (in_total) {
-        CU(h, cudaMemcpyAsync(h->staging, h->host_pack, in_total * 8, cudaMemcpyHostToDevice, h->stream));
+    if (plan.in_total) {
+        CU(h, cudaMemcpyAsync(h->staging, h->host_pack, plan.in_total * 8, cudaMemcpyHostToDevice, h->stream));
         CU(h, launch_multi_transpose(mi, h->n_bodies, h->ld, true, h->stream));
         h->timings.kernel_launches++;
     }
-    rc = launch_ticks(h, 0, h->desc.n_worlds, n_ticks, h->stream);
-    if (rc) return rc;
+    if ((rc = launch_ticks(h, 0, h->desc.n_worlds, n_ticks, h->stream))) return rc;
     commit_ping_pong(h, n_ticks);
-    for (uint32_t k = 0; k < mo.n; ++k) mo.col[k].soa = h->find(h->output_ids[out_map[k].first])->dev; // after a ping-pong swap
-    h->ticks_done += n_ticks;
-    h->tick += n_ticks;
-    h->timings.ticks += n_ticks;
-    if (out_total) {
+    advance_ticks(h, n_ticks);
+    for (const BatchPlan::Col &c : plan.out) // after a ping-pong swap: the columns' planes are the live ones
+        if (c.role == BatchPlan::DOWNLOAD) mo.col[mo.n++] = {c.offset, c.col->dev, c.col->width, 0};
+    if (plan.out_total) {
         CU(h, launch_multi_transpose(mo, h->n_bodies, h->ld, false, h->stream));
         h->timings.kernel_launches++;
-        CU(h, cudaMemcpyAsync(h->host_pack, h->staging, out_total * 8, cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaMemcpyAsync(h->host_pack, h->staging, plan.out_total * 8, cudaMemcpyDeviceToHost, h->stream));
     }
     CU(h, cudaStreamSynchronize(h->stream));
-    for (auto &m : out_map) {
-        const Column *c = h->find(h->output_ids[m.first]);
-        std::memcpy(out_cols[m.first], h->host_pack + m.second, h->n_bodies * c->width * 8);
-    }
-    for (size_t i = 0; i < h->output_ids.size(); ++i) {
-        const Column *c = h->find(h->output_ids[i]);
-        if (!out_cols[i]) continue;
-        if (c->global) { rc = do_download(h, c->id, out_cols[i], 8); if (rc) return rc; continue; }
-        if (!output_is_pass_through(c->id)) continue;
-        bool filled = false;
-        for (size_t k = 0; k < h->input_ids.size(); ++k)
-            if (h->input_ids[k] == c->id && in_cols[k]) {
-                if (in_cols[k] != out_cols[i]) std::memcpy(out_cols[i], in_cols[k], h->n_bodies * c->width * 8);
-                filled = true;
-            }
-        if (!filled) { rc = do_download(h, c->id, out_cols[i], h->n_bodies * c->width * 8); if (rc) return rc; } // input was not dirty: the device copy is the value
+    for (const BatchPlan::Col &c : plan.out)
+        if (c.role == BatchPlan::DOWNLOAD) std::memcpy(c.dst, h->host_pack + c.offset * 8, column_bytes(h, *c.col));
+    for (const BatchPlan::Col &c : plan.out) {
+        if (c.role == BatchPlan::GLOBAL && (rc = do_download(h, c.col->id, c.dst, 8))) return rc;
+        if (c.role != BatchPlan::PASS_THROUGH) continue;
+        if (!c.src) { // input was not dirty: the device copy is the value
+            if ((rc = do_download(h, c.col->id, c.dst, column_bytes(h, *c.col)))) return rc;
+        } else if (c.src != c.dst) {
+            std::memcpy(c.dst, c.src, column_bytes(h, *c.col));
+        }
     }
     h->timings.h2d_upload_ms = h->timings.kernel_invoke_ms = h->timings.d2h_download_ms = 0.0; // not separable here
     return B200_OK;
 }
 
-static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8_t *const *out_cols, uint64_t n_ticks,
-                            uint64_t worlds_per_chunk)
+static int invoke_pipelined(b200_sixdof *h, const BatchPlan &plan, uint64_t n_ticks, uint64_t worlds_per_chunk)
 {
     const uint64_t N = h->desc.n_entities, M = h->desc.n_worlds;
     const uint64_t n_chunks = (M + worlds_per_chunk - 1) / worlds_per_chunk;
@@ -903,63 +944,30 @@ static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8
         h->chunk_in.push_back(a);
         h->chunk_out.push_back(b);
     }
-    // whole-batch AoS staging: column c of the inputs lives at in_off[c] (doubles)
-    std::vector<uint64_t> in_off(h->input_ids.size(), 0), out_off(h->output_ids.size(), 0);
-    uint64_t in_total = 0, out_total = 0;
-    for (size_t i = 0; i < h->input_ids.size(); ++i) {
-        const Column *c = h->find(h->input_ids[i]);
-        in_off[i] = in_total;
-        if (in_cols[i] && !c->global && input_is_live(h, c->id)) in_total += h->n_bodies * c->width;
-    }
-    for (size_t i = 0; i < h->output_ids.size(); ++i) {
-        const Column *c = h->find(h->output_ids[i]);
-        out_off[i] = out_total;
-        if (out_cols[i] && !c->global && !output_is_pass_through(c->id)) out_total += h->n_bodies * c->width;
-    }
-    // host-to-host fill of the pass-through outputs, split over a few worker threads
-    std::vector<size_t> late_downloads;
+    int rc;
+    // the pass-through outputs whose input is here: by the copy engine when either side is device memory, else
+    // host-to-host on a few worker threads, while the PCIe link carries the columns that did change
     std::vector<std::thread> fillers;
     struct Joiner { std::vector<std::thread> &v; ~Joiner() { for (auto &t : v) if (t.joinable()) t.join(); } } joiner{fillers};
-    for (size_t i = 0; i < h->output_ids.size(); ++i) {
-        const Column *c = h->find(h->output_ids[i]);
-        if (!out_cols[i] || c->global || !output_is_pass_through(c->id)) continue;
-        const uint8_t *src = nullptr;
-        for (size_t k = 0; k < h->input_ids.size(); ++k) if (h->input_ids[k] == c->id) src = in_cols[k];
-        if (!src) { late_downloads.push_back(i); continue; } // input not dirty: its value is the device-resident column
-        if (src == out_cols[i]) continue;
-        cudaPointerAttributes a_in{}, a_out{};
-        const bool dev_in = cudaPointerGetAttributes(&a_in, src) == cudaSuccess && a_in.type == cudaMemoryTypeDevice;
-        const bool dev_out = cudaPointerGetAttributes(&a_out, out_cols[i]) == cudaSuccess && a_out.type == cudaMemoryTypeDevice;
-        (void)cudaGetLastError();
-        const uint64_t bytes = h->n_bodies * c->width * 8ull;
-        if (dev_in || dev_out) { // device-resident caller buffers: let the copy engine do it
-            CU(h, cudaMemcpyAsync(out_cols[i], src, bytes, cudaMemcpyDefault, h->copy_out));
+    for (const BatchPlan::Col &c : plan.out) {
+        if (c.role != BatchPlan::PASS_THROUGH || !c.src || c.src == c.dst) continue;
+        const uint64_t bytes = column_bytes(h, *c.col);
+        if (c.device) {
+            CU(h, cudaMemcpyAsync(c.dst, c.src, bytes, cudaMemcpyDefault, h->copy_out));
             continue;
         }
         const unsigned parts = bytes >= (8u << 20) ? 4u : 1u;
         for (unsigned t = 0; t < parts; ++t) {
             const uint64_t o0 = bytes * t / parts, o1 = bytes * (t + 1) / parts;
-            uint8_t *dst = out_cols[i];
-            fillers.emplace_back([dst, src, o0, o1] { std::memcpy(dst + o0, src + o0, o1 - o0); });
+            fillers.emplace_back([dst = c.dst, src = c.src, o0, o1] { std::memcpy(dst + o0, src + o0, o1 - o0); });
         }
     }
-    if (h->stage_in_bytes < in_total * 8) {
-        if (h->stage_in) CU(h, cudaFree(h->stage_in));
-        h->stage_in = nullptr; h->stage_in_bytes = 0;
-        CU(h, cudaMalloc(&h->stage_in, std::max<uint64_t>(in_total * 8, 8)));
-        h->stage_in_bytes = in_total * 8;
-    }
-    if (h->stage_out_bytes < out_total * 8) {
-        if (h->stage_out) CU(h, cudaFree(h->stage_out));
-        h->stage_out = nullptr; h->stage_out_bytes = 0;
-        CU(h, cudaMalloc(&h->stage_out, std::max<uint64_t>(out_total * 8, 8)));
-        h->stage_out_bytes = out_total * 8;
-    }
+    // whole-batch AoS staging: an UPLOAD / DOWNLOAD column lives at its plan offset (doubles)
+    if ((rc = grow_device(h, &h->stage_in, &h->stage_in_bytes, plan.in_total * 8))) return rc;
+    if ((rc = grow_device(h, &h->stage_out, &h->stage_out_bytes, plan.out_total * 8))) return rc;
     // globals first (host-resident scalars)
-    for (size_t i = 0; i < h->input_ids.size(); ++i) {
-        const Column *c = h->find(h->input_ids[i]);
-        if (c->global && in_cols[i]) { int rc = do_upload(h, c->id, in_cols[i], 8); if (rc) return rc; }
-    }
+    for (const BatchPlan::Col &c : plan.in)
+        if (c.role == BatchPlan::GLOBAL && (rc = do_upload(h, c.col->id, c.src, 8))) return rc;
     // the copy streams must not run ahead of work already queued on the compute stream
     CU(h, cudaEventRecord(h->ev[2], h->stream));
     CU(h, cudaStreamWaitEvent(h->copy_in, h->ev[2], 0));
@@ -971,33 +979,30 @@ static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8
         const uint64_t w0 = k * worlds_per_chunk, nw = std::min(worlds_per_chunk, M - w0);
         const uint64_t b0 = w0 * N, nb = nw * N;
         // H2D of this world range, every live input column (copy engine 1)
-        for (size_t i = 0; i < h->input_ids.size(); ++i) {
-            const Column *c = h->find(h->input_ids[i]);
-            if (!in_cols[i] || c->global || !input_is_live(h, c->id)) continue;
-            CU(h, cudaMemcpyAsync(h->stage_in + in_off[i] + b0 * c->width, (const double *)in_cols[i] + b0 * c->width,
-                                  nb * c->width * 8, cudaMemcpyDefault, h->copy_in));
+        for (const BatchPlan::Col &c : plan.in) {
+            if (c.role != BatchPlan::UPLOAD) continue;
+            const uint32_t w = c.col->width;
+            CU(h, cudaMemcpyAsync(h->stage_in + c.offset + b0 * w, (const double *)c.src + b0 * w, nb * w * 8, cudaMemcpyDefault,
+                                  h->copy_in));
         }
         CU(h, cudaEventRecord(h->chunk_in[k], h->copy_in));
         if (k + 1 == n_chunks) CU(h, cudaEventRecord(h->ev[1], h->copy_in));
         // compute stream: AoS -> SoA, n ticks, SoA -> AoS
         CU(h, cudaStreamWaitEvent(h->stream, h->chunk_in[k], 0));
-        for (size_t i = 0; i < h->input_ids.size(); ++i) {
-            const Column *c = h->find(h->input_ids[i]);
-            if (!in_cols[i] || c->global || !input_is_live(h, c->id)) continue;
-            if (c->id == B200_ID_INERTIA) { int rc = clear_mass_class(h, b0, nb); if (rc) return rc; }
-            CU(h, launch_aos_to_soa(h->stage_in + in_off[i] + b0 * c->width, c->dev + b0, nb, c->width, h->ld, h->stream));
+        for (const BatchPlan::Col &c : plan.in) {
+            if (c.role != BatchPlan::UPLOAD) continue;
+            if (c.col->id == B200_ID_INERTIA && (rc = clear_mass_class(h, b0, nb))) return rc;
+            CU(h, launch_aos_to_soa(h->stage_in + c.offset + b0 * c.col->width, c.col->dev + b0, nb, c.col->width, h->ld, h->stream));
             h->timings.kernel_launches++;
         }
-        int rc = launch_ticks(h, w0, nw, n_ticks, h->stream);
-        if (rc) return rc;
+        if ((rc = launch_ticks(h, w0, nw, n_ticks, h->stream))) return rc;
         const bool flipped = h->nbody_fused && (n_ticks & 1); // live pose / velocity sit in the other plane set
-        for (size_t i = 0; i < h->output_ids.size(); ++i) {
-            const Column *c = h->find(h->output_ids[i]);
-            if (!out_cols[i] || c->global || output_is_pass_through(c->id)) continue;
-            const double *live = c->dev;
-            if (flipped && c->id == B200_ID_WORLD_POS) live = h->pos_alt;
-            if (flipped && c->id == B200_ID_WORLD_VEL) live = h->vel_alt;
-            CU(h, launch_soa_to_aos(live + b0, h->stage_out + out_off[i] + b0 * c->width, nb, c->width, h->ld, h->stream));
+        for (const BatchPlan::Col &c : plan.out) {
+            if (c.role != BatchPlan::DOWNLOAD) continue;
+            const double *live = c.col->dev;
+            if (flipped && c.col->id == B200_ID_WORLD_POS) live = h->pos_alt;
+            if (flipped && c.col->id == B200_ID_WORLD_VEL) live = h->vel_alt;
+            CU(h, launch_soa_to_aos(live + b0, h->stage_out + c.offset + b0 * c.col->width, nb, c.col->width, h->ld, h->stream));
             h->timings.kernel_launches++;
         }
         CU(h, cudaEventRecord(h->chunk_out[k], h->stream));
@@ -1005,11 +1010,11 @@ static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8
         // D2H of this world range (copy engine 2) overlaps the next range's H2D and ticks
         CU(h, cudaStreamWaitEvent(h->copy_out, h->chunk_out[k], 0));
         if (k == 0) CU(h, cudaEventRecord(h->ev[4], h->copy_out));
-        for (size_t i = 0; i < h->output_ids.size(); ++i) {
-            const Column *c = h->find(h->output_ids[i]);
-            if (!out_cols[i] || c->global || output_is_pass_through(c->id)) continue;
-            CU(h, cudaMemcpyAsync((double *)out_cols[i] + b0 * c->width, h->stage_out + out_off[i] + b0 * c->width,
-                                  nb * c->width * 8, cudaMemcpyDefault, h->copy_out));
+        for (const BatchPlan::Col &c : plan.out) {
+            if (c.role != BatchPlan::DOWNLOAD) continue;
+            const uint32_t w = c.col->width;
+            CU(h, cudaMemcpyAsync((double *)c.dst + b0 * w, h->stage_out + c.offset + b0 * w, nb * w * 8, cudaMemcpyDefault,
+                                  h->copy_out));
         }
         if (trace) {
             cudaEvent_t e;
@@ -1020,22 +1025,16 @@ static int invoke_pipelined(b200_sixdof *h, const uint8_t *const *in_cols, uint8
     }
     host_loop1 = host_ms();
     commit_ping_pong(h, n_ticks);
-    h->ticks_done += n_ticks;
-    h->tick += n_ticks;
-    h->timings.ticks += n_ticks;
-    for (size_t i = 0; i < h->output_ids.size(); ++i) {
-        const Column *c = h->find(h->output_ids[i]);
-        if (c->global && out_cols[i]) { int rc = do_download(h, c->id, out_cols[i], 8); if (rc) return rc; }
-    }
+    advance_ticks(h, n_ticks);
+    for (const BatchPlan::Col &c : plan.out)
+        if (c.role == BatchPlan::GLOBAL && (rc = do_download(h, c.col->id, c.dst, 8))) return rc;
     CU(h, cudaEventRecord(h->ev[5], h->copy_out));
     CU(h, cudaStreamSynchronize(h->copy_out));
     CU(h, cudaStreamSynchronize(h->stream));
     CU(h, cudaStreamSynchronize(h->copy_in));
-    for (size_t i : late_downloads) {
-        const Column *c = h->find(h->output_ids[i]);
-        int rc = do_download(h, c->id, out_cols[i], h->n_bodies * c->width * 8ull);
-        if (rc) return rc;
-    }
+    for (const BatchPlan::Col &c : plan.out) // input not dirty: its value is the device-resident column
+        if (c.role == BatchPlan::PASS_THROUGH && !c.src && (rc = do_download(h, c.col->id, c.dst, column_bytes(h, *c.col))))
+            return rc;
     if (trace) {
         fprintf(stderr, "[b200 pipe] host: enqueue loop %.3f..%.3f ms, synced at %.3f ms; device times from the first upload's start:\n",
                 host_loop0, host_loop1, host_ms());
@@ -1058,8 +1057,6 @@ int b200_sixdof_invoke_batch(b200_sixdof *h, const uint8_t *const *in_cols, uint
     if (!in_cols || !out_cols) return fail(B200_ERR_INVALID_ARGUMENT, "null column tables");
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     CU(h, cudaSetDevice(h->device));
-    // A NULL in_cols[i] means "not dirty" (World::dirty_components, world.rs:43,249-252): the device-resident copy of
-    // that column stands.  A NULL out_cols[j] means the caller does not read that column after this batch.
     n_ticks = std::max<uint64_t>(n_ticks, 1); // `n.max(1)`, cranelift_exec.rs:135
 
     // World ranges of ~kChunkBodies bodies: range k's PCIe download overlaps range k+1's upload
@@ -1072,23 +1069,11 @@ int b200_sixdof_invoke_batch(b200_sixdof *h, const uint8_t *const *in_cols, uint
     if (h->n_bodies == 0) wpc = std::max<uint64_t>(h->desc.n_worlds, 1);
 
     auto t0 = std::chrono::steady_clock::now();
-    // host pointers only on the small path (it packs with memcpy); device-resident callers use the pipeline
-    bool small = h->n_bodies > 0 && h->n_bodies * 32ull * 8ull <= (256ull << 10) && h->input_ids.size() <= 16 &&
-                 !h->desc.invoke_chunk_bodies;
-    if (small) { // the packed path memcpy()s: only for host-resident caller buffers
-        for (size_t i = 0; i < h->input_ids.size() && small; ++i) {
-            if (!in_cols[i] || h->find(h->input_ids[i])->global) continue;
-            cudaPointerAttributes at{};
-            if (cudaPointerGetAttributes(&at, in_cols[i]) == cudaSuccess && at.type == cudaMemoryTypeDevice) small = false;
-        }
-        for (size_t i = 0; i < h->output_ids.size() && small; ++i) {
-            if (!out_cols[i] || h->find(h->output_ids[i])->global) continue;
-            cudaPointerAttributes at{};
-            if (cudaPointerGetAttributes(&at, out_cols[i]) == cudaSuccess && at.type == cudaMemoryTypeDevice) small = false;
-        }
-        (void)cudaGetLastError();
-    }
-    int rc = small ? invoke_small(h, in_cols, out_cols, n_ticks) : invoke_pipelined(h, in_cols, out_cols, n_ticks, wpc);
+    const BatchPlan plan = plan_batch(h, in_cols, out_cols);
+    // the packed path memcpy()s: only for host-resident caller buffers; device-resident callers use the pipeline
+    const bool small = h->n_bodies > 0 && h->n_bodies * 32ull * 8ull <= (256ull << 10) && h->input_ids.size() <= 16 &&
+                       !h->desc.invoke_chunk_bodies && !plan.device_buffers;
+    int rc = small ? invoke_small(h, plan, n_ticks) : invoke_pipelined(h, plan, n_ticks, wpc);
     if (rc) {
         // copies into the caller's buffers may still be queued: they must not outlive this call
         (void)cudaStreamSynchronize(h->stream);
@@ -1150,10 +1135,8 @@ uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h) { return (h && h->tr
 // staging buffer.
 static bool device_destination(const b200_sixdof *h, const void *dst)
 {
-    cudaPointerAttributes a{};
-    const bool device = cudaPointerGetAttributes(&a, dst) == cudaSuccess && a.type == cudaMemoryTypeDevice && a.device == h->device;
-    (void)cudaGetLastError();
-    return device;
+    int device = -1;
+    return is_device_pointer(dst, &device) && device == h->device;
 }
 
 // A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu) into dst, `bytes` already
@@ -1460,13 +1443,8 @@ int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_thres
     h->sum_begun = false;
     if (extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 125ull * h->ld * 8ull));
     const uint64_t thr_bytes = h->desc.n_worlds * n_thresholds * 26ull * 8ull;
-    if (thr_bytes > h->sum_thr_bytes) {
-        if (h->sum_thr) CU(h, cudaFree(h->sum_thr));
-        h->sum_thr = nullptr;
-        h->sum_thr_bytes = 0;
-        CU(h, cudaMalloc(&h->sum_thr, thr_bytes));
-        h->sum_thr_bytes = thr_bytes;
-    }
+    const int rc = grow_device(h, &h->sum_thr, &h->sum_thr_bytes, thr_bytes);
+    if (rc) return rc;
     h->sum_extrema = extrema != 0;
     h->sum_thr_list.assign(t, t + n_thresholds);
     int launches = 0;

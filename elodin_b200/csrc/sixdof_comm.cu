@@ -285,23 +285,12 @@ int b200_sixdof_trajectory_allgather(b200_sixdof *h, b200_comm *c, const uint64_
     if (want == 0) return B200_OK;
     const uint64_t row = S * N * W; // doubles per world
     const uint64_t mine = h->desc.n_worlds * row;
-    if (c->send_bytes < mine * 8) {
-        if (c->send) CU(h, cudaFree(c->send));
-        c->send = nullptr; c->send_bytes = 0;
-        CU(h, cudaMalloc(&c->send, std::max<uint64_t>(mine * 8, 8)));
-        c->send_bytes = mine * 8;
-    }
-    cudaPointerAttributes at{};
-    const bool dst_dev = cudaPointerGetAttributes(&at, dst) == cudaSuccess && at.type == cudaMemoryTypeDevice;
-    (void)cudaGetLastError();
+    int rc = grow_device(h, &c->send, &c->send_bytes, mine * 8);
+    if (rc) return rc;
+    const bool dst_dev = is_device_pointer(dst);
     double *recv = (double *)dst;
     if (!dst_dev) {
-        if (c->recv_bytes < want) {
-            if (c->recv) CU(h, cudaFree(c->recv));
-            c->recv = nullptr; c->recv_bytes = 0;
-            CU(h, cudaMalloc(&c->recv, want));
-            c->recv_bytes = want;
-        }
+        if ((rc = grow_device(h, &c->recv, &c->recv_bytes, want))) return rc;
         recv = c->recv;
     }
     CU(h, cudaEventRecord(c->ev0, h->stream));
@@ -463,7 +452,6 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
     CU(h, cudaSetDevice(h->device));
     const uint64_t rows = N / R, i0 = rows * (uint64_t)c->rank;
     const bool exact = h->desc.math_mode == B200_MATH_EXACT;
-    const b200_effector &e = h->effectors[h->graph_eff];
     static const int peer_env = env_int("B200_ROW_PEER", 1);
     // (a window attached to another handle — or to a destroyed one whose address this handle reuses — is ignored)
     const bool peer = peer_env && c->win.owner == h && c->win.owner_serial == h->serial && c->win.ld == h->ld;
@@ -479,17 +467,17 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
         CU(h, cudaGetLastError());
         h->timings.kernel_launches++;
     }
+    // gravity folds over the whole world (every row is a target of this rank's source rows); the body kernel runs on
+    // this rank's rows only, which keep their entity numbering.  (The shift of aforce is a no-op: no EGM08 effector
+    // here, so it is NULL.)  No mass_class: a rank's rows need not start on a segment boundary.
+    GraphParams G = graph_params(h, range_step_params(h, 0, N), 1);
+    G.src0 = (uint32_t)i0; G.src_n = (uint32_t)rows;
+    StepParams P = range_step_params(h, i0, rows);
+    P.ent0 = (uint32_t)i0;
+    P.n_ticks = 1;
     for (uint64_t t = 0; t < n_ticks; ++t) {
         const bool last = t + 1 == n_ticks;
         const unsigned long long T = h->ticks_done + t;
-        StepParams P;
-        fill_step_params(h, P);
-        GraphParams G{};
-        G.pos = P.pos; G.vel = P.vel; G.ine = P.ine; G.gforce = h->gforce;
-        G.ld = h->ld; G.n_entities = (uint32_t)N; G.n_worlds = 1;
-        G.dt_stage = P.dt_stage; G.kind = e.kind; G.integrator = h->desc.integrator;
-        G.p0 = e.p[0]; G.p1 = e.p[1]; G.row_ptr = h->row_ptr; G.col_idx = h->col_idx; G.max_deg = h->max_deg;
-        G.src0 = (uint32_t)i0; G.src_n = (uint32_t)rows;
         if (peer) {
             // gravity reads every row's x, v from the window half of this tick count (the fold kernels touch planes
             // 4..6 of pos and 3..5 of vel only), once every rank's rows of that count have landed
@@ -502,14 +490,6 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
             }
         }
         CU(h, launch_graph_force(G, (int)h->desc.math_mode, true, h->stream));
-        // the body kernel on this rank's rows only: shift every per-body plane, keep the entity numbering
-        P.pos += i0; P.vel += i0; P.acc += i0; P.frc += i0; P.ine += i0;
-        if (P.gforce) P.gforce += i0;
-        if (P.traj) P.traj += i0;
-        for (uint32_t k = 0; k < P.n_eff; ++k) if (P.eff[k].col) P.eff[k].col += i0;
-        P.n_bodies = rows;
-        P.ent0 = (uint32_t)i0;
-        P.n_ticks = 1;
         P.tick0 = T;
         P.write_fa = (exact || last) ? 1u : 0u;
         CU(h, launch_body_step(P, (int)h->desc.integrator, (int)h->desc.math_mode, h->stream));
@@ -542,9 +522,7 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
         if (r != ncclSuccess) { nccl().GroupEnd(); return nccl_fail(r, "ncclAllGather(row slice)"); }
         NC(nccl().GroupEnd());
     }
-    h->ticks_done += n_ticks;
-    h->tick += n_ticks;
-    h->timings.ticks += n_ticks;
+    advance_ticks(h, n_ticks); // (no ping-pong commit: this route never runs the one-launch n-body tick)
     return B200_OK;
 }
 

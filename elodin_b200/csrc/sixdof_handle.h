@@ -102,12 +102,49 @@ namespace b200 {
 
 int cuda_fail(b200_sixdof *h, cudaError_t e, const char *what);
 int ensure_staging(b200_sixdof *h, uint64_t bytes);
-void fill_step_params(b200_sixdof *h, StepParams &P); // every plane base, constant and effector of the handle
+// Every plane base, constant and effector of the handle, as the body kernels see bodies [b0, b0 + nb): each per-body
+// plane base starts at body b0; rows inside a world keep their index.
+StepParams range_step_params(b200_sixdof *h, uint64_t b0, uint64_t nb);
+// The edge_fold gravity launch over the planes of P: the graph effector's kind and constants, the CSR arrays and the
+// integrator, for n_worlds worlds starting where P starts.
+GraphParams graph_params(const b200_sixdof *h, const StepParams &P, uint64_t n_worlds);
 
 #define CU(h, call)                                                        \
     do {                                                                   \
         cudaError_t e_ = (call);                                           \
         if (e_ != cudaSuccess) return b200::cuda_fail((h), e_, #call);     \
     } while (0)
+
+// Grow-only device buffer: *ptr holds at least need_bytes afterwards (its content is not kept).  need > have >= 0, so
+// nothing is ever allocated with 0 bytes.
+inline int grow_device(b200_sixdof *h, double **ptr, uint64_t *have_bytes, uint64_t need_bytes)
+{
+    if (*have_bytes >= need_bytes) return B200_OK;
+    if (*ptr) CU(h, cudaFree(*ptr));
+    *ptr = nullptr;
+    *have_bytes = 0;
+    CU(h, cudaMalloc(ptr, need_bytes));
+    *have_bytes = need_bytes;
+    return B200_OK;
+}
+
+// Is p device memory (of any GPU; *device receives which)?  Host pointers the runtime has never seen make the query
+// fail: that error is cleared here, not left for the next call to find.
+inline bool is_device_pointer(const void *p, int *device = nullptr)
+{
+    cudaPointerAttributes a{};
+    const bool dev = cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice;
+    (void)cudaGetLastError();
+    if (dev && device) *device = a.device;
+    return dev;
+}
+
+// n ticks happened: the trajectory slot base, the Tick column and the tick counter of the timings.
+inline void advance_ticks(b200_sixdof *h, uint64_t n)
+{
+    h->ticks_done += n;
+    h->tick += n;
+    h->timings.ticks += n;
+}
 
 } // namespace b200
