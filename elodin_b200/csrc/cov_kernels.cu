@@ -7,7 +7,7 @@
 // tile is every entity), marks the complete worlds, then thread (entity, tile) accumulates a 4 x 4 register tile of the
 // upper triangle of M over the chunk's complete worlds in world order.  Shift: K = the chunk's first complete world's
 // row, y = x - K, sums S_a = sum y_a (diagonal tiles) and Q_ab = sum y_a y_b (fma); the chunk's record is
-// mean_a = K_a + S_a / n, M_ab = Q_ab - S_a S_b / n.  Each entry is a sequential sum over the same worlds whatever the
+// mean_a = K_a + S_a / n, M_ab = Q_ab - lo (hi / n) with (lo, hi) = (min, max)(S_a, S_b), and M_aa = +inf where Q_aa overflowed.  Each entry is a sequential sum over the same worlds whatever the
 // selection, the entity tile or the other planes, so an entry has the same bits in any selection with the same complete
 // worlds.  With C > 1 a second launch merges the chunk records left to right with cov_merge, one thread per (group,
 // upper entry).  The partials live in scratch; groups run in slices that keep it under kScratchCap.  No atomics.
@@ -206,8 +206,12 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chu
                     const uint32_t b = 4 * bb + j;
                     if (b >= p || (diag && j < i)) continue;
                     const double sb = diag ? Ssum[j] : ss[b * Et + el];
-                    double m = Q[i * 4 + j] - sa * sb / dn;
-                    if (a == b) m = fmax(m, 0.0);
+                    // as Shifted::group in stats_kernels.cu: one sum divided before the product (so it does not
+                    // overflow where M is finite), the smaller first (so (a, b) and (b, a) get the same bits), and an
+                    // overflowed Q_aa means M_aa at the top of the range
+                    const double lo = fmin(sa, sb), hi = fmax(sa, sb);
+                    double m = Q[i * 4 + j] - lo * (hi / dn);
+                    if (a == b) m = Q[i * 4 + j] > DBL_MAX ? HUGE_VAL : fmax(m, 0.0);
                     if (!n) m = fin ? nan : 0.0;
                     o[1 + p + a * p + b] = m;
                     o[1 + p + b * p + a] = m;

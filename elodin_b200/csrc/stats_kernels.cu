@@ -77,7 +77,9 @@ struct Shifted {
         if (n) {
             const double dn = (double)n;
             g.mean = K + s1 / dn;
-            g.m2 = fmax(s2 - s1 * s1 / dn, 0.0);
+            // s2 = m2 + n (mean - K)^2 <= (2n + 1) m2 (K is one of the values), so an overflowed s2 means m2 is at the
+            // top of the range: +inf, never inf - inf = NaN clamped to 0.  s1 * (s1 / n) <= s2 does not overflow.
+            g.m2 = s2 > DBL_MAX ? HUGE_VAL : fmax(s2 - s1 * (s1 / dn), 0.0);
         }
         return g;
     }

@@ -280,7 +280,9 @@ int b200_sixdof_trajectory_reset(b200_sixdof *h);
  * one entity:  count  = worlds whose value is finite (a double, exact up to 2^53),
  *              mean, m2 = sum (x - mean)^2, min, max  over those finite values only  (std = sqrt(m2 / count));
  * a group with count = 0 holds NaN in the other four.  A non-finite world is therefore never averaged in: a diverged
- * run shows up as a missing count.  Partial groups are merged with Chan et al.'s pairwise update in a fixed order (no
+ * run shows up as a missing count.  Near the top of the f64 range: where m2 exceeds DBL_MAX (and every |x| <= 2^1000)
+ * m2 is +inf, never 0 or NaN; mean and m2 may be non-finite only where max|x| or m2 exceeds about 2^990; a finite
+ * result always keeps full accuracy.  Partial groups are merged with Chan et al.'s pairwise update in a fixed order (no
  * atomics): the same input gives the same bits on every call, and a sample's bits do not depend on how many other
  * samples are reduced with it.  Both device entries run on the handle's stream, return once dst is filled (like
  * b200_sixdof_trajectory_download), count their launches in timings.kernel_launches, and take host or device dst;
@@ -336,7 +338,9 @@ double b200_sixdof_quantile_reads(const b200_sixdof *h);
  *   mean[n_p]   over those worlds,
  *   M[n_p][n_p] the co-moments sum (x_a - mean_a)(x_b - mean_b), row-major, M[b][a] the same bits as M[a][b]
  *               (covariance = M / n, numpy's ddof = 0);
- * a group with n = 0 holds NaN after n.  Chunks of worlds are summed shifted by the chunk's first complete world and
+ * a group with n = 0 holds NaN after n.  Near the top of the f64 range, as for the statistics: M[a][a] beyond DBL_MAX
+ * (every |x_a| <= 2^1000) is +inf, never 0 or NaN; an entry (a, b) may be non-finite only where max|x_a|, max|x_b|,
+ * M[a][a] or M[b][b] exceeds about 2^990.  Chunks of worlds are summed shifted by the chunk's first complete world and
  * merged with Chan et al.'s update in a fixed order (no atomics); the chunking depends on (n_worlds, n_entities) alone,
  * so the same input gives the same bits on every call, a sample's bits do not depend on the ring, and an entry (a, b)
  * has the same bits in any selection that holds both planes and has the same complete worlds.  Device scratch (in the
