@@ -19,9 +19,9 @@ from . import _lib, effectors
 from ._lib import B200Error, B200ValueError, component_id
 from .effectors import (DragQuadratic, GravityConst, GravityEGM08, GravityEdges, GravityFrame, GravityJ2, Pipe, System, ThrustBody,
                         TorqueBodyFold, WrenchBody, WrenchWorld, all_pairs_edges)
-from .executor import B200Exec, device_count, merge_covariance, merge_stats, pinned_empty, pinned_free
-from .world import (Annotated, Archetype, Body, Component, ComponentType, Edge, EntityId, Exec, Force, HostSystem,
-                    Inertia, Integrator, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
+from .executor import B200Exec, device_count, merge_covariance, merge_histograms, merge_stats, pinned_empty, pinned_free
+from .world import (Annotated, Archetype, Body, Component, ComponentType, Edge, EntityId, Exec, Force, Histogram,
+                    HostSystem, Inertia, Integrator, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
                     SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, Threshold, World, WorldAccel,
                     WorldPos, WorldVel, dataclass, host_system, quantised_time_step, six_dof, ticks_per_telemetry)
 

@@ -64,12 +64,15 @@ SYMBOLS = [
     "b200_sixdof_extrema_download", "b200_sixdof_thresholds_download",
     "b200_sixdof_trajectory_quantiles", "b200_sixdof_state_quantiles", "b200_sixdof_quantile_reads",
     "b200_sixdof_trajectory_covariance", "b200_sixdof_state_covariance", "b200_covariance_merge",
+    "b200_sixdof_trajectory_histograms", "b200_sixdof_state_histograms",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
 MAX_THRESHOLDS = 8
 MAX_QUANTILES = 16  # levels per quantile call
 MAX_COV_PLANES = 25  # planes per covariance selection
+MAX_HISTOGRAMS = 8  # specs per histogram call
+MAX_HISTOGRAM_CELLS = 4096  # bins of one spec (na * nb for 2D)
 COMM_ID_BYTES = 128
 
 
@@ -129,6 +132,18 @@ class Threshold(C.Structure):
         ("plane", C.c_uint32),
         ("above", C.c_int32),
         ("value", C.c_double),
+    ]
+
+
+class Histogram(C.Structure):
+    _fields_ = [
+        ("entity", C.c_uint64),
+        ("n_axes", C.c_uint32),
+        ("plane", C.c_uint32 * 2),
+        ("bins", C.c_uint32 * 2),
+        ("reserved", C.c_uint32),
+        ("lo", C.c_double * 2),
+        ("hi", C.c_double * 2),
     ]
 
 
@@ -213,6 +228,8 @@ def lib():
     L.b200_sixdof_trajectory_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_state_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_covariance_merge.argtypes = [C.POINTER(C.c_double), u32, u64, u32, C.POINTER(C.c_double)]
+    L.b200_sixdof_trajectory_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_state_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1314,6 +1314,107 @@ int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_
     return run_covariance(h, state_planes, 25, planes, n_p, dst, bytes, "state");
 }
 
+// np.linspace(lo, hi, n + 1) into e[0 .. n]: i * step + lo, the product rounded before the sum (never an fma), e[n] = hi.
+// Refused (non-zero) where numpy's histogram rules would be ill-defined: lo or hi not finite, lo >= hi, hi - lo not
+// finite, step = 0, or edges that are not strictly increasing.
+static int linspace_edges(double lo, double hi, uint32_t n, double *e)
+{
+    if (!std::isfinite(lo) || !std::isfinite(hi) || !(lo < hi) || !std::isfinite(hi - lo)) return 1;
+    const double step = (hi - lo) / (double)n;
+    if (step == 0.0) return 1;
+    for (uint32_t i = 0; i < n; ++i) {
+        volatile double m = (double)i * step;
+        e[i] = m + lo;
+    }
+    e[n] = hi;
+    for (uint32_t i = 0; i < n; ++i)
+        if (!(e[i] < e[i + 1])) return 1;
+    return 0;
+}
+
+// Histograms of the specs over the worlds (hist_kernels.cu) into dst: the handle's status checked, then the specs (each
+// plane < width), then `bytes`.  The edges are computed here and copied to the device ahead of the launch.
+static int run_histograms(b200_sixdof *h, PlaneSource source, uint32_t width, const b200_histogram *specs, uint32_t n_specs,
+                          void *dst, uint64_t bytes, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    HistParams P{};
+    static_cast<StatsParams &>(P) = source(h);
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (n_specs == 0 || n_specs > B200_MAX_HISTOGRAMS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u histograms: 1 to %u", n_specs, B200_MAX_HISTOGRAMS);
+    if (!specs) return fail(B200_ERR_INVALID_ARGUMENT, "null histogram specs");
+    std::vector<double> edges;
+    for (uint32_t k = 0; k < n_specs; ++k) {
+        const b200_histogram &hs = specs[k];
+        HistParams::Spec &sp = P.spec[k];
+        if (hs.n_axes != 1 && hs.n_axes != 2)
+            return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: %u axes, 1 or 2", k, hs.n_axes);
+        if (hs.reserved != 0) return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: reserved field is not 0", k);
+        if (hs.entity >= P.n_entities)
+            return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: entity %llu of %llu", k, (unsigned long long)hs.entity,
+                        (unsigned long long)P.n_entities);
+        uint64_t cells = 1;
+        for (uint32_t a = 0; a < hs.n_axes; ++a) {
+            if (hs.plane[a] >= width)
+                return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: plane %u, the %s has %u planes", k, hs.plane[a], what, width);
+            if (hs.bins[a] == 0) return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: 0 bins", k);
+            cells *= hs.bins[a];
+        }
+        if (hs.n_axes == 2 && hs.plane[0] == hs.plane[1])
+            return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: plane %u twice", k, hs.plane[0]);
+        if (cells > B200_MAX_HISTOGRAM_CELLS)
+            return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: %llu cells, at most %u", k, (unsigned long long)cells,
+                        B200_MAX_HISTOGRAM_CELLS);
+        sp.entity = hs.entity;
+        sp.n_axes = hs.n_axes;
+        sp.rec_off = P.record_len;
+        sp.edge_off = edges.size();
+        uint32_t n_edges = 0;
+        for (uint32_t a = 0; a < hs.n_axes; ++a) {
+            sp.plane[a] = hs.plane[a];
+            sp.bins[a] = hs.bins[a];
+            sp.lo[a] = hs.lo[a];
+            sp.hi[a] = hs.hi[a];
+            edges.resize(edges.size() + hs.bins[a] + 1);
+            if (linspace_edges(hs.lo[a], hs.hi[a], hs.bins[a], edges.data() + edges.size() - (hs.bins[a] + 1)))
+                return fail(B200_ERR_INVALID_ARGUMENT,
+                            "histogram %u: range (%.17g, %.17g) in %u bins has no strictly increasing finite edges", k,
+                            hs.lo[a], hs.hi[a], hs.bins[a]);
+            n_edges += hs.bins[a] + 1;
+        }
+        sp.den = sp.hi[0] - sp.lo[0];
+        P.smem_edges = std::max(P.smem_edges, n_edges);
+        P.record_len += hs.n_axes == 2 ? 2 + cells : 3 + cells;
+    }
+    P.n_specs = n_specs;
+    const uint64_t n_s = P.planes_per_sample ? P.n_planes / P.planes_per_sample : 0;
+    const uint64_t want = n_s * P.record_len * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s histograms are %llu bytes, got %llu", what, (unsigned long long)want,
+                    (unsigned long long)bytes);
+    const uint64_t edge_bytes = edges.size() * 8ull;
+    return run_world_reduction(h, edge_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
+        cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes, cudaMemcpyHostToDevice, h->stream);
+        if (e != cudaSuccess) return e;
+        P.out = out;
+        P.edges = (const double *)scratch;
+        return launch_histograms(P, n, h->stream);
+    });
+}
+
+int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                      uint64_t bytes)
+{
+    return run_histograms(h, trajectory_planes, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes)
+{
+    return run_histograms(h, state_planes, 25, specs, n_specs, dst, bytes, "state");
+}
+
 // Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.
 int b200_covariance_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, uint32_t n_p, double *out)
 {

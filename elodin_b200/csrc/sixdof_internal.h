@@ -238,6 +238,34 @@ uint64_t cov_scratch_bytes(const CovParams &S);
 // one chunk launch, and a merge launch when the worlds take more than one chunk, per slice of groups (*launches)
 cudaError_t launch_covariance(const CovParams &S, void *scratch, int *launches, cudaStream_t s);
 
+// Ensemble histograms over the world axis (hist_kernels.cu): the samples of a StatsParams and n_specs specs, each one
+// entity and one or two planes of a sample.  Sample s, spec k goes to out[s * record_len + spec[k].rec_off ..]: a 1D
+// record [nonfinite, below, above, c_0 .. c_{n-1}] or a 2D one [nonfinite, outside, c_00 .. c_{na-1,nb-1}].  The edges
+// of axis a of spec k are edges[spec[k].edge_off + (a ? bins[0] + 1 : 0) ..] (device memory, np.linspace's values).
+struct HistParams : StatsParams {
+    struct Spec {
+        uint64_t entity;
+        uint32_t n_axes;
+        uint32_t plane[2];
+        uint32_t bins[2];
+        double lo[2], hi[2];
+        double den;        // hi[0] - lo[0]: the 1D rule's divisor
+        uint64_t rec_off;  // f64 from the start of a sample's row
+        uint64_t edge_off; // f64 from `edges`
+    } spec[B200_MAX_HISTOGRAMS];
+    uint32_t n_specs;
+    uint32_t smem_edges;   // the most edges one spec has (both axes)
+    uint64_t record_len;   // f64 per sample: every spec's record
+    const double *edges;
+};
+// worlds per chunk and chunks of a call over n_groups (sample, spec) pairs
+struct HistChunks {
+    uint64_t Wc, C;
+};
+HistChunks hist_chunks(uint64_t n_worlds, uint64_t n_groups);
+// zeroes out (a memset) and counts every (sample, spec) in one launch on s (*launches = 1; 0 with nothing to count)
+cudaError_t launch_histograms(const HistParams &P, int *launches, cudaStream_t s);
+
 // Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
 // row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.
 //   ext: extrema accumulators, plane p * 5 + f of ld doubles (f = min, max, min_tick, max_tick, first_nonfinite_tick),

@@ -309,6 +309,37 @@ class B200Exec:
         sel = self._selection(planes)
         return self._reduce("covariance", False, sel, self._planes(ring=False)[:-1] + (1 + sel[1] + sel[1] ** 2,))
 
+    # ---- ensemble histograms (bin counts over the world axis, on the device) ---------------------------------------
+    @staticmethod
+    def _hist_specs(specs) -> tuple:
+        """specs -> ((specs, n_specs) arguments of the histogram entries, f64 per row).  A spec is (entity row, planes,
+        bins, lo, hi): one number each for 1D (plane of the 25-plane sample layout), a pair each for 2D."""
+        specs = list(specs)
+        arr = (_lib.Histogram * max(len(specs), 1))()
+        row = 0
+        for k, (entity, planes, bins, lo, hi) in enumerate(specs):
+            planes, bins, lo, hi = (np.atleast_1d(np.asarray(v)).ravel() for v in (planes, bins, lo, hi))
+            h = arr[k]
+            h.entity, h.n_axes = int(entity), len(planes)
+            for a in range(min(len(planes), 2)):
+                h.plane[a], h.bins[a], h.lo[a], h.hi[a] = int(planes[a]), int(bins[a]), float(lo[a]), float(hi[a])
+            cells = int(np.prod([int(b) for b in bins[:2]]))
+            row += (2 if len(planes) == 2 else 3) + min(max(cells, 0), _lib.MAX_HISTOGRAM_CELLS)  # refused specs: C says why
+        return (arr, len(specs)), row
+
+    def trajectory_histograms(self, specs, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
+        """The ring's samples: [samples, sum of the record lengths] f64, each row the specs' records in spec order -- 1D
+        [nonfinite, below, above, counts[n]], 2D [nonfinite, outside, counts[na * nb]] (row-major), integer counts over
+        the worlds with numpy's histogram / histogram2d rules.  With `out_ptr` (a host or device pointer) the table is
+        written there and nothing is returned."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("histograms", True, args, (self.trajectory_len(), row), out_ptr)
+
+    def state_histograms(self, specs) -> np.ndarray:
+        """The current state: [sum of the record lengths] f64, records as trajectory_histograms()."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("histograms", False, args, (row,))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
@@ -402,6 +433,19 @@ def merge_covariance(tables: Sequence[np.ndarray]) -> np.ndarray:
     dp = C.POINTER(C.c_double)
     _lib.check(_lib.lib().b200_covariance_merge(stacked.ctypes.data_as(dp), len(stacked), out.size // rec, p(rec),
                                                  out.ctypes.data_as(dp)))
+    return out
+
+
+def merge_histograms(tables: Sequence[np.ndarray]) -> np.ndarray:
+    """Merge histogram tables of the same shape (e.g. one per rank of a world-sharded campaign, or per handle): their
+    elementwise sum, which is exactly the table of the union of their worlds.  Every value must be a count (a
+    non-negative integer) and every sum at most 2^53, where f64 counts stay exact."""
+    stacked = _stack(tables, "merge_histograms", "records", lambda rec: rec >= 3)
+    if not np.all((stacked >= 0) & (stacked == np.floor(stacked))):
+        raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "merge_histograms: a value is not a count")
+    out = stacked.sum(axis=0)
+    if np.any(out > 2.0 ** 53):
+        raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "merge_histograms: a count exceeds 2^53")
     return out
 
 

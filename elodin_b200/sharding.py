@@ -83,6 +83,16 @@ def gather_covariance(table, group=None) -> np.ndarray:
     return merge_covariance(_all_gather_tables(table, group))
 
 
+def gather_histograms(table, group=None) -> np.ndarray:
+    """Ensemble histograms of a world-sharded campaign: every rank passes the table of its own worlds (from
+    `B200Exec.trajectory_histograms` / `state_histograms`, numpy or torch, the same specs on every rank), the tables are
+    all-gathered and summed with `merge_histograms`.  The counts are integers, so every rank gets the same bits: exactly
+    the histogram of the union of the worlds."""
+    from .executor import merge_histograms
+
+    return merge_histograms(_all_gather_tables(table, group))
+
+
 def total_entity_steps(local_entity_steps: int, group=None) -> int:
     import torch
     import torch.distributed as dist

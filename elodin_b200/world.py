@@ -438,7 +438,7 @@ class World:
               world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
               thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
-              covariance: Optional[Sequence] = None) -> "Exec":
+              covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -447,7 +447,8 @@ class World:
         levels in [0, 1]) also records numpy's linear quantiles over the worlds for every row (`Exec.quantiles`), and
         `covariance` the covariance over the worlds of a selection of components for every row and entity
         (`Exec.covariance`): items are a component name ("world_pos": all its planes) or (component, indices), e.g.
-        covariance=[("world_pos", (4, 5, 6)), ("world_vel", (3, 4, 5))], at most 25 distinct planes."""
+        covariance=[("world_pos", (4, 5, 6)), ("world_vel", (3, 4, 5))], at most 25 distinct planes; `histograms` (1 to
+        8 `Histogram`s) the bin counts over the worlds of one or two components for every row (`Exec.histogram`)."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -455,7 +456,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -575,6 +576,18 @@ def _covariance_planes(spec):
     return planes, labels
 
 
+def _histogram_specs(histograms) -> List["Histogram"]:
+    """World.build(..., histograms=...): 1 to MAX_HISTOGRAMS el.Histogram objects."""
+    if isinstance(histograms, (str, bytes)) or not isinstance(histograms, Sequence):
+        raise TypeError(f"histograms take a sequence of el.Histogram objects, got {histograms!r}")
+    for h in histograms:
+        if not isinstance(h, Histogram):
+            raise TypeError(f"histograms take el.Histogram objects, got {h!r}")
+    if not 1 <= len(histograms) <= _lib.MAX_HISTOGRAMS:
+        raise ValueError(f"{len(histograms)} histograms: 1 to {_lib.MAX_HISTOGRAMS}")
+    return list(histograms)
+
+
 class Threshold:
     """A per-world event for `World.build(..., ensemble=True, thresholds=[...])`: the first telemetry row at which
     component `index` of `pair` ("<entity>.<component>": world_pos, world_vel, world_accel or force) is strictly
@@ -594,6 +607,69 @@ class Threshold:
 
     def __repr__(self) -> str:
         return f"Threshold({self.pair!r}, {self.index}, {'above' if self.above else 'below'}={self.value!r})"
+
+
+class Histogram:
+    """A per-row histogram for `World.build(..., ensemble=True, histograms=[...])`: for every telemetry row, the bin
+    counts over the worlds of component `index` of `pair` ("<entity>.<component>": world_pos, world_vel, world_accel or
+    force), as np.histogram(x, bins=bins, range=range) counts them, or of the components of a pair of indices, as
+    np.histogram2d(x, y, bins=bins, range=range) does -- over the finite values, with numpy's edges and rules, exactly.
+    `range` is (lo, hi) for 1D and ((lo_x, hi_x), (lo_y, hi_y)) for 2D; `bins` an int (every axis) or one per axis, at
+    most 4096 cells in all.  The edges (`edges`) must be finite and strictly increasing."""
+
+    def __init__(self, pair: str, index, range, bins=10):
+        where = f"Histogram({pair!r}, {index!r})"
+        self.entity, span = _sampled_span(pair, "histograms")
+        two = isinstance(index, (tuple, list))
+        if two and len(index) != 2:
+            raise ValueError(f"{where}: one index (1D) or a pair of indices (2D)")
+        idx = tuple(index) if two else (index,)
+        self.planes = tuple(_sampled_plane(span, i, where) for i in idx)  # in the 25-plane row layout
+        if two and self.planes[0] == self.planes[1]:
+            raise ValueError(f"{where}: the same component on both axes")
+        bins_t = tuple(bins) if isinstance(bins, (tuple, list)) else (bins,) * len(idx)
+        if len(bins_t) != len(idx) or any(isinstance(b, (bool, np.bool_)) or not isinstance(b, (int, np.integer)) or b < 1
+                                          for b in bins_t):
+            raise ValueError(f"{where}: bins {bins!r} is not a positive integer per axis")
+        self.bins = tuple(int(b) for b in bins_t)
+        cells = int(np.prod(self.bins))
+        if cells > _lib.MAX_HISTOGRAM_CELLS:
+            raise ValueError(f"{where}: {cells} cells, at most {_lib.MAX_HISTOGRAM_CELLS}")
+        ranges = tuple(range) if two and isinstance(range, (tuple, list)) else (range,)
+        if len(ranges) != len(idx) or not all(isinstance(r, (tuple, list)) and len(r) == 2 for r in ranges):
+            raise ValueError(f"{where}: range {range!r} is not " + ("((lo, hi), (lo, hi))" if two else "(lo, hi)"))
+        self.range, self._edges = [], []
+        for (lo, hi), n in zip(ranges, self.bins):
+            if not all(isinstance(v, (int, float, np.integer, np.floating)) and not isinstance(v, (bool, np.bool_))
+                       for v in (lo, hi)):
+                raise ValueError(f"{where}: range ({lo!r}, {hi!r}) is not two real numbers")
+            lo, hi = float(lo), float(hi)
+            # the edges numpy uses, checked as b200_sixdof_*_histograms checks them
+            ok = np.isfinite(lo) and np.isfinite(hi) and lo < hi and np.isfinite(hi - lo) and (hi - lo) / n != 0.0
+            e = np.linspace(lo, hi, n + 1) if ok else None
+            if not ok or not np.all(e[:-1] < e[1:]):
+                raise ValueError(f"{where}: range ({lo!r}, {hi!r}) in {n} bins has no finite, strictly increasing edges")
+            self.range.append((lo, hi))
+            self._edges.append(e)
+        self.range = tuple(self.range)
+        self.pair, self.index = pair, tuple(int(i) for i in idx) if two else int(index)
+        self.record_len = (2 if two else 3) + cells  # f64 of its record in a row of the table
+
+    @property
+    def edges(self):
+        """np.linspace(lo, hi, bins + 1) of the axis (1D), or of each axis (2D: a pair)."""
+        e = [a.copy() for a in self._edges]
+        return e[0] if len(e) == 1 else tuple(e)
+
+    def _spec(self, row: int) -> tuple:
+        """The B200Exec.trajectory_histograms spec of this histogram on the Body row `row`."""
+        lo, hi = zip(*self.range)
+        return (row, self.planes, self.bins, lo, hi)
+
+    def __repr__(self) -> str:
+        r = self.range[0] if len(self.range) == 1 else self.range
+        b = self.bins[0] if len(self.bins) == 1 else self.bins
+        return f"Histogram({self.pair!r}, {self.index!r}, range={r!r}, bins={b!r})"
 
 
 class _Row(np.ndarray):
@@ -617,7 +693,7 @@ class Exec:
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
                  thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
-                 covariance: Optional[Sequence] = None):
+                 covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -657,7 +733,8 @@ class Exec:
         self._extrema = bool(extrema)
         self._thresholds = list(thresholds or [])
         given = [name for name, on in (("extrema", self._extrema), ("thresholds", self._thresholds),
-                                       ("quantiles", quantiles is not None), ("covariance", covariance is not None)) if on]
+                                       ("quantiles", quantiles is not None), ("covariance", covariance is not None),
+                                       ("histograms", histograms is not None)) if on]
         if given and not ensemble:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{', '.join(given)}: need World.build(..., ensemble=True)")
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
@@ -681,6 +758,18 @@ class Exec:
         if covariance is not None:
             planes, self._cov_labels = _covariance_planes(covariance)
             self._ens_args["covariance"] = (planes,)
+        if histograms is not None:
+            self._histograms = _histogram_specs(histograms)
+            specs = []
+            for h in self._histograms:  # the entity resolved against the Body entities, as for thresholds
+                try:
+                    ent = world.entity_by_name(h.entity)
+                except _lib.B200ValueError:
+                    ent = None
+                if ent not in bodies:
+                    raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {h.pair}")
+                specs.append(h._spec(bodies.index(ent)))
+            self._ens_args["histograms"] = (specs,)
         self._ens_rows: Dict[str, List[np.ndarray]] = {kind: [] for kind in self._ens_args}
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
@@ -1074,6 +1163,26 @@ class Exec:
         with np.errstate(invalid="ignore", divide="ignore"):
             cov = t[:, 1 + p:].reshape(-1, p, p) / count[:, None, None]
         return {"count": count, "mean": np.ascontiguousarray(t[:, 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
+
+    def histogram(self, i: int) -> Dict[str, object]:
+        """`exec.histogram(i)` -> for histogram i of World.build(..., histograms=[...]) and every telemetry row (row 0 =
+        the initial state), int64 counts over the worlds: "counts" [rows, bins] (1D) or [rows, bins_x, bins_y] (2D,
+        np.histogram2d's layout), "nonfinite" [rows] (worlds whose value, or either value, is NaN / inf), 1D "below" and
+        "above" [rows] (finite values out of the range on each side), 2D "outside" [rows] (both finite, at least one out
+        of range), and "edges" (np.linspace's; a pair for 2D).  Every world is counted once per row."""
+        if "histograms" not in self._ens_rows:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "histogram(): build the Exec with World.build(..., ensemble=True, histograms=[...])")
+        if not 0 <= i < len(self._histograms):
+            raise IndexError(f"histogram {i}: this Exec has {len(self._histograms)}")
+        h = self._histograms[i]
+        off = sum(x.record_len for x in self._histograms[:i])
+        t = np.concatenate(self._ens_rows["histograms"])[:, off:off + h.record_len].astype(np.int64)
+        if len(h.bins) == 1:
+            return {"counts": np.ascontiguousarray(t[:, 3:]), "nonfinite": t[:, 0].copy(), "below": t[:, 1].copy(),
+                    "above": t[:, 2].copy(), "edges": h.edges}
+        return {"counts": np.ascontiguousarray(t[:, 2:]).reshape(-1, *h.bins), "nonfinite": t[:, 0].copy(),
+                "outside": t[:, 1].copy(), "edges": h.edges}
 
     def _ensemble_rows(self, kind: str, pair: str, what: str, method: str, option: str, per_plane: bool = True):
         """The recorded rows of table `kind` for the entity of `pair`, sliced to the planes of its component when the

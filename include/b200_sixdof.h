@@ -296,7 +296,8 @@ int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes);
 int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes);
 /* host-only: merge n_parts tables of n_groups stat groups each ([n_parts][n_groups][5]), left to right in part order,
  * into out[n_groups][5] — the cross-rank step of a world-sharded campaign (ranks exchange their tables over any channel;
- * every rank that merges the same tables in the same order gets the same bits).  Needs no GPU. */
+ * every rank that merges the same tables in the same order gets the same bits).  Needs no GPU.  Histogram tables
+ * (b200_sixdof_trajectory_histograms) need no merge entry: they are integer counts and merge by elementwise addition. */
 int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, double *out);
 
 /* ---- ensemble quantiles: per-row percentile envelopes over the worlds, on the device.  For one group (one sampled
@@ -358,6 +359,45 @@ int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_
  * part order, into out[n_groups][1 + n_p + n_p^2], with the update the kernels use (M[a][b] is read from a <= b).
  * A negative or NaN count is B200_ERR_INVALID_ARGUMENT.  Needs no GPU. */
 int b200_covariance_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, uint32_t n_p, double *out);
+
+/* ---- ensemble histograms: per-row bin counts over the worlds, on the device.  A spec is one entity row and one or two
+ * axes; an axis is a plane of the B200_TRAJ_FULL sample layout, a range lo < hi and n bins.  Its edges are
+ * np.linspace(lo, hi, n + 1)'s: step = (hi - lo) / n, edge_i = i * step + lo (multiply, then add), edge_n = hi.
+ * Only finite values are counted in bins, as in the statistics.
+ *   1D record, 3 + n f64:  nonfinite (worlds whose value is NaN / +-inf), below (x < lo), above (x > hi), then the
+ *     counts of np.histogram(x[np.isfinite(x)], bins=n, range=(lo, hi)), with numpy's own rule, operation for operation
+ *     (uncontracted, correctly rounded, in both math modes): keep lo <= x <= hi; f = ((x - lo) / (hi - lo)) * n;
+ *     i = trunc(f); i == n -> n - 1; then i - 1 if x < edge_i, and i + 1 if x >= edge_{i+1} and i != n - 1.
+ *   2D record, 2 + na * nb f64:  nonfinite (either value non-finite), outside (both finite, at least one out of range),
+ *     then the counts of np.histogram2d(x, y, bins=(na, nb), range=((lo_a, hi_a), (lo_b, hi_b))) over the worlds with
+ *     both values finite, row-major; per axis searchsorted(edges, v, side='right') - 1, with v == hi in the last bin.
+ * Every world is counted once: 1D nonfinite + below + above + sum(counts) = n_worlds, 2D nonfinite + outside +
+ * sum(counts) = n_worlds.  Counts are f64, exact below 2^53, and integer sums are exact in any order, so the table does
+ * not depend on the launch shape or the order of the device's atomics, and the tables of a world-sharded campaign merge
+ * by elementwise addition into exactly the table of the union of their worlds (there is no merge entry: add them).
+ * A row's records are the specs' records concatenated in spec order: the ring's dst = [trajectory_len][sum of the record
+ * lengths] f64 (an empty ring takes bytes = 0 and launches nothing), the state's dst = [sum of the record lengths].
+ * Both entries return B200_ERR_INVALID_ARGUMENT for a null handle, then the handle's sticky status if it has failed,
+ * then B200_ERR_INVALID_ARGUMENT for: null specs, n_specs of 0 or above B200_MAX_HISTOGRAMS, n_axes not 1 or 2, a
+ * reserved field that is not 0, entity >= n_entities, a plane >= the width (b200_sixdof_trajectory_width for the ring,
+ * 25 for the state), a 2D spec with the same plane twice, n = 0, more than B200_MAX_HISTOGRAM_CELLS cells (n for 1D,
+ * na * nb for 2D), lo or hi not finite, lo >= hi, hi - lo not finite, step = 0, or edges that are not strictly
+ * increasing (a range too narrow for its bins); then B200_ERR_VALUE_SIZE_MISMATCH unless `bytes` matches exactly.  They
+ * run on the handle's stream (one memset and one launch), return once dst (host or device) is filled and count their
+ * launches in timings.kernel_launches. ---- */
+#define B200_MAX_HISTOGRAMS 8u
+#define B200_MAX_HISTOGRAM_CELLS 4096u
+typedef struct b200_histogram {
+    uint64_t entity;     /* entity row within a world                                   */
+    uint32_t n_axes;     /* 1 or 2                                                      */
+    uint32_t plane[2];   /* B200_TRAJ_FULL layout; plane[1] unused for 1D               */
+    uint32_t bins[2];
+    uint32_t reserved;   /* must be 0                                                   */
+    double   lo[2], hi[2];
+} b200_histogram;
+int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                      uint64_t bytes);
+int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes);
 
 /* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
  * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the
