@@ -65,6 +65,8 @@ SYMBOLS = [
     "b200_sixdof_trajectory_quantiles", "b200_sixdof_state_quantiles", "b200_sixdof_quantile_reads",
     "b200_sixdof_trajectory_covariance", "b200_sixdof_state_covariance", "b200_covariance_merge",
     "b200_sixdof_trajectory_histograms", "b200_sixdof_state_histograms",
+    "b200_sixdof_set_world_groups", "b200_sixdof_world_groups", "b200_sixdof_trajectory_group_stats",
+    "b200_sixdof_state_group_stats", "b200_sixdof_trajectory_group_histograms", "b200_sixdof_state_group_histograms",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -73,6 +75,7 @@ MAX_QUANTILES = 16  # levels per quantile call
 MAX_COV_PLANES = 25  # planes per covariance selection
 MAX_HISTOGRAMS = 8  # specs per histogram call
 MAX_HISTOGRAM_CELLS = 4096  # bins of one spec (na * nb for 2D)
+MAX_WORLD_GROUPS = 1024  # groups of a grouped ensemble
 COMM_ID_BYTES = 128
 
 
@@ -230,6 +233,13 @@ def lib():
     L.b200_covariance_merge.argtypes = [C.POINTER(C.c_double), u32, u64, u32, C.POINTER(C.c_double)]
     L.b200_sixdof_trajectory_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_state_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_set_world_groups.argtypes = [vp, C.POINTER(u64), u32]
+    L.b200_sixdof_world_groups.argtypes = [vp]
+    L.b200_sixdof_world_groups.restype = u32
+    L.b200_sixdof_trajectory_group_stats.argtypes = [vp, vp, u64]
+    L.b200_sixdof_state_group_stats.argtypes = [vp, vp, u64]
+    L.b200_sixdof_trajectory_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_state_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1,15 +1,19 @@
-// Ensemble histograms over the world axis: for every (sample, spec) one record of integer counts over the worlds
-// (include/b200_sixdof.h b200_sixdof_trajectory_histograms / _state_histograms).
+// Ensemble histograms over the world axis: for every (sample, world group, spec) one record of integer counts over the
+// group's worlds (include/b200_sixdof.h b200_sixdof_trajectory_histograms / _state_histograms, and the
+// _group_histograms entries).  A world group is a contiguous world range; the ungrouped entries are the one-group case
+// [0, n_worlds) of the same code.
 //
 // A value's cell is a pure function of the value and the spec's edges (numpy's own rules, below), so the table is a set
 // of integer counts, and integer-valued f64 sums below 2^53 are exact in any order: the result does not depend on the
-// launch shape or on the order of the atomics.  Shape of the reduction: the table is zeroed with one memset, then one
-// launch; block task = (chunk of worlds, sample, spec).  A block clears its spec's record (<= 4099 u32 cells) and copies
-// its edges (<= 4099 f64) into shared memory, walks the chunk with consecutive lanes on consecutive worlds (four loads in
-// flight per thread), classifies each value, and adds one per world to its cell.  Lanes of a warp that hit the same
-// cell are counted together (__match_any_sync) before one shared atomic, so a warp whose 32 worlds share a bin (early
-// rows of a campaign) costs one atomic, not 32 serialised ones.  The block then adds its non-zero cells to the f64
-// table with atomicAdd.  No scratch beyond the edges, no merge pass.
+// launch shape or on the order of the atomics, and a group's record is the ungrouped table of a batch of its worlds.
+// Shape of the reduction: the table is zeroed with one memset, then one launch; block task = (chunk of worlds of one
+// group, sample, spec).  The chunks of all groups are numbered through the group table (WorldGroup::k0) and a block
+// finds its group by binary search.  A block clears its spec's record (<= 4099 u32 cells) and copies its edges (<= 4099
+// f64) into shared memory, walks the chunk with consecutive lanes on consecutive worlds (four loads in flight per
+// thread), classifies each value, and adds one per world to its cell.  Lanes of a warp that hit the same cell are
+// counted together (__match_any_sync) before one shared atomic, so a warp whose 32 worlds share a bin (early rows of a
+// campaign) costs one atomic, not 32 serialised ones.  The block then adds its non-zero cells to its group's record of
+// the f64 table with atomicAdd.  No scratch beyond the edges and the group table, no merge pass.
 #include <algorithm>
 #include <cfloat>
 
@@ -81,16 +85,19 @@ __device__ __forceinline__ void count(uint32_t *cells, uint32_t c)
     if (c != kNone && (threadIdx.x & 31) == (unsigned)(__ffs(same) - 1)) atomicAdd(&cells[c], (unsigned)__popc(same));
 }
 
-__global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, HistChunks ck, uint64_t n_samples)
+__global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, const WorldGroup *groups, uint64_t G, uint64_t Q,
+                                                        uint64_t n_samples)
 {
     extern __shared__ double smem[];
     double *edges = smem;                                   // [P.smem_edges]
     uint32_t *cells = (uint32_t *)(smem + P.smem_edges);   // [record length]
     const uint64_t E = P.n_entities;
-    const uint64_t n_tasks = ck.C * n_samples * P.n_specs;
+    const uint64_t n_tasks = Q * n_samples * P.n_specs;  // Q = the chunks of all groups
     for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
-        const uint64_t c = task % ck.C, s = (task / ck.C) % n_samples;
-        const HistParams::Spec sp = spec_of(P, (uint32_t)(task / (ck.C * n_samples)));
+        const uint64_t k = task % Q, s = (task / Q) % n_samples;
+        const HistParams::Spec sp = spec_of(P, (uint32_t)(task / (Q * n_samples)));
+        const uint64_t g = group_of_chunk(groups, 0, G, k);
+        const WorldGroup wg = groups[g];
         const bool two = sp.n_axes == 2;
         const uint32_t R = two ? 2 + sp.bins[0] * sp.bins[1] : 3 + sp.bins[0];
         const uint32_t ne = sp.bins[0] + 1 + (two ? sp.bins[1] + 1 : 0);
@@ -102,7 +109,7 @@ __global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, HistChunks
         const double *xa = stats_plane(P, s * P.planes_per_sample + sp.plane[0]) + sp.entity;
         const double *xb = two ? stats_plane(P, s * P.planes_per_sample + sp.plane[1]) + sp.entity : xa;
         const ex::Rcp r = ex::rcp_prep(sp.den);
-        const uint64_t w0 = c * ck.Wc, w1 = min(w0 + ck.Wc, P.n_worlds);
+        const uint64_t w0 = wg.o + (k - wg.k0) * wg.Wc, w1 = min(w0 + wg.Wc, wg.o + wg.n);
         for (uint64_t base = w0; base < w1; base += (uint64_t)kUnroll * blockDim.x) { // uniform trip count per warp
             double va[kUnroll], vb[kUnroll];
 #pragma unroll
@@ -120,7 +127,7 @@ __global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, HistChunks
             }
         }
         __syncthreads();
-        double *o = P.out + s * P.record_len + sp.rec_off;
+        double *o = P.out + (s * G + g) * P.record_len + sp.rec_off;
         for (uint32_t i = threadIdx.x; i < R; i += blockDim.x)
             if (cells[i]) atomicAdd(o + i, (double)cells[i]);
     }
@@ -128,32 +135,48 @@ __global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, HistChunks
 
 } // namespace
 
-HistChunks hist_chunks(uint64_t n_worlds, uint64_t n_groups)
+std::vector<WorldGroup> hist_group_table(const uint64_t *sizes, uint64_t n_groups, uint64_t n_pairs)
 {
-    const uint64_t want = std::max<uint64_t>(1, (kChunkTasks + n_groups - 1) / std::max<uint64_t>(n_groups, 1));
-    const uint64_t C = std::max<uint64_t>(1, std::min(want, n_worlds / kMinWorlds));
-    HistChunks ck;
-    ck.Wc = (n_worlds + C - 1) / C;
-    ck.C = (n_worlds + ck.Wc - 1) / ck.Wc;
-    return ck;
+    uint64_t n_worlds = 0;
+    for (uint64_t g = 0; g < n_groups; ++g) n_worlds += sizes[g];
+    std::vector<WorldGroup> t(n_groups);
+    uint64_t o = 0, k0 = 0;
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        const uint64_t n = sizes[g];
+        uint64_t C = 0, Wc = 0;
+        if (n) {  // the group's share of kChunkTasks over the call's pairs, rounded up: ceil(kChunkTasks / n_pairs) for one group
+            const uint64_t pairs = std::max<uint64_t>(n_pairs, 1);
+            const uint64_t want = std::max<uint64_t>(1, (kChunkTasks * n + n_worlds * pairs - 1) / (n_worlds * pairs));
+            C = std::max<uint64_t>(1, std::min(want, n / kMinWorlds));
+            Wc = (n + C - 1) / C;
+            C = (n + Wc - 1) / Wc;
+        }
+        t[g] = {o, n, Wc, C, k0};
+        o += n;
+        k0 += C;
+    }
+    return t;
 }
 
-cudaError_t launch_histograms(const HistParams &P, int *launches, cudaStream_t s)
+cudaError_t launch_histograms(const HistParams &P, const WorldGroup *groups, const std::vector<WorldGroup> &table,
+                              int *launches, cudaStream_t s)
 {
     *launches = 0;
     const uint64_t n_s = P.planes_per_sample ? P.n_planes / P.planes_per_sample : 0;
-    if (n_s == 0 || P.n_worlds == 0 || P.n_entities == 0) return cudaSuccess;
-    cudaError_t e = cudaMemsetAsync(P.out, 0, n_s * P.record_len * 8ull, s);
+    const uint64_t G = table.size();
+    if (n_s == 0 || G == 0 || P.n_entities == 0) return cudaSuccess;
+    cudaError_t e = cudaMemsetAsync(P.out, 0, n_s * G * P.record_len * 8ull, s);
     if (e != cudaSuccess) return e;
+    const uint64_t Q = table.back().k0 + table.back().C;
+    if (Q == 0) return cudaSuccess;  // no worlds: the zeroed table
     uint32_t R = 0;
     for (uint32_t k = 0; k < P.n_specs; ++k)
         R = std::max(R, P.spec[k].n_axes == 2 ? 2 + P.spec[k].bins[0] * P.spec[k].bins[1] : 3 + P.spec[k].bins[0]);
     const size_t smem = P.smem_edges * 8ull + R * 4ull;
     e = cudaFuncSetAttribute(hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    const HistChunks ck = hist_chunks(P.n_worlds, n_s * P.n_specs);
-    const uint64_t tasks = ck.C * n_s * P.n_specs;
-    hist_kernel<<<(unsigned)std::min<uint64_t>(tasks, 64ull * kNumSMs * 8), kThreads, smem, s>>>(P, ck, n_s);
+    const uint64_t tasks = Q * n_s * P.n_specs;
+    hist_kernel<<<(unsigned)std::min<uint64_t>(tasks, 64ull * kNumSMs * 8), kThreads, smem, s>>>(P, groups, G, Q, n_s);
     *launches = 1;
     return cudaGetLastError();
 }

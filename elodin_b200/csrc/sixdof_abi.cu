@@ -535,6 +535,8 @@ void b200_host_free(void *p)
 // device allocation.  On failure the caller destroys the handle, which frees whatever was allocated by then.
 static int init_handle(b200_sixdof *h, const b200_sixdof_desc *d);
 
+static int upload_group_table(b200_sixdof *h, const std::vector<WorldGroup> &t, WorldGroup **dev);
+
 int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
 {
     if (!d || !out) return fail(B200_ERR_INVALID_ARGUMENT, "null descriptor / out pointer");
@@ -571,7 +573,11 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
     h->ld = round_up(std::max<uint64_t>(h->n_bodies, 1), 128); // whole 128-body tiles inside every plane
     h->sim_time_step = d->sim_time_step;
 
-    const int rc = init_handle(h, d);
+    int rc = init_handle(h, d);
+    if (!rc) {  // the ungrouped statistics' one-group table {n_worlds}, on the device for the handle's life
+        h->all_table = world_group_table(&h->desc.n_worlds, 1, h->desc.n_entities);
+        rc = upload_group_table(h, h->all_table, &h->all_table_dev);
+    }
     if (rc) { b200_sixdof_destroy(h); return rc; }
     *out = h;
     return B200_OK;
@@ -725,6 +731,8 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->traj) cudaFree(h->traj);
     if (h->sum_ext) cudaFree(h->sum_ext);
     if (h->sum_thr) cudaFree(h->sum_thr);
+    if (h->all_table_dev) cudaFree(h->all_table_dev);
+    if (h->group_table_dev) cudaFree(h->group_table_dev);
     for (auto &e : h->chunk_in) if (e) cudaEventDestroy(e);
     for (auto &e : h->chunk_out) if (e) cudaEventDestroy(e);
     if (h->host_pack) cudaFreeHost(h->host_pack);
@@ -1201,30 +1209,94 @@ static StatsParams state_planes(const b200_sixdof *h)
 // The reduction entries below run over one of these; `what` names it in error messages.
 using PlaneSource = StatsParams (*)(const b200_sixdof *);
 
-// Statistics of the planes over the worlds (stats_kernels.cu) into dst: `bytes` checked, then the handle's status.
-static int run_world_stats(b200_sixdof *h, PlaneSource source, void *dst, uint64_t bytes, const char *what)
+// A statistics group table into device memory (*dev, replaced): the stream is drained first, so that no reduction still
+// in flight reads the table it replaces.
+static int upload_group_table(b200_sixdof *h, const std::vector<WorldGroup> &t, WorldGroup **dev)
+{
+    CU(h, cudaStreamSynchronize(h->stream));
+    if (*dev) CU(h, cudaFree(*dev));
+    *dev = nullptr;
+    if (t.empty()) return B200_OK;
+    CU(h, cudaMalloc(dev, t.size() * sizeof(WorldGroup)));
+    CU(h, cudaMemcpy(*dev, t.data(), t.size() * sizeof(WorldGroup), cudaMemcpyHostToDevice));
+    return B200_OK;
+}
+
+int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (n_groups > B200_MAX_WORLD_GROUPS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u world groups: at most %u", n_groups, B200_MAX_WORLD_GROUPS);
+    if (n_groups && !sizes) return fail(B200_ERR_INVALID_ARGUMENT, "null world group sizes");
+    uint64_t sum = 0;
+    for (uint32_t g = 0; g < n_groups; ++g) {
+        if (sizes[g] > h->desc.n_worlds - sum)
+            return fail(B200_ERR_INVALID_ARGUMENT, "world group sizes exceed the %llu worlds at group %u",
+                        (unsigned long long)h->desc.n_worlds, g);
+        sum += sizes[g];
+    }
+    if (n_groups && sum != h->desc.n_worlds)
+        return fail(B200_ERR_INVALID_ARGUMENT, "world group sizes sum to %llu, not to the %llu worlds", (unsigned long long)sum,
+                    (unsigned long long)h->desc.n_worlds);
+    CU(h, cudaSetDevice(h->device));
+    h->group_sizes.assign(sizes, sizes + n_groups);
+    h->group_table = world_group_table(sizes, n_groups, h->desc.n_entities);
+    return upload_group_table(h, h->group_table, &h->group_table_dev);
+}
+
+uint32_t b200_sixdof_world_groups(const b200_sixdof *h) { return h ? (uint32_t)h->group_sizes.size() : 0; }
+
+// The world sizes a reduction runs over: the groups set (grouped), else all worlds as one group.
+static std::vector<uint64_t> reduction_groups(const b200_sixdof *h, bool grouped)
+{
+    return grouped ? h->group_sizes : std::vector<uint64_t>{h->desc.n_worlds};
+}
+
+static int no_groups(const char *what)
+{
+    return fail(B200_ERR_INVALID_ARGUMENT, "grouped %s: call b200_sixdof_set_world_groups first", what);
+}
+
+// Statistics of the planes over the worlds, per group when `grouped` (stats_kernels.cu), into dst: the groups checked,
+// then `bytes`, then the handle's status.
+static int run_world_stats(b200_sixdof *h, PlaneSource source, bool grouped, void *dst, uint64_t bytes, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     StatsParams S = source(h);
-    const uint64_t want = S.n_planes * S.n_entities * 5ull * 8ull;
+    const uint64_t G = grouped ? h->group_sizes.size() : 1;
+    const uint64_t want = S.n_planes * G * S.n_entities * 5ull * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s statistics are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    return run_world_reduction(h, world_stats_scratch_doubles(S) * 8ull, dst, bytes, [&](double *out, void *scratch, int *n) {
+    const std::vector<WorldGroup> &table = grouped ? h->group_table : h->all_table;
+    const WorldGroup *groups = grouped ? h->group_table_dev : h->all_table_dev;
+    const uint64_t scratch = bytes && h->status == B200_OK ? world_stats_scratch_doubles(S, table) * 8ull : 0;
+    return run_world_reduction(h, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
-        return launch_world_stats(S, (double *)scratch, n, h->stream);
+        return launch_world_stats(S, groups, table, (double *)scr, n, h->stream);
     });
 }
 
 int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, trajectory_planes, dst, bytes, "trajectory");
+    return run_world_stats(h, trajectory_planes, false, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, state_planes, dst, bytes, "state");
+    return run_world_stats(h, state_planes, false, dst, bytes, "state");
+}
+
+int b200_sixdof_trajectory_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return run_world_stats(h, trajectory_planes, true, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return run_world_stats(h, state_planes, true, dst, bytes, "state");
 }
 
 // Quantiles of the planes over the worlds (quantile_kernels.cu) into dst: the handle's status checked, then the levels,
@@ -1332,12 +1404,14 @@ static int linspace_edges(double lo, double hi, uint32_t n, double *e)
     return 0;
 }
 
-// Histograms of the specs over the worlds (hist_kernels.cu) into dst: the handle's status checked, then the specs (each
-// plane < width), then `bytes`.  The edges are computed here and copied to the device ahead of the launch.
-static int run_histograms(b200_sixdof *h, PlaneSource source, uint32_t width, const b200_histogram *specs, uint32_t n_specs,
-                          void *dst, uint64_t bytes, const char *what)
+// Histograms of the specs over the worlds, per group when `grouped` (hist_kernels.cu), into dst: the groups checked,
+// then the handle's status, then the specs (each plane < width), then `bytes`.  The edges and the group table are
+// computed here and copied to the device ahead of the launch.
+static int run_histograms(b200_sixdof *h, PlaneSource source, bool grouped, uint32_t width, const b200_histogram *specs,
+                          uint32_t n_specs, void *dst, uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     HistParams P{};
     static_cast<StatsParams &>(P) = source(h);
@@ -1390,29 +1464,47 @@ static int run_histograms(b200_sixdof *h, PlaneSource source, uint32_t width, co
     }
     P.n_specs = n_specs;
     const uint64_t n_s = P.planes_per_sample ? P.n_planes / P.planes_per_sample : 0;
-    const uint64_t want = n_s * P.record_len * 8ull;
+    const std::vector<uint64_t> sizes = reduction_groups(h, grouped);
+    const uint64_t want = n_s * sizes.size() * P.record_len * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s histograms are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    const uint64_t edge_bytes = edges.size() * 8ull;
-    return run_world_reduction(h, edge_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
-        cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes, cudaMemcpyHostToDevice, h->stream);
+    const std::vector<WorldGroup> table = hist_group_table(sizes.data(), sizes.size(), n_s * n_specs);
+    const uint64_t edge_bytes = edges.size() * 8ull, table_bytes = table.size() * sizeof(WorldGroup);
+    edges.resize(edges.size() + table_bytes / 8);  // one copy to the device: the edges, then the group table
+    std::memcpy(edges.data() + edge_bytes / 8, table.data(), table_bytes);
+    return run_world_reduction(h, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
+        cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes + table_bytes, cudaMemcpyHostToDevice, h->stream);
         if (e != cudaSuccess) return e;
         P.out = out;
         P.edges = (const double *)scratch;
-        return launch_histograms(P, n, h->stream);
+        return launch_histograms(P, (const WorldGroup *)((char *)scratch + edge_bytes), table, n, h->stream);
     });
 }
 
 int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                       uint64_t bytes)
 {
-    return run_histograms(h, trajectory_planes, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes, "trajectory");
+    return run_histograms(h, trajectory_planes, false, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes,
+                          "trajectory");
 }
 
 int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes)
 {
-    return run_histograms(h, state_planes, 25, specs, n_specs, dst, bytes, "state");
+    return run_histograms(h, state_planes, false, 25, specs, n_specs, dst, bytes, "state");
+}
+
+int b200_sixdof_trajectory_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                            uint64_t bytes)
+{
+    return run_histograms(h, trajectory_planes, true, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes,
+                          "trajectory");
+}
+
+int b200_sixdof_state_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                       uint64_t bytes)
+{
+    return run_histograms(h, state_planes, true, 25, specs, n_specs, dst, bytes, "state");
 }
 
 // Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.

@@ -60,6 +60,11 @@ struct b200_sixdof {
     uint64_t staging_bytes = 0;
     double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
+    // statistics group tables (stats_kernels.cu): all worlds as one group (built at creation) and the groups of
+    // b200_sixdof_set_world_groups (sizes empty = none set), each with its device copy
+    std::vector<b200::WorldGroup> all_table, group_table;
+    b200::WorldGroup *all_table_dev = nullptr, *group_table_dev = nullptr;
+    std::vector<uint64_t> group_sizes;
     // trajectory
     double *traj = nullptr;
     uint32_t traj_planes = 13;   // 25 with B200_TRAJ_FULL

@@ -3,6 +3,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include <vector>
 
 #include "../../include/b200_sixdof.h"
 
@@ -187,10 +188,34 @@ __device__ inline const double *stats_plane(const StatsParams &S, uint64_t i)
     }
     return p; // i < n_planes: always set
 }
-// f64 of device scratch the reduction needs for this shape (0: one pass, no scratch)
-uint64_t world_stats_scratch_doubles(const StatsParams &S);
-// one or two launches on s (written to *launches); `scratch` holds world_stats_scratch_doubles(S) f64
-cudaError_t launch_world_stats(const StatsParams &S, double *scratch, int *launches, cudaStream_t s);
+// A world group of a grouped reduction: the worlds [o, o + n), reduced in C chunks of Wc worlds; k0 = the chunks of the
+// groups before it, which numbers the block tasks of a launch and places the group's partials.
+struct WorldGroup {
+    uint64_t o, n, Wc, C, k0;
+};
+// the group of chunk k among the groups [g0, g1) of t: the last one whose first chunk is at most k (empty groups of the
+// histogram table share their successor's k0 and are never chosen)
+__device__ inline uint64_t group_of_chunk(const WorldGroup *t, uint64_t g0, uint64_t g1, uint64_t k)
+{
+    uint64_t lo = g0, hi = g1 - 1;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi + 1) / 2;
+        if (t[mid].k0 <= k) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+// The statistics table of consecutive groups of sizes[0 .. n_groups) (stats_shape per group; an empty group has one
+// chunk of no worlds).  The ungrouped statistics are the one-group table {n_worlds}.
+std::vector<WorldGroup> world_group_table(const uint64_t *sizes, uint64_t n_groups, uint64_t n_entities);
+// f64 of device scratch the reduction over the groups of `table` needs (0: one pass, no scratch); at most 256 MiB
+// unless one group-plane alone needs more
+uint64_t world_stats_scratch_doubles(const StatsParams &S, const std::vector<WorldGroup> &table);
+// One or two launches per slice of groups and planes on s (written to *launches); `groups` is `table` in device memory
+// and `scratch` holds world_stats_scratch_doubles(S, table) f64.  Group g of G = table.size() goes to
+// out[(((i / W) * G + g) * n_entities + e) * W + i % W][5].
+cudaError_t launch_world_stats(const StatsParams &S, const WorldGroup *groups, const std::vector<WorldGroup> &table,
+                               double *scratch, int *launches, cudaStream_t s);
 
 // Ensemble quantiles over the world axis (quantile_kernels.cu): the planes of a StatsParams, and n_q levels.  Group
 // (plane i, entity e) goes to out[((i / W) * n_entities + e) * W + i % W][n_q].
@@ -258,13 +283,14 @@ struct HistParams : StatsParams {
     uint64_t record_len;   // f64 per sample: every spec's record
     const double *edges;
 };
-// worlds per chunk and chunks of a call over n_groups (sample, spec) pairs
-struct HistChunks {
-    uint64_t Wc, C;
-};
-HistChunks hist_chunks(uint64_t n_worlds, uint64_t n_groups);
-// zeroes out (a memset) and counts every (sample, spec) in one launch on s (*launches = 1; 0 with nothing to count)
-cudaError_t launch_histograms(const HistParams &P, int *launches, cudaStream_t s);
+// The histogram table of consecutive groups of sizes[0 .. n_groups) of a call over n_pairs (sample, spec) pairs: each
+// group's chunks (none for an empty group), about 2 block tasks per SM over the whole call.
+std::vector<WorldGroup> hist_group_table(const uint64_t *sizes, uint64_t n_groups, uint64_t n_pairs);
+// Zeroes out (a memset) and counts every (sample, group, spec) in one launch on s (*launches = 1; 0 with nothing to
+// count).  `groups` is `table` in device memory; sample s, group g of G = table.size() goes to
+// out[(s * G + g) * record_len ..].
+cudaError_t launch_histograms(const HistParams &P, const WorldGroup *groups, const std::vector<WorldGroup> &table,
+                              int *launches, cudaStream_t s);
 
 // Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
 // row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.

@@ -340,6 +340,38 @@ class B200Exec:
         args, row = self._hist_specs(specs)
         return self._reduce("histograms", False, args, (row,))
 
+    # ---- grouped ensembles (the statistics and histograms above, one table per contiguous world range) ----------
+    def set_world_groups(self, sizes) -> None:
+        """Split the worlds into consecutive groups of `sizes` worlds (each >= 0, summing to n_worlds, at most
+        MAX_WORLD_GROUPS); an empty `sizes` clears the setting.  The ungrouped tables are unchanged by it."""
+        sz = np.ascontiguousarray(np.asarray(list(sizes), dtype=np.uint64).ravel())
+        _lib.check(self._L.b200_sixdof_set_world_groups(self._h, sz.ctypes.data_as(C.POINTER(C.c_uint64)), sz.size))
+
+    @property
+    def world_groups(self) -> int:
+        """The number of groups set, 0 = none."""
+        return int(self._L.b200_sixdof_world_groups(self._h))
+
+    def trajectory_group_stats(self) -> np.ndarray:
+        """trajectory_stats() per group: [samples, G, n_entities, width, 5]; group g's record has the bits of
+        trajectory_stats() on a batch of exactly its worlds."""
+        n, E, W = self._planes(ring=True)
+        return self._reduce("group_stats", True, (), (n, self.world_groups, E, W, _lib.STATS_FIELDS))
+
+    def state_group_stats(self) -> np.ndarray:
+        """state_stats() per group: [G, n_entities, 25, 5]."""
+        return self._reduce("group_stats", False, (), (self.world_groups,) + self._planes(ring=False) + (_lib.STATS_FIELDS,))
+
+    def trajectory_group_histograms(self, specs) -> np.ndarray:
+        """trajectory_histograms(specs) per group: [samples, G, sum of the record lengths]."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("group_histograms", True, args, (self.trajectory_len(), self.world_groups, row))
+
+    def state_group_histograms(self, specs) -> np.ndarray:
+        """state_histograms(specs) per group: [G, sum of the record lengths]."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("group_histograms", False, args, (self.world_groups, row))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =

@@ -27,6 +27,20 @@ def shard_sizes(n_worlds: int, world_size: int) -> List[int]:
     return [shard_worlds(n_worlds, r, world_size)[1] - shard_worlds(n_worlds, r, world_size)[0] for r in range(world_size)]
 
 
+def shard_groups(sizes: Sequence[int], rank: int, world_size: int) -> List[int]:
+    """The world groups of `rank` in a world-sharded grouped campaign: the global group sizes cut to the rank's world
+    range (shard_worlds), zeros kept, so every rank has the same number of groups and group g of every rank's grouped
+    tables is part of global group g.  gather_ensemble / gather_histograms then merge the grouped tables as they merge
+    the ungrouped ones (a count-0 part is the identity of the merge)."""
+    w0, w1 = shard_worlds(sum(int(s) for s in sizes), rank, world_size)
+    out, g0 = [], 0
+    for s in sizes:
+        g1 = g0 + int(s)
+        out.append(max(0, min(g1, w1) - max(g0, w0)))
+        g0 = g1
+    return out
+
+
 def gather_worlds(local, n_worlds: int, group=None):
     """End-of-run gather of a per-world tensor [w_local, ...] from every rank into the global
     world order [n_worlds, ...] (all ranks get the result).  Ragged shards are padded to the

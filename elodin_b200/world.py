@@ -438,7 +438,8 @@ class World:
               world_params: Optional[Dict[str, np.ndarray]] = None, resident: Optional[bool] = None,
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
               thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
-              covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None) -> "Exec":
+              covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
+              groups: Optional[Sequence[int]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -448,7 +449,11 @@ class World:
         `covariance` the covariance over the worlds of a selection of components for every row and entity
         (`Exec.covariance`): items are a component name ("world_pos": all its planes) or (component, indices), e.g.
         covariance=[("world_pos", (4, 5, 6)), ("world_vel", (3, 4, 5))], at most 25 distinct planes; `histograms` (1 to
-        8 `Histogram`s) the bin counts over the worlds of one or two components for every row (`Exec.histogram`)."""
+        8 `Histogram`s) the bin counts over the worlds of one or two components for every row (`Exec.histogram`).
+        `groups` (1 to 1024 world counts summing to n_worlds) splits the worlds into consecutive groups, e.g. the sweep
+        points of a plan ordered by `monte_carlo.plan_groups`, and also records the statistics and histograms of every
+        group (`Exec.ensemble(pair, groups=True)`, `Exec.histogram(i, groups=True)`); quantiles and covariance stay over
+        all worlds."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -456,7 +461,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -576,6 +581,23 @@ def _covariance_planes(spec):
     return planes, labels
 
 
+def _world_groups(groups, n_worlds: int) -> List[int]:
+    """World.build(..., groups=...): 1 to MAX_WORLD_GROUPS non-negative integer world counts summing to n_worlds."""
+    if isinstance(groups, (str, bytes)) or not isinstance(groups, (Sequence, np.ndarray)):
+        raise TypeError(f"groups take a sequence of world counts, got {groups!r}")
+    sizes = list(np.asarray(groups).ravel()) if isinstance(groups, np.ndarray) else list(groups)
+    for x in sizes:
+        if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)):
+            raise TypeError(f"groups: world count {x!r} is not an integer")
+        if x < 0:
+            raise ValueError(f"groups: world count {x} is negative")
+    if not 1 <= len(sizes) <= _lib.MAX_WORLD_GROUPS:
+        raise ValueError(f"{len(sizes)} groups: 1 to {_lib.MAX_WORLD_GROUPS}")
+    if sum(int(x) for x in sizes) != n_worlds:
+        raise ValueError(f"groups: the world counts sum to {sum(int(x) for x in sizes)}, not to n_worlds = {n_worlds}")
+    return [int(x) for x in sizes]
+
+
 def _histogram_specs(histograms) -> List["Histogram"]:
     """World.build(..., histograms=...): 1 to MAX_HISTOGRAMS el.Histogram objects."""
     if isinstance(histograms, (str, bytes)) or not isinstance(histograms, Sequence):
@@ -693,7 +715,8 @@ class Exec:
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
                  thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
-                 covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None):
+                 covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
+                 groups: Optional[Sequence[int]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -737,6 +760,9 @@ class Exec:
                                        ("histograms", histograms is not None)) if on]
         if given and not ensemble:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{', '.join(given)}: need World.build(..., ensemble=True)")
+        if groups is not None and not ensemble:
+            raise ValueError("groups: need World.build(..., ensemble=True)")
+        self.groups = _world_groups(groups, self.n_worlds) if groups is not None else None
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
         self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
@@ -770,6 +796,10 @@ class Exec:
                     raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {h.pair}")
                 specs.append(h._spec(bodies.index(ent)))
             self._ens_args["histograms"] = (specs,)
+        if self.groups is not None:  # the same tables per group of worlds
+            self._ens_args["group_stats"] = ()
+            if histograms is not None:
+                self._ens_args["group_histograms"] = self._ens_args["histograms"]
         self._ens_rows: Dict[str, List[np.ndarray]] = {kind: [] for kind in self._ens_args}
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
@@ -824,6 +854,8 @@ class Exec:
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._extrema or self._thresholds:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
+        if self.groups is not None:
+            self.backend.set_world_groups(self.groups)
         if self._ensemble:
             self._history = {}
             self._upload_inputs()
@@ -1129,13 +1161,18 @@ class Exec:
         row = col.row_of(self.world.entity_by_name(ent))
         return np.stack([h[:, row] for h in self._history[col.component.id]])
 
-    def ensemble(self, pair: str) -> Dict[str, np.ndarray]:
+    def ensemble(self, pair: str, groups: bool = False) -> Dict[str, np.ndarray]:
         """`exec.ensemble("rocket.world_pos")` -> {"count", "mean", "std", "min", "max"}, each [rows, width]: one row
         per telemetry cycle (row 0 = the initial state), taken over the worlds whose value is finite; count = the
         number of such worlds (a diverged world is missing from it), std = sqrt(m2 / count) (numpy's ddof=0), NaN
         where no world is finite.  Needs World.build(..., ensemble=True); the sampled components are world_pos,
-        world_vel, world_accel and force."""
-        t = self._ensemble_rows("stats", pair, "ensemble statistics", "ensemble()", "")  # [rows, width, 5]
+        world_vel, world_accel and force.  With groups=True (World.build(..., groups=[...])) each is [rows, G, width],
+        taken over the worlds of each group."""
+        if groups:
+            t = self._ensemble_rows("group_stats", pair, "ensemble statistics", "ensemble(groups=True)", ", groups=[...]",
+                                    grouped=True)  # [rows, G, width, 5]
+        else:
+            t = self._ensemble_rows("stats", pair, "ensemble statistics", "ensemble()", "")  # [rows, width, 5]
         count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
             std = np.sqrt(t[..., 2] / count)
@@ -1164,33 +1201,42 @@ class Exec:
             cov = t[:, 1 + p:].reshape(-1, p, p) / count[:, None, None]
         return {"count": count, "mean": np.ascontiguousarray(t[:, 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
 
-    def histogram(self, i: int) -> Dict[str, object]:
+    def histogram(self, i: int, groups: bool = False) -> Dict[str, object]:
         """`exec.histogram(i)` -> for histogram i of World.build(..., histograms=[...]) and every telemetry row (row 0 =
         the initial state), int64 counts over the worlds: "counts" [rows, bins] (1D) or [rows, bins_x, bins_y] (2D,
         np.histogram2d's layout), "nonfinite" [rows] (worlds whose value, or either value, is NaN / inf), 1D "below" and
         "above" [rows] (finite values out of the range on each side), 2D "outside" [rows] (both finite, at least one out
-        of range), and "edges" (np.linspace's; a pair for 2D).  Every world is counted once per row."""
-        if "histograms" not in self._ens_rows:
+        of range), and "edges" (np.linspace's; a pair for 2D).  Every world is counted once per row.  With groups=True
+        (World.build(..., groups=[...])) a group axis follows the row axis: [rows, G, ...], over the worlds of each
+        group."""
+        kind = "group_histograms" if groups else "histograms"
+        if kind not in self._ens_rows:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "histogram(): build the Exec with World.build(..., ensemble=True, histograms=[...])")
+                                 f"histogram({'groups=True' if groups else ''}): build the Exec with World.build(..., "
+                                 f"ensemble=True, histograms=[...]{', groups=[...]' if groups else ''})")
         if not 0 <= i < len(self._histograms):
             raise IndexError(f"histogram {i}: this Exec has {len(self._histograms)}")
         h = self._histograms[i]
         off = sum(x.record_len for x in self._histograms[:i])
-        t = np.concatenate(self._ens_rows["histograms"])[:, off:off + h.record_len].astype(np.int64)
+        t = np.concatenate(self._ens_rows[kind])[..., off:off + h.record_len].astype(np.int64)
         if len(h.bins) == 1:
-            return {"counts": np.ascontiguousarray(t[:, 3:]), "nonfinite": t[:, 0].copy(), "below": t[:, 1].copy(),
-                    "above": t[:, 2].copy(), "edges": h.edges}
-        return {"counts": np.ascontiguousarray(t[:, 2:]).reshape(-1, *h.bins), "nonfinite": t[:, 0].copy(),
-                "outside": t[:, 1].copy(), "edges": h.edges}
+            return {"counts": np.ascontiguousarray(t[..., 3:]), "nonfinite": t[..., 0].copy(), "below": t[..., 1].copy(),
+                    "above": t[..., 2].copy(), "edges": h.edges}
+        return {"counts": np.ascontiguousarray(t[..., 2:]).reshape(*t.shape[:-1], *h.bins), "nonfinite": t[..., 0].copy(),
+                "outside": t[..., 1].copy(), "edges": h.edges}
 
-    def _ensemble_rows(self, kind: str, pair: str, what: str, method: str, option: str, per_plane: bool = True):
-        """The recorded rows of table `kind` for the entity of `pair`, sliced to the planes of its component when the
-        table is `per_plane`; refused (ERR_INVALID_ARGUMENT) by `method` if this Exec was not built with `option`."""
+    def _ensemble_rows(self, kind: str, pair: str, what: str, method: str, option: str, per_plane: bool = True,
+                       grouped: bool = False):
+        """The recorded rows of table `kind` for the entity of `pair` (after the group axis when the table is
+        `grouped`), sliced to the planes of its component when the table is `per_plane`; refused (ERR_INVALID_ARGUMENT)
+        by `method` if this Exec was not built with `option`."""
         if kind not in self._ens_rows:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{method}: build the Exec with World.build(..., ensemble=True{option})")
         row, (lo, hi) = self._sampled_row(pair, what)
-        t = np.concatenate(self._ens_rows[kind])[:, row]
+        t = np.concatenate(self._ens_rows[kind])
+        if grouped:
+            return t[:, :, row, lo:hi] if per_plane else t[:, :, row]
+        t = t[:, row]
         return t[:, lo:hi] if per_plane else t
 
     def _sampled_row(self, pair: str, what: str):

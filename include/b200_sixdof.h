@@ -399,6 +399,37 @@ int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *spec
                                       uint64_t bytes);
 int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes);
 
+/* ---- grouped ensembles: the statistics and histograms above, one table per group of worlds (one sweep point of a
+ * campaign).  A group is a contiguous world range: group g holds the worlds [sizes[0] + .. + sizes[g-1], .. + sizes[g]);
+ * a host reorders its plan so that every sweep point is contiguous.  Empty groups are allowed.  Group g's record has the
+ * same bits as the ungrouped entry on a handle whose n_worlds = sizes[g] holds exactly those worlds (statistics: the
+ * chunking of a group depends on its size and n_entities alone; histograms: integer counts, exact in any order); an
+ * empty group has count 0 and NaN in its statistics, and zero counts.  The grouped tables put the group axis after the
+ * sample axis; with G = 1 and sizes = {n_worlds} they are the ungrouped tables.  Setting groups changes nothing the
+ * ungrouped entries return.  The grouped entries check what the ungrouped ones check, in the same order, and return
+ * B200_ERR_INVALID_ARGUMENT while no groups are set; they run on the handle's stream, return once dst (host or device)
+ * is filled and count their launches in timings.kernel_launches (statistics: one or two per slice of groups and planes,
+ * slices keeping the chunk partials in the staging buffer at most 256 MiB; histograms: one memset and one launch).
+ * Grouped quantiles and covariance do not exist: those tables are over all worlds. ---- */
+#define B200_MAX_WORLD_GROUPS 1024u
+/* sizes[0 .. n_groups): consecutive world counts, each >= 0, summing to n_worlds; n_groups = 0 clears the setting.
+ * B200_ERR_INVALID_ARGUMENT for a null handle, more than B200_MAX_WORLD_GROUPS groups, null sizes with n_groups > 0 or
+ * sizes that do not sum to n_worlds (the setting is then unchanged).  The group table is built and copied to the device
+ * here, once per setting. */
+int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups);
+/* the current number of groups, 0 = none */
+uint32_t b200_sixdof_world_groups(const b200_sixdof *h);
+/* the ring's samples: dst = [trajectory_len][G][n_entities][trajectory_width][5] f64 */
+int b200_sixdof_trajectory_group_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* the current state: dst = [G][n_entities][25][5] f64 */
+int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* the ring's samples: dst = [trajectory_len][G][sum of the record lengths] f64 */
+int b200_sixdof_trajectory_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                            uint64_t bytes);
+/* the current state: dst = [G][sum of the record lengths] f64 */
+int b200_sixdof_state_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                       uint64_t bytes);
+
 /* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
  * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the
  * B200_TRAJ_FULL layout (world_pos[7], world_vel[6], world_accel[6], force[6]: planes 0..24) at one tick.
