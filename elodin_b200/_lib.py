@@ -67,6 +67,8 @@ SYMBOLS = [
     "b200_sixdof_trajectory_histograms", "b200_sixdof_state_histograms",
     "b200_sixdof_set_world_groups", "b200_sixdof_world_groups", "b200_sixdof_trajectory_group_stats",
     "b200_sixdof_state_group_stats", "b200_sixdof_trajectory_group_histograms", "b200_sixdof_state_group_histograms",
+    "b200_sixdof_trajectory_group_quantiles", "b200_sixdof_state_group_quantiles",
+    "b200_sixdof_trajectory_group_covariance", "b200_sixdof_state_group_covariance",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -240,6 +242,10 @@ def lib():
     L.b200_sixdof_state_group_stats.argtypes = [vp, vp, u64]
     L.b200_sixdof_trajectory_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_state_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_trajectory_group_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_state_group_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_trajectory_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_state_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -1,16 +1,23 @@
-// Ensemble covariance over the world axis: for every (sample, entity) one record (n, mean[p], M[p][p]) over the worlds
-// whose p selected values are all finite (include/b200_sixdof.h b200_sixdof_trajectory_covariance / _state_covariance).
+// Ensemble covariance over the world axis: for every (sample, world group, entity) one record (n, mean[p], M[p][p])
+// over the group's worlds whose p selected values are all finite (include/b200_sixdof.h
+// b200_sixdof_trajectory_covariance / _state_covariance and the _group_covariance entries).  A world group is a
+// contiguous world range; the ungrouped entries are the one-group case [0, n_worlds) of the same code.
 //
-// Shape of the reduction.  The worlds are cut into C chunks of Wc consecutive worlds; Wc and C depend on (n_worlds,
-// n_entities) alone.  A block reduces one chunk of one sample for a tile of Et entities: it stages Wt worlds x p planes x
+// Shape of the reduction.  A group's worlds are cut into C chunks of Wc consecutive worlds; Wc and C depend on (the
+// group's size, n_entities) alone (cov_chunks), and chunk c of a group starting at world o reads o + [c Wc, (c + 1) Wc),
+// so a group's record has the bits of the ungrouped call on a batch of exactly its worlds.  The chunks of all groups
+// are numbered through the group table (WorldGroup, k0 = the chunks of the groups before it) and a block finds the
+// group of its chunk by binary search, as the statistics do; an empty group is one chunk of no worlds, which writes
+// n = 0 and NaN.  A block reduces one chunk of one sample for a tile of Et entities: it stages Wt worlds x p planes x
 // Et entities at a time in shared memory (lanes read consecutive doubles of one plane: entities, then worlds when the
 // tile is every entity), marks the complete worlds, then thread (entity, tile) accumulates a 4 x 4 register tile of the
 // upper triangle of M over the chunk's complete worlds in world order.  Shift: K = the chunk's first complete world's
 // row, y = x - K, sums S_a = sum y_a (diagonal tiles) and Q_ab = sum y_a y_b (fma); the chunk's record is
 // mean_a = K_a + S_a / n, M_ab = Q_ab - lo (hi / n) with (lo, hi) = (min, max)(S_a, S_b), and M_aa = +inf where Q_aa overflowed.  Each entry is a sequential sum over the same worlds whatever the
 // selection, the entity tile or the other planes, so an entry has the same bits in any selection with the same complete
-// worlds.  With C > 1 a second launch merges the chunk records left to right with cov_merge, one thread per (group,
-// upper entry).  The partials live in scratch; groups run in slices that keep it under kScratchCap.  No atomics.
+// worlds.  Where a group has C > 1 a second launch merges its chunk records left to right with cov_merge, one thread per
+// (group, sample, entity, upper entry).  The partials live in scratch; groups and samples run in slices that keep it
+// under kScratchCap.  No atomics.
 #include <algorithm>
 #include <cfloat>
 
@@ -35,6 +42,7 @@ struct Chunks {
 
 inline Chunks cov_chunks(uint64_t n_worlds, uint64_t E)
 {
+    if (n_worlds == 0 || E == 0) return Chunks{n_worlds, 1};  // one chunk: of no worlds, or of no entities to reduce
     const uint64_t tiles = (E + kEntTile - 1) / kEntTile;
     uint64_t C = std::max<uint64_t>(1, (kChunkTasks + tiles - 1) / tiles);
     C = std::min(C, std::max<uint64_t>(1, (n_worlds + kMinWorlds - 1) / kMinWorlds));
@@ -64,17 +72,19 @@ inline Geo cov_geo(const CovParams &S)
     return g;
 }
 
-// A slice of the groups: samples [s0, s0 + ns) x entities [e0, e0 + ne) (every entity, e0 = 0); local group
-// gl = (s - s0) * ne + (e - e0)
+// A slice: the groups [g0, g1) of a table of G groups, their chunks k0 .. k0 + K, and the samples [s0, s0 + ns)
 struct Slice {
-    uint64_t s0, ns, e0, ne;
+    const WorldGroup *groups;
+    uint64_t G, g0, g1, k0, K, s0, ns;
 };
 
-__device__ inline double *record(const CovParams &S, const Slice &sl, double *scratch, uint64_t c, uint64_t s, uint64_t e)
+// the final record of (sample s, group g, entity e), or, with scratch, the partial record of chunk q of the slice
+__device__ inline double *record(const CovParams &S, const Slice &sl, double *scratch, uint64_t q, uint64_t g, uint64_t s,
+                                 uint64_t e)
 {
     const uint64_t R = 1 + S.n_p + (uint64_t)S.n_p * S.n_p;
-    if (scratch) return scratch + (c * sl.ns * sl.ne + (s - sl.s0) * sl.ne + (e - sl.e0)) * R;
-    return S.out + (s * S.n_entities + e) * R;
+    if (scratch) return scratch + ((q * sl.ns + (s - sl.s0)) * S.n_entities + e) * R;
+    return S.out + ((s * sl.G + g) * S.n_entities + e) * R;
 }
 
 __device__ inline void tile_of(uint32_t t, uint32_t nb, uint32_t &ab, uint32_t &bb)
@@ -84,9 +94,9 @@ __device__ inline void tile_of(uint32_t t, uint32_t nb, uint32_t &ab, uint32_t &
     bb = ab + t;
 }
 
-// pass 1: task = (sample s of the slice, chunk c, entity tile) -> the chunk's record per entity: final (NaN where
-// n = 0) when C = 1, else a partial record in scratch
-__global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chunks ck, Geo geo, Slice sl, double *scratch)
+// pass 1: task = (sample s of the slice, chunk q of the slice, entity tile) -> the chunk's record per entity: final
+// (NaN where n = 0) when its group has C = 1, else a partial record in scratch
+__global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Geo geo, Slice sl, double *scratch)
 {
     extern __shared__ double smem[];
     const uint32_t p = S.n_p, Et = geo.Et, Wt = geo.Wt;
@@ -94,8 +104,8 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chu
     double *ss = xs + (uint64_t)Wt * p * Et;              // [p][Et]: the diagonal tiles' S_a
     unsigned char *ok = (unsigned char *)(ss + p * Et);   // [Wt][Et]
     const uint64_t E = S.n_entities;
-    const uint64_t n_et = (sl.ne + Et - 1) / Et;
-    const uint64_t n_tasks = sl.ns * ck.C * n_et;
+    const uint64_t n_et = (E + Et - 1) / Et;
+    const uint64_t n_tasks = sl.ns * sl.K * n_et;
     const unsigned t = threadIdx.x;
     const uint32_t el = t % Et, tile = t / Et, nb = (p + 3) / 4;
     const bool active = tile < geo.T;
@@ -109,10 +119,14 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chu
         ib[k] = min(4 * bb + k, p - 1);
     }
     for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
-        const uint64_t et = task % n_et, c = (task / n_et) % ck.C, s = sl.s0 + task / (n_et * ck.C);
-        const uint64_t e0 = sl.e0 + et * Et;
-        const uint32_t ne = (uint32_t)min((uint64_t)Et, sl.e0 + sl.ne - e0);
-        const uint64_t w0 = c * ck.Wc, w1 = min(w0 + ck.Wc, S.n_worlds);
+        const uint64_t et = task % n_et, q = (task / n_et) % sl.K, s = sl.s0 + task / (n_et * sl.K);
+        const uint64_t g = group_of_chunk(sl.groups, sl.g0, sl.g1, sl.k0 + q);
+        const WorldGroup wg = sl.groups[g];
+        const uint64_t c = sl.k0 + q - wg.k0;
+        const uint64_t e0 = et * Et;
+        const uint32_t ne = (uint32_t)min((uint64_t)Et, E - e0);
+        const uint64_t w0 = wg.o + c * wg.Wc, w1 = wg.o + min((c + 1) * wg.Wc, wg.n);
+        const bool fin = wg.C == 1;  // a final record holds NaN where n = 0; a partial leaves them (unread)
         double K[8], Q[16], Ssum[4];
 #pragma unroll
         for (int k = 0; k < 8; ++k) K[k] = 0.0;
@@ -190,9 +204,8 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chu
                 if (4 * ab + k < p) ss[(4 * ab + k) * Et + el] = Ssum[k];
         __syncthreads();
         if (active && el < ne) {
-            double *o = record(S, sl, ck.C > 1 ? scratch : nullptr, c, s, e0 + el);
+            double *o = record(S, sl, fin ? nullptr : scratch, q, g, s, e0 + el);
             const double nan = __longlong_as_double(0x7ff8000000000000ll);
-            const bool fin = ck.C == 1;  // a final record holds NaN where n = 0; a partial leaves them (unread)
             const double dn = (double)n;
             if (tile == 0) o[0] = dn;
 #pragma unroll
@@ -221,34 +234,38 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Chu
     }
 }
 
-// pass 2 (C > 1): thread = (group of the slice, upper entry (a, b)) folds the C chunk records left to right
-__global__ void __launch_bounds__(256) cov_merge_kernel(CovParams S, Chunks ck, Slice sl, const double *scratch)
+// pass 2: thread = (group of the slice with C > 1, sample, entity, upper entry (a, b)) folds the group's C chunk
+// records left to right
+__global__ void __launch_bounds__(256) cov_merge_kernel(CovParams S, Slice sl, const double *scratch)
 {
     const uint32_t p = S.n_p;
-    const uint64_t U = (uint64_t)p * (p + 1) / 2, R = 1 + p + (uint64_t)p * p, Gs = sl.ns * sl.ne;
+    const uint64_t U = (uint64_t)p * (p + 1) / 2, R = 1 + p + (uint64_t)p * p, SE = sl.ns * S.n_entities;
+    const uint64_t n = (sl.g1 - sl.g0) * SE * U;
     const double nan = __longlong_as_double(0x7ff8000000000000ll);
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < Gs * U; i += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t gl = i / U;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t g = sl.g0 + i / (SE * U), gl = i / U % SE;  // gl = (s - s0) * E + e
+        const WorldGroup wg = sl.groups[g];
+        if (wg.C == 1) continue;  // finished by pass 1
         uint32_t k = (uint32_t)(i % U), a = 0;
         while (k >= p - a) { k -= p - a; ++a; }
         const uint32_t b = a + k;
         CovEntry acc{0.0, 0.0, 0.0, 0.0};
-        const double *r = scratch + gl * R;
-        for (uint64_t c0 = 0; c0 < ck.C; c0 += kMergeBatch) { // the batch's loads are in flight before the first fold
+        const double *r = scratch + ((wg.k0 - sl.k0) * SE + gl) * R;
+        for (uint64_t c0 = 0; c0 < wg.C; c0 += kMergeBatch) { // the batch's loads are in flight before the first fold
             CovEntry v[kMergeBatch];
 #pragma unroll
             for (unsigned u = 0; u < kMergeBatch; ++u) {
                 v[u].n = 0.0;
-                if (c0 + u < ck.C) {
-                    const double *q = r + (c0 + u) * Gs * R;
+                if (c0 + u < wg.C) {
+                    const double *q = r + (c0 + u) * SE * R;
                     v[u] = CovEntry{q[0], q[1 + a], q[1 + b], q[1 + p + a * p + b]};
                 }
             }
 #pragma unroll
             for (unsigned u = 0; u < kMergeBatch; ++u) cov_merge(acc, v[u]);
         }
-        const uint64_t s = sl.s0 + gl / sl.ne, e = sl.e0 + gl % sl.ne;
-        double *o = S.out + (s * S.n_entities + e) * R;
+        const uint64_t s = sl.s0 + gl / S.n_entities, e = gl % S.n_entities;
+        double *o = S.out + ((s * sl.G + g) * S.n_entities + e) * R;
         const bool any = acc.n > 0.0;
         if (a == 0 && b == 0) o[0] = acc.n;
         if (a == b) o[1 + a] = any ? acc.ma : nan;
@@ -257,53 +274,81 @@ __global__ void __launch_bounds__(256) cov_merge_kernel(CovParams S, Chunks ck, 
     }
 }
 
-inline uint64_t partial_bytes(const CovParams &S, const Chunks &ck)
-{
-    return ck.C > 1 ? ck.C * (1 + S.n_p + (uint64_t)S.n_p * S.n_p) * 8ull : 0;
-}
-
-// Slices are whole samples: with C > 1 (fewer than kChunkTasks entity tiles of kEntTile), a sample's E * C partial
-// records number at most kEntTile * 2 * kChunkTasks, which fit in kScratchCap at the largest record.
+// Slices of groups and samples: consecutive groups while their chunks' partials for one sample fit in kScratchCap
+// (counting every chunk of the slice's groups, as the scratch is indexed by chunk), then as many samples as fit; a
+// slice whose groups all have one chunk needs no scratch and takes every sample.  With C > 1 (fewer than kChunkTasks
+// entity tiles of kEntTile), one (group, sample)'s E * C partial records number at most kEntTile * 2 * kChunkTasks,
+// which fit in kScratchCap at the largest record, so a slice always holds at least one group and one sample.  The
+// one-group table gives the slices of whole samples the ungrouped call always had.
 static_assert(kEntTile * 2 * kChunkTasks * (1 + B200_MAX_COV_PLANES + B200_MAX_COV_PLANES * B200_MAX_COV_PLANES) * 8 <= kScratchCap,
               "one sample's partials must fit in the scratch");
-inline Slice slice_shape(const CovParams &S, const Chunks &ck)
+std::vector<Slice> cov_slices(const CovParams &S, const std::vector<WorldGroup> &table, uint64_t *scratch)
 {
-    const uint64_t per = partial_bytes(S, ck);
-    const uint64_t G = per ? kScratchCap / per : ~0ull;
-    return Slice{0, std::max<uint64_t>(1, G / S.n_entities), 0, S.n_entities};
+    std::vector<Slice> out;
+    *scratch = 0;
+    const uint64_t n_s = S.n_planes / S.planes_per_sample, G = table.size();
+    const uint64_t per_chunk = S.n_entities * (1 + S.n_p + (uint64_t)S.n_p * S.n_p) * 8ull;  // bytes per chunk and sample
+    for (uint64_t g0 = 0; g0 < G;) {
+        uint64_t g1 = g0 + 1, chunks = table[g0].C;
+        bool merge = table[g0].C > 1;
+        while (g1 < G && (chunks + table[g1].C) * per_chunk <= kScratchCap) {
+            chunks += table[g1].C;
+            merge = merge || table[g1].C > 1;
+            ++g1;
+        }
+        const uint64_t ns = merge ? std::max<uint64_t>(1, kScratchCap / (chunks * per_chunk)) : n_s;
+        for (uint64_t s0 = 0; s0 < n_s; s0 += ns) {
+            out.push_back(Slice{nullptr, G, g0, g1, table[g0].k0, chunks, s0, std::min(ns, n_s - s0)});
+            if (merge) *scratch = std::max(*scratch, chunks * per_chunk * out.back().ns);
+        }
+        g0 = g1;
+    }
+    return out;
 }
 
 } // namespace
 
-uint64_t cov_scratch_bytes(const CovParams &S)
+std::vector<WorldGroup> cov_group_table(const uint64_t *sizes, uint64_t n_groups, uint64_t n_entities)
 {
-    const uint64_t n_s = S.n_planes / S.planes_per_sample;
-    if (n_s == 0 || S.n_worlds == 0 || S.n_entities == 0) return 0;
-    const Chunks ck = cov_chunks(S.n_worlds, S.n_entities);
-    const Slice sh = slice_shape(S, ck);
-    return std::min(sh.ns, n_s) * sh.ne * partial_bytes(S, ck);
+    std::vector<WorldGroup> t(n_groups);
+    uint64_t o = 0, k0 = 0;
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        const Chunks ck = cov_chunks(sizes[g], n_entities);
+        t[g] = {o, sizes[g], ck.Wc, ck.C, k0};
+        o += sizes[g];
+        k0 += ck.C;
+    }
+    return t;
 }
 
-cudaError_t launch_covariance(const CovParams &S, void *scratch, int *launches, cudaStream_t s)
+uint64_t cov_scratch_bytes(const CovParams &S, const std::vector<WorldGroup> &table)
+{
+    uint64_t scratch = 0;
+    if (S.n_planes && S.n_entities) cov_slices(S, table, &scratch);
+    return scratch;
+}
+
+cudaError_t launch_covariance(const CovParams &S, const WorldGroup *groups, const std::vector<WorldGroup> &table,
+                              void *scratch, int *launches, cudaStream_t s)
 {
     *launches = 0;
-    const uint64_t n_s = S.n_planes / S.planes_per_sample;
-    if (n_s == 0 || S.n_worlds == 0 || S.n_entities == 0) return cudaSuccess;
-    const Chunks ck = cov_chunks(S.n_worlds, S.n_entities);
+    if (S.n_planes == 0 || S.n_entities == 0) return cudaSuccess;
     const Geo geo = cov_geo(S);
     const size_t smem = ((uint64_t)geo.Wt * S.n_p * geo.Et + (uint64_t)S.n_p * geo.Et) * 8 + (uint64_t)geo.Wt * geo.Et;
     cudaError_t e = cudaFuncSetAttribute(cov_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    const Slice sh = slice_shape(S, ck);
     const uint64_t cap = 64ull * kNumSMs * 8;
-    for (uint64_t s0 = 0; s0 < n_s; s0 += sh.ns) {
-        const Slice sl{s0, std::min(sh.ns, n_s - s0), 0, S.n_entities};
-        const uint64_t tasks = sl.ns * ck.C * ((sl.ne + geo.Et - 1) / geo.Et);
-        cov_chunk_kernel<<<(unsigned)std::min(tasks, cap), geo.threads, smem, s>>>(S, ck, geo, sl, (double *)scratch);
+    uint64_t unused;
+    for (Slice sl : cov_slices(S, table, &unused)) {
+        sl.groups = groups;
+        const uint64_t tasks = sl.ns * sl.K * ((S.n_entities + geo.Et - 1) / geo.Et);
+        cov_chunk_kernel<<<(unsigned)std::min(tasks, cap), geo.threads, smem, s>>>(S, geo, sl, (double *)scratch);
         *launches += 1;
-        if (ck.C > 1) {
-            const uint64_t work = sl.ns * sl.ne * ((uint64_t)S.n_p * (S.n_p + 1) / 2);
-            cov_merge_kernel<<<(unsigned)std::min((work + 255) / 256, cap), 256, 0, s>>>(S, ck, sl, (const double *)scratch);
+        bool merge = false;
+        for (uint64_t g = sl.g0; g < sl.g1; ++g) merge = merge || table[g].C > 1;
+        if (merge) {
+            const uint64_t work = (sl.g1 - sl.g0) * sl.ns * S.n_entities * ((uint64_t)S.n_p * (S.n_p + 1) / 2);
+            cov_merge_kernel<<<(unsigned)std::min((work + 255) / 256, cap), 256, 0, s>>>(S, sl, (const double *)scratch);
             *launches += 1;
         }
     }

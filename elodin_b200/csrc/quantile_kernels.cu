@@ -1,12 +1,16 @@
-// Ensemble quantiles over the world axis: for every (plane, entity) group and every level q, numpy's default
-// ("linear") quantile of the finite values of all worlds (include/b200_sixdof.h b200_sixdof_trajectory_quantiles /
-// _state_quantiles).  The result is two order statistics and a fixed lerp, so it needs no floating-point reduction:
-// it is exact, and independent of the launch shape and of the order of any atomic.
+// Ensemble quantiles over the world axis: for every (world group, plane, entity) triple and every level q, numpy's
+// default ("linear") quantile of the finite values of the group's worlds (include/b200_sixdof.h
+// b200_sixdof_trajectory_quantiles / _state_quantiles and the _group_quantiles entries).  A world group is a contiguous
+// world range [o, o + n) of the group table (WorldGroup; only o and n are read here); the ungrouped entries are the
+// one-group case [0, n_worlds).  The result is two order statistics and a fixed lerp, so it needs no floating-point
+// reduction: it is exact, and independent of the route, the launch shape and the order of any atomic, so a triple has
+// the bits of the ungrouped call on a batch of exactly its group's worlds whatever the other groups of the call.
 //
-// Values are ordered by the IEEE totalOrder key (key(-0) < key(+0); NaN and +-inf are dropped before).  Two routes,
-// chosen from n_worlds alone:
-//  - small groups (n_worlds <= kSmallMax): a warp (n_worlds <= 256) or a block per group loads the group's finite keys
-//    into shared memory, sorts them (bitonic) and reads off the ranks.  One read of the planes, one launch, no scratch.
+// Values are ordered by the IEEE totalOrder key (key(-0) < key(+0); NaN and +-inf are dropped before).  Three routes,
+// chosen per world group from its size n alone (quantile_order lists the groups by route); one call can take all three:
+//  - small groups (n <= kSmallMax): a warp (n <= 256, empty groups included) or a block per triple loads the triple's
+//    finite keys into shared memory, sorts them (bitonic) and reads off the ranks.  One read of the planes, one launch
+//    per route that has groups, no scratch; the block route's shared memory is sized by its largest group.
 //  - large groups: a radix select on the key with a fixed launch sequence, pass 0 and passes 1..kLevels:
 //      pass 0   per group: finite count n and min / max key (integer atomics)
 //      plan     every rank a level needs is in [kmin, kmax]
@@ -20,9 +24,12 @@
 //    range, at least 2^9 for up to 32), so every rank is finished after pass kLevels = 7: at most 8 reads of the planes
 //    on any data.  On continuous data pass 1 leaves buckets of a few thousand keys, so the planes are read 3 times
 //    (count, histogram, compaction).  A pass reads nothing of a group whose ranks are all finished.
-//    Scratch per group: kBins u32 + kGroupCap u64 keys + the plan (QGroup), about 198 KB.  The groups run in slices of
-//    at most kSliceGroups (whole planes, or entity ranges of one plane when a plane has more entities), the same launch
-//    sequence per slice, so the scratch stays under kScratchCap = 256 MiB whatever the ring or entity count.
+//    Scratch per triple: kBins u32 + kGroupCap u64 keys + the plan (QGroup), about 198 KB.  The triples of the large
+//    groups form rows (large group, plane), large group outermost; they run in slices of at most kSliceGroups triples
+//    (whole rows, or entity ranges of one row when a row has more entities), the same launch sequence per slice, so the
+//    scratch stays under kScratchCap = 256 MiB whatever the ring, group or entity count.  Each row of a slice is chunked
+//    by pass_shape over its own group's size; a block task finds its row through the slice's row table (QRow, copied
+//    to the scratch ahead of the slice's launches) by binary search over the rows' first chunks.
 // Counts and keys are integers, so the order in which atomics land changes no result.
 #include <algorithm>
 #include <cfloat>
@@ -61,15 +68,24 @@ struct QGroup {
     QSlot slot[kSlots];
 };
 
-// A slice of the groups the fixed launch sequence runs on: planes [i0, i0 + ni) x entities [e0, e0 + ne); local group
-// g = (i - i0) * ne + (e - e0).  Slices keep the scratch under kScratchCap whatever the ring or entity count.
+// One row (large world group g, plane i) of a radix slice: the group's worlds [o, o + n) in C chunks of Wc worlds
+// (pass_shape), k0 = the chunks of the slice's rows before it
+struct QRow {
+    uint32_t o, n, Wc, C, k0, g, i, pad;
+};
+
+// A slice of the triples the fixed launch sequence runs on: rows [r0, r0 + nr) of the large groups' (group, plane)
+// rows x entities [e0, e0 + ne), K chunks over its rows (Cu chunks each where every row has as many, else 0, and a
+// task searches the row table); local triple t = (r - r0) * ne + (e - e0).  Slices keep the scratch under kScratchCap
+// whatever the ring, group or entity count.
 struct Slice {
-    uint64_t i0, ni, e0, ne;
+    uint64_t r0, nr, e0, ne, K, Cu;
 };
 
 struct Layout {
-    uint64_t G;                   // groups of the slice
-    unsigned long long *reads;    // reads of the planes, summed over the groups of every slice of the call
+    uint64_t G;                   // triples of the slice
+    unsigned long long *reads;    // reads of the planes, summed over the triples of the call
+    const QRow *rows;             // [nr] the slice's rows
     QGroup *grp;                  // [G]
     uint32_t *hist;               // [G][kBins]
     unsigned long long *area;     // [G][kGroupCap]
@@ -101,10 +117,10 @@ __device__ inline const double *plane_of(const QuantileParams &S, uint64_t i)
     return p;
 }
 
-__device__ __forceinline__ double *out_of(const QuantileParams &S, uint64_t i, uint64_t e)
+__device__ __forceinline__ double *out_of(const QuantileParams &S, uint64_t g, uint64_t i, uint64_t e)
 {
     const uint64_t W = S.planes_per_sample;
-    return S.out + (((i / W) * S.n_entities + e) * W + i % W) * S.n_q;
+    return S.out + ((((i / W) * S.n_groups + g) * S.n_entities + e) * W + i % W) * S.n_q;
 }
 
 // numpy's linear quantile of the n sorted keys, rank -> key given by `at`
@@ -153,15 +169,16 @@ __device__ __forceinline__ uint32_t pow2_at_least(uint32_t n)
 
 // ---- small groups ---------------------------------------------------------------------------------------------------
 
-// load the finite keys of group (i, e) into a[], pad to a power of two with ~0 (above every finite key), sort
+// load the finite keys of triple (world group wg, i, e) into a[], pad to a power of two with ~0 (above every finite
+// key), sort
 template <class Sync>
-__device__ uint32_t load_sort(const QuantileParams &S, uint64_t i, uint64_t e, unsigned long long *a, uint32_t *cnt,
-                              uint32_t tid, uint32_t team, Sync sync)
+__device__ uint32_t load_sort(const QuantileParams &S, const WorldGroup &wg, uint64_t i, uint64_t e,
+                              unsigned long long *a, uint32_t *cnt, uint32_t tid, uint32_t team, Sync sync)
 {
     if (tid == 0) *cnt = 0;
     sync();
-    const double *p = plane_of(S, i) + e;
-    for (uint64_t w = tid; w < S.n_worlds; w += team) {
+    const double *p = plane_of(S, i) + wg.o * S.n_entities + e;
+    for (uint64_t w = tid; w < wg.n; w += team) {
         const double x = p[w * S.n_entities];
         if (finite(x)) a[atomicAdd(cnt, 1u)] = order_key(x);
     }
@@ -173,33 +190,52 @@ __device__ uint32_t load_sort(const QuantileParams &S, uint64_t i, uint64_t e, u
     return n;
 }
 
-// a warp per group, eight groups per block (n_worlds <= kWarpMax)
-__global__ void __launch_bounds__(256) quantile_warp_kernel(QuantileParams S)
+// Item x of a small route over the world groups order[first .. first + n_groups): triple (group order[first + x / PE],
+// plane (x % PE) / E, entity x % E), PE = planes x entities
+struct Item {
+    uint64_t g, i, e;
+    WorldGroup wg;
+};
+
+__device__ __forceinline__ Item item_of(const QuantileParams &S, uint32_t first, uint64_t x)
+{
+    const uint64_t PE = S.n_planes * S.n_entities;
+    Item it;
+    it.g = S.order[first + x / PE];
+    it.i = (x % PE) / S.n_entities;
+    it.e = x % S.n_entities;
+    it.wg = S.groups[it.g];
+    return it;
+}
+
+// a warp per triple, eight triples per block (groups of at most kWarpMax worlds)
+__global__ void __launch_bounds__(256) quantile_warp_kernel(QuantileParams S, uint32_t first, uint64_t n_groups)
 {
     __shared__ unsigned long long keys[8][kWarpMax];
     __shared__ uint32_t cnt[8];
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const uint64_t G = S.n_planes * S.n_entities;
-    for (uint64_t g = blockIdx.x * 8ull + wid; g < G; g += gridDim.x * 8ull) {
-        const uint64_t i = g / S.n_entities, e = g % S.n_entities;
-        const uint32_t n = load_sort(S, i, e, keys[wid], &cnt[wid], lane, 32, []() { __syncwarp(); });
-        double *o = out_of(S, i, e);
+    const uint64_t G = n_groups * S.n_planes * S.n_entities;
+    for (uint64_t x = blockIdx.x * 8ull + wid; x < G; x += gridDim.x * 8ull) {
+        const Item it = item_of(S, first, x);
+        const uint32_t n = load_sort(S, it.wg, it.i, it.e, keys[wid], &cnt[wid], lane, 32, []() { __syncwarp(); });
+        double *o = out_of(S, it.g, it.i, it.e);
         for (uint32_t l = lane; l < S.n_q; l += 32)
             o[l] = quantile_of(n, S.q[l], [&](uint32_t r) { return keys[wid][r]; });
         __syncwarp();
     }
 }
 
-// a block per group (kWarpMax < n_worlds <= kSmallMax); dynamic shared memory: pow2(n_worlds) keys
-__global__ void __launch_bounds__(512) quantile_block_kernel(QuantileParams S)
+// a block per triple (groups of kWarpMax < n <= kSmallMax worlds); dynamic shared memory: pow2 of the largest group's
+// size in keys
+__global__ void __launch_bounds__(512) quantile_block_kernel(QuantileParams S, uint32_t first, uint64_t n_groups)
 {
     extern __shared__ unsigned long long keys[];
     __shared__ uint32_t cnt;
-    const uint64_t G = S.n_planes * S.n_entities;
-    for (uint64_t g = blockIdx.x; g < G; g += gridDim.x) {
-        const uint64_t i = g / S.n_entities, e = g % S.n_entities;
-        const uint32_t n = load_sort(S, i, e, keys, &cnt, threadIdx.x, blockDim.x, []() { __syncthreads(); });
-        double *o = out_of(S, i, e);
+    const uint64_t G = n_groups * S.n_planes * S.n_entities;
+    for (uint64_t x = blockIdx.x; x < G; x += gridDim.x) {
+        const Item it = item_of(S, first, x);
+        const uint32_t n = load_sort(S, it.wg, it.i, it.e, keys, &cnt, threadIdx.x, blockDim.x, []() { __syncthreads(); });
+        double *o = out_of(S, it.g, it.i, it.e);
         for (uint32_t l = threadIdx.x; l < S.n_q; l += blockDim.x)
             o[l] = quantile_of(n, S.q[l], [&](uint32_t r) { return keys[r]; });
         __syncthreads();
@@ -208,8 +244,9 @@ __global__ void __launch_bounds__(512) quantile_block_kernel(QuantileParams S)
 
 // ---- large groups ---------------------------------------------------------------------------------------------------
 
-// Thread mapping of the passes (as in stats_kernels.cu): a task is (plane, world chunk, tile of Et entities); thread t
-// takes entity t % Et of the tile and every J-th world of the chunk, so a warp reads consecutive doubles.
+// Thread mapping of the passes (as in stats_kernels.cu): a task is (row, world chunk, tile of Et entities); thread t
+// takes entity t % Et of the tile and every J-th world of the chunk, so a warp reads consecutive doubles.  The chunking
+// of a row is pass_shape over its group's size, the entities and the rows of its slice.
 struct PassShape {
     uint64_t Et, J, T, Wc, C;
 };
@@ -229,22 +266,36 @@ inline PassShape pass_shape(uint64_t n_worlds, uint64_t E, uint64_t n_planes)
     return s;
 }
 
-// pass 0: finite count and min / max key per group
+// the row of chunk k of a slice: the last of rows[0 .. nr) whose first chunk is at most k
+__device__ inline uint64_t row_of_chunk(const QRow *rows, uint64_t nr, uint64_t k)
+{
+    uint64_t lo = 0, hi = nr - 1;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi + 1) / 2;
+        if (rows[mid].k0 <= k) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// pass 0: finite count and min / max key per triple
 __global__ void __launch_bounds__(kPassThreads) quantile_count_kernel(QuantileParams S, Slice sl, PassShape sp, Layout L)
 {
     const uint64_t E = S.n_entities;
     const unsigned t = threadIdx.x, el = t % (unsigned)sp.Et, j = t / (unsigned)sp.Et;
-    const uint64_t n_tasks = sl.ni * sp.C * sp.T;
+    const uint64_t n_tasks = sl.K * sp.T;
     for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
-        const uint64_t tile = task % sp.T, c = (task / sp.T) % sp.C, il = task / (sp.T * sp.C);
+        const uint64_t tile = task % sp.T, k = task / sp.T, il = sl.Cu ? k / sl.Cu : row_of_chunk(L.rows, sl.nr, k);
+        const QRow r = L.rows[il];
+        const uint64_t c = k - r.k0;
         const uint64_t e = tile * sp.Et + el;  // within the slice
         uint32_t n = 0;
         unsigned long long mn = ~0ull, mx = 0;
         const bool live = j < sp.J && e < sl.ne;
         if (live) {
-            const double *p = plane_of(S, sl.i0 + il) + sl.e0 + e;
-            const uint64_t w1 = min((c + 1) * sp.Wc, S.n_worlds);
-            for (uint64_t w = c * sp.Wc + j; w < w1; w += sp.J) {
+            const double *p = plane_of(S, r.i) + sl.e0 + e;
+            const uint64_t w1 = r.o + min((c + 1) * r.Wc, (uint64_t)r.n);
+            for (uint64_t w = r.o + c * r.Wc + j; w < w1; w += sp.J) {
                 const double x = p[w * E];
                 if (finite(x)) {
                     const unsigned long long k = order_key(x);
@@ -280,9 +331,11 @@ __global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantilePar
     const uint64_t E = S.n_entities;
     const bool shared_hist = sl.ne == 1;
     const unsigned t = threadIdx.x, el = t % (unsigned)sp.Et, j = t / (unsigned)sp.Et;
-    const uint64_t n_tasks = sl.ni * sp.C * sp.T;
+    const uint64_t n_tasks = sl.K * sp.T;
     for (uint64_t task = blockIdx.x; task < n_tasks; task += gridDim.x) {
-        const uint64_t tile = task % sp.T, c = (task / sp.T) % sp.C, il = task / (sp.T * sp.C);
+        const uint64_t tile = task % sp.T, k = task / sp.T, il = sl.Cu ? k / sl.Cu : row_of_chunk(L.rows, sl.nr, k);
+        const QRow r = L.rows[il];
+        const uint64_t c = k - r.k0;
         const uint64_t e = tile * sp.Et + el;  // within the slice
         const bool live = j < sp.J && e < sl.ne;
         const uint64_t g = il * sl.ne + (live ? e : 0);
@@ -303,11 +356,11 @@ __global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantilePar
         if (live && G.todo) {
             uint32_t *hist = L.hist + g * kBins;
             unsigned long long *area = L.area + g * kGroupCap;
-            const double *p = plane_of(S, sl.i0 + il) + sl.e0 + e;
-            const uint64_t w1 = min((c + 1) * sp.Wc, S.n_worlds);
+            const double *p = plane_of(S, r.i) + sl.e0 + e;
+            const uint64_t w1 = r.o + min((c + 1) * r.Wc, (uint64_t)r.n);
             const unsigned long long kmin = G.kmin, kmax = G.kmax;
             const uint32_t n_act = G.n_act;
-            for (uint64_t w = c * sp.Wc + j; w < w1; w += sp.J) {
+            for (uint64_t w = r.o + c * r.Wc + j; w < w1; w += sp.J) {
                 const double x = p[w * E];
                 if (!finite(x)) continue;
                 const unsigned long long k = order_key(x);
@@ -478,7 +531,8 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_finish_kernel(QuantileP
         if (t < kSlots && G.slot[t].owner == a) rank_key[t] = keys[G.slot[t].rr];
         __syncthreads();
     }
-    double *out = out_of(S, sl.i0 + blockIdx.x / sl.ne, sl.e0 + blockIdx.x % sl.ne);
+    const QRow &r = L.rows[blockIdx.x / sl.ne];
+    double *out = out_of(S, r.g, r.i, sl.e0 + blockIdx.x % sl.ne);
     for (uint32_t l = t; l < S.n_q; l += blockDim.x) {
         // slot 2l holds rank i (or n - 1), slot 2l + 1 rank i + 1: map the two ranks quantile_of asks for onto them
         uint32_t r0 = 0, r1 = 0;
@@ -490,7 +544,9 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_finish_kernel(QuantileP
 
 constexpr uint64_t kScratchCap = 256ull << 20;  // device scratch of a large-group call, whatever the ring holds
 constexpr uint64_t kGroupBytes = (sizeof(QGroup) + 7) / 8 * 8 + kBins * 4ull + kGroupCap * 8ull;
-constexpr uint64_t kSliceGroups = (kScratchCap - 256) / kGroupBytes;  // about 1350 groups per slice
+constexpr uint64_t kSliceGroups = (kScratchCap - 256) / kGroupBytes;  // about 1350 triples per slice
+constexpr uint64_t kRowBytes = kSliceGroups * sizeof(QRow);           // a slice has at most kSliceGroups rows
+static_assert(256 + kRowBytes + kSliceGroups * kGroupBytes <= kScratchCap, "a slice's scratch must fit in kScratchCap");
 
 inline Layout layout_of(uint64_t G, void *scratch)
 {
@@ -499,6 +555,8 @@ inline Layout layout_of(uint64_t G, void *scratch)
     char *p = (char *)scratch;
     L.reads = (unsigned long long *)p;
     p += 256;
+    L.rows = (const QRow *)p;
+    p += kRowBytes;
     L.grp = (QGroup *)p;
     p += G * ((sizeof(QGroup) + 7) / 8 * 8);
     L.hist = (uint32_t *)p;
@@ -507,9 +565,10 @@ inline Layout layout_of(uint64_t G, void *scratch)
     return L;
 }
 
-__global__ void quantile_init_kernel(Layout L, bool first)
+// first: the reads counter starts at `reads0`, the reads of the small routes' triples
+__global__ void quantile_init_kernel(Layout L, bool first, unsigned long long reads0)
 {
-    if (first && blockIdx.x == 0 && threadIdx.x == 0) *L.reads = 0;
+    if (first && blockIdx.x == 0 && threadIdx.x == 0) *L.reads = reads0;
     for (uint64_t g = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; g < L.G; g += (uint64_t)gridDim.x * blockDim.x) {
         L.grp[g].kmin = ~0ull;
         L.grp[g].kmax = 0;
@@ -521,66 +580,114 @@ __global__ void quantile_init_kernel(Layout L, bool first)
     }
 }
 
-// groups per slice along each axis: whole planes while a plane's entities fit, else entity ranges of one plane
-inline Slice slice_shape(const QuantileParams &S)
+// triples per slice along each axis: whole rows while a row's entities fit, else entity ranges of one row
+inline Slice slice_shape(uint64_t E)
 {
-    if (S.n_entities <= kSliceGroups) return Slice{0, std::max<uint64_t>(1, kSliceGroups / S.n_entities), 0, S.n_entities};
-    return Slice{0, 1, 0, kSliceGroups};
+    if (E <= kSliceGroups) return Slice{0, std::max<uint64_t>(1, kSliceGroups / E), 0, E, 0, 0};
+    return Slice{0, 1, 0, kSliceGroups, 0, 0};
+}
+
+// the groups of each route: order[0 .. warp) warp, [warp, block) block, [block, size) radix
+struct Routes {
+    uint32_t warp, block;
+};
+
+inline Routes routes_of(const std::vector<WorldGroup> &table, const std::vector<uint32_t> &order)
+{
+    Routes r{0, 0};
+    for (uint32_t g : order) {
+        r.warp += table[g].n <= kWarpMax;
+        r.block += table[g].n <= kSmallMax;
+    }
+    return r;
 }
 
 } // namespace
 
-bool quantile_large(const QuantileParams &S) { return S.n_worlds > kSmallMax; }
-
-uint64_t quantile_scratch_bytes(const QuantileParams &S)
+std::vector<uint32_t> quantile_order(const std::vector<WorldGroup> &table)
 {
-    if (S.n_planes == 0 || S.n_worlds == 0 || S.n_entities == 0 || !quantile_large(S)) return 0;
-    const Slice sh = slice_shape(S);
-    const uint64_t G = std::min(sh.ni, S.n_planes) * sh.ne;
-    return 256 + G * kGroupBytes;
+    std::vector<uint32_t> order;
+    for (int route = 0; route < 3; ++route)
+        for (uint32_t g = 0; g < table.size(); ++g) {
+            const uint64_t n = table[g].n;
+            if ((n <= kWarpMax ? 0 : n <= kSmallMax ? 1 : 2) == route) order.push_back(g);
+        }
+    return order;
 }
 
-cudaError_t launch_quantiles(const QuantileParams &S, void *scratch, int *launches, unsigned long long *reads,
-                             cudaStream_t s)
+uint64_t quantile_scratch_bytes(const QuantileParams &S, const std::vector<WorldGroup> &table)
+{
+    uint64_t large = 0;
+    for (const WorldGroup &wg : table) large += wg.n > kSmallMax;
+    if (S.n_planes == 0 || S.n_entities == 0 || large == 0) return 0;
+    const Slice sh = slice_shape(S.n_entities);
+    return 256 + kRowBytes + std::min(sh.nr, large * S.n_planes) * sh.ne * kGroupBytes;
+}
+
+cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGroup> &table,
+                             const std::vector<uint32_t> &order, void *scratch, int *launches,
+                             unsigned long long *reads, cudaStream_t s)
 {
     *launches = 0;
-    if (S.n_planes == 0 || S.n_worlds == 0 || S.n_entities == 0) return cudaSuccess;
-    const uint64_t G = S.n_planes * S.n_entities;
+    if (S.n_planes == 0 || S.n_entities == 0) return cudaSuccess;
+    const uint64_t PE = S.n_planes * S.n_entities;
     const uint64_t cap = 64ull * kNumSMs * 8;
-    if (!quantile_large(S)) {
-        if (S.n_worlds <= kWarpMax) {
-            quantile_warp_kernel<<<(unsigned)std::min((G + 7) / 8, cap), 256, 0, s>>>(S);
-        } else {
-            uint32_t P = 1;
-            while (P < S.n_worlds) P <<= 1;
-            const size_t smem = P * 8ull;
-            cudaError_t e = cudaFuncSetAttribute(quantile_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-            quantile_block_kernel<<<(unsigned)std::min(G, cap), 512, smem, s>>>(S);
-        }
-        *launches = 1;
-        return cudaGetLastError();
+    const Routes rt = routes_of(table, order);
+    cudaError_t e = cudaSuccess;
+    if (rt.warp > 0) {
+        quantile_warp_kernel<<<(unsigned)std::min((rt.warp * PE + 7) / 8, cap), 256, 0, s>>>(S, 0, rt.warp);
+        *launches += 1;
     }
-    cudaError_t e = cudaFuncSetAttribute(quantile_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
+    if (rt.block > rt.warp) {
+        uint64_t n = 0;
+        for (uint32_t k = rt.warp; k < rt.block; ++k) n = std::max(n, table[order[k]].n);
+        uint32_t P = 1;
+        while (P < n) P <<= 1;
+        const size_t smem = P * 8ull;
+        e = cudaFuncSetAttribute(quantile_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+        quantile_block_kernel<<<(unsigned)std::min((rt.block - rt.warp) * PE, cap), 512, smem, s>>>(S, rt.warp,
+                                                                                                    rt.block - rt.warp);
+        *launches += 1;
+    }
+    const uint64_t large = order.size() - rt.block;
+    if (large == 0) return cudaGetLastError();
+    e = cudaFuncSetAttribute(quantile_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
     if (e == cudaSuccess)
         e = cudaFuncSetAttribute(quantile_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
     if (e == cudaSuccess)
         e = cudaFuncSetAttribute(quantile_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBucketCap * 8));
     if (e != cudaSuccess) return e;
-    const Slice sh = slice_shape(S);
+    const Slice sh = slice_shape(S.n_entities);
     const Layout L0 = layout_of(0, scratch);
+    const uint64_t n_rows = large * S.n_planes;
+    std::vector<QRow> rows;
     bool first = true;
-    // The same fixed sequence on every slice (one slice unless the groups need more than kScratchCap of scratch);
-    // each plan clears the histograms it leaves for the next pass, so the scratch needs no clearing in between.
-    for (uint64_t i0 = 0; i0 < S.n_planes; i0 += sh.ni) {
+    // The same fixed sequence on every slice (one slice unless the triples need more than kScratchCap of scratch);
+    // each plan clears the histograms it leaves for the next pass, so the scratch needs no clearing in between.  The
+    // slice's row table is copied ahead of its launches, in stream order, into the scratch the previous slice is done
+    // with.
+    for (uint64_t r0 = 0; r0 < n_rows; r0 += sh.nr) {
         for (uint64_t e0 = 0; e0 < S.n_entities; e0 += sh.ne) {
-            const Slice sl{i0, std::min(sh.ni, S.n_planes - i0), e0, std::min(sh.ne, S.n_entities - e0)};
-            const uint64_t Gs = sl.ni * sl.ne;
+            Slice sl{r0, std::min(sh.nr, n_rows - r0), e0, std::min(sh.ne, S.n_entities - e0), 0, 0};
+            rows.clear();
+            for (uint64_t r = r0; r < r0 + sl.nr; ++r) {
+                const uint32_t g = order[rt.block + r / S.n_planes];
+                const WorldGroup &wg = table[g];
+                const PassShape sp = pass_shape(wg.n, sl.ne, sl.nr);
+                rows.push_back(QRow{(uint32_t)wg.o, (uint32_t)wg.n, (uint32_t)sp.Wc, (uint32_t)sp.C, (uint32_t)sl.K, g,
+                                    (uint32_t)(r % S.n_planes), 0});
+                sl.K += sp.C;
+                sl.Cu = r == r0 || sl.Cu == sp.C ? sp.C : 0;
+            }
+            const uint64_t Gs = sl.nr * sl.ne;
             const Layout L = layout_of(Gs, scratch);
-            const PassShape sp = pass_shape(S.n_worlds, sl.ne, sl.ni);
-            const unsigned grid = (unsigned)std::min(sl.ni * sp.C * sp.T, cap);
+            const PassShape sp = pass_shape(0, sl.ne, sl.nr);  // the tiles (Et, J, T): the slice's entities alone
+            const unsigned grid = (unsigned)std::min(sl.K * sp.T, cap);
             const size_t hist_smem = sl.ne == 1 ? kBins * 4ull : 0;
-            quantile_init_kernel<<<(unsigned)std::min((Gs + 255) / 256, cap), 256, 0, s>>>(L, first);
+            e = cudaMemcpyAsync((void *)L.rows, rows.data(), rows.size() * sizeof(QRow), cudaMemcpyHostToDevice, s);
+            if (e != cudaSuccess) return e;
+            quantile_init_kernel<<<(unsigned)std::min((Gs + 255) / 256, cap), 256, 0, s>>>(L, first, rt.block * PE);
             quantile_count_kernel<<<grid, kPassThreads, 0, s>>>(S, sl, sp, L);
             quantile_plan_kernel<<<(unsigned)Gs, kPlanThreads, kBins * 4, s>>>(S, L, 0);
             *launches += 3;

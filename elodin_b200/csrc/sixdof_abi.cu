@@ -535,7 +535,7 @@ void b200_host_free(void *p)
 // device allocation.  On failure the caller destroys the handle, which frees whatever was allocated by then.
 static int init_handle(b200_sixdof *h, const b200_sixdof_desc *d);
 
-static int upload_group_table(b200_sixdof *h, const std::vector<WorldGroup> &t, WorldGroup **dev);
+static int build_group_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped);
 
 int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
 {
@@ -574,10 +574,8 @@ int b200_sixdof_create(const b200_sixdof_desc *d, b200_sixdof **out)
     h->sim_time_step = d->sim_time_step;
 
     int rc = init_handle(h, d);
-    if (!rc) {  // the ungrouped statistics' one-group table {n_worlds}, on the device for the handle's life
-        h->all_table = world_group_table(&h->desc.n_worlds, 1, h->desc.n_entities);
-        rc = upload_group_table(h, h->all_table, &h->all_table_dev);
-    }
+    if (!rc)  // the ungrouped reductions' one-group tables {n_worlds}, on the device for the handle's life
+        rc = build_group_tables(h, &h->desc.n_worlds, 1, false);
     if (rc) { b200_sixdof_destroy(h); return rc; }
     *out = h;
     return B200_OK;
@@ -731,8 +729,9 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->traj) cudaFree(h->traj);
     if (h->sum_ext) cudaFree(h->sum_ext);
     if (h->sum_thr) cudaFree(h->sum_thr);
-    if (h->all_table_dev) cudaFree(h->all_table_dev);
-    if (h->group_table_dev) cudaFree(h->group_table_dev);
+    for (void *t : {(void *)h->all_table_dev, (void *)h->group_table_dev, (void *)h->all_cov_dev, (void *)h->group_cov_dev,
+                    (void *)h->all_order_dev, (void *)h->group_order_dev})
+        if (t) cudaFree(t);
     for (auto &e : h->chunk_in) if (e) cudaEventDestroy(e);
     for (auto &e : h->chunk_out) if (e) cudaEventDestroy(e);
     if (h->host_pack) cudaFreeHost(h->host_pack);
@@ -1209,17 +1208,37 @@ static StatsParams state_planes(const b200_sixdof *h)
 // The reduction entries below run over one of these; `what` names it in error messages.
 using PlaneSource = StatsParams (*)(const b200_sixdof *);
 
-// A statistics group table into device memory (*dev, replaced): the stream is drained first, so that no reduction still
+// A group table of `bytes` into device memory (*dev, replaced): the stream is drained first, so that no reduction still
 // in flight reads the table it replaces.
-static int upload_group_table(b200_sixdof *h, const std::vector<WorldGroup> &t, WorldGroup **dev)
+static int upload_group_table(b200_sixdof *h, const void *t, uint64_t bytes, void **dev)
 {
     CU(h, cudaStreamSynchronize(h->stream));
     if (*dev) CU(h, cudaFree(*dev));
     *dev = nullptr;
-    if (t.empty()) return B200_OK;
-    CU(h, cudaMalloc(dev, t.size() * sizeof(WorldGroup)));
-    CU(h, cudaMemcpy(*dev, t.data(), t.size() * sizeof(WorldGroup), cudaMemcpyHostToDevice));
+    if (bytes == 0) return B200_OK;
+    CU(h, cudaMalloc(dev, bytes));
+    CU(h, cudaMemcpy(*dev, t, bytes, cudaMemcpyHostToDevice));
     return B200_OK;
+}
+
+// The tables of consecutive groups of sizes[0 .. n_groups), each with its device copy: the statistics' group table, the
+// quantiles' route order over it and the covariance's group table; the grouped entries' tables, else the all-worlds ones.
+static int build_group_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped)
+{
+    std::vector<WorldGroup> &stats = grouped ? h->group_table : h->all_table, &cov = grouped ? h->group_cov : h->all_cov;
+    std::vector<uint32_t> &order = grouped ? h->group_order : h->all_order;
+    stats = world_group_table(sizes, n_groups, h->desc.n_entities);
+    cov = cov_group_table(sizes, n_groups, h->desc.n_entities);
+    order = quantile_order(stats);
+    int rc = upload_group_table(h, stats.data(), stats.size() * sizeof(WorldGroup),
+                                (void **)(grouped ? &h->group_table_dev : &h->all_table_dev));
+    if (!rc)
+        rc = upload_group_table(h, cov.data(), cov.size() * sizeof(WorldGroup),
+                                (void **)(grouped ? &h->group_cov_dev : &h->all_cov_dev));
+    if (!rc)
+        rc = upload_group_table(h, order.data(), order.size() * sizeof(uint32_t),
+                                (void **)(grouped ? &h->group_order_dev : &h->all_order_dev));
+    return rc;
 }
 
 int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups)
@@ -1240,8 +1259,7 @@ int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t
                     (unsigned long long)h->desc.n_worlds);
     CU(h, cudaSetDevice(h->device));
     h->group_sizes.assign(sizes, sizes + n_groups);
-    h->group_table = world_group_table(sizes, n_groups, h->desc.n_entities);
-    return upload_group_table(h, h->group_table, &h->group_table_dev);
+    return build_group_tables(h, sizes, n_groups, true);
 }
 
 uint32_t b200_sixdof_world_groups(const b200_sixdof *h) { return h ? (uint32_t)h->group_sizes.size() : 0; }
@@ -1299,12 +1317,13 @@ int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
     return run_world_stats(h, state_planes, true, dst, bytes, "state");
 }
 
-// Quantiles of the planes over the worlds (quantile_kernels.cu) into dst: the handle's status checked, then the levels,
-// then `bytes`.
-static int run_quantiles(b200_sixdof *h, PlaneSource source, const double *q, uint32_t n_q, void *dst, uint64_t bytes,
-                         const char *what)
+// Quantiles of the planes over the worlds, per group when `grouped` (quantile_kernels.cu), into dst: the groups checked,
+// then the handle's status, then the levels, then `bytes`.
+static int run_quantiles(b200_sixdof *h, PlaneSource source, bool grouped, const double *q, uint32_t n_q, void *dst,
+                         uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     QuantileParams S{};
     static_cast<StatsParams &>(S) = source(h);
@@ -1314,40 +1333,57 @@ static int run_quantiles(b200_sixdof *h, PlaneSource source, const double *q, ui
     if (!q) return fail(B200_ERR_INVALID_ARGUMENT, "null quantile levels");
     for (uint32_t l = 0; l < n_q; ++l)
         if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
-    const uint64_t want = S.n_planes * S.n_entities * n_q * 8ull;
+    const std::vector<WorldGroup> &table = grouped ? h->group_table : h->all_table;
+    const std::vector<uint32_t> &order = grouped ? h->group_order : h->all_order;
+    const uint64_t G = reduction_groups(h, grouped).size();
+    const uint64_t want = S.n_planes * G * S.n_entities * n_q * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s quantiles are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
     S.n_q = n_q;
     for (uint32_t l = 0; l < n_q; ++l) S.q[l] = q[l];
-    const uint64_t groups = S.n_planes * S.n_entities;
-    h->quantile_read_sum = groups;  // the small-group route reads every group once
-    int rc = run_world_reduction(h, quantile_scratch_bytes(S), dst, bytes, [&](double *out, void *scratch, int *n) {
+    S.groups = grouped ? h->group_table_dev : h->all_table_dev;
+    S.order = grouped ? h->group_order_dev : h->all_order_dev;
+    S.n_groups = G;
+    const uint64_t triples = S.n_planes * G * S.n_entities;
+    h->quantile_read_sum = triples;  // the small-group routes read every triple once
+    int rc = run_world_reduction(h, quantile_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
-        return launch_quantiles(S, scratch, n, &h->quantile_read_sum, h->stream);
+        return launch_quantiles(S, table, order, scratch, n, &h->quantile_read_sum, h->stream);
     });
-    h->quantile_reads = rc == B200_OK && bytes && groups ? (double)h->quantile_read_sum / (double)groups : 0.0;
+    h->quantile_reads = rc == B200_OK && bytes && triples ? (double)h->quantile_read_sum / (double)triples : 0.0;
     return rc;
 }
 
 int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, trajectory_planes, q, n_q, dst, bytes, "trajectory");
+    return run_quantiles(h, trajectory_planes, false, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, state_planes, q, n_q, dst, bytes, "state");
+    return run_quantiles(h, state_planes, false, q, n_q, dst, bytes, "state");
+}
+
+int b200_sixdof_trajectory_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    return run_quantiles(h, trajectory_planes, true, q, n_q, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    return run_quantiles(h, state_planes, true, q, n_q, dst, bytes, "state");
 }
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
-// Covariance of the selection `planes` (each < width) of every sample over the worlds (cov_kernels.cu) into dst: the
-// handle's status checked, then the selection, then `bytes`.
-static int run_covariance(b200_sixdof *h, PlaneSource source, uint32_t width, const uint32_t *planes, uint32_t n_p,
-                          void *dst, uint64_t bytes, const char *what)
+// Covariance of the selection `planes` (each < width) of every sample over the worlds, per group when `grouped`
+// (cov_kernels.cu), into dst: the groups checked, then the handle's status, then the selection, then `bytes`.
+static int run_covariance(b200_sixdof *h, PlaneSource source, bool grouped, uint32_t width, const uint32_t *planes,
+                          uint32_t n_p, void *dst, uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     CovParams S{};
     static_cast<StatsParams &>(S) = source(h);
@@ -1363,27 +1399,43 @@ static int run_covariance(b200_sixdof *h, PlaneSource source, uint32_t width, co
         seen |= 1u << planes[k];
     }
     const uint64_t n_s = S.planes_per_sample ? S.n_planes / S.planes_per_sample : 0;
-    const uint64_t want = n_s * S.n_entities * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
+    const uint64_t G = reduction_groups(h, grouped).size();
+    const uint64_t want = n_s * G * S.n_entities * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s covariance is %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
     S.n_p = n_p;
     for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
-    return run_world_reduction(h, cov_scratch_bytes(S), dst, bytes, [&](double *out, void *scratch, int *n) {
+    const std::vector<WorldGroup> &table = grouped ? h->group_cov : h->all_cov;
+    const WorldGroup *groups = grouped ? h->group_cov_dev : h->all_cov_dev;
+    return run_world_reduction(h, cov_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
-        return launch_covariance(S, scratch, n, h->stream);
+        return launch_covariance(S, groups, table, scratch, n, h->stream);
     });
 }
 
 // The ring's width, not its planes per sample: a handle without a ring refuses every plane.
 int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, trajectory_planes, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes, "trajectory");
+    return run_covariance(h, trajectory_planes, false, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes,
+                          "trajectory");
 }
 
 int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, state_planes, 25, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, state_planes, false, 25, planes, n_p, dst, bytes, "state");
+}
+
+int b200_sixdof_trajectory_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
+                                            uint64_t bytes)
+{
+    return run_covariance(h, trajectory_planes, true, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes,
+                          "trajectory");
+}
+
+int b200_sixdof_state_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_covariance(h, state_planes, true, 25, planes, n_p, dst, bytes, "state");
 }
 
 // np.linspace(lo, hi, n + 1) into e[0 .. n]: i * step + lo, the product rounded before the sum (never an fma), e[n] = hi.

@@ -61,9 +61,13 @@ struct b200_sixdof {
     double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
     // statistics group tables (stats_kernels.cu): all worlds as one group (built at creation) and the groups of
-    // b200_sixdof_set_world_groups (sizes empty = none set), each with its device copy
-    std::vector<b200::WorldGroup> all_table, group_table;
-    b200::WorldGroup *all_table_dev = nullptr, *group_table_dev = nullptr;
+    // b200_sixdof_set_world_groups (sizes empty = none set), each with its device copy; the quantiles read the same
+    // tables' worlds, in the route order of quantile_order (quantile_kernels.cu), and the covariance has its own
+    // chunking (cov_group_table, cov_kernels.cu), both built at the same two points
+    std::vector<b200::WorldGroup> all_table, group_table, all_cov, group_cov;
+    b200::WorldGroup *all_table_dev = nullptr, *group_table_dev = nullptr, *all_cov_dev = nullptr, *group_cov_dev = nullptr;
+    std::vector<uint32_t> all_order, group_order;
+    uint32_t *all_order_dev = nullptr, *group_order_dev = nullptr;
     std::vector<uint64_t> group_sizes;
     // trajectory
     double *traj = nullptr;

@@ -217,19 +217,29 @@ uint64_t world_stats_scratch_doubles(const StatsParams &S, const std::vector<Wor
 cudaError_t launch_world_stats(const StatsParams &S, const WorldGroup *groups, const std::vector<WorldGroup> &table,
                                double *scratch, int *launches, cudaStream_t s);
 
-// Ensemble quantiles over the world axis (quantile_kernels.cu): the planes of a StatsParams, and n_q levels.  Group
-// (plane i, entity e) goes to out[((i / W) * n_entities + e) * W + i % W][n_q].
+// Ensemble quantiles over the world axis (quantile_kernels.cu): the planes of a StatsParams, n_q levels and the world
+// groups of a group table (only o and n are read).  Triple (group g of G = n_groups, plane i, entity e) goes to
+// out[(((i / W) * G + g) * n_entities + e) * W + i % W][n_q].
 struct QuantileParams : StatsParams {
     uint32_t n_q;
     double q[B200_MAX_QUANTILES];
+    const WorldGroup *groups;  // the group table, in device memory
+    const uint32_t *order;     // quantile_order(table), in device memory
+    uint64_t n_groups;
 };
-// bytes of device scratch the call needs: 0 below the large-group size (one pass, no scratch), else at most 256 MiB
-uint64_t quantile_scratch_bytes(const QuantileParams &S);
-// a fixed launch sequence per slice of groups (written to *launches); `scratch` holds quantile_scratch_bytes(S).  On
-// the large-group route *reads (host memory) receives, once the stream reaches it, the reads of the planes summed
-// over the groups; it is left alone on the small-group route (one read).
-cudaError_t launch_quantiles(const QuantileParams &S, void *scratch, int *launches, unsigned long long *reads,
-                             cudaStream_t s);
+// the groups of a table listed by route, each route in table order: at most 256 worlds (the warp route, empty groups
+// included), then at most 8192 (the block route), then the rest (the radix select)
+std::vector<uint32_t> quantile_order(const std::vector<WorldGroup> &table);
+// bytes of device scratch the call over the groups of `table` needs: 0 without a group above 8192 worlds (one pass,
+// no scratch), else at most 256 MiB
+uint64_t quantile_scratch_bytes(const QuantileParams &S, const std::vector<WorldGroup> &table);
+// one launch per small route that has groups, and a fixed launch sequence per slice of the large groups' triples
+// (written to *launches); `scratch` holds quantile_scratch_bytes(S, table), `order` is quantile_order(table).  With a
+// large group *reads (host memory) receives, once the stream reaches it, the reads of the planes summed over every
+// triple; it is left alone otherwise (one read per triple).
+cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGroup> &table,
+                             const std::vector<uint32_t> &order, void *scratch, int *launches,
+                             unsigned long long *reads, cudaStream_t s);
 
 // Ensemble covariance over the world axis (cov_kernels.cu).  One entry (a, b) of a group over a set of worlds: the
 // count n, the means of planes a and b, and the co-moment m = sum (x_a - mean_a)(x_b - mean_b); while n = 0 the other
@@ -253,15 +263,23 @@ __host__ __device__ inline void cov_merge(CovEntry &x, const CovEntry &y)
 }
 
 // The samples of a StatsParams (n_planes / planes_per_sample of them) and a selection of n_p distinct planes of a
-// sample.  Group (sample s, entity e) goes to out[(s * n_entities + e) * (1 + n_p + n_p^2)]: n, mean[n_p], M[n_p][n_p].
+// sample.  A record is n, mean[n_p], M[n_p][n_p] over the worlds of one (sample, world group, entity).
 struct CovParams : StatsParams {
     uint32_t n_p;
     uint32_t planes[B200_MAX_COV_PLANES];
 };
-// bytes of device scratch the call needs (0: one chunk, no scratch); at most 256 MiB
-uint64_t cov_scratch_bytes(const CovParams &S);
-// one chunk launch, and a merge launch when the worlds take more than one chunk, per slice of groups (*launches)
-cudaError_t launch_covariance(const CovParams &S, void *scratch, int *launches, cudaStream_t s);
+// The covariance table of consecutive groups of sizes[0 .. n_groups): cov_chunks per group (an empty group has one chunk
+// of no worlds), k0 = the chunks of the groups before it.  It depends on the sizes and n_entities alone; the ungrouped
+// covariance is the one-group table {n_worlds}.
+std::vector<WorldGroup> cov_group_table(const uint64_t *sizes, uint64_t n_groups, uint64_t n_entities);
+// bytes of device scratch the call over the groups of `table` needs (0: one chunk per group, no scratch); at most
+// 256 MiB
+uint64_t cov_scratch_bytes(const CovParams &S, const std::vector<WorldGroup> &table);
+// One chunk launch, and a merge launch where a group of the slice takes more than one chunk, per slice of groups and
+// samples (*launches); `groups` is `table` in device memory.  Sample s, group g of G = table.size(), entity e goes to
+// out[((s * G + g) * n_entities + e) * (1 + n_p + n_p^2)].
+cudaError_t launch_covariance(const CovParams &S, const WorldGroup *groups, const std::vector<WorldGroup> &table,
+                              void *scratch, int *launches, cudaStream_t s);
 
 // Ensemble histograms over the world axis (hist_kernels.cu): the samples of a StatsParams and n_specs specs, each one
 // entity and one or two planes of a sample.  Sample s, spec k goes to out[s * record_len + spec[k].rec_off ..]: a 1D

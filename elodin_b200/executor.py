@@ -372,6 +372,33 @@ class B200Exec:
         args, row = self._hist_specs(specs)
         return self._reduce("group_histograms", False, args, (self.world_groups, row))
 
+    def trajectory_group_quantiles(self, q) -> np.ndarray:
+        """trajectory_quantiles(q) per group: [samples, G, n_entities, width, n_q]; group g's quantiles have the bits of
+        trajectory_quantiles(q) on a batch of exactly its worlds (NaN for an empty group).  Like the ungrouped tables,
+        they do not merge across the ranks of a world-sharded campaign: each rank gets its own."""
+        lv = self._levels(q)
+        n, E, W = self._planes(ring=True)
+        return self._reduce("group_quantiles", True, lv, (n, self.world_groups, E, W, lv[1]))
+
+    def state_group_quantiles(self, q) -> np.ndarray:
+        """state_quantiles(q) per group: [G, n_entities, 25, n_q]."""
+        lv = self._levels(q)
+        return self._reduce("group_quantiles", False, lv, (self.world_groups,) + self._planes(ring=False) + (lv[1],))
+
+    def trajectory_group_covariance(self, planes) -> np.ndarray:
+        """trajectory_covariance(planes) per group: [samples, G, n_entities, 1 + p + p*p]; group g's records have the
+        bits of trajectory_covariance(planes) on a batch of exactly its worlds (n = 0 and NaN for an empty group).
+        The tables of a world-sharded campaign, with groups cut by sharding.shard_groups, merge with
+        merge_covariance."""
+        sel = self._selection(planes)
+        n, E, _ = self._planes(ring=True)
+        return self._reduce("group_covariance", True, sel, (n, self.world_groups, E, 1 + sel[1] + sel[1] ** 2))
+
+    def state_group_covariance(self, planes) -> np.ndarray:
+        """state_covariance(planes) per group: [G, n_entities, 1 + p + p*p]."""
+        sel = self._selection(planes)
+        return self._reduce("group_covariance", False, sel, (self.world_groups, self.n_entities, 1 + sel[1] + sel[1] ** 2))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =

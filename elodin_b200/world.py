@@ -451,9 +451,11 @@ class World:
         covariance=[("world_pos", (4, 5, 6)), ("world_vel", (3, 4, 5))], at most 25 distinct planes; `histograms` (1 to
         8 `Histogram`s) the bin counts over the worlds of one or two components for every row (`Exec.histogram`).
         `groups` (1 to 1024 world counts summing to n_worlds) splits the worlds into consecutive groups, e.g. the sweep
-        points of a plan ordered by `monte_carlo.plan_groups`, and also records the statistics and histograms of every
-        group (`Exec.ensemble(pair, groups=True)`, `Exec.histogram(i, groups=True)`); quantiles and covariance stay over
-        all worlds."""
+        points of a plan ordered by `monte_carlo.plan_groups`, and also records the statistics of every group
+        (`Exec.ensemble(pair, groups=True)`) and, where `histograms`, `quantiles` or `covariance` is given, the
+        histograms, quantiles and covariance of every group (`Exec.histogram(i, groups=True)`,
+        `Exec.quantiles(pair, groups=True)`, `Exec.covariance(entity, groups=True)`), beside the all-worlds tables.
+        Group g's tables equal those of an Exec over exactly its worlds."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -798,8 +800,9 @@ class Exec:
             self._ens_args["histograms"] = (specs,)
         if self.groups is not None:  # the same tables per group of worlds
             self._ens_args["group_stats"] = ()
-            if histograms is not None:
-                self._ens_args["group_histograms"] = self._ens_args["histograms"]
+            for kind in ("histograms", "quantiles", "covariance"):
+                if kind in self._ens_args:
+                    self._ens_args[f"group_{kind}"] = self._ens_args[kind]
         self._ens_rows: Dict[str, List[np.ndarray]] = {kind: [] for kind in self._ens_args}
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
@@ -1179,27 +1182,40 @@ class Exec:
         return {"count": count, "mean": np.ascontiguousarray(t[..., 1]), "std": std,
                 "min": np.ascontiguousarray(t[..., 3]), "max": np.ascontiguousarray(t[..., 4])}
 
-    def quantiles(self, pair: str) -> np.ndarray:
+    def quantiles(self, pair: str, groups: bool = False) -> np.ndarray:
         """`exec.quantiles("rocket.world_pos")` -> [rows, n_q, width] f64: for every telemetry row (row 0 = the initial
         state) numpy's linear quantile over the worlds whose value is finite, at each level of World.build(...,
         quantiles=...) in the order given -- the layout of np.quantile(rows_k, q, axis=0) stacked over rows.  NaN where no
-        world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates."""
+        world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates.
+        With groups=True (World.build(..., groups=[...])) -> [rows, G, n_q, width], over the worlds of each group.
+        Quantile tables do not merge across the ranks of a world-sharded campaign: each rank has its own."""
+        if groups:
+            t = self._ensemble_rows("group_quantiles", pair, "ensemble quantiles", "quantiles(groups=True)",
+                                    ", quantiles=[...], groups=[...]", grouped=True)  # [rows, G, width, n_q]
+            return np.ascontiguousarray(t.transpose(0, 1, 3, 2))
         t = self._ensemble_rows("quantiles", pair, "ensemble quantiles", "quantiles()", ", quantiles=[...]")  # [rows, width, n_q]
         return np.ascontiguousarray(t.transpose(0, 2, 1))
 
-    def covariance(self, entity: str) -> Dict[str, object]:
+    def covariance(self, entity: str, groups: bool = False) -> Dict[str, object]:
         """`exec.covariance("rocket")` -> {"count" [rows], "mean" [rows, p], "cov" [rows, p, p], "planes" [p] labels such
         as "world_pos[4]"}: for every telemetry row (row 0 = the initial state) the covariance over the worlds of the
         selection of World.build(..., covariance=...), in its order.  Only worlds whose p selected values are all
         finite count (listwise deletion, unlike Exec.ensemble, which counts per component); cov = co-moments / count
-        (numpy's ddof=0, as Exec.ensemble's std), exactly symmetric, NaN where count = 0."""
-        t = self._ensemble_rows("covariance", f"{entity}.world_pos", "ensemble covariance", "covariance()",
-                                ", covariance=[...]", per_plane=False)  # [rows, 1 + p + p*p]
+        (numpy's ddof=0, as Exec.ensemble's std), exactly symmetric, NaN where count = 0.  With groups=True
+        (World.build(..., groups=[...])) a group axis follows the row axis: count [rows, G], mean [rows, G, p], cov
+        [rows, G, p, p], over the worlds of each group."""
+        if groups:
+            t = self._ensemble_rows("group_covariance", f"{entity}.world_pos", "ensemble covariance",
+                                    "covariance(groups=True)", ", covariance=[...], groups=[...]", per_plane=False,
+                                    grouped=True)  # [rows, G, 1 + p + p*p]
+        else:
+            t = self._ensemble_rows("covariance", f"{entity}.world_pos", "ensemble covariance", "covariance()",
+                                    ", covariance=[...]", per_plane=False)  # [rows, 1 + p + p*p]
         p = len(self._cov_labels)
-        count = np.ascontiguousarray(t[:, 0])
+        count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
-            cov = t[:, 1 + p:].reshape(-1, p, p) / count[:, None, None]
-        return {"count": count, "mean": np.ascontiguousarray(t[:, 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
+            cov = t[..., 1 + p:].reshape(*t.shape[:-1], p, p) / count[..., None, None]
+        return {"count": count, "mean": np.ascontiguousarray(t[..., 1:1 + p]), "cov": cov, "planes": list(self._cov_labels)}
 
     def histogram(self, i: int, groups: bool = False) -> Dict[str, object]:
         """`exec.histogram(i)` -> for histogram i of World.build(..., histograms=[...]) and every telemetry row (row 0 =

@@ -326,7 +326,8 @@ int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, d
 int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
 /* the current world_pos, world_vel, world_accel, force planes: dst = [n_entities][25][n_q] f64 */
 int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
-/* reads of the reduced planes the last quantile call made, averaged over its groups (1 on the shared-memory route) */
+/* reads of the reduced planes the last quantile call (grouped or not) made, averaged over its (world group, plane,
+ * entity) triples (1 on the shared-memory routes) */
 double b200_sixdof_quantile_reads(const b200_sixdof *h);
 
 /* ---- ensemble covariance: the joint spread of chosen components over the worlds, on the device.  A selection is
@@ -410,7 +411,17 @@ int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, ui
  * B200_ERR_INVALID_ARGUMENT while no groups are set; they run on the handle's stream, return once dst (host or device)
  * is filled and count their launches in timings.kernel_launches (statistics: one or two per slice of groups and planes,
  * slices keeping the chunk partials in the staging buffer at most 256 MiB; histograms: one memset and one launch).
- * Grouped quantiles and covariance do not exist: those tables are over all worlds. ---- */
+ * Quantiles: a result is two order statistics and a fixed lerp, so any route gives a group the bits of its own handle.
+ * Each group takes the route of its own size: up to 256 worlds (empty groups included) the warp sort, up to 8192 the
+ * block sort, above that the radix select.  A call launches once per sort route that has groups, plus 18 launches per
+ * slice of the large groups' (group, plane, entity) triples (at most about 1350 triples a slice, whole (group, plane)
+ * rows or entity ranges of one row); b200_sixdof_quantile_reads averages the reads over every (group, plane, entity).
+ * An empty group gives NaN at every level.  Grouped quantile tables do not merge across ranks, as the ungrouped ones.
+ * Covariance: group g is chunked as a batch of sizes[g] worlds would be, and an empty group is one chunk of no worlds,
+ * with n = 0 and NaN after it.  A call launches one chunk launch, plus a merge launch where a group of the slice has
+ * more than one chunk, per slice of groups and samples, slices keeping the chunk partials at most 256 MiB.  Grouped
+ * covariance tables of a world-sharded campaign, with each rank's groups cut to its worlds, merge with
+ * b200_covariance_merge (a group a rank does not hold has n = 0, the identity of the merge). ---- */
 #define B200_MAX_WORLD_GROUPS 1024u
 /* sizes[0 .. n_groups): consecutive world counts, each >= 0, summing to n_worlds; n_groups = 0 clears the setting.
  * B200_ERR_INVALID_ARGUMENT for a null handle, more than B200_MAX_WORLD_GROUPS groups, null sizes with n_groups > 0 or
@@ -429,6 +440,15 @@ int b200_sixdof_trajectory_group_histograms(b200_sixdof *h, const b200_histogram
 /* the current state: dst = [G][sum of the record lengths] f64 */
 int b200_sixdof_state_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                        uint64_t bytes);
+/* the ring's samples: dst = [trajectory_len][G][n_entities][trajectory_width][n_q] f64 */
+int b200_sixdof_trajectory_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* the current state: dst = [G][n_entities][25][n_q] f64 */
+int b200_sixdof_state_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* the ring's samples: dst = [trajectory_len][G][n_entities][1 + n_p + n_p^2] f64 */
+int b200_sixdof_trajectory_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
+                                            uint64_t bytes);
+/* the current state: dst = [G][n_entities][1 + n_p + n_p^2] f64 */
+int b200_sixdof_state_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
 
 /* ---- run summaries: the time axis reduced on the device, per world, so that a Monte-Carlo campaign keeps each run's
  * extrema and threshold events without moving its trajectory to the host.  A row is one recorded state in the

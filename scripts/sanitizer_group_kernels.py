@@ -1,5 +1,6 @@
 """compute-sanitizer target for the grouped ensemble entries (world_stats_chunk_kernel / world_stats_merge_kernel and
-hist_kernel driven by a world-group table):
+hist_kernel driven by a world-group table; the quantile kernels and cov_chunk_kernel / cov_merge_kernel driven by the
+quantiles' route order and the covariance group table):
 
     compute-sanitizer --tool memcheck python scripts/sanitizer_group_kernels.py
 
@@ -9,7 +10,11 @@ run in two slices of planes (E = 300, a 512-world group of 64 chunks, 16 samples
 arithmetic an out-of-bounds access would come from: the binary search over the table, the empty groups (one empty
 statistics chunk, no histogram chunk), the group table placed after the edges in the staging buffer and the per-slice
 scratch offsets.  Each case also checks what a wrong index would change: group counts against numpy, and the sum of the
-grouped histograms against the ungrouped table.  Small sizes: the tool slows every kernel by 10-50x."""
+grouped histograms against the ungrouped table.  The grouped quantiles and covariance: empty leading, middle and
+trailing groups in a call that takes the warp, block and radix routes at once; a radix call whose (group, plane) rows
+run in two slices (E = 30, 45 rows a slice); and a covariance call whose groups run in two slices of partials (100
+groups of 528 chunks at p = 25).  The quantiles are checked against np.quantile per group, the covariance counts
+against the complete worlds of each group.  Small sizes: the tool slows every kernel by 10-50x."""
 import os
 import sys
 
@@ -47,7 +52,68 @@ def run(sizes, E, samples):
 run([0, 5, 0, 700, 1, 0], 3, 3)          # empty first / middle / last groups; 700 worlds = 2 chunks at E = 3
 run([0, 512, 3, 0], 300, 16)             # 64 chunks at E = 300; 400 planes of partials in two slices
 run([1] * 40 + [0] * 20 + [5000], 1, 2)  # many one-chunk groups, a run of empty ones, one group of 3 chunks
+
+
+def state(M, E, seed):
+    rng = np.random.default_rng(seed)
+    x = rng.normal(size=(M, E, 25)) + np.arange(M)[:, None, None] * 1e-3
+    x[rng.random(x.shape) < 0.02] = np.nan
+    return x
+
+
+def handle(x):
+    M, E, _ = x.shape
+    ine = np.broadcast_to(np.array([1.0, 1.0, 1.0, 0.0, 0.0, 0.0, 1.0]), (M, E, 7))
+    ex = el.B200Exec(E, M, 0.01, None, [], "rk4", "exact", trajectory_every=1, trajectory_capacity=1, trajectory_full=True)
+    ex.set_state(x[..., :7], x[..., 7:13], ine, accel=x[..., 13:19], force=x[..., 19:25])
+    return ex
+
+
+Q = (0.0, 0.01, 0.5, 0.99, 1.0)
+SEL = (4, 5, 6, 10, 11, 12)
+
+
+def run_quantiles(sizes, E, planes=range(25)):
+    x = state(sum(sizes), E, sum(sizes) + E)
+    with handle(x) as ex:
+        ex.set_world_groups(sizes)
+        st = ex.state_group_quantiles(Q)
+        ex.step(1)
+        tr = ex.trajectory_group_quantiles(Q)
+        traj = ex.trajectory()
+    o = np.concatenate([[0], np.cumsum(sizes)])
+    for g in range(len(sizes)):
+        for e in range(E):
+            for i in planes:
+                for got, v in ((st[g, e, i], x[o[g]:o[g + 1], e, i]), (tr[0, g, e, i], traj[0, o[g]:o[g + 1], e, i])):
+                    f = v[np.isfinite(v)]
+                    want = np.quantile(f, Q) if f.size else np.full(len(Q), np.nan)
+                    assert np.array_equal(got, want, equal_nan=True), (g, e, i)
+
+
+def run_covariance(sizes, E, p_planes=SEL):
+    x = state(sum(sizes), E, sum(sizes) + 2 * E)
+    with handle(x) as ex:
+        ex.set_world_groups(sizes)
+        st = ex.state_group_covariance(p_planes)
+        ex.step(1)
+        tr = ex.trajectory_group_covariance(p_planes)
+        traj = ex.trajectory()
+    o = np.concatenate([[0], np.cumsum(sizes)])
+    for g in range(len(sizes)):
+        ok = np.isfinite(x[o[g]:o[g + 1]][..., list(p_planes)]).all(-1).sum(0)
+        assert np.array_equal(st[g, :, 0], ok), g
+        ok = np.isfinite(traj[0, o[g]:o[g + 1]][..., list(p_planes)]).all(-1).sum(0)
+        assert np.array_equal(tr[0, g, :, 0], ok), g
+
+
+run_quantiles([0, 5, 0, 300, 9000, 0], 2)      # empty first / middle / last groups; warp, block and radix routes
+run_quantiles([3, 8193, 8200], 30, (0, 24))    # 50 (group, plane) rows of the radix groups: two slices of 45 rows
+run_covariance([0, 5, 0, 700, 64, 65, 0], 3)   # empty first / middle / last groups, one- and several-chunk groups
+run_covariance([528 * 64] * 100, 1, tuple(range(25)))  # 2.75 MB of partials per group: slices of 97 and 3 groups
 with el.B200Exec(0, 4, 0.01, None, [], "rk4", "exact") as ex:  # a world without entities takes groups too
     ex.set_world_groups([4, 0])
     assert ex.state_group_stats().shape == (2, 0, 25, 5)
+    assert ex.state_group_quantiles(Q).shape == (2, 0, 25, len(Q))
+    assert ex.state_group_covariance(SEL).shape == (2, 0, 1 + 6 + 36)
 print("done")
