@@ -69,6 +69,7 @@ SYMBOLS = [
     "b200_sixdof_state_group_stats", "b200_sixdof_trajectory_group_histograms", "b200_sixdof_state_group_histograms",
     "b200_sixdof_trajectory_group_quantiles", "b200_sixdof_state_group_quantiles",
     "b200_sixdof_trajectory_group_covariance", "b200_sixdof_state_group_covariance",
+    "b200_sixdof_trajectory_download_worlds", "b200_sixdof_state_download_worlds",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -78,6 +79,9 @@ MAX_COV_PLANES = 25  # planes per covariance selection
 MAX_HISTOGRAMS = 8  # specs per histogram call
 MAX_HISTOGRAM_CELLS = 4096  # bins of one spec (na * nb for 2D)
 MAX_WORLD_GROUPS = 1024  # groups of a grouped ensemble
+# retained worlds x entities of an ensemble Exec (World.build(..., retain=...)): the default mode's device-resident
+# threshold, so that the host rows of the retained worlds stay the size of an interactive run's
+MAX_RETAINED_BODIES = 65536
 COMM_ID_BYTES = 128
 
 
@@ -218,6 +222,8 @@ def lib():
     L.b200_sixdof_trajectory_width.restype = C.c_uint32
     L.b200_sixdof_trajectory_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_trajectory_reset.argtypes = [vp]
+    L.b200_sixdof_trajectory_download_worlds.argtypes = [vp, C.POINTER(u64), u32, vp, u64]
+    L.b200_sixdof_state_download_worlds.argtypes = [vp, C.POINTER(u64), u32, vp, u64]
     L.b200_sixdof_trajectory_stats.argtypes = [vp, vp, u64]
     L.b200_sixdof_state_stats.argtypes = [vp, vp, u64]
     L.b200_stats_merge.argtypes = [C.POINTER(C.c_double), u32, u64, C.POINTER(C.c_double)]

@@ -67,6 +67,32 @@ __global__ void __launch_bounds__(kTile) multi_transpose_kernel(const __grid_con
     }
 }
 
+// Rows of chosen worlds (b200_sixdof_{trajectory,state}_download_worlds): sample s0 + blockIdx.y of S, whose plane p is
+// plane (s0 + blockIdx.y) * W + p of the concatenated segments (W = planes_per_sample).  Output body i < rows is entity
+// i % E of world worlds[i / E]; it goes to S.out[(blockIdx.y * rows + i) * W + p].  One pass: every value is read once
+// and written once.  The reads of a plane are coalesced along the entities of a world, and a tile of kTile output bodies
+// is staged through shared memory so that its W * kTile writes are one contiguous run.
+__global__ void __launch_bounds__(kTile) gather_worlds_kernel(const __grid_constant__ StatsParams S,
+                                                              const uint64_t *__restrict__ worlds, uint64_t rows,
+                                                              uint64_t s0)
+{
+    extern __shared__ double tile[]; // kTile * (W | 1)
+    __shared__ const double *plane[32];
+    const uint32_t W = S.planes_per_sample, pitch = W | 1u;
+    const uint64_t base = (uint64_t)blockIdx.x * kTile;
+    const uint32_t nb = (uint32_t)min((uint64_t)kTile, rows - base);
+    if (threadIdx.x < W) plane[threadIdx.x] = stats_plane(S, (s0 + blockIdx.y) * W + threadIdx.x);
+    __syncthreads();
+    if (threadIdx.x < nb) {
+        const uint64_t i = base + threadIdx.x, E = S.n_entities;
+        const uint64_t b = worlds[i / E] * E + i % E;
+        for (uint32_t p = 0; p < W; ++p) tile[threadIdx.x * pitch + p] = __ldg(plane[p] + b);
+    }
+    __syncthreads();
+    double *dst = S.out + ((uint64_t)blockIdx.y * rows + base) * W;
+    for (uint32_t i = threadIdx.x; i < nb * W; i += kTile) dst[i] = tile[(i / W) * pitch + (i % W)];
+}
+
 // FP64 FMA throughput probe: 8 independent chains per thread
 __global__ void __launch_bounds__(256) probe_fp64_kernel(double *out, int iters)
 {
@@ -132,6 +158,25 @@ cudaError_t launch_multi_transpose(const MultiColumns &mc, uint64_t n_bodies, ui
     if (e != cudaSuccess) return e;
     const dim3 grid((unsigned)((n_bodies + kTile - 1) / kTile), mc.n);
     multi_transpose_kernel<<<grid, kTile, smem, s>>>(mc, n_bodies, ld, to_soa ? 1 : 0);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_gather_worlds(const StatsParams &S, const uint64_t *worlds, uint64_t n_worlds, uint64_t s0,
+                                 uint64_t n_samples, int *launches, cudaStream_t s)
+{
+    *launches = 0;
+    const uint64_t rows = n_worlds * S.n_entities, W = S.planes_per_sample;
+    if (rows == 0 || n_samples == 0) return cudaSuccess;
+    const size_t smem = (size_t)kTile * (W | 1u) * sizeof(double); // 25 planes: 52 KB, above the 48 KB default
+    const cudaError_t e = ensure_dynamic_smem(gather_worlds_kernel, smem);
+    if (e != cudaSuccess) return e;
+    StatsParams P = S;
+    for (uint64_t k = 0; k < n_samples; k += 32768) { // gridDim.y <= 65535
+        const unsigned ny = (unsigned)min((uint64_t)32768, n_samples - k);
+        P.out = S.out + k * rows * W;
+        gather_worlds_kernel<<<dim3((unsigned)((rows + kTile - 1) / kTile), ny), kTile, smem, s>>>(P, worlds, rows, s0 + k);
+        ++*launches;
+    }
     return cudaGetLastError();
 }
 

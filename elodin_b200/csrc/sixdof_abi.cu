@@ -1208,6 +1208,59 @@ static StatsParams state_planes(const b200_sixdof *h)
 // The reduction entries below run over one of these; `what` names it in error messages.
 using PlaneSource = StatsParams (*)(const b200_sixdof *);
 
+// The rows of worlds[0 .. n) of the planes of `source` into dst (gather_worlds_kernel): the arguments checked, then
+// `bytes`, then the handle's status.  The index list goes to the device once, at the front of the staging buffer.  A
+// device destination on the handle's GPU takes the rows straight from the kernel; any other gets them through the
+// staging buffer in slices of at most 256 MiB of samples (one sample at least).
+static int download_worlds(b200_sixdof *h, PlaneSource source, const uint64_t *worlds, uint32_t n, void *dst,
+                           uint64_t bytes, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (n == 0) return fail(B200_ERR_INVALID_ARGUMENT, "%s rows of 0 worlds: list at least one", what);
+    if (!worlds) return fail(B200_ERR_INVALID_ARGUMENT, "null world list");
+    for (uint32_t j = 0; j < n; ++j)
+        if (worlds[j] >= h->desc.n_worlds)
+            return fail(B200_ERR_INVALID_ARGUMENT, "world index %llu (entry %u) is not below the %llu worlds",
+                        (unsigned long long)worlds[j], j, (unsigned long long)h->desc.n_worlds);
+    CU(h, cudaSetDevice(h->device));
+    StatsParams S = source(h);
+    const uint64_t W = S.planes_per_sample, n_samples = S.n_planes / W;
+    const uint64_t per_sample = (uint64_t)n * S.n_entities * W * 8ull, want = n_samples * per_sample;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s rows of %u worlds are %llu bytes, got %llu", what, n,
+                    (unsigned long long)want, (unsigned long long)bytes);
+    if (want == 0) return B200_OK;
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    const bool direct = device_destination(h, dst);
+    const uint64_t list = (uint64_t)n * 8ull;
+    const uint64_t chunk = direct ? n_samples : std::max<uint64_t>(1, std::min<uint64_t>(n_samples, (256ull << 20) / per_sample));
+    int rc = ensure_staging(h, list + (direct ? 0 : chunk * per_sample));
+    if (rc) return rc;
+    const uint64_t *dev_worlds = (const uint64_t *)h->staging;
+    CU(h, cudaMemcpyAsync(h->staging, worlds, list, cudaMemcpyHostToDevice, h->stream));
+    for (uint64_t s0 = 0; s0 < n_samples; s0 += chunk) {
+        const uint64_t ns = std::min(chunk, n_samples - s0);
+        S.out = direct ? (double *)((char *)dst + s0 * per_sample) : (double *)((char *)h->staging + list);
+        int launches = 0;
+        CU(h, launch_gather_worlds(S, dev_worlds, n, s0, ns, &launches, h->stream));
+        h->timings.kernel_launches += (uint64_t)launches;
+        if (!direct) CU(h, cudaMemcpyAsync((char *)dst + s0 * per_sample, S.out, ns * per_sample, cudaMemcpyDefault, h->stream));
+    }
+    CU(h, cudaStreamSynchronize(h->stream));
+    return B200_OK;
+}
+
+int b200_sixdof_trajectory_download_worlds(b200_sixdof *h, const uint64_t *worlds, uint32_t n, void *dst, uint64_t bytes)
+{
+    return download_worlds(h, trajectory_planes, worlds, n, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_download_worlds(b200_sixdof *h, const uint64_t *worlds, uint32_t n, void *dst, uint64_t bytes)
+{
+    return download_worlds(h, state_planes, worlds, n, dst, bytes, "state");
+}
+
 // A group table of `bytes` into device memory (*dev, replaced): the stream is drained first, so that no reduction still
 // in flight reads the table it replaces.
 static int upload_group_table(b200_sixdof *h, const void *t, uint64_t bytes, void **dev)

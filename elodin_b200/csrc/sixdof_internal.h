@@ -188,6 +188,12 @@ __device__ inline const double *stats_plane(const StatsParams &S, uint64_t i)
     }
     return p; // i < n_planes: always set
 }
+// Rows of chosen worlds (layout_kernels.cu:gather_worlds_kernel): samples [s0, s0 + n_samples) of S's planes for the
+// worlds worlds[0 .. n_worlds) (device memory, each < S.n_worlds, repeats allowed) into S.out =
+// [n_samples][n_worlds][n_entities][planes_per_sample], the layout of b200_sixdof_trajectory_download restricted to
+// those worlds.  One launch per 32768 samples on s (*launches); none without rows.
+cudaError_t launch_gather_worlds(const StatsParams &S, const uint64_t *worlds, uint64_t n_worlds, uint64_t s0,
+                                 uint64_t n_samples, int *launches, cudaStream_t s);
 // A world group of a grouped reduction: the worlds [o, o + n), reduced in C chunks of Wc worlds; k0 = the chunks of the
 // groups before it, which numbers the block tasks of a launch and places the group's partials.
 struct WorldGroup {

@@ -381,6 +381,14 @@ def sample_timestamps(start_us: int, sim_time_step: float, sample_ticks) -> np.n
     return out
 
 
+def history_slot(exec_, world: int, what: str) -> int:
+    """The index of campaign world `world` on the world axis of `exec_._history` (rows are indexed h[slot, row]): the
+    Exec's own mapping (world.Exec._history_slot: the world itself, or its slot among an ensemble Exec's retained
+    worlds, refusing any other), else the world itself for an object that only carries `_history`."""
+    slot = getattr(exec_, "_history_slot", None)
+    return int(world) if slot is None else slot(world, what)
+
+
 class LiveDbWriter:
     """The telemetry sink while a run is in flight: `init_db` once (every (entity, component) pair registered, row 0 =
     the initial state), then `flush()` appends the history rows recorded since the last flush — one
@@ -392,6 +400,7 @@ class LiveDbWriter:
         from .export import _entity_key
 
         self.exec_, self.world, self.start = exec_, int(world), int(start_timestamp_us)
+        self._slot = history_slot(exec_, world, "attach_db() / write_db()")
         self.sink = DbSink(path, start_timestamp_us)
         self.rows_written = 0
         w = exec_.world
@@ -433,7 +442,7 @@ class LiveDbWriter:
         for (pid, prim), k in zip(self._globals, (0, 1)):
             self.sink.commit_many(pid, ts, np.asarray([x[k] for x in g[i0:i1]], dtype=Schema(prim).dtype))
         for pid, cid, row, dtype in self._pairs:
-            rows = np.stack([h[self.world, row] for h in ex._history[cid][i0:i1]]).astype(dtype, copy=False)
+            rows = np.stack([h[self._slot, row] for h in ex._history[cid][i0:i1]]).astype(dtype, copy=False)
             self.sink.commit_many(pid, ts, rows)
         self.rows_written = i1
         return i1 - i0

@@ -236,6 +236,33 @@ class B200Exec:
     def trajectory_reset(self) -> None:
         _lib.check(self._L.b200_sixdof_trajectory_reset(self._h))
 
+    # ---- retained worlds (full rows of chosen worlds, gathered on the device) -----------------------------------
+    def _download_worlds(self, ring: bool, worlds, shape, out_ptr: Optional[int], nbytes: Optional[int]):
+        """b200_sixdof_{trajectory|state}_download_worlds(h, worlds, n, dst, bytes) into `out_ptr` (returning nothing)
+        or into a new [shape] f64 array, returned."""
+        ws = np.ascontiguousarray(np.asarray(worlds, dtype=np.uint64).ravel())
+        fn = getattr(self._L, f"b200_sixdof_{'trajectory' if ring else 'state'}_download_worlds")
+        out = None if out_ptr is not None else np.empty(shape)
+        ptr = out_ptr if out is None else out.ctypes.data
+        _lib.check(fn(self._h, ws.ctypes.data_as(C.POINTER(C.c_uint64)), ws.size, C.c_void_p(ptr),
+                      int(np.prod(shape)) * 8 if nbytes is None else nbytes))
+        return out
+
+    def trajectory_worlds(self, worlds, out_ptr: Optional[int] = None, nbytes: Optional[int] = None):
+        """The ring's samples of the worlds `worlds` (indices below n_worlds, in that order, repeats allowed):
+        [samples, k, n_entities, width], equal to trajectory()[:, worlds] bit for bit, gathered on the device.  With
+        `out_ptr` (a host or device pointer, e.g. a torch CUDA tensor's data_ptr()) and its `nbytes` the rows are
+        written there and nothing is returned."""
+        n, E, W = self._planes(ring=True)
+        return self._download_worlds(True, worlds, (n, len(np.atleast_1d(worlds)), E, W), out_ptr, nbytes)
+
+    def state_worlds(self, worlds, out_ptr: Optional[int] = None, nbytes: Optional[int] = None):
+        """The current state of the worlds `worlds`: [k, n_entities, 25] -- world_pos[7], world_vel[6], world_accel[6],
+        force[6] (the B200_TRAJ_FULL sample layout), equal to the downloaded columns at `worlds` bit for bit.
+        `out_ptr` / `nbytes` as trajectory_worlds()."""
+        return self._download_worlds(False, worlds, (len(np.atleast_1d(worlds)),) + self._planes(ring=False), out_ptr,
+                                     nbytes)
+
     # ---- ensemble statistics (reductions over the world axis, on the device) ------------------------------------
     def _reduce(self, kind: str, ring: bool, args: tuple, shape, out_ptr: Optional[int] = None,
                 nbytes: Optional[int] = None) -> Optional[np.ndarray]:

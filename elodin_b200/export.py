@@ -51,13 +51,15 @@ def _fmt(v) -> str:
 
 
 def export_csv(exec_, out_dir: str, start_timestamp: Optional[_dt.datetime] = None, world: int = 0) -> List[str]:
-    """Write one CSV per (entity, component) of `exec_`'s recorded history (world `world`)."""
+    """Write one CSV per (entity, component) of `exec_`'s recorded history (world `world`: the campaign's world index,
+    a retained one for an ensemble Exec)."""
+    from .db_sink import history_slot, sample_timestamps
+
+    slot = history_slot(exec_, world, "export_csv()")
     os.makedirs(out_dir, exist_ok=True)
     w = exec_.world
     t0 = start_timestamp or _dt.datetime(2026, 1, 1)
     # the same time base as the elodin-db sink: row k is stamped by the ticks it really covers (exec.rs:134-152)
-    from .db_sink import sample_timestamps
-
     us = sample_timestamps(0, exec_.sim_time_step, [g[0] for g in exec_._globals_hist])
     times = [(t0 + _dt.timedelta(microseconds=int(u))).isoformat() for u in us]
     written = []
@@ -83,6 +85,6 @@ def export_csv(exec_, out_dir: str, start_timestamp: Optional[_dt.datetime] = No
             key = _entity_key(ename)
             base = f"{key}.{comp.name}"
             header = [base] if (col.width == 1 and not names) else [f"{base}_{e}" for e in elems]
-            series = [h[world, row] for h in exec_._history[cid]]
+            series = [h[slot, row] for h in exec_._history[cid]]
             write(base, header, series)
     return written

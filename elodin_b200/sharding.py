@@ -41,6 +41,14 @@ def shard_groups(sizes: Sequence[int], rank: int, world_size: int) -> List[int]:
     return out
 
 
+def shard_retained(retain: Sequence[int], n_worlds: int, rank: int, world_size: int) -> List[int]:
+    """The entries of a global `retain` list (World.build(..., ensemble=True, retain=...)) that fall in `rank`'s world
+    range (shard_worlds), as indices local to that range, in the given order: every rank of a world-sharded campaign
+    retains the global runs it holds.  A rank may get none (then it builds without `retain`)."""
+    w0, w1 = shard_worlds(n_worlds, rank, world_size)
+    return [int(w) - w0 for w in retain if w0 <= int(w) < w1]
+
+
 def gather_worlds(local, n_worlds: int, group=None):
     """End-of-run gather of a per-world tensor [w_local, ...] from every rank into the global
     world order [n_worlds, ...] (all ranks get the result).  Ragged shards are padded to the

@@ -439,7 +439,7 @@ class World:
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
               thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
               covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
-              groups: Optional[Sequence[int]] = None) -> "Exec":
+              groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -455,7 +455,11 @@ class World:
         (`Exec.ensemble(pair, groups=True)`) and, where `histograms`, `quantiles` or `covariance` is given, the
         histograms, quantiles and covariance of every group (`Exec.histogram(i, groups=True)`,
         `Exec.quantiles(pair, groups=True)`, `Exec.covariance(entity, groups=True)`), beside the all-worlds tables.
-        Group g's tables equal those of an Exec over exactly its worlds."""
+        Group g's tables equal those of an Exec over exactly its worlds.  `retain` (distinct world indices, at least one,
+        at most MAX_RETAINED_BODIES worlds x entities) also records the full rows of those worlds, gathered on the
+        device, so that `history_worlds`, `history` (world 0, if retained), `attach_db`, `write_db`,
+        `export.export_csv` and `monte_carlo.write_run_databases` work for them as in the default mode, with the same
+        rows bit for bit; `Exec.retained` is the tuple in the order given."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -463,7 +467,7 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -600,6 +604,31 @@ def _world_groups(groups, n_worlds: int) -> List[int]:
     return [int(x) for x in sizes]
 
 
+def _retained_worlds(retain, n_worlds: int, n_entities: int) -> tuple:
+    """World.build(..., retain=...): 1 or more distinct integer world indices in [0, n_worlds), order kept, at most
+    MAX_RETAINED_BODIES worlds x entities."""
+    if isinstance(retain, (str, bytes)) or not isinstance(retain, (Sequence, np.ndarray)):
+        raise TypeError(f"retain takes a sequence of world indices, got {retain!r}")
+    worlds = list(np.asarray(retain).ravel()) if isinstance(retain, np.ndarray) else list(retain)
+    for w in worlds:
+        if isinstance(w, (bool, np.bool_)) or not isinstance(w, (int, np.integer)):
+            raise TypeError(f"retain: world index {w!r} is not an integer")
+        if not 0 <= w < n_worlds:
+            raise ValueError(f"retain: world index {w} is not in [0, {n_worlds})")
+    worlds = [int(w) for w in worlds]
+    if not worlds:
+        raise ValueError("retain: list at least one world")
+    seen = set()
+    for w in worlds:
+        if w in seen:
+            raise ValueError(f"retain: world {w} is listed twice")
+        seen.add(w)
+    if len(worlds) * n_entities > _lib.MAX_RETAINED_BODIES:
+        raise ValueError(f"retain: {len(worlds)} worlds x {n_entities} entities = {len(worlds) * n_entities} bodies, "
+                         f"at most {_lib.MAX_RETAINED_BODIES}")
+    return tuple(worlds)
+
+
 def _histogram_specs(histograms) -> List["Histogram"]:
     """World.build(..., histograms=...): 1 to MAX_HISTOGRAMS el.Histogram objects."""
     if isinstance(histograms, (str, bytes)) or not isinstance(histograms, Sequence):
@@ -718,7 +747,7 @@ class Exec:
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
                  thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
                  covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
-                 groups: Optional[Sequence[int]] = None):
+                 groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -765,6 +794,9 @@ class Exec:
         if groups is not None and not ensemble:
             raise ValueError("groups: need World.build(..., ensemble=True)")
         self.groups = _world_groups(groups, self.n_worlds) if groups is not None else None
+        if retain is not None and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "retain: need World.build(..., ensemble=True)")
+        self._retain = _retained_worlds(retain, self.n_worlds, len(bodies)) if retain is not None else None
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
         self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
@@ -860,7 +892,8 @@ class Exec:
         if self.groups is not None:
             self.backend.set_world_groups(self.groups)
         if self._ensemble:
-            self._history = {}
+            if self._retain is None:
+                self._history = {}
             self._upload_inputs()
             self._add_ensemble_rows(ring=False)  # row 0: the initial state
         else:
@@ -938,10 +971,11 @@ class Exec:
             else:
                 be.upload(cid, self.world.columns[cid].buffer)
 
-    def _add_ensemble_rows(self, ring: bool) -> None:
+    def _add_ensemble_rows(self, ring: bool, host_rows: bool = False) -> None:
         """Record one batch of ensemble rows, on the device: the ring's samples (ring=True; ticks_per_telemetry ticks
         apart, the last one at the current tick) or the current state as one row.  Reduces every table this Exec
-        records, folds the run summaries and appends the rows' globals."""
+        records, folds the run summaries, records the retained worlds' rows (from the host columns when `host_rows`)
+        and appends the rows' globals."""
         be = self.backend
         for kind, args in self._ens_args.items():
             rows = getattr(be, f"trajectory_{kind}")(*args) if ring else getattr(be, f"state_{kind}")(*args)[None]
@@ -950,7 +984,31 @@ class Exec:
             (be.summary_add_trajectory if ring else be.summary_add_state)()
             self._summary_tables.clear()
         k, tpt = rows.shape[0], self.ticks_per_telemetry
+        if self._retain is not None:
+            self._add_retained_rows(ring, host_rows)
         self._globals_hist.extend((self.tick - (k - 1 - i) * tpt, self.sim_time_step) for i in range(k))
+        if self._db is not None:
+            self._db.flush()  # the k cycles of this batch, each with its own timestamp
+
+    def _add_retained_rows(self, ring: bool, host_rows: bool) -> None:
+        """The rows of the retained worlds for the batch _add_ensemble_rows records, as the default mode records them.
+        With `host_rows` (the invoke_batch route: one row, the host columns current after the cycle's host systems and
+        callbacks) every column comes from the host columns at those worlds, as in Exec._record, so that a host
+        system's write to a sampled component is in the row.  Otherwise (the resident route, where no host code runs
+        between the ticks) the sampled components are gathered on the device (the ring's samples, or the current
+        state) and every other column comes from the host columns, as in Exec._run_resident."""
+        be, idx = self.backend, list(self._retain)
+        if host_rows:
+            for cid, col in self.world.columns.items():
+                self._history[cid].append(col.buffer[idx])
+            return
+        rows = be.trajectory_worlds(idx) if ring else be.state_worlds(idx)[None]  # [k, R, n_entities, 25]
+        for name, (lo, hi) in _SAMPLED.items():
+            self._history[component_id(name)].extend(np.ascontiguousarray(rows[..., lo:hi]))
+        sampled = {component_id(name) for name in _SAMPLED}
+        for cid, col in self.world.columns.items():
+            if cid not in sampled:                                    # pass-through, as on the resident route
+                self._history[cid].extend([col.buffer[idx]] * rows.shape[0])
 
     def _run_ensemble(self, ticks: int, is_canceled, pre_step, post_step) -> None:
         """Ensemble mode: one row of world-axis statistics per telemetry cycle, reduced on the device from the
@@ -1012,7 +1070,7 @@ class Exec:
                     post_step(self.tick, ctx)
                 done += per_call
             t_hist = time.perf_counter()
-            self._add_ensemble_rows(ring=n == tpt)
+            self._add_ensemble_rows(ring=n == tpt, host_rows=True)
             self._prof["add_to_history"].append((time.perf_counter() - t_hist) * 1e3)
             remaining -= n
             if is_canceled is not None and is_canceled():
@@ -1021,7 +1079,28 @@ class Exec:
     def _no_rows(self, what: str):
         raise _lib.B200Error(_lib.ERR_UNSUPPORTED,
                              f"{what}: this Exec was built with ensemble=True and records statistics over the worlds, "
-                             "not per-world rows; read them with Exec.ensemble('<entity>.<component>')")
+                             "not per-world rows; read them with Exec.ensemble('<entity>.<component>'), or keep the "
+                             "rows of chosen worlds with World.build(..., ensemble=True, retain=[...])")
+
+    @property
+    def retained(self) -> Optional[tuple]:
+        """The worlds of World.build(..., ensemble=True, retain=[...]) whose rows this Exec records, in that order;
+        None without `retain`."""
+        return self._retain
+
+    def _history_slot(self, world: int, what: str) -> int:
+        """The index of campaign world `world` on the world axis of the recorded history: the world itself in the
+        default mode, its position in `retain` in ensemble mode.  `what` names the caller in the refusals: an ensemble
+        Exec without `retain`, or a world it does not retain."""
+        if not self._ensemble:
+            return int(world)
+        if self._retain is None:
+            self._no_rows(what)
+        if world not in self._retain:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 f"{what}: world {world!r} has no rows; this ensemble Exec records the rows of "
+                                 f"retain={list(self._retain)}")
+        return self._retain.index(world)
 
     def _run_resident(self, cycles: int) -> None:
         """`cycles` whole telemetry cycles without leaving the device: upload the host columns once, step,
@@ -1107,8 +1186,7 @@ class Exec:
     def history(self, names: Union[str, Sequence[str]]):
         """`exec.history("e1.world_pos")` -> {name: rows[T, width]} (world 0; use
         `history_worlds` for the batch).  The reference returns a polars frame."""
-        if self._ensemble:
-            self._no_rows("history()")
+        slot = self._history_slot(0, "history()")
         if isinstance(names, str):
             names = [names]
         out = {}
@@ -1123,17 +1201,17 @@ class Exec:
             if col is None:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
             row = col.row_of(self.world.entity_by_name(ent))
-            out[pair] = np.stack([h[0, row] for h in self._history[cid]]).view(_Series)
+            out[pair] = np.stack([h[slot, row] for h in self._history[cid]]).view(_Series)
         return out
 
     def attach_db(self, path: str, start_timestamp_us: Optional[int] = None, world: int = 0):
         """Stream the telemetry of world `world` into an elodin-db directory while the run is in flight: `init_db` now
         (every pair registered, the rows recorded so far committed), then one commit per telemetry cycle
         (`commit_world_head_unified`, impeller2_server.rs:390-438) — per ring read-back on the device-resident route.
-        `close_db()` finishes the directory."""
+        `close_db()` finishes the directory.  `world` is the campaign's world index, a retained one in ensemble mode."""
         from . import db_sink
 
-        if self._ensemble:
+        if self._ensemble and self._retain is None:
             self._no_rows("attach_db()")
         if getattr(self, "_db", None) is not None:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "a database is already attached")
@@ -1147,17 +1225,20 @@ class Exec:
 
     def write_db(self, path: str, start_timestamp_us: Optional[int] = None, world: int = 0):
         """Write the recorded telemetry as an elodin-db directory (`elodin_b200.db_sink`): what the
-        reference's `init_db` + `commit_world_head_unified` leave on disk for `elodin-db export` / the editor."""
+        reference's `init_db` + `commit_world_head_unified` leave on disk for `elodin-db export` / the editor.
+        `world` is the campaign's world index, a retained one in ensemble mode."""
         from . import db_sink
 
-        if self._ensemble:
+        if self._ensemble and self._retain is None:
             self._no_rows("write_db()")
         if start_timestamp_us is None:
             return db_sink.write_db(self, path, world=world)
         return db_sink.write_db(self, path, start_timestamp_us, world)
 
     def history_worlds(self, pair: str) -> np.ndarray:
-        if self._ensemble:
+        """`<entity>.<component>` -> [rows, n_worlds, width]: every recorded row of every world; in ensemble mode
+        [rows, k, width] for the worlds of `retain`, in that order."""
+        if self._ensemble and self._retain is None:
             self._no_rows("history_worlds()")
         ent, comp = pair.rsplit(".", 1)
         col = self.world.columns[component_id(comp)]

@@ -275,6 +275,20 @@ uint32_t b200_sixdof_trajectory_width(const b200_sixdof *h);
 int b200_sixdof_trajectory_download(b200_sixdof *h, void *dst, uint64_t bytes);
 int b200_sixdof_trajectory_reset(b200_sixdof *h);
 
+/* ---- retained worlds: the full rows of chosen worlds, gathered on the device, so that an ensemble campaign keeps a
+ * few real trajectories (the nominal run, a sample for a spaghetti plot, flagged runs) beside its statistics.
+ * worlds[0 .. n) are world indices below n_worlds, in any order, repeats allowed; a null handle, n = 0, a null list or
+ * an index >= n_worlds returns B200_ERR_INVALID_ARGUMENT (naming the index), a wrong `bytes`
+ * B200_ERR_VALUE_SIZE_MISMATCH.  The list goes to the device once per call.  dst may be host memory or device memory
+ * on the handle's GPU (written directly); host rows go through the staging buffer in slices of at most 256 MiB of
+ * samples.  Both entries run on the handle's stream, return once dst is filled and count their launches in
+ * timings.kernel_launches. ---- */
+/* rows of chosen worlds: dst = [trajectory_len][n][n_entities][trajectory_width] f64, the rows of
+ * b200_sixdof_trajectory_download for worlds[0..n) in that order.  An empty ring takes bytes = 0 and launches nothing. */
+int b200_sixdof_trajectory_download_worlds(b200_sixdof *h, const uint64_t *worlds, uint32_t n, void *dst, uint64_t bytes);
+/* the current state of chosen worlds: dst = [n][n_entities][25] f64 (world_pos, world_vel, world_accel, force) */
+int b200_sixdof_state_download_worlds(b200_sixdof *h, const uint64_t *worlds, uint32_t n, void *dst, uint64_t bytes);
+
 /* ---- ensemble statistics: the world axis reduced on the device, so that a Monte-Carlo campaign records dispersion
  * over time without moving every world's state to the host.  A group is 5 f64 over the worlds of one sampled value of
  * one entity:  count  = worlds whose value is finite (a double, exact up to 2^53),
