@@ -20,8 +20,8 @@ from ._lib import B200Error, B200ValueError, component_id
 from .effectors import (DragQuadratic, GravityConst, GravityEGM08, GravityEdges, GravityFrame, GravityJ2, Pipe, System, ThrustBody,
                         TorqueBodyFold, WrenchBody, WrenchWorld, all_pairs_edges)
 from .executor import B200Exec, device_count, merge_covariance, merge_histograms, merge_stats, pinned_empty, pinned_free
-from .world import (Annotated, Archetype, Body, Component, ComponentType, Edge, EntityId, Exec, Force, Histogram,
-                    HostSystem, Inertia, Integrator, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
+from .world import (Annotated, Archetype, AxisAngle, Body, Channel, Component, ComponentType, Edge, EntityId, Exec, Force, Histogram,
+                    HostSystem, Inertia, Integrator, Norm, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
                     SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, Threshold, World, WorldAccel,
                     WorldPos, WorldVel, dataclass, host_system, quantised_time_step, six_dof, ticks_per_telemetry)
 

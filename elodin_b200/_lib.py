@@ -70,6 +70,7 @@ SYMBOLS = [
     "b200_sixdof_trajectory_group_quantiles", "b200_sixdof_state_group_quantiles",
     "b200_sixdof_trajectory_group_covariance", "b200_sixdof_state_group_covariance",
     "b200_sixdof_trajectory_download_worlds", "b200_sixdof_state_download_worlds",
+    "b200_sixdof_set_channels", "b200_sixdof_channels", "b200_sixdof_trajectory_channels", "b200_sixdof_state_channels",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -82,6 +83,11 @@ MAX_WORLD_GROUPS = 1024  # groups of a grouped ensemble
 # retained worlds x entities of an ensemble Exec (World.build(..., retain=...)): the default mode's device-resident
 # threshold, so that the host rows of the retained worlds stay the size of an interactive run's
 MAX_RETAINED_BODIES = 65536
+# derived channels (b200_sixdof_set_channels): per-body values of a row, reduced as planes 25 + k
+MAX_CHANNELS = 8
+CHANNEL_NORM = 1
+CHANNEL_AXIS_ANGLE = 2
+ROW_PLANES = 25  # planes of a B200_TRAJ_FULL row; channel k is plane ROW_PLANES + k of an ensemble table
 COMM_ID_BYTES = 128
 
 
@@ -154,6 +160,31 @@ class Histogram(C.Structure):
         ("lo", C.c_double * 2),
         ("hi", C.c_double * 2),
     ]
+
+
+class Channel(C.Structure):
+    _fields_ = [
+        ("kind", C.c_uint32),
+        ("n", C.c_uint32),
+        ("plane", C.c_uint32 * 3),
+        ("reserved", C.c_uint32),
+        ("c", C.c_double * 3),
+        ("d", C.c_double * 3),
+        ("r0", C.c_double),
+    ]
+
+
+def channel(kind: int, n: int, planes=(), c=(), d=(), r0: float = 0.0) -> Channel:
+    """A Channel record; unnamed fields are zero."""
+    ch = Channel()
+    ch.kind, ch.n, ch.r0 = int(kind), int(n), float(r0)
+    for i, v in enumerate(list(planes)[:3]):
+        ch.plane[i] = int(v)
+    for i, v in enumerate(list(c)[:3]):
+        ch.c[i] = float(v)
+    for i, v in enumerate(list(d)[:3]):
+        ch.d[i] = float(v)
+    return ch
 
 
 class B200Error(RuntimeError):
@@ -252,6 +283,11 @@ def lib():
     L.b200_sixdof_state_group_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
     L.b200_sixdof_trajectory_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_state_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_set_channels.argtypes = [vp, C.POINTER(Channel), u32]
+    L.b200_sixdof_channels.argtypes = [vp]
+    L.b200_sixdof_channels.restype = u32
+    L.b200_sixdof_trajectory_channels.argtypes = [vp, vp, u64]
+    L.b200_sixdof_state_channels.argtypes = [vp, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -99,6 +99,7 @@ __device__ inline void tile_of(uint32_t t, uint32_t nb, uint32_t &ab, uint32_t &
 __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Geo geo, Slice sl, double *scratch)
 {
     extern __shared__ double smem[];
+    __shared__ const double *src_plane[B200_MAX_COV_PLANES];  // the selected planes of the task's sample
     const uint32_t p = S.n_p, Et = geo.Et, Wt = geo.Wt;
     double *xs = smem;                                    // [Wt][p][Et]
     double *ss = xs + (uint64_t)Wt * p * Et;              // [p][Et]: the diagonal tiles' S_a
@@ -127,6 +128,8 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Geo
         const uint32_t ne = (uint32_t)min((uint64_t)Et, E - e0);
         const uint64_t w0 = wg.o + c * wg.Wc, w1 = wg.o + min((c + 1) * wg.Wc, wg.n);
         const bool fin = wg.C == 1;  // a final record holds NaN where n = 0; a partial leaves them (unread)
+        // read after the barrier that opens each tile; the previous task's reads all precede its last tile's barrier
+        if (t < p) src_plane[t] = sample_plane(S, s, S.planes[t]);
         double K[8], Q[16], Ssum[4];
 #pragma unroll
         for (int k = 0; k < 8; ++k) K[k] = 0.0;
@@ -147,8 +150,7 @@ __global__ void __launch_bounds__(kMaxThreads) cov_chunk_kernel(CovParams S, Geo
                     const uint32_t i = i0 + u * blockDim.x;
                     if (i < items) {
                         const uint32_t q = i / per_plane, r = i % per_plane, w = r / ne, j = r % ne;
-                        const double *src = stats_plane(S, s * S.planes_per_sample + S.planes[q]);
-                        v[u] = __ldcs(src + (wa + w) * E + e0 + j);
+                        v[u] = __ldcs(src_plane[q] + (wa + w) * E + e0 + j);
                         dst[u] = (w * p + q) * Et + j;
                     }
                 }

@@ -106,8 +106,8 @@ __global__ void __launch_bounds__(kThreads) hist_kernel(HistParams P, const Worl
         for (uint32_t i = threadIdx.x; i < ne; i += blockDim.x) edges[i] = P.edges[sp.edge_off + i];
         __syncthreads();
         const double *ea = edges, *eb = edges + sp.bins[0] + 1;
-        const double *xa = stats_plane(P, s * P.planes_per_sample + sp.plane[0]) + sp.entity;
-        const double *xb = two ? stats_plane(P, s * P.planes_per_sample + sp.plane[1]) + sp.entity : xa;
+        const double *xa = sample_plane(P, s, sp.plane[0]) + sp.entity;
+        const double *xb = two ? sample_plane(P, s, sp.plane[1]) + sp.entity : xa;
         const ex::Rcp r = ex::rcp_prep(sp.den);
         const uint64_t w0 = wg.o + (k - wg.k0) * wg.Wc, w1 = min(w0 + wg.Wc, wg.o + wg.n);
         for (uint64_t base = w0; base < w1; base += (uint64_t)kUnroll * blockDim.x) { // uniform trip count per warp

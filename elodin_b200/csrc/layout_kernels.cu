@@ -81,7 +81,7 @@ __global__ void __launch_bounds__(kTile) gather_worlds_kernel(const __grid_const
     const uint32_t W = S.planes_per_sample, pitch = W | 1u;
     const uint64_t base = (uint64_t)blockIdx.x * kTile;
     const uint32_t nb = (uint32_t)min((uint64_t)kTile, rows - base);
-    if (threadIdx.x < W) plane[threadIdx.x] = stats_plane(S, (s0 + blockIdx.y) * W + threadIdx.x);
+    if (threadIdx.x < W) plane[threadIdx.x] = sample_plane(S, s0 + blockIdx.y, threadIdx.x);
     __syncthreads();
     if (threadIdx.x < nb) {
         const uint64_t i = base + threadIdx.x, E = S.n_entities;

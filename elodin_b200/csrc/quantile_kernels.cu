@@ -104,19 +104,6 @@ __device__ __forceinline__ double key_value(unsigned long long k)
 
 __device__ __forceinline__ bool finite(double x) { return fabs(x) <= DBL_MAX; }
 
-__device__ inline const double *plane_of(const QuantileParams &S, uint64_t i)
-{
-    const double *p = nullptr;
-#pragma unroll
-    for (uint32_t k = 0; k < 4; ++k) {
-        if (!p && k < S.n_segs) {
-            if (i < S.seg[k].n_planes) p = S.seg[k].base + i * S.ld;
-            else i -= S.seg[k].n_planes;
-        }
-    }
-    return p;
-}
-
 __device__ __forceinline__ double *out_of(const QuantileParams &S, uint64_t g, uint64_t i, uint64_t e)
 {
     const uint64_t W = S.planes_per_sample;
@@ -177,7 +164,7 @@ __device__ uint32_t load_sort(const QuantileParams &S, const WorldGroup &wg, uin
 {
     if (tid == 0) *cnt = 0;
     sync();
-    const double *p = plane_of(S, i) + wg.o * S.n_entities + e;
+    const double *p = stats_plane(S, i) + wg.o * S.n_entities + e;
     for (uint64_t w = tid; w < wg.n; w += team) {
         const double x = p[w * S.n_entities];
         if (finite(x)) a[atomicAdd(cnt, 1u)] = order_key(x);
@@ -293,7 +280,7 @@ __global__ void __launch_bounds__(kPassThreads) quantile_count_kernel(QuantilePa
         unsigned long long mn = ~0ull, mx = 0;
         const bool live = j < sp.J && e < sl.ne;
         if (live) {
-            const double *p = plane_of(S, r.i) + sl.e0 + e;
+            const double *p = stats_plane(S, r.i) + sl.e0 + e;
             const uint64_t w1 = r.o + min((c + 1) * r.Wc, (uint64_t)r.n);
             for (uint64_t w = r.o + c * r.Wc + j; w < w1; w += sp.J) {
                 const double x = p[w * E];
@@ -356,7 +343,7 @@ __global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantilePar
         if (live && G.todo) {
             uint32_t *hist = L.hist + g * kBins;
             unsigned long long *area = L.area + g * kGroupCap;
-            const double *p = plane_of(S, r.i) + sl.e0 + e;
+            const double *p = stats_plane(S, r.i) + sl.e0 + e;
             const uint64_t w1 = r.o + min((c + 1) * r.Wc, (uint64_t)r.n);
             const unsigned long long kmin = G.kmin, kmax = G.kmax;
             const uint32_t n_act = G.n_act;

@@ -728,6 +728,8 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->stage_out) cudaFree(h->stage_out);
     if (h->traj) cudaFree(h->traj);
     if (h->sum_ext) cudaFree(h->sum_ext);
+    if (h->chan_ring) cudaFree(h->chan_ring);
+    if (h->chan_state) cudaFree(h->chan_state);
     if (h->sum_thr) cudaFree(h->sum_thr);
     for (void *t : {(void *)h->all_table_dev, (void *)h->group_table_dev, (void *)h->all_cov_dev, (void *)h->group_cov_dev,
                     (void *)h->all_order_dev, (void *)h->group_order_dev})
@@ -1178,7 +1180,7 @@ static StatsParams trajectory_planes(const b200_sixdof *h)
     const uint64_t n = b200_sixdof_trajectory_len(h);
     const uint64_t W = h->traj_planes;
     StatsParams S{};
-    S.seg[0] = {h->traj, n * W};
+    S.seg[0] = {h->traj, W, W * h->ld};
     S.n_segs = 1;
     S.planes_per_sample = (uint32_t)W;
     S.n_planes = n * W;
@@ -1194,7 +1196,7 @@ static StatsParams state_planes(const b200_sixdof *h)
     const uint64_t ids[4] = {B200_ID_WORLD_POS, B200_ID_WORLD_VEL, B200_ID_WORLD_ACCEL, B200_ID_FORCE};
     for (int k = 0; k < 4; ++k) {
         const Column *c = h->find(ids[k]);
-        S.seg[k] = {c->dev, c->width};
+        S.seg[k] = {c->dev, c->width, 0};
     }
     S.n_segs = 4;
     S.planes_per_sample = 25;
@@ -1205,8 +1207,54 @@ static StatsParams state_planes(const b200_sixdof *h)
     return S;
 }
 
-// The reduction entries below run over one of these; `what` names it in error messages.
+// download_worlds runs over one of these; `what` names it in error messages.
 using PlaneSource = StatsParams (*)(const b200_sixdof *);
+
+// The rows every ensemble reduction and run summary reads, R = 25 + n_c planes per sample: the sampled planes of the
+// ring's samples (ring) or of the state, then the channel planes (b200_sixdof_set_channels) as a segment of its own.
+static StatsParams ensemble_rows(const b200_sixdof *h, bool ring)
+{
+    StatsParams S = ring ? trajectory_planes(h) : state_planes(h);
+    const uint64_t n_c = h->channels.size();
+    if (n_c) {
+        const uint64_t n_s = S.n_planes / S.planes_per_sample;
+        S.seg[S.n_segs++] = {ring ? h->chan_ring : h->chan_state, n_c, n_c * h->ld};
+        S.planes_per_sample += (uint32_t)n_c;
+        S.n_planes = n_s * S.planes_per_sample;
+    }
+    return S;
+}
+
+// The planes of a row of the ring (0 without a ring) or of the state: what a plane index is checked against.
+static uint32_t row_width(const b200_sixdof *h, bool ring)
+{
+    const uint32_t n_c = (uint32_t)h->channels.size();
+    return ring ? (h->traj ? h->traj_planes + n_c : 0) : 25 + n_c;
+}
+
+// Recompute the channel planes of every sample now in the ring (ring) or of the state, on the handle's stream (one
+// launch, none without channels or samples).  Always recomputed, never cached: b200_sixdof_device_plane hands out
+// writable planes.
+static int refresh_channels(b200_sixdof *h, bool ring)
+{
+    if (h->channels.empty()) return B200_OK;
+    const StatsParams S = ring ? trajectory_planes(h) : state_planes(h);
+    ChannelParams P{};
+    uint32_t p = 0;
+    for (uint32_t k = 0; k < S.n_segs; ++k)
+        for (uint64_t j = 0; j < S.seg[k].n_planes && p < 25; ++j) P.row[p++] = S.seg[k].base + j * S.ld;
+    P.row_stride = S.seg[0].stride;
+    P.out = ring ? h->chan_ring : h->chan_state;
+    P.ld = h->ld;
+    P.n_bodies = h->n_bodies;
+    P.n_samples = S.n_planes / S.planes_per_sample;
+    P.n_c = (uint32_t)h->channels.size();
+    for (uint32_t k = 0; k < P.n_c; ++k) P.c[k] = h->channels[k];
+    int launches = 0;
+    CU(h, launch_channels(P, &launches, h->stream));
+    h->timings.kernel_launches += (uint64_t)launches;
+    return B200_OK;
+}
 
 // The rows of worlds[0 .. n) of the planes of `source` into dst (gather_worlds_kernel): the arguments checked, then
 // `bytes`, then the handle's status.  The index list goes to the device once, at the front of the staging buffer.  A
@@ -1330,12 +1378,12 @@ static int no_groups(const char *what)
 
 // Statistics of the planes over the worlds, per group when `grouped` (stats_kernels.cu), into dst: the groups checked,
 // then `bytes`, then the handle's status.
-static int run_world_stats(b200_sixdof *h, PlaneSource source, bool grouped, void *dst, uint64_t bytes, const char *what)
+static int run_world_stats(b200_sixdof *h, bool ring, bool grouped, void *dst, uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
-    StatsParams S = source(h);
+    StatsParams S = ensemble_rows(h, ring);
     const uint64_t G = grouped ? h->group_sizes.size() : 1;
     const uint64_t want = S.n_planes * G * S.n_entities * 5ull * 8ull;
     if (bytes != want)
@@ -1344,6 +1392,10 @@ static int run_world_stats(b200_sixdof *h, PlaneSource source, bool grouped, voi
     const std::vector<WorldGroup> &table = grouped ? h->group_table : h->all_table;
     const WorldGroup *groups = grouped ? h->group_table_dev : h->all_table_dev;
     const uint64_t scratch = bytes && h->status == B200_OK ? world_stats_scratch_doubles(S, table) * 8ull : 0;
+    if (bytes && h->status == B200_OK && dst) {
+        const int rc = refresh_channels(h, ring);
+        if (rc) return rc;
+    }
     return run_world_reduction(h, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
         return launch_world_stats(S, groups, table, (double *)scr, n, h->stream);
@@ -1352,34 +1404,34 @@ static int run_world_stats(b200_sixdof *h, PlaneSource source, bool grouped, voi
 
 int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, trajectory_planes, false, dst, bytes, "trajectory");
+    return run_world_stats(h, true, false, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, state_planes, false, dst, bytes, "state");
+    return run_world_stats(h, false, false, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, trajectory_planes, true, dst, bytes, "trajectory");
+    return run_world_stats(h, true, true, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, state_planes, true, dst, bytes, "state");
+    return run_world_stats(h, false, true, dst, bytes, "state");
 }
 
 // Quantiles of the planes over the worlds, per group when `grouped` (quantile_kernels.cu), into dst: the groups checked,
 // then the handle's status, then the levels, then `bytes`.
-static int run_quantiles(b200_sixdof *h, PlaneSource source, bool grouped, const double *q, uint32_t n_q, void *dst,
+static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *q, uint32_t n_q, void *dst,
                          uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     QuantileParams S{};
-    static_cast<StatsParams &>(S) = source(h);
+    static_cast<StatsParams &>(S) = ensemble_rows(h, ring);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_q == 0 || n_q > B200_MAX_QUANTILES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u quantile levels: 1 to %u", n_q, B200_MAX_QUANTILES);
@@ -1400,6 +1452,10 @@ static int run_quantiles(b200_sixdof *h, PlaneSource source, bool grouped, const
     S.n_groups = G;
     const uint64_t triples = S.n_planes * G * S.n_entities;
     h->quantile_read_sum = triples;  // the small-group routes read every triple once
+    if (bytes && dst) {
+        const int rc = refresh_channels(h, ring);
+        if (rc) return rc;
+    }
     int rc = run_world_reduction(h, quantile_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
         return launch_quantiles(S, table, order, scratch, n, &h->quantile_read_sum, h->stream);
@@ -1410,46 +1466,49 @@ static int run_quantiles(b200_sixdof *h, PlaneSource source, bool grouped, const
 
 int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, trajectory_planes, false, q, n_q, dst, bytes, "trajectory");
+    return run_quantiles(h, true, false, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, state_planes, false, q, n_q, dst, bytes, "state");
+    return run_quantiles(h, false, false, q, n_q, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, trajectory_planes, true, q, n_q, dst, bytes, "trajectory");
+    return run_quantiles(h, true, true, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, state_planes, true, q, n_q, dst, bytes, "state");
+    return run_quantiles(h, false, true, q, n_q, dst, bytes, "state");
 }
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
 // Covariance of the selection `planes` (each < width) of every sample over the worlds, per group when `grouped`
 // (cov_kernels.cu), into dst: the groups checked, then the handle's status, then the selection, then `bytes`.
-static int run_covariance(b200_sixdof *h, PlaneSource source, bool grouped, uint32_t width, const uint32_t *planes,
-                          uint32_t n_p, void *dst, uint64_t bytes, const char *what)
+static int run_covariance(b200_sixdof *h, bool ring, bool grouped, const uint32_t *planes, uint32_t n_p, void *dst,
+                          uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     CovParams S{};
-    static_cast<StatsParams &>(S) = source(h);
+    static_cast<StatsParams &>(S) = ensemble_rows(h, ring);
+    const uint32_t width = row_width(h, ring);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_p == 0 || n_p > B200_MAX_COV_PLANES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u covariance planes: 1 to %u", n_p, B200_MAX_COV_PLANES);
     if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null covariance planes");
-    uint32_t seen = 0;
+    uint64_t seen = 0;
+    bool channel = false;
     for (uint32_t k = 0; k < n_p; ++k) {
         if (planes[k] >= width)
             return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u is %u: the %s has %u planes", k, planes[k], what, width);
-        if (seen & (1u << planes[k])) return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u listed twice", planes[k]);
-        seen |= 1u << planes[k];
+        if (seen & (1ull << planes[k])) return fail(B200_ERR_INVALID_ARGUMENT, "covariance plane %u listed twice", planes[k]);
+        seen |= 1ull << planes[k];
+        channel = channel || planes[k] >= 25;
     }
     const uint64_t n_s = S.planes_per_sample ? S.n_planes / S.planes_per_sample : 0;
     const uint64_t G = reduction_groups(h, grouped).size();
@@ -1461,34 +1520,36 @@ static int run_covariance(b200_sixdof *h, PlaneSource source, bool grouped, uint
     for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
     const std::vector<WorldGroup> &table = grouped ? h->group_cov : h->all_cov;
     const WorldGroup *groups = grouped ? h->group_cov_dev : h->all_cov_dev;
+    if (channel && bytes && dst) {
+        const int rc = refresh_channels(h, ring);
+        if (rc) return rc;
+    }
     return run_world_reduction(h, cov_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
         return launch_covariance(S, groups, table, scratch, n, h->stream);
     });
 }
 
-// The ring's width, not its planes per sample: a handle without a ring refuses every plane.
+// The ring's width (row_width), not its planes per sample: a handle without a ring refuses every plane.
 int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, trajectory_planes, false, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes,
-                          "trajectory");
+    return run_covariance(h, true, false, planes, n_p, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, state_planes, false, 25, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, false, false, planes, n_p, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
                                             uint64_t bytes)
 {
-    return run_covariance(h, trajectory_planes, true, b200_sixdof_trajectory_width(h), planes, n_p, dst, bytes,
-                          "trajectory");
+    return run_covariance(h, true, true, planes, n_p, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, state_planes, true, 25, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, false, true, planes, n_p, dst, bytes, "state");
 }
 
 // np.linspace(lo, hi, n + 1) into e[0 .. n]: i * step + lo, the product rounded before the sum (never an fma), e[n] = hi.
@@ -1512,14 +1573,16 @@ static int linspace_edges(double lo, double hi, uint32_t n, double *e)
 // Histograms of the specs over the worlds, per group when `grouped` (hist_kernels.cu), into dst: the groups checked,
 // then the handle's status, then the specs (each plane < width), then `bytes`.  The edges and the group table are
 // computed here and copied to the device ahead of the launch.
-static int run_histograms(b200_sixdof *h, PlaneSource source, bool grouped, uint32_t width, const b200_histogram *specs,
-                          uint32_t n_specs, void *dst, uint64_t bytes, const char *what)
+static int run_histograms(b200_sixdof *h, bool ring, bool grouped, const b200_histogram *specs, uint32_t n_specs,
+                          void *dst, uint64_t bytes, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     if (grouped && h->group_sizes.empty()) return no_groups(what);
     CU(h, cudaSetDevice(h->device));
     HistParams P{};
-    static_cast<StatsParams &>(P) = source(h);
+    static_cast<StatsParams &>(P) = ensemble_rows(h, ring);
+    const uint32_t width = row_width(h, ring);
+    bool channel = false;
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_specs == 0 || n_specs > B200_MAX_HISTOGRAMS)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u histograms: 1 to %u", n_specs, B200_MAX_HISTOGRAMS);
@@ -1540,6 +1603,7 @@ static int run_histograms(b200_sixdof *h, PlaneSource source, bool grouped, uint
                 return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: plane %u, the %s has %u planes", k, hs.plane[a], what, width);
             if (hs.bins[a] == 0) return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: 0 bins", k);
             cells *= hs.bins[a];
+            channel = channel || hs.plane[a] >= 25;
         }
         if (hs.n_axes == 2 && hs.plane[0] == hs.plane[1])
             return fail(B200_ERR_INVALID_ARGUMENT, "histogram %u: plane %u twice", k, hs.plane[0]);
@@ -1578,6 +1642,10 @@ static int run_histograms(b200_sixdof *h, PlaneSource source, bool grouped, uint
     const uint64_t edge_bytes = edges.size() * 8ull, table_bytes = table.size() * sizeof(WorldGroup);
     edges.resize(edges.size() + table_bytes / 8);  // one copy to the device: the edges, then the group table
     std::memcpy(edges.data() + edge_bytes / 8, table.data(), table_bytes);
+    if (channel && bytes && dst) {
+        const int rc = refresh_channels(h, ring);
+        if (rc) return rc;
+    }
     return run_world_reduction(h, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
         cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes + table_bytes, cudaMemcpyHostToDevice, h->stream);
         if (e != cudaSuccess) return e;
@@ -1590,26 +1658,24 @@ static int run_histograms(b200_sixdof *h, PlaneSource source, bool grouped, uint
 int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                       uint64_t bytes)
 {
-    return run_histograms(h, trajectory_planes, false, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes,
-                          "trajectory");
+    return run_histograms(h, true, false, specs, n_specs, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes)
 {
-    return run_histograms(h, state_planes, false, 25, specs, n_specs, dst, bytes, "state");
+    return run_histograms(h, false, false, specs, n_specs, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                             uint64_t bytes)
 {
-    return run_histograms(h, trajectory_planes, true, b200_sixdof_trajectory_width(h), specs, n_specs, dst, bytes,
-                          "trajectory");
+    return run_histograms(h, true, true, specs, n_specs, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                        uint64_t bytes)
 {
-    return run_histograms(h, state_planes, true, 25, specs, n_specs, dst, bytes, "state");
+    return run_histograms(h, false, true, specs, n_specs, dst, bytes, "state");
 }
 
 // Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.
@@ -1685,14 +1751,11 @@ static SummaryParams summary_params(const b200_sixdof *h)
         const b200_threshold &t = h->sum_thr_list[i];
         S.t[i] = {(uint32_t)t.entity, t.plane, t.above ? 1 : 0, 0u, t.value};
     }
-    uint32_t seen = 0;
-    for (uint32_t p = 0; p < 25; ++p) {
+    S.width = row_width(h, false);
+    for (uint32_t p = 0; p < S.width; ++p) {
         bool used = h->sum_extrema;
         for (uint32_t i = 0; i < S.n_thr; ++i) used = used || S.t[i].plane == p;
-        if (used && !((seen >> p) & 1u)) {
-            seen |= 1u << p;
-            S.planes[S.n_planes++] = (uint8_t)p;
-        }
+        if (used) S.planes[S.n_planes++] = (uint8_t)p;
     }
     return S;
 }
@@ -1704,15 +1767,24 @@ static int summary_ready(b200_sixdof *h, const char *what)
     return B200_OK;
 }
 
-// Fold the samples of P as rows, sample k at tick tick0 + k * tick_step: row[p] is plane p of sample 0, and each sample
-// starts planes_per_sample planes after the one before it.
-static int run_summary_fold(b200_sixdof *h, const StatsParams &P, uint64_t tick0, uint64_t tick_step)
+// Fold the samples of the ring (ring) or the state as rows, sample k at tick tick0 + k * tick_step: row[p] is plane p of
+// sample 0, and each sample's planes start one segment stride after the one before it.  The channel planes are
+// recomputed first where the fold reads one: with extrema, or a threshold on a channel plane.
+static int run_summary_fold(b200_sixdof *h, bool ring, uint64_t tick0, uint64_t tick_step)
 {
     SummaryParams S = summary_params(h);
+    const StatsParams P = ensemble_rows(h, ring);
+    bool channel = false;
+    for (uint32_t i = 0; i < S.n_planes; ++i) channel = channel || S.planes[i] >= 25;
+    if (channel) {
+        const int rc = refresh_channels(h, ring);
+        if (rc) return rc;
+    }
     uint32_t p = 0;
     for (uint32_t k = 0; k < P.n_segs; ++k)
-        for (uint64_t j = 0; j < P.seg[k].n_planes && p < 25; ++j) S.row[p++] = P.seg[k].base + j * P.ld;
-    S.row_stride = P.planes_per_sample * P.ld;
+        for (uint64_t j = 0; j < P.seg[k].n_planes && p < kMaxRow; ++j) S.row[p++] = P.seg[k].base + j * P.ld;
+    S.row_stride = P.seg[0].stride;
+    S.chan_stride = P.seg[P.n_segs - 1].stride;
     S.n_rows = P.n_planes / P.planes_per_sample;
     S.tick0 = tick0;
     S.tick_step = tick_step;
@@ -1735,11 +1807,13 @@ int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_thres
         if (t[i].entity >= h->desc.n_entities)
             return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: entity row %llu, the world has %llu", i,
                         (unsigned long long)t[i].entity, (unsigned long long)h->desc.n_entities);
-        if (t[i].plane >= 25) return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: plane %u, a row has 25", i, t[i].plane);
+        if (t[i].plane >= row_width(h, false))
+            return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: plane %u, a row has %u", i, t[i].plane, row_width(h, false));
         if (std::isnan(t[i].value)) return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: the bound is NaN", i);
     }
     h->sum_begun = false;
-    if (extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 125ull * h->ld * 8ull));
+    h->sum_ever = true;  // the channel set, and so R, stays as it is from here on
+    if (extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 5ull * row_width(h, false) * h->ld * 8ull));
     const uint64_t thr_bytes = h->desc.n_worlds * n_thresholds * 26ull * 8ull;
     const int rc = grow_device(h, &h->sum_thr, &h->sum_thr_bytes, thr_bytes);
     if (rc) return rc;
@@ -1758,7 +1832,7 @@ int b200_sixdof_summary_add_state(b200_sixdof *h)
     CU(h, cudaSetDevice(h->device));
     int rc = summary_ready(h, "summary_add_state");
     if (rc) return rc;
-    return run_summary_fold(h, state_planes(h), h->tick, 0);
+    return run_summary_fold(h, false, h->tick, 0);
 }
 
 int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
@@ -1771,7 +1845,7 @@ int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
         return fail(B200_ERR_INVALID_ARGUMENT, "summary_add_trajectory needs a B200_TRAJ_FULL trajectory ring");
     // sample k was recorded when the ticks since the reset reached (k + 1) * every (sixdof_tick.cuh traj slots)
     const uint64_t every = h->desc.trajectory_every;
-    return run_summary_fold(h, trajectory_planes(h), h->tick - h->ticks_done + every, every);
+    return run_summary_fold(h, true, h->tick - h->ticks_done + every, every);
 }
 
 // dst on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer in
@@ -1783,7 +1857,8 @@ int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
     int rc = summary_ready(h, "extrema_download");
     if (rc) return rc;
     if (!h->sum_extrema) return fail(B200_ERR_INVALID_ARGUMENT, "extrema_download: summary_begin had no extrema");
-    const uint64_t per_body = 125ull * 8ull;
+    const uint32_t width = row_width(h, false);
+    const uint64_t per_body = 5ull * width * 8ull;
     const uint64_t want = h->n_bodies * per_body;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "extrema are %llu bytes, got %llu", (unsigned long long)want,
@@ -1796,7 +1871,7 @@ int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
     for (uint64_t b0 = 0; b0 < h->n_bodies; b0 += chunk) {
         const uint64_t nb = std::min(chunk, h->n_bodies - b0);
         double *out = direct ? (double *)dst : h->staging;
-        CU(h, launch_extrema_table(h->sum_ext, h->ld, b0, nb, out, h->stream));
+        CU(h, launch_extrema_table(h->sum_ext, h->ld, width, b0, nb, out, h->stream));
         h->timings.kernel_launches++;
         if (!direct) CU(h, cudaMemcpyAsync((char *)dst + b0 * per_body, out, nb * per_body, cudaMemcpyDefault, h->stream));
         CU(h, cudaStreamSynchronize(h->stream)); // the staging buffer is reused by the next chunk
@@ -1820,6 +1895,117 @@ int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes)
     CU(h, cudaMemcpyAsync(dst, h->sum_thr, want, cudaMemcpyDefault, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
+}
+
+// ---- derived channels (channel_kernels.cu)
+
+// channel k of c: 0 when it keeps the contract of include/b200_sixdof.h, else the refusal
+static int check_channel(const b200_channel &ch, uint32_t k)
+{
+    auto finite3 = [](const double *v) { return std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2]); };
+    auto zero3 = [](const double *v) { return v[0] == 0.0 && v[1] == 0.0 && v[2] == 0.0; };
+    if (ch.reserved != 0) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: reserved field is not 0", k);
+    if (ch.kind == B200_CHANNEL_NORM) {
+        if (ch.n < 1 || ch.n > 3) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: a norm of %u planes, 1 to 3", k, ch.n);
+        for (uint32_t i = 0; i < ch.n; ++i) {
+            if (ch.plane[i] >= 25) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: plane %u, a row has 25", k, ch.plane[i]);
+            for (uint32_t j = 0; j < i; ++j)
+                if (ch.plane[j] == ch.plane[i]) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: plane %u twice", k, ch.plane[i]);
+            if (!std::isfinite(ch.c[i])) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: offset %u is not finite", k, i);
+        }
+        if (!std::isfinite(ch.r0)) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: r0 is not finite", k);
+        return B200_OK;
+    }
+    if (ch.kind == B200_CHANNEL_AXIS_ANGLE) {
+        if (ch.n != 0 && ch.n != 3)
+            return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: an axis angle takes n = 0 (fixed direction) or 3 (planes), not %u",
+                        k, ch.n);
+        if (ch.n == 3 && ch.plane[0] > 22)
+            return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: planes %u .. %u run past plane 24", k, ch.plane[0], ch.plane[0] + 2);
+        if (!finite3(ch.c)) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: the body axis is not finite", k);
+        if (zero3(ch.c)) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: the body axis is zero", k);
+        if (ch.n == 0 && !finite3(ch.d)) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: the direction is not finite", k);
+        if (ch.n == 0 && zero3(ch.d)) return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: the direction is zero", k);
+        return B200_OK;
+    }
+    return fail(B200_ERR_INVALID_ARGUMENT, "channel %u: unknown kind %u", k, ch.kind);
+}
+
+int b200_sixdof_set_channels(b200_sixdof *h, const b200_channel *c, uint32_t n)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (n > B200_MAX_CHANNELS) return fail(B200_ERR_INVALID_ARGUMENT, "%u channels: at most %u", n, B200_MAX_CHANNELS);
+    if (n && !c) return fail(B200_ERR_INVALID_ARGUMENT, "null channels");
+    if (h->traj && h->traj_planes != 25)
+        return fail(B200_ERR_INVALID_ARGUMENT, "channels need a B200_TRAJ_FULL trajectory ring: this one is %u wide",
+                    h->traj_planes);
+    if (h->sum_ever)
+        return fail(B200_ERR_INVALID_ARGUMENT, "set_channels after b200_sixdof_summary_begin: the summary's row width is fixed");
+    for (uint32_t k = 0; k < n; ++k) {
+        const int rc = check_channel(c[k], k);
+        if (rc) return rc;
+    }
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaStreamSynchronize(h->stream));  // no reduction in flight still reads the planes replaced here
+    double *ring = nullptr, *state = nullptr;
+    if (n) {
+        const cudaError_t e = cudaMalloc(&state, (uint64_t)n * h->ld * 8ull);
+        if (e != cudaSuccess) return cuda_fail(h, e, "cudaMalloc(channel state planes)");
+        if (h->traj) {
+            const cudaError_t e2 = cudaMalloc(&ring, h->desc.trajectory_capacity * n * h->ld * 8ull);
+            if (e2 != cudaSuccess) {
+                cudaFree(state);
+                return cuda_fail(h, e2, "cudaMalloc(channel ring planes)");
+            }
+        }
+    }
+    if (h->chan_ring) CU(h, cudaFree(h->chan_ring));
+    if (h->chan_state) CU(h, cudaFree(h->chan_state));
+    h->chan_ring = ring;
+    h->chan_state = state;
+    h->channels.assign(c, c + n);
+    return B200_OK;
+}
+
+uint32_t b200_sixdof_channels(const b200_sixdof *h) { return h ? (uint32_t)h->channels.size() : 0; }
+
+// The channel planes of the ring's samples (ring) or of the state, recomputed, into dst = [samples][n_bodies][n_c] in
+// slices of at most 256 MiB of samples through the staging buffer.
+static int download_channels(b200_sixdof *h, bool ring, void *dst, uint64_t bytes, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t n = ring ? b200_sixdof_trajectory_len(h) : 1, W = h->channels.size();
+    const uint64_t per_sample = h->n_bodies * W * 8ull, want = n * per_sample;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s channels are %llu bytes, got %llu", what, (unsigned long long)want,
+                    (unsigned long long)bytes);
+    if (want == 0) return B200_OK;
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    int rc = refresh_channels(h, ring);
+    if (rc) return rc;
+    const double *planes = ring ? h->chan_ring : h->chan_state;
+    const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(n, (256ull << 20) / per_sample));
+    if ((rc = ensure_staging(h, chunk * per_sample))) return rc;
+    for (uint64_t s0 = 0; s0 < n; s0 += chunk) {
+        const uint64_t ns = std::min(chunk, n - s0);
+        CU(h, launch_traj_to_aos(planes + s0 * W * h->ld, h->staging, ns, h->n_bodies, h->ld, (uint32_t)W, h->stream));
+        h->timings.kernel_launches++;
+        CU(h, cudaMemcpyAsync((char *)dst + s0 * per_sample, h->staging, ns * per_sample, cudaMemcpyDefault, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+    }
+    return B200_OK;
+}
+
+int b200_sixdof_trajectory_channels(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return download_channels(h, true, dst, bytes, "trajectory");
+}
+
+int b200_sixdof_state_channels(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return download_channels(h, false, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_reset(b200_sixdof *h)

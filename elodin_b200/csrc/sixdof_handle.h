@@ -72,11 +72,16 @@ struct b200_sixdof {
     // trajectory
     double *traj = nullptr;
     uint32_t traj_planes = 13;   // 25 with B200_TRAJ_FULL
+    // derived channels (b200_sixdof_set_channels): the channel set and its planes, [capacity][n_c][ld] for the ring and
+    // [n_c][ld] for the state, recomputed by every entry that reads them (channel_kernels.cu)
+    std::vector<b200_channel> channels;
+    double *chan_ring = nullptr, *chan_state = nullptr;
     // run summaries (b200_sixdof_summary_*): device accumulators, allocated on first use, kept across begins
     bool sum_begun = false;
+    bool sum_ever = false;           // summary_begin has been called: the channel set (the row width) is fixed
     bool sum_extrema = false;
     std::vector<b200_threshold> sum_thr_list;
-    double *sum_ext = nullptr;       // 125 planes of ld (SummaryParams::ext)
+    double *sum_ext = nullptr;       // 5 R planes of ld, R = 25 + channels (SummaryParams::ext)
     double *sum_thr = nullptr;       // [n_worlds][thresholds][26] (SummaryParams::thr)
     uint64_t sum_thr_bytes = 0;
     // plumbing

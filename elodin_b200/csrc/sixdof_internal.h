@@ -159,14 +159,18 @@ __host__ __device__ inline void stats_merge(StatsGroup &a, const StatsGroup &b)
     a.n = n;
 }
 
-// Planes to reduce: segment s holds n_planes planes at base + k*ld (k < n_planes); plane i of the launch is plane i of
-// the concatenated segments.  Group (plane i, entity e) goes to out[((i / W) * n_entities + e) * W + i % W][5],
-// W = planes_per_sample.  Only bodies b = w * n_entities + e with w < n_worlds are read (never the padding to ld).
+// Planes to reduce: the planes of a sample are the concatenated segments' planes, segment k holding n_planes planes per
+// sample, plane j of sample s at base + s * stride + j * ld; plane i of the launch is plane i % W of sample i / W,
+// W = planes_per_sample = the sum of the segments' n_planes.  Group (plane i, entity e) goes to
+// out[((i / W) * n_entities + e) * W + i % W][5].  Only bodies b = w * n_entities + e with w < n_worlds are read (never
+// the padding to ld).  A ring of W planes per sample is one segment of stride W * ld, so plane i is at base + i * ld.
+constexpr uint32_t kMaxSegs = 5; // the state's four columns, then the channel planes (sixdof_abi.cu:ensemble_rows)
 struct StatsParams {
     struct Seg {
         const double *base;
         uint64_t n_planes;
-    } seg[4];
+        uint64_t stride;
+    } seg[kMaxSegs];
     uint32_t n_segs;
     uint32_t planes_per_sample;
     uint64_t n_planes;
@@ -175,18 +179,24 @@ struct StatsParams {
     uint64_t n_entities;
     double *out;
 };
-// plane i (< n_planes) of the concatenated segments
-__device__ inline const double *stats_plane(const StatsParams &S, uint64_t i)
+// plane j (< planes_per_sample) of sample s
+__device__ inline const double *sample_plane(const StatsParams &S, uint64_t s, uint64_t j)
 {
     const double *p = nullptr;
 #pragma unroll
-    for (uint32_t k = 0; k < 4; ++k) { // constant indices: the segment table stays in the parameter space
+    for (uint32_t k = 0; k < kMaxSegs; ++k) { // constant indices: the segment table stays in the parameter space
         if (!p && k < S.n_segs) {
-            if (i < S.seg[k].n_planes) p = S.seg[k].base + i * S.ld;
-            else i -= S.seg[k].n_planes;
+            if (j < S.seg[k].n_planes) p = S.seg[k].base + s * S.seg[k].stride + j * S.ld;
+            else j -= S.seg[k].n_planes;
         }
     }
-    return p; // i < n_planes: always set
+    return p; // j < planes_per_sample: always set
+}
+// plane i (< n_planes) of the concatenated samples
+__device__ inline const double *stats_plane(const StatsParams &S, uint64_t i)
+{
+    const uint64_t s = i / S.planes_per_sample;
+    return sample_plane(S, s, i - s * S.planes_per_sample);
 }
 // Rows of chosen worlds (layout_kernels.cu:gather_worlds_kernel): samples [s0, s0 + n_samples) of S's planes for the
 // worlds worlds[0 .. n_worlds) (device memory, each < S.n_worlds, repeats allowed) into S.out =
@@ -316,16 +326,19 @@ std::vector<WorldGroup> hist_group_table(const uint64_t *sizes, uint64_t n_group
 cudaError_t launch_histograms(const HistParams &P, const WorldGroup *groups, const std::vector<WorldGroup> &table,
                               int *launches, cudaStream_t s);
 
-// Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows: plane p of row r at
-// row[p] + r * row_stride + b for body b < n_bodies, at tick tick0 + r * tick_step.
+// Run summaries over the time axis (summary_kernels.cu).  A fold reads n_rows rows of R = 25 + n_channels planes:
+// plane p of row r at row[p] + r * (p < 25 ? row_stride : chan_stride) + b for body b < n_bodies, at tick
+// tick0 + r * tick_step.
 //   ext: extrema accumulators, plane p * 5 + f of ld doubles (f = min, max, min_tick, max_tick, first_nonfinite_tick),
-//        i.e. body b's 125 values read in plane order are its row of the public table; nullptr = no extrema.
-//   thr: the public threshold table itself, [n_worlds][n_thr][26] f64 (tick, 25 planes); nullptr = no thresholds.
+//        i.e. body b's 5 R values read in plane order are its row of the public table; nullptr = no extrema.
+//   thr: the public threshold table itself, [n_worlds][n_thr][26] f64 (tick, the 25 raw planes); nullptr = no thresholds.
 // Ticks are stored as f64 (exact below 2^53), -1 = none; every accumulator has one owning thread per fold.
-// A fold reads only the planes listed in planes[0 .. n_planes): all 25 with extrema, else the thresholds' planes.
+// A fold reads only the planes listed in planes[0 .. n_planes): all R with extrema, else the thresholds' planes.
+constexpr uint32_t kMaxRow = 25 + B200_MAX_CHANNELS;
 struct SummaryParams {
-    const double *row[25];
+    const double *row[kMaxRow];
     uint64_t row_stride;
+    uint64_t chan_stride;
     uint64_t n_rows;
     uint64_t tick0, tick_step;
     uint64_t ld, n_bodies;
@@ -334,7 +347,8 @@ struct SummaryParams {
     double *ext;
     double *thr;
     uint32_t n_planes;
-    uint8_t planes[25];
+    uint32_t width;    // R: the planes of a row, and of an extrema table row
+    uint8_t planes[kMaxRow];
     struct Thr {
         uint32_t entity, plane;
         int32_t above;
@@ -346,7 +360,23 @@ struct SummaryParams {
 cudaError_t launch_summary_clear(const SummaryParams &S, int *launches, cudaStream_t s);
 // fold S's rows into the accumulators; launches written to *launches (0 when there are no rows, else 1)
 cudaError_t launch_summary_fold(const SummaryParams &S, int *launches, cudaStream_t s);
-// extrema accumulators of bodies [b0, b0 + nb) -> out[nb][125] (the public table's rows)
-cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint64_t b0, uint64_t nb, double *out, cudaStream_t s);
+// extrema accumulators of rows of R planes, bodies [b0, b0 + nb) -> out[nb][5 R] (the public table's rows)
+cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint32_t R, uint64_t b0, uint64_t nb, double *out,
+                                 cudaStream_t s);
+
+// Derived channels (channel_kernels.cu, include/b200_sixdof.h b200_channel): n_c values per body of samples
+// [0, n_samples), from the 25 planes of each sample (plane p of sample s at row[p] + s * row_stride) into
+// out + (s * n_c + k) * ld + b, for bodies b < n_bodies only.
+struct ChannelParams {
+    const double *row[25];
+    uint64_t row_stride;
+    double *out;
+    uint64_t ld, n_bodies, n_samples;
+    uint32_t n_c;
+    uint32_t pad;
+    b200_channel c[B200_MAX_CHANNELS];
+};
+// one launch on s (*launches = 1; 0 without samples, bodies or channels)
+cudaError_t launch_channels(const ChannelParams &P, int *launches, cudaStream_t s);
 
 } // namespace b200

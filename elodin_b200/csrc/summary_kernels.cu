@@ -1,7 +1,8 @@
 // Run summaries over the time axis: per (world, entity, plane) extrema and per (world, threshold) first events
 // (include/b200_sixdof.h b200_sixdof_summary_*).
 //
-// Shape of a fold.  Rows are SoA planes (the trajectory ring [samples][25][ld], or the state columns), so a thread owns
+// Shape of a fold.  Rows are SoA planes (the trajectory ring [samples][25][ld], or the state columns, then the channel
+// planes of sixdof_abi.cu:ensemble_rows), so a thread owns
 // one (body, plane): block (x, y) takes 256 consecutive bodies of plane planes[y], and every thread walks the fold's rows
 // in order, one coalesced double per row, four loads in flight.  The thread's accumulators (5 extrema planes of ld,
 // and the tick of each threshold on its (entity, plane)) are read once before the walk and written once after it; a
@@ -71,7 +72,7 @@ __global__ void __launch_bounds__(kSumThreads, 4) summary_fold_kernel(const __gr
         }
     };
     const double *src = S.row[p] + b;
-    const uint64_t st = S.row_stride;
+    const uint64_t st = p < 25 ? S.row_stride : S.chan_stride;
     uint64_t r = 0;
     for (; r + 4 <= S.n_rows; r += 4) { // four loads in flight before the first is used
         const double x0 = __ldcs(src + r * st), x1 = __ldcs(src + (r + 1) * st), x2 = __ldcs(src + (r + 2) * st),
@@ -94,7 +95,7 @@ __global__ void __launch_bounds__(kSumThreads, 4) summary_fold_kernel(const __gr
     for (uint32_t i = 0; i < B200_MAX_THRESHOLDS; ++i) {
         if (at[i] != ~0u) { // fired inside this fold, earlier than anything folded before: capture the row
             double *o = S.thr + (w * S.n_thr + i) * kThrFields;
-            const uint64_t off = (uint64_t)at[i] * st + b;
+            const uint64_t off = (uint64_t)at[i] * S.row_stride + b;
             o[0] = best[i];
 #pragma unroll
             for (uint32_t j = 0; j < 25; ++j) o[1 + j] = S.row[j][off];
@@ -103,20 +104,22 @@ __global__ void __launch_bounds__(kSumThreads, 4) summary_fold_kernel(const __gr
 }
 
 // extrema planes: min, max = NaN, the three ticks = -1; threshold table: tick = -1, planes = NaN
-__global__ void __launch_bounds__(kSumThreads) summary_clear_kernel(double *ext, uint64_t ld, double *thr, uint64_t thr_len)
+__global__ void __launch_bounds__(kSumThreads) summary_clear_kernel(double *ext, uint64_t ld, uint32_t R, double *thr,
+                                                                    uint64_t thr_len)
 {
-    const uint64_t ext_len = ext ? 125 * ld : 0;
+    const uint64_t ext_len = ext ? 5ull * R * ld : 0;
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < ext_len + thr_len; i += (uint64_t)gridDim.x * blockDim.x) {
         if (i < ext_len) ext[i] = (i / ld) % 5 < 2 ? nan_value() : -1.0;
         else thr[i - ext_len] = (i - ext_len) % kThrFields == 0 ? -1.0 : nan_value();
     }
 }
 
-__global__ void __launch_bounds__(kSumThreads) extrema_table_kernel(const double *__restrict__ ext, uint64_t ld, uint64_t b0,
-                                                                    uint64_t nb, double *__restrict__ out)
+__global__ void __launch_bounds__(kSumThreads) extrema_table_kernel(const double *__restrict__ ext, uint64_t ld, uint32_t R,
+                                                                    uint64_t b0, uint64_t nb, double *__restrict__ out)
 {
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nb * 125; i += (uint64_t)gridDim.x * blockDim.x)
-        out[i] = ext[(i % 125) * ld + b0 + i / 125];
+    const uint64_t F = 5ull * R;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nb * F; i += (uint64_t)gridDim.x * blockDim.x)
+        out[i] = ext[(i % F) * ld + b0 + i / F];
 }
 
 } // namespace
@@ -124,11 +127,11 @@ __global__ void __launch_bounds__(kSumThreads) extrema_table_kernel(const double
 cudaError_t launch_summary_clear(const SummaryParams &S, int *launches, cudaStream_t s)
 {
     *launches = 0;
-    const uint64_t ext_len = S.ext ? 125 * S.ld : 0;
+    const uint64_t ext_len = S.ext ? 5ull * S.width * S.ld : 0;
     const uint64_t thr_len = (S.thr && S.n_entities) ? S.n_bodies / S.n_entities * S.n_thr * kThrFields : 0;
     if (ext_len + thr_len == 0) return cudaSuccess;
     const uint64_t blocks = std::min<uint64_t>((ext_len + thr_len + kSumThreads - 1) / kSumThreads, 64ull * kNumSMs * 8);
-    summary_clear_kernel<<<(unsigned)blocks, kSumThreads, 0, s>>>(S.ext, S.ld, S.thr, thr_len);
+    summary_clear_kernel<<<(unsigned)blocks, kSumThreads, 0, s>>>(S.ext, S.ld, S.width, S.thr, thr_len);
     *launches = 1;
     return cudaGetLastError();
 }
@@ -143,11 +146,12 @@ cudaError_t launch_summary_fold(const SummaryParams &S, int *launches, cudaStrea
     return cudaGetLastError();
 }
 
-cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint64_t b0, uint64_t nb, double *out, cudaStream_t s)
+cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint32_t R, uint64_t b0, uint64_t nb, double *out,
+                                 cudaStream_t s)
 {
     if (nb == 0) return cudaSuccess;
-    const uint64_t blocks = std::min<uint64_t>((nb * 125 + kSumThreads - 1) / kSumThreads, 64ull * kNumSMs * 8);
-    extrema_table_kernel<<<(unsigned)blocks, kSumThreads, 0, s>>>(ext, ld, b0, nb, out);
+    const uint64_t blocks = std::min<uint64_t>((nb * 5 * R + kSumThreads - 1) / kSumThreads, 64ull * kNumSMs * 8);
+    extrema_table_kernel<<<(unsigned)blocks, kSumThreads, 0, s>>>(ext, ld, R, b0, nb, out);
     return cudaGetLastError();
 }
 

@@ -222,6 +222,12 @@ class B200Exec:
             return (self.trajectory_len(), self.n_entities, max(self.trajectory_width(), 13))
         return (self.n_entities, 25)
 
+    def _rows(self, ring: bool) -> tuple:
+        """The rows an ensemble reduction or run summary reads, as table axes: _planes() with the row widened by the
+        channels (set_channels; channel k is plane 25 + k)."""
+        p = self._planes(ring)
+        return p[:-1] + (p[-1] + self.n_channels,)
+
     def trajectory(self) -> np.ndarray:
         """[samples, n_worlds, n_entities, width] — see trajectory_width()."""
         self.sync()
@@ -277,7 +283,7 @@ class B200Exec:
     def trajectory_stats(self, out: Optional[np.ndarray] = None) -> np.ndarray:
         """The ring's samples reduced over the worlds: [samples, n_entities, width, 5] with the fields (count, mean,
         m2 = sum (x - mean)^2, min, max) over the finite values (count = 0: NaN in the other four)."""
-        shape = self._planes(ring=True) + (_lib.STATS_FIELDS,)
+        shape = self._rows(ring=True) + (_lib.STATS_FIELDS,)
         if out is None:
             return self._reduce("stats", True, (), shape)
         if out.shape != shape or out.dtype != np.float64 or not out.flags.c_contiguous:
@@ -292,7 +298,7 @@ class B200Exec:
     def state_stats(self) -> np.ndarray:
         """The current state reduced over the worlds: [n_entities, 25, 5] — world_pos[7], world_vel[6],
         world_accel[6], force[6] (the B200_TRAJ_FULL sample layout), fields as trajectory_stats()."""
-        return self._reduce("stats", False, (), self._planes(ring=False) + (_lib.STATS_FIELDS,))
+        return self._reduce("stats", False, (), self._rows(ring=False) + (_lib.STATS_FIELDS,))
 
     # ---- ensemble quantiles (order statistics over the world axis, on the device) -------------------------------
     @staticmethod
@@ -306,12 +312,12 @@ class B200Exec:
         [samples, n_entities, width, n_q] (NaN where no world is finite).  With `out_ptr` (a host or device pointer,
         e.g. a torch CUDA tensor's data_ptr()) the table is written there and nothing is returned."""
         lv = self._levels(q)
-        return self._reduce("quantiles", True, lv, self._planes(ring=True) + (lv[1],), out_ptr)
+        return self._reduce("quantiles", True, lv, self._rows(ring=True) + (lv[1],), out_ptr)
 
     def state_quantiles(self, q) -> np.ndarray:
         """The current state: quantiles over the worlds, [n_entities, 25, n_q] in the B200_TRAJ_FULL plane layout."""
         lv = self._levels(q)
-        return self._reduce("quantiles", False, lv, self._planes(ring=False) + (lv[1],))
+        return self._reduce("quantiles", False, lv, self._rows(ring=False) + (lv[1],))
 
     def quantile_reads(self) -> float:
         """Reads of the reduced planes the last quantile call made, averaged over its groups."""
@@ -382,12 +388,12 @@ class B200Exec:
     def trajectory_group_stats(self) -> np.ndarray:
         """trajectory_stats() per group: [samples, G, n_entities, width, 5]; group g's record has the bits of
         trajectory_stats() on a batch of exactly its worlds."""
-        n, E, W = self._planes(ring=True)
+        n, E, W = self._rows(ring=True)
         return self._reduce("group_stats", True, (), (n, self.world_groups, E, W, _lib.STATS_FIELDS))
 
     def state_group_stats(self) -> np.ndarray:
         """state_stats() per group: [G, n_entities, 25, 5]."""
-        return self._reduce("group_stats", False, (), (self.world_groups,) + self._planes(ring=False) + (_lib.STATS_FIELDS,))
+        return self._reduce("group_stats", False, (), (self.world_groups,) + self._rows(ring=False) + (_lib.STATS_FIELDS,))
 
     def trajectory_group_histograms(self, specs) -> np.ndarray:
         """trajectory_histograms(specs) per group: [samples, G, sum of the record lengths]."""
@@ -404,13 +410,13 @@ class B200Exec:
         trajectory_quantiles(q) on a batch of exactly its worlds (NaN for an empty group).  Like the ungrouped tables,
         they do not merge across the ranks of a world-sharded campaign: each rank gets its own."""
         lv = self._levels(q)
-        n, E, W = self._planes(ring=True)
+        n, E, W = self._rows(ring=True)
         return self._reduce("group_quantiles", True, lv, (n, self.world_groups, E, W, lv[1]))
 
     def state_group_quantiles(self, q) -> np.ndarray:
         """state_quantiles(q) per group: [G, n_entities, 25, n_q]."""
         lv = self._levels(q)
-        return self._reduce("group_quantiles", False, lv, (self.world_groups,) + self._planes(ring=False) + (lv[1],))
+        return self._reduce("group_quantiles", False, lv, (self.world_groups,) + self._rows(ring=False) + (lv[1],))
 
     def trajectory_group_covariance(self, planes) -> np.ndarray:
         """trajectory_covariance(planes) per group: [samples, G, n_entities, 1 + p + p*p]; group g's records have the
@@ -426,10 +432,36 @@ class B200Exec:
         sel = self._selection(planes)
         return self._reduce("group_covariance", False, sel, (self.world_groups, self.n_entities, 1 + sel[1] + sel[1] ** 2))
 
+    # ---- derived channels (per-body values computed on the device, reduced as planes 25 + k) --------------------
+    def set_channels(self, channels: Sequence) -> None:
+        """Replace the channel set with `channels` (at most MAX_CHANNELS _lib.Channel records, or tuples (kind, n,
+        planes, c, d, r0)); an empty set clears it.  Channel k is plane 25 + k of every ensemble table's rows.  Must come
+        before summary_begin."""
+        chans = list(channels)
+        arr = (_lib.Channel * max(len(chans), 1))()
+        for k, c in enumerate(chans):
+            arr[k] = c if isinstance(c, _lib.Channel) else _lib.channel(*c)
+        _lib.check(self._L.b200_sixdof_set_channels(self._h, arr, len(chans)))
+
+    @property
+    def n_channels(self) -> int:
+        """The number of channels set, 0 = none."""
+        return int(self._L.b200_sixdof_channels(self._h))
+
+    def trajectory_channels(self, out_ptr: Optional[int] = None) -> Optional[np.ndarray]:
+        """The channels of the ring's samples, recomputed on the device: [samples, n_worlds, n_entities, n_c].  With
+        `out_ptr` (a host or device pointer) they are written there and nothing is returned."""
+        return self._reduce("channels", True, (), (self.trajectory_len(), self.n_worlds, self.n_entities,
+                                                   self.n_channels), out_ptr)
+
+    def state_channels(self) -> np.ndarray:
+        """The channels of the current state: [n_worlds, n_entities, n_c]."""
+        return self._reduce("channels", False, (), (self.n_worlds, self.n_entities, self.n_channels))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
         """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
-        up to 8 (entity row, plane 0..24, above, value) tuples, each firing on value > bound (above) or < bound."""
+        up to 8 (entity row, plane 0..24 or 25 + channel, above, value) tuples, each firing on value > bound (above) or < bound."""
         ts = list(thresholds)
         arr = (_lib.Threshold * max(len(ts), 1))()
         for i, (entity, plane, above, value) in enumerate(ts):
@@ -446,10 +478,10 @@ class B200Exec:
         _lib.check(self._L.b200_sixdof_summary_add_trajectory(self._h))
 
     def extrema(self) -> np.ndarray:
-        """[n_worlds, n_entities, 25, 5]: (min, max, min_tick, max_tick, first_nonfinite_tick) of every plane of the
-        B200_TRAJ_FULL row layout over the rows folded; min / max over the finite values (NaN if none), ticks -1 where
+        """[n_worlds, n_entities, 25 + n_c, 5]: (min, max, min_tick, max_tick, first_nonfinite_tick) of every plane of
+        the B200_TRAJ_FULL row layout, then of every channel, over the rows folded; min / max over the finite values (NaN if none), ticks -1 where
         they never applied."""
-        out = np.empty((self.n_worlds, self.n_entities, 25, _lib.EXTREMA_FIELDS))
+        out = np.empty((self.n_worlds,) + self._rows(ring=False) + (_lib.EXTREMA_FIELDS,))
         _lib.check(self._L.b200_sixdof_extrema_download(self._h, out.ctypes.data, out.nbytes))
         return out
 

@@ -439,7 +439,8 @@ class World:
               ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
               thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
               covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
-              groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None) -> "Exec":
+              groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
+              channels: Optional[Sequence["Channel"]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -459,7 +460,11 @@ class World:
         at most MAX_RETAINED_BODIES worlds x entities) also records the full rows of those worlds, gathered on the
         device, so that `history_worlds`, `history` (world 0, if retained), `attach_db`, `write_db`,
         `export.export_csv` and `monte_carlo.write_run_databases` work for them as in the default mode, with the same
-        rows bit for bit; `Exec.retained` is the tuple in the order given."""
+        rows bit for bit; `Exec.retained` is the tuple in the order given.  `channels` (up to 8 `Norm` / `AxisAngle`
+        objects with distinct names) adds derived values computed on the device from each body's row -- speeds,
+        distances, altitudes, pointing angles -- as the component "<entity>.channels" (channel k at index k, in the
+        order given; `Exec.channels` lists the names), which every ensemble table, the extrema and the thresholds
+        cover like the sampled components."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -467,7 +472,8 @@ class World:
         if backend == "b200-fast":
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
-                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain)
+                    ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain,
+                    channels)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -523,10 +529,16 @@ _SAMPLED = {"world_pos": (0, 7), "world_vel": (7, 13), "world_accel": (13, 19), 
 _ENSEMBLE_RING_BYTES = 256 << 20  # device memory of the ensemble mode's trajectory ring
 
 
+# the derived channels of World.build(..., channels=[...]) in ensemble mode: planes 25 + k of an ensemble row, addressed
+# as one more component, at most MAX_CHANNELS wide (build checks an index against the channels it has)
+_CHANNELS = "channels"
+_CHANNEL_SPAN = (_lib.ROW_PLANES, _lib.ROW_PLANES + _lib.MAX_CHANNELS)
+
+
 def _sampled_span(pair: str, what: str):
-    """`<entity>.<component>` -> (entity, (first, end) plane of the component in a 25-plane row)."""
+    """`<entity>.<component>` -> (entity, (first, end) plane of the component in a 25-plane row, or of the channels)."""
     ent, _, comp = pair.rpartition(".")
-    span = _SAMPLED.get(comp)
+    span = _CHANNEL_SPAN if comp == _CHANNELS else _SAMPLED.get(comp)
     if not ent or span is None:
         raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
                                   f"component not found: {pair} ({what} cover {', '.join(_SAMPLED)})")
@@ -558,8 +570,9 @@ def _quantile_levels(levels) -> np.ndarray:
     return np.array(out)
 
 
-def _covariance_planes(spec):
-    """World.build(..., covariance=...) -> (planes of the 25-plane row layout, labels), selection order kept."""
+def _covariance_planes(spec, channel_names=()):
+    """World.build(..., covariance=...) -> (planes of the 25-plane row layout, channel k at 25 + k, labels), selection
+    order kept; a channel's label is its name."""
     if isinstance(spec, (str, bytes)) or not isinstance(spec, Sequence):
         raise TypeError(f"covariance takes a sequence of components or (component, indices) pairs, got {spec!r}")
     planes, labels = [], []
@@ -572,16 +585,20 @@ def _covariance_planes(spec):
             comp, idx = None, None
         if not isinstance(comp, str):
             raise TypeError(f"covariance item {item!r}: a component name or a (component, indices) pair")
-        span = _SAMPLED.get(comp)
+        span = (_lib.ROW_PLANES, _lib.ROW_PLANES + len(channel_names)) if comp == _CHANNELS else _SAMPLED.get(comp)
         if span is None:
             raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
                                       f"component not found: {comp} (ensemble covariance covers {', '.join(_SAMPLED)})")
         for i in range(span[1] - span[0]) if idx is None else idx:
+            if comp == _CHANNELS:
+                _sampled_plane(_CHANNEL_SPAN, i, f"covariance item {item!r}")
+                if i >= len(channel_names):
+                    raise ValueError(f"covariance item {item!r}: channel {int(i)}, this Exec has {len(channel_names)}")
             plane = _sampled_plane(span, i, f"covariance item {item!r}")
             if plane in planes:
                 raise ValueError(f"covariance selects {comp}[{int(i)}] twice")
             planes.append(plane)
-            labels.append(f"{comp}[{int(i)}]")
+            labels.append(channel_names[int(i)] if comp == _CHANNELS else f"{comp}[{int(i)}]")
     if not 1 <= len(planes) <= _lib.MAX_COV_PLANES:
         raise ValueError(f"covariance selects {len(planes)} planes: 1 to {_lib.MAX_COV_PLANES}")
     return planes, labels
@@ -639,6 +656,114 @@ def _histogram_specs(histograms) -> List["Histogram"]:
     if not 1 <= len(histograms) <= _lib.MAX_HISTOGRAMS:
         raise ValueError(f"{len(histograms)} histograms: 1 to {_lib.MAX_HISTOGRAMS}")
     return list(histograms)
+
+
+def _finite3(v, where: str) -> tuple:
+    """A finite, non-zero 3-vector, as floats."""
+    a = np.asarray(v, dtype=np.float64) if not isinstance(v, str) else np.zeros(0)
+    if a.shape != (3,) or not np.all(np.isfinite(a)):
+        raise ValueError(f"{where}: {v!r} is not a finite 3-vector")
+    if not np.any(a != 0.0):
+        raise ValueError(f"{where}: the vector is zero")
+    return tuple(float(x) for x in a)
+
+
+class Channel:
+    """A derived channel of World.build(..., ensemble=True, channels=[...]): see `Norm` and `AxisAngle`."""
+
+    name: str
+
+    def _record(self) -> "_lib.Channel":
+        raise NotImplementedError
+
+
+class Norm(Channel):
+    """`Norm(name, component, indices, center=None, minus=0.0)`: sqrt(sum_i (x_i - center_i)^2) - minus over 1 to 3
+    distinct components `indices` of a sampled component (world_pos, world_vel, world_accel, force), per body and row,
+    in correctly rounded f64 operations summed in index order (numpy's bits for the same expression).  Speed:
+    Norm("speed", "world_vel", (3, 4, 5)); range from a pad: Norm("range", "world_pos", (4, 5), center=(x0, y0));
+    altitude over a sphere: Norm("alt", "world_pos", (4, 5, 6), minus=R)."""
+
+    def __init__(self, name: str, component: str, indices, center=None, minus: float = 0.0):
+        where = f"Norm({name!r}, {component!r}, {indices!r})"
+        if not isinstance(name, str) or not name:
+            raise ValueError(f"{where}: the name must be a non-empty string")
+        span = _SAMPLED.get(component)
+        if span is None:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                      f"component not found: {component} (channels cover {', '.join(_SAMPLED)})")
+        idx = tuple(indices) if isinstance(indices, (tuple, list)) else (indices,)
+        if not 1 <= len(idx) <= 3:
+            raise ValueError(f"{where}: 1 to 3 indices")
+        self.planes = tuple(_sampled_plane(span, i, where) for i in idx)
+        if len(set(self.planes)) != len(self.planes):
+            raise ValueError(f"{where}: an index listed twice")
+        c = (0.0,) * len(idx) if center is None else tuple(np.asarray(center, dtype=np.float64).ravel())
+        if len(c) != len(idx) or not all(np.isfinite(c)):
+            raise ValueError(f"{where}: center {center!r} is not {len(idx)} finite numbers")
+        if isinstance(minus, (bool, np.bool_)) or not np.isfinite(float(minus)):
+            raise ValueError(f"{where}: minus {minus!r} is not a finite number")
+        self.name, self.center, self.minus = name, tuple(float(x) for x in c), float(minus)
+
+    def _record(self) -> "_lib.Channel":
+        return _lib.channel(_lib.CHANNEL_NORM, len(self.planes), self.planes, self.center, (), self.minus)
+
+    def __repr__(self) -> str:
+        return f"Norm({self.name!r}, planes={self.planes}, center={self.center}, minus={self.minus})"
+
+
+class AxisAngle(Channel):
+    """`AxisAngle(name, axis, toward)`: the angle in radians, in [0, pi], between the body-frame `axis` rotated into the
+    world frame by the body's world_pos quaternion and the world direction `toward` -- a fixed 3-vector, or
+    (component, indices) of three consecutive components of a sampled component, e.g. ("world_vel", (3, 4, 5)) for the
+    velocity (inertial angle of attack, flight-path angle).  atan2(|u x v|, u . v) with CUDA's double atan2 (2 ulp);
+    neither the quaternion nor the direction needs to be unit.  A zero direction (a body at rest) gives 0.  Pitch from
+    vertical of a body whose nose is -x: AxisAngle("pitch", (-1, 0, 0), (0, 0, 1))."""
+
+    def __init__(self, name: str, axis, toward):
+        where = f"AxisAngle({name!r}, {axis!r}, {toward!r})"
+        if not isinstance(name, str) or not name:
+            raise ValueError(f"{where}: the name must be a non-empty string")
+        self.axis = _finite3(axis, f"{where}: axis")
+        if isinstance(toward, (tuple, list)) and len(toward) == 2 and isinstance(toward[0], str):
+            comp, idx = toward
+            span = _SAMPLED.get(comp)
+            if span is None:
+                raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                          f"component not found: {comp} (channels cover {', '.join(_SAMPLED)})")
+            idx = tuple(idx) if isinstance(idx, (tuple, list)) else (idx,)
+            planes = tuple(_sampled_plane(span, i, where) for i in idx)
+            if len(planes) != 3 or planes != (planes[0], planes[0] + 1, planes[0] + 2):
+                raise ValueError(f"{where}: toward takes three consecutive indices of one component")
+            self.plane, self.direction = planes[0], None
+        else:
+            self.plane, self.direction = None, _finite3(toward, f"{where}: toward")
+        self.name = name
+
+    def _record(self) -> "_lib.Channel":
+        if self.plane is None:
+            return _lib.channel(_lib.CHANNEL_AXIS_ANGLE, 0, (), self.axis, self.direction)
+        return _lib.channel(_lib.CHANNEL_AXIS_ANGLE, 3, (self.plane,), self.axis)
+
+    def __repr__(self) -> str:
+        toward = self.direction if self.plane is None else f"planes {self.plane}..{self.plane + 2}"
+        return f"AxisAngle({self.name!r}, axis={self.axis}, toward={toward})"
+
+
+def _channel_list(channels) -> List[Channel]:
+    """World.build(..., channels=...): 1 to MAX_CHANNELS Norm / AxisAngle objects with distinct names."""
+    if isinstance(channels, (str, bytes)) or not isinstance(channels, Sequence):
+        raise TypeError(f"channels take a sequence of el.Norm / el.AxisAngle objects, got {channels!r}")
+    for c in channels:
+        if not isinstance(c, Channel):
+            raise TypeError(f"channels take el.Norm / el.AxisAngle objects, got {c!r}")
+    if not 1 <= len(channels) <= _lib.MAX_CHANNELS:
+        raise ValueError(f"{len(channels)} channels: 1 to {_lib.MAX_CHANNELS}")
+    names = [c.name for c in channels]
+    for n in names:
+        if names.count(n) > 1:
+            raise ValueError(f"channels: the name {n!r} is used twice")
+    return list(channels)
 
 
 class Threshold:
@@ -747,7 +872,8 @@ class Exec:
                  ensemble: bool = False, ensemble_ring: Optional[int] = None, extrema: bool = False,
                  thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
                  covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
-                 groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None):
+                 groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
+                 channels: Optional[Sequence[Channel]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -797,6 +923,10 @@ class Exec:
         if retain is not None and not ensemble:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "retain: need World.build(..., ensemble=True)")
         self._retain = _retained_worlds(retain, self.n_worlds, len(bodies)) if retain is not None else None
+        if channels is not None and not ensemble:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "channels: need World.build(..., ensemble=True)")
+        self._channels = _channel_list(channels) if channels is not None else []
+        n_rows = _lib.ROW_PLANES + len(self._channels)  # planes of an ensemble row
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
         self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
@@ -809,6 +939,8 @@ class Exec:
                 ent = None
             if ent not in bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
+            if t.plane >= n_rows:
+                raise ValueError(f"{t!r}: channel {t.index}, this Exec has {len(self._channels)}")
             self._threshold_rows.append((bodies.index(ent), t.plane, t.above, t.value))
         # ensemble rows, per kind of table: the arguments of B200Exec.trajectory_<kind> / state_<kind>, and the blocks
         # of rows recorded so far ([k, n_entities, ...] each)
@@ -816,7 +948,7 @@ class Exec:
         if quantiles is not None:
             self._ens_args["quantiles"] = (_quantile_levels(quantiles),)
         if covariance is not None:
-            planes, self._cov_labels = _covariance_planes(covariance)
+            planes, self._cov_labels = _covariance_planes(covariance, [c.name for c in self._channels])
             self._ens_args["covariance"] = (planes,)
         if histograms is not None:
             self._histograms = _histogram_specs(histograms)
@@ -828,6 +960,8 @@ class Exec:
                     ent = None
                 if ent not in bodies:
                     raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {h.pair}")
+                if max(h.planes) >= n_rows:
+                    raise ValueError(f"Histogram({h.pair!r}, ...): a channel index, this Exec has {len(self._channels)}")
                 specs.append(h._spec(bodies.index(ent)))
             self._ens_args["histograms"] = (specs,)
         if self.groups is not None:  # the same tables per group of worlds
@@ -869,7 +1003,7 @@ class Exec:
             # Ensemble mode: the state never leaves the device between the initial upload and the end of run();
             # each ring-full of telemetry samples is reduced over the worlds in place, then the ring is reset.
             ld = (n_bodies + 127) // 128 * 128
-            cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max(25 * ld * 8, 1)
+            cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max(n_rows * ld * 8, 1)
             self._ring_cap = int(max(1, min(4096, cap)))
         elif resident and n_bodies:
             ld = (n_bodies + 127) // 128 * 128
@@ -887,6 +1021,8 @@ class Exec:
         self._history: Dict[int, List[np.ndarray]] = {cid: [] for cid in self.world.columns}
         self._globals_hist: List[tuple] = []
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
+        if self._channels:  # before summary_begin, which fixes the row width
+            self.backend.set_channels([c._record() for c in self._channels])
         if self._extrema or self._thresholds:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
         if self.groups is not None:
@@ -1336,9 +1472,20 @@ class Exec:
         t = t[:, row]
         return t[:, lo:hi] if per_plane else t
 
+    @property
+    def channels(self) -> List[str]:
+        """The names of the channels of World.build(..., channels=[...]), in order: index k of "<entity>.channels"."""
+        return [c.name for c in self._channels]
+
     def _sampled_row(self, pair: str, what: str):
-        """`<entity>.<component>` -> (Body row of the entity, plane span of the component in a 25-plane row)."""
+        """`<entity>.<component>` -> (Body row of the entity, plane span of the component in an ensemble row: 25 planes,
+        then the channels)."""
         ent, span = _sampled_span(pair, what)
+        if span == _CHANNEL_SPAN:
+            if not self._channels:
+                raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                     f"{pair}: build the Exec with World.build(..., ensemble=True, channels=[...])")
+            span = (span[0], span[0] + len(self._channels))
         ent_id = self.world.entity_by_name(ent)
         col = self.world.columns[component_id("world_pos")]
         if ent_id not in col.entity_ids:

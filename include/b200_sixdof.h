@@ -507,6 +507,55 @@ int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes);
 /* Both downloads take host or device dst, return once it is filled, need `bytes` to match exactly (else
  * B200_ERR_VALUE_SIZE_MISMATCH) and count their launches in timings.kernel_launches, as the statistics entries do. */
 
+/* ---- derived channels: per-body quantities computed on the device from a body's 25-plane row (B200_TRAJ_FULL layout)
+ * and reduced like the state components.  With n_c channels set, channel k is plane 25 + k of the row every ensemble
+ * entry reduces, ring and state alike, so a row is R = 25 + n_c planes wide in: the statistics and quantiles (plain and
+ * grouped: dst [..][n_entities][R][..]), covariance selections and histogram specs (a plane < R), and the run summaries
+ * (threshold planes < R; extrema dst = [n_worlds][n_entities][R][5]).  A threshold record stays tick + the 25 raw planes.
+ * trajectory_download, trajectory_width, the *_download_worlds entries, the NCCL all-gather and both merge entries do not
+ * change.  With n_c = 0 (the default) every entry is what it is without this section; with channels set, planes 0..24 of
+ * every table keep their bits.
+ *   B200_CHANNEL_NORM: n in 1..3 distinct planes p[0..n) (each < 25), offsets c[0..n), r0:
+ *     d_i = x[p_i] - c_i;  s = d_0*d_0;  s = s + d_1*d_1;  s = s + d_2*d_2  (terms i < n, in that order);  sqrt(s) - r0
+ *     every operation correctly rounded and uncontracted in both math modes: numpy's bits for the same expression.
+ *     Squares that overflow give +inf.  Speed: planes (10, 11, 12); distance from a point: (4, 5, 6) with c = the point;
+ *     altitude over a sphere: r0 = its radius.
+ *   B200_CHANNEL_AXIS_ANGLE: the angle in [0, pi] between the body-frame axis c (finite, not zero) rotated into the world
+ *     frame and a world direction v: the fixed vector d (n = 0, finite, not zero), or planes plane[0] .. plane[0] + 2
+ *     of the row (n = 3; plane[0] = 10 gives the velocity: inertial angle of attack / flight-path angle):
+ *       u = qrot(q, c)  (q = planes 0..3; the EXACT rotation of the tick, q * [c, 0] * q.inverse(), in both math modes)
+ *       x = u cross v;  s = sqrt((x.x*x.x + x.y*x.y) + x.z*x.z);  t = (u.x*v.x + u.y*v.y) + u.z*v.z;  atan2(s, t)
+ *     correctly rounded and uncontracted up to s and t; atan2 is CUDA's double atan2 (2 ulp maximum error, CUDA Math API).
+ *     Neither q nor v needs to be normalised.  A zero v (a body at rest) gives atan2(0, 0) = 0.
+ * NaN or +-inf inputs give non-finite values, which the reductions drop like any other non-finite value.  Every entry
+ * that reads a channel plane recomputes the channels first (one launch on the handle's stream, counted in
+ * timings.kernel_launches): statistics, quantiles and extrema whenever n_c > 0; covariance, histograms and thresholds
+ * only when their selection names a channel plane. ---- */
+#define B200_MAX_CHANNELS 8u
+enum { B200_CHANNEL_NORM = 1, B200_CHANNEL_AXIS_ANGLE = 2 };
+typedef struct b200_channel {
+    uint32_t kind;       /* B200_CHANNEL_*                                                              */
+    uint32_t n;          /* NORM: 1..3 planes; AXIS_ANGLE: 0 = fixed direction d, 3 = planes plane[0] .. +2 */
+    uint32_t plane[3];   /* planes of the 25-plane row                                                  */
+    uint32_t reserved;   /* must be 0                                                                   */
+    double   c[3];       /* NORM: offsets; AXIS_ANGLE: body axis                                        */
+    double   d[3];       /* AXIS_ANGLE with n = 0: world direction                                      */
+    double   r0;         /* NORM: subtracted from the norm                                              */
+} b200_channel;
+/* c[0 .. n) replaces the channel set; n = 0 clears it.  B200_ERR_INVALID_ARGUMENT, with the setting unchanged, for: a
+ * null handle, n > B200_MAX_CHANNELS, null c with n > 0, an unknown kind, a bad n, a plane >= 25, duplicate NORM planes,
+ * an AXIS_ANGLE plane triple past plane 24, a non-zero reserved field, a non-finite constant, a zero axis or fixed
+ * direction, a 13-wide ring (a handle without a ring is allowed), or a handle on which b200_sixdof_summary_begin was
+ * called (it fixes the row width of its accumulators).  Allocates capacity * n * ld f64 for the ring's channels and
+ * n * ld for the state's. */
+int b200_sixdof_set_channels(b200_sixdof *h, const b200_channel *c, uint32_t n);
+/* the number of channels set (0 for a null handle) */
+uint32_t b200_sixdof_channels(const b200_sixdof *h);
+/* the channels of the ring's samples: dst = [trajectory_len][n_worlds][n_entities][n_c] f64 (host or device) */
+int b200_sixdof_trajectory_channels(b200_sixdof *h, void *dst, uint64_t bytes);
+/* the channels of the current state: dst = [n_worlds][n_entities][n_c] f64 (host or device) */
+int b200_sixdof_state_channels(b200_sixdof *h, void *dst, uint64_t bytes);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
