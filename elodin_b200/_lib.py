@@ -71,10 +71,14 @@ SYMBOLS = [
     "b200_sixdof_trajectory_group_covariance", "b200_sixdof_state_group_covariance",
     "b200_sixdof_trajectory_download_worlds", "b200_sixdof_state_download_worlds",
     "b200_sixdof_set_channels", "b200_sixdof_channels", "b200_sixdof_trajectory_channels", "b200_sixdof_state_channels",
+    "b200_sixdof_summary_start", "b200_sixdof_moments_download", "b200_sixdof_dwells_download",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
 MAX_THRESHOLDS = 8
+MOMENT_FIELDS = 3  # n, mean, m2 = sum (x - mean)^2 over a world's finite rows
+MAX_DWELLS = 8
+DWELL_FIELDS = 3  # rows, first_tick, last_tick of the rows beyond a dwell's bound
 MAX_QUANTILES = 16  # levels per quantile call
 MAX_COV_PLANES = 25  # planes per covariance selection
 MAX_HISTOGRAMS = 8  # specs per histogram call
@@ -147,6 +151,18 @@ class Threshold(C.Structure):
         ("plane", C.c_uint32),
         ("above", C.c_int32),
         ("value", C.c_double),
+    ]
+
+
+class SummarySpec(C.Structure):
+    _fields_ = [
+        ("extrema", C.c_uint32),
+        ("n_thresholds", C.c_uint32),
+        ("thresholds", C.POINTER(Threshold)),
+        ("n_moments", C.c_uint32),
+        ("n_dwells", C.c_uint32),
+        ("moments", C.POINTER(C.c_uint32)),
+        ("dwells", C.POINTER(Threshold)),
     ]
 
 
@@ -263,6 +279,9 @@ def lib():
     L.b200_sixdof_summary_add_trajectory.argtypes = [vp]
     L.b200_sixdof_extrema_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_thresholds_download.argtypes = [vp, vp, u64]
+    L.b200_sixdof_summary_start.argtypes = [vp, C.POINTER(SummarySpec)]
+    L.b200_sixdof_moments_download.argtypes = [vp, vp, u64]
+    L.b200_sixdof_dwells_download.argtypes = [vp, vp, u64]
     L.b200_sixdof_trajectory_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
     L.b200_sixdof_state_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
     L.b200_sixdof_quantile_reads.argtypes = [vp]

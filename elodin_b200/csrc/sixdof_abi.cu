@@ -731,6 +731,8 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->chan_ring) cudaFree(h->chan_ring);
     if (h->chan_state) cudaFree(h->chan_state);
     if (h->sum_thr) cudaFree(h->sum_thr);
+    if (h->sum_mom) cudaFree(h->sum_mom);
+    if (h->sum_dwell) cudaFree(h->sum_dwell);
     for (void *t : {(void *)h->all_table_dev, (void *)h->group_table_dev, (void *)h->all_cov_dev, (void *)h->group_cov_dev,
                     (void *)h->all_order_dev, (void *)h->group_order_dev})
         if (t) cudaFree(t);
@@ -1751,11 +1753,26 @@ static SummaryParams summary_params(const b200_sixdof *h)
         const b200_threshold &t = h->sum_thr_list[i];
         S.t[i] = {(uint32_t)t.entity, t.plane, t.above ? 1 : 0, 0u, t.value};
     }
+    S.n_mom = (uint32_t)h->sum_mom_planes.size();
+    S.mom = S.n_mom ? h->sum_mom : nullptr;
+    S.n_dwell = (uint32_t)h->sum_dwell_list.size();
+    S.dwell = S.n_dwell ? h->sum_dwell : nullptr;
+    for (uint32_t i = 0; i < S.n_dwell; ++i) {
+        const b200_threshold &t = h->sum_dwell_list[i];
+        S.d[i] = {(uint32_t)t.entity, t.plane, t.above ? 1 : 0, 0u, t.value};
+    }
     S.width = row_width(h, false);
     for (uint32_t p = 0; p < S.width; ++p) {
         bool used = h->sum_extrema;
         for (uint32_t i = 0; i < S.n_thr; ++i) used = used || S.t[i].plane == p;
-        if (used) S.planes[S.n_planes++] = (uint8_t)p;
+        for (uint32_t i = 0; i < S.n_dwell; ++i) used = used || S.d[i].plane == p;
+        uint8_t slot = kNoMoment;
+        for (uint32_t j = 0; j < S.n_mom; ++j)
+            if (h->sum_mom_planes[j] == p) slot = (uint8_t)j;
+        if (used || slot != kNoMoment) {
+            S.mom_slot[S.n_planes] = slot;
+            S.planes[S.n_planes++] = (uint8_t)p;
+        }
     }
     return S;
 }
@@ -1769,7 +1786,7 @@ static int summary_ready(b200_sixdof *h, const char *what)
 
 // Fold the samples of the ring (ring) or the state as rows, sample k at tick tick0 + k * tick_step: row[p] is plane p of
 // sample 0, and each sample's planes start one segment stride after the one before it.  The channel planes are
-// recomputed first where the fold reads one: with extrema, or a threshold on a channel plane.
+// recomputed first where the fold reads one: with extrema, or a threshold, moment or dwell on a channel plane.
 static int run_summary_fold(b200_sixdof *h, bool ring, uint64_t tick0, uint64_t tick_step)
 {
     SummaryParams S = summary_params(h);
@@ -1794,36 +1811,83 @@ static int run_summary_fold(b200_sixdof *h, bool ring, uint64_t tick0, uint64_t 
     return B200_OK;
 }
 
-int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_threshold *t, uint32_t n_thresholds)
+// A threshold or dwell condition `what` i: 0 when it keeps the contract of include/b200_sixdof.h, else the refusal.
+static int check_condition(const b200_sixdof *h, const b200_threshold &t, const char *what, uint32_t i)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (t.entity >= h->desc.n_entities)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%s %u: entity row %llu, the world has %llu", what, i,
+                    (unsigned long long)t.entity, (unsigned long long)h->desc.n_entities);
+    if (t.plane >= row_width(h, false))
+        return fail(B200_ERR_INVALID_ARGUMENT, "%s %u: plane %u, a row has %u", what, i, t.plane, row_width(h, false));
+    if (std::isnan(t.value)) return fail(B200_ERR_INVALID_ARGUMENT, "%s %u: the bound is NaN", what, i);
+    return B200_OK;
+}
+
+// summary_begin and summary_start (`nothing`: the refusal of a spec that requests nothing): every argument checked
+// before anything changes, then the accumulators allocated on first use, the spec stored and everything cleared on the
+// handle's stream.
+static int summary_start(b200_sixdof *h, const b200_summary_spec &sp, const char *nothing)
+{
     CU(h, cudaSetDevice(h->device));
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
-    if (n_thresholds > B200_MAX_THRESHOLDS)
-        return fail(B200_ERR_INVALID_ARGUMENT, "%u thresholds: at most %u", n_thresholds, B200_MAX_THRESHOLDS);
-    if (!extrema && n_thresholds == 0) return fail(B200_ERR_INVALID_ARGUMENT, "summary_begin: neither extrema nor thresholds");
-    if (n_thresholds && !t) return fail(B200_ERR_INVALID_ARGUMENT, "null thresholds");
-    for (uint32_t i = 0; i < n_thresholds; ++i) {
-        if (t[i].entity >= h->desc.n_entities)
-            return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: entity row %llu, the world has %llu", i,
-                        (unsigned long long)t[i].entity, (unsigned long long)h->desc.n_entities);
-        if (t[i].plane >= row_width(h, false))
-            return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: plane %u, a row has %u", i, t[i].plane, row_width(h, false));
-        if (std::isnan(t[i].value)) return fail(B200_ERR_INVALID_ARGUMENT, "threshold %u: the bound is NaN", i);
+    if (sp.n_thresholds > B200_MAX_THRESHOLDS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u thresholds: at most %u", sp.n_thresholds, B200_MAX_THRESHOLDS);
+    if (!sp.extrema && sp.n_thresholds == 0 && sp.n_moments == 0 && sp.n_dwells == 0)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%s", nothing);
+    if (sp.n_thresholds && !sp.thresholds) return fail(B200_ERR_INVALID_ARGUMENT, "null thresholds");
+    for (uint32_t i = 0; i < sp.n_thresholds; ++i) {
+        const int rc = check_condition(h, sp.thresholds[i], "threshold", i);
+        if (rc) return rc;
+    }
+    const uint32_t R = row_width(h, false);
+    if (sp.n_moments && !sp.moments) return fail(B200_ERR_INVALID_ARGUMENT, "null moment planes");
+    for (uint32_t j = 0; j < sp.n_moments; ++j) {
+        if (sp.moments[j] >= R) return fail(B200_ERR_INVALID_ARGUMENT, "moment %u: plane %u, a row has %u", j, sp.moments[j], R);
+        for (uint32_t i = 0; i < j; ++i)
+            if (sp.moments[i] == sp.moments[j])
+                return fail(B200_ERR_INVALID_ARGUMENT, "moments: plane %u twice", sp.moments[j]);
+    }
+    if (sp.n_dwells > B200_MAX_DWELLS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "%u dwells: at most %u", sp.n_dwells, B200_MAX_DWELLS);
+    if (sp.n_dwells && !sp.dwells) return fail(B200_ERR_INVALID_ARGUMENT, "null dwells");
+    for (uint32_t i = 0; i < sp.n_dwells; ++i) {
+        const int rc = check_condition(h, sp.dwells[i], "dwell", i);
+        if (rc) return rc;
     }
     h->sum_begun = false;
     h->sum_ever = true;  // the channel set, and so R, stays as it is from here on
-    if (extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 5ull * row_width(h, false) * h->ld * 8ull));
-    const uint64_t thr_bytes = h->desc.n_worlds * n_thresholds * 26ull * 8ull;
-    const int rc = grow_device(h, &h->sum_thr, &h->sum_thr_bytes, thr_bytes);
+    if (sp.extrema && !h->sum_ext) CU(h, cudaMalloc(&h->sum_ext, 5ull * R * h->ld * 8ull));
+    const uint64_t thr_bytes = h->desc.n_worlds * sp.n_thresholds * 26ull * 8ull;
+    int rc = grow_device(h, &h->sum_thr, &h->sum_thr_bytes, thr_bytes);
     if (rc) return rc;
-    h->sum_extrema = extrema != 0;
-    h->sum_thr_list.assign(t, t + n_thresholds);
+    if ((rc = grow_device(h, &h->sum_mom, &h->sum_mom_bytes, 4ull * sp.n_moments * h->ld * 8ull))) return rc;
+    if ((rc = grow_device(h, &h->sum_dwell, &h->sum_dwell_bytes, h->desc.n_worlds * sp.n_dwells * 3ull * 8ull))) return rc;
+    h->sum_extrema = sp.extrema != 0;
+    h->sum_thr_list.assign(sp.thresholds, sp.thresholds + sp.n_thresholds);
+    h->sum_mom_planes.assign(sp.moments, sp.moments + sp.n_moments);
+    h->sum_dwell_list.assign(sp.dwells, sp.dwells + sp.n_dwells);
     int launches = 0;
     CU(h, launch_summary_clear(summary_params(h), &launches, h->stream));
     h->timings.kernel_launches += (uint64_t)launches;
     h->sum_begun = true;
     return B200_OK;
+}
+
+int b200_sixdof_summary_begin(b200_sixdof *h, uint32_t extrema, const b200_threshold *t, uint32_t n_thresholds)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    b200_summary_spec sp{};
+    sp.extrema = extrema;
+    sp.n_thresholds = n_thresholds;
+    sp.thresholds = t;
+    return summary_start(h, sp, "summary_begin: neither extrema nor thresholds");
+}
+
+int b200_sixdof_summary_start(b200_sixdof *h, const b200_summary_spec *spec)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (!spec) return fail(B200_ERR_INVALID_ARGUMENT, "null summary spec");
+    return summary_start(h, *spec, "summary_start: no extrema, thresholds, moments or dwells");
 }
 
 int b200_sixdof_summary_add_state(b200_sixdof *h)
@@ -1848,8 +1912,30 @@ int b200_sixdof_summary_add_trajectory(b200_sixdof *h)
     return run_summary_fold(h, true, h->tick - h->ticks_done + every, every);
 }
 
-// dst on the handle's GPU takes the table straight from the kernel; any other goes through the staging buffer in
-// chunks of 256 MB.
+// A per-body table of per_body bytes into dst, `table` writing bodies [b0, b0 + nb) of it: dst on the handle's GPU
+// takes the table straight from the kernel; any other goes through the staging buffer in chunks of 256 MB.
+extern "C++" {
+template <class Table>
+static int body_table_download(b200_sixdof *h, void *dst, uint64_t per_body, Table table)
+{
+    if (h->n_bodies * per_body == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    const bool direct = device_destination(h, dst);
+    const uint64_t chunk = direct ? h->n_bodies : std::max<uint64_t>(1, std::min<uint64_t>(h->n_bodies, (256ull << 20) / per_body));
+    int rc = B200_OK;
+    if (!direct && (rc = ensure_staging(h, chunk * per_body))) return rc;
+    for (uint64_t b0 = 0; b0 < h->n_bodies; b0 += chunk) {
+        const uint64_t nb = std::min(chunk, h->n_bodies - b0);
+        double *out = direct ? (double *)dst : h->staging;
+        CU(h, table(b0, nb, out));
+        h->timings.kernel_launches++;
+        if (!direct) CU(h, cudaMemcpyAsync((char *)dst + b0 * per_body, out, nb * per_body, cudaMemcpyDefault, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream)); // the staging buffer is reused by the next chunk
+    }
+    return B200_OK;
+}
+}
+
 int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
@@ -1863,20 +1949,27 @@ int b200_sixdof_extrema_download(b200_sixdof *h, void *dst, uint64_t bytes)
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "extrema are %llu bytes, got %llu", (unsigned long long)want,
                     (unsigned long long)bytes);
-    if (want == 0) return B200_OK;
-    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
-    const bool direct = device_destination(h, dst);
-    const uint64_t chunk = direct ? h->n_bodies : std::max<uint64_t>(1, std::min<uint64_t>(h->n_bodies, (256ull << 20) / per_body));
-    if (!direct && (rc = ensure_staging(h, chunk * per_body))) return rc;
-    for (uint64_t b0 = 0; b0 < h->n_bodies; b0 += chunk) {
-        const uint64_t nb = std::min(chunk, h->n_bodies - b0);
-        double *out = direct ? (double *)dst : h->staging;
-        CU(h, launch_extrema_table(h->sum_ext, h->ld, width, b0, nb, out, h->stream));
-        h->timings.kernel_launches++;
-        if (!direct) CU(h, cudaMemcpyAsync((char *)dst + b0 * per_body, out, nb * per_body, cudaMemcpyDefault, h->stream));
-        CU(h, cudaStreamSynchronize(h->stream)); // the staging buffer is reused by the next chunk
-    }
-    return B200_OK;
+    return body_table_download(h, dst, per_body, [&](uint64_t b0, uint64_t nb, double *out) {
+        return launch_extrema_table(h->sum_ext, h->ld, width, b0, nb, out, h->stream);
+    });
+}
+
+int b200_sixdof_moments_download(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "moments_download");
+    if (rc) return rc;
+    const uint32_t k = (uint32_t)h->sum_mom_planes.size();
+    if (k == 0) return fail(B200_ERR_INVALID_ARGUMENT, "moments_download: the summary has no moments");
+    const uint64_t per_body = 3ull * k * 8ull;
+    const uint64_t want = h->n_bodies * per_body;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "moments are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    return body_table_download(h, dst, per_body, [&](uint64_t b0, uint64_t nb, double *out) {
+        return launch_moment_table(h->sum_mom, h->ld, k, b0, nb, out, h->stream);
+    });
 }
 
 int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes)
@@ -1893,6 +1986,24 @@ int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes)
     if (want == 0) return B200_OK;
     if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
     CU(h, cudaMemcpyAsync(dst, h->sum_thr, want, cudaMemcpyDefault, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return B200_OK;
+}
+
+int b200_sixdof_dwells_download(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    CU(h, cudaSetDevice(h->device));
+    int rc = summary_ready(h, "dwells_download");
+    if (rc) return rc;
+    if (h->sum_dwell_list.empty()) return fail(B200_ERR_INVALID_ARGUMENT, "dwells_download: the summary has no dwells");
+    const uint64_t want = h->desc.n_worlds * h->sum_dwell_list.size() * 3ull * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "dwell records are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    if (want == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    CU(h, cudaMemcpyAsync(dst, h->sum_dwell, want, cudaMemcpyDefault, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
 }

@@ -84,6 +84,12 @@ struct b200_sixdof {
     double *sum_ext = nullptr;       // 5 R planes of ld, R = 25 + channels (SummaryParams::ext)
     double *sum_thr = nullptr;       // [n_worlds][thresholds][26] (SummaryParams::thr)
     uint64_t sum_thr_bytes = 0;
+    std::vector<uint32_t> sum_mom_planes;     // selected moment planes, in table order
+    std::vector<b200_threshold> sum_dwell_list;
+    double *sum_mom = nullptr;       // 4 planes of ld per selected plane (SummaryParams::mom)
+    uint64_t sum_mom_bytes = 0;
+    double *sum_dwell = nullptr;     // [n_worlds][dwells][3] (SummaryParams::dwell)
+    uint64_t sum_dwell_bytes = 0;
     // plumbing
     cudaStream_t stream = nullptr;
     bool own_stream = true;

@@ -332,8 +332,12 @@ cudaError_t launch_histograms(const HistParams &P, const WorldGroup *groups, con
 //   ext: extrema accumulators, plane p * 5 + f of ld doubles (f = min, max, min_tick, max_tick, first_nonfinite_tick),
 //        i.e. body b's 5 R values read in plane order are its row of the public table; nullptr = no extrema.
 //   thr: the public threshold table itself, [n_worlds][n_thr][26] f64 (tick, the 25 raw planes); nullptr = no thresholds.
+//   mom: moment accumulators (n, K, S1, S2) of selected plane j at plane j * 4 + f of ld doubles; mom_slot[y] = j when
+//        planes[y] is selected plane j, kNoMoment otherwise; nullptr = no moments.
+//   dwell: the public dwell table itself, [n_worlds][n_dwell][3] f64 (rows, first_tick, last_tick); nullptr = none.
 // Ticks are stored as f64 (exact below 2^53), -1 = none; every accumulator has one owning thread per fold.
-// A fold reads only the planes listed in planes[0 .. n_planes): all R with extrema, else the thresholds' planes.
+// A fold reads only the planes listed in planes[0 .. n_planes): all R with extrema, else the union of the thresholds',
+// moments' and dwells' planes.  With mom and dwell null the fold is the extrema / threshold kernel alone.
 constexpr uint32_t kMaxRow = 25 + B200_MAX_CHANNELS;
 struct SummaryParams {
     const double *row[kMaxRow];
@@ -355,14 +359,25 @@ struct SummaryParams {
         uint32_t pad;
         double value;
     } t[B200_MAX_THRESHOLDS];
+    double *mom;
+    double *dwell;
+    uint32_t n_mom;
+    uint32_t n_dwell;
+    uint8_t mom_slot[kMaxRow];
+    Thr d[B200_MAX_DWELLS];
 };
-// the accumulators of S (ext and / or thr) set to "nothing seen yet"; launches written to *launches (0 or 1)
+constexpr uint8_t kNoMoment = 0xff;
+// the accumulators of S (ext, thr, mom, dwell) set to "nothing seen yet"; launches written to *launches (0, 1 or 2:
+// one for ext / thr, one for mom / dwell)
 cudaError_t launch_summary_clear(const SummaryParams &S, int *launches, cudaStream_t s);
 // fold S's rows into the accumulators; launches written to *launches (0 when there are no rows, else 1)
 cudaError_t launch_summary_fold(const SummaryParams &S, int *launches, cudaStream_t s);
 // extrema accumulators of rows of R planes, bodies [b0, b0 + nb) -> out[nb][5 R] (the public table's rows)
 cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint32_t R, uint64_t b0, uint64_t nb, double *out,
                                  cudaStream_t s);
+// moment accumulators of k selected planes, bodies [b0, b0 + nb) -> out[nb][k][3] (n, mean, m2: the public table's rows)
+cudaError_t launch_moment_table(const double *mom, uint64_t ld, uint32_t k, uint64_t b0, uint64_t nb, double *out,
+                                cudaStream_t s);
 
 // Derived channels (channel_kernels.cu, include/b200_sixdof.h b200_channel): n_c values per body of samples
 // [0, n_samples), from the 25 planes of each sample (plane p of sample s at row[p] + s * row_stride) into

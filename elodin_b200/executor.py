@@ -459,15 +459,31 @@ class B200Exec:
         return self._reduce("channels", False, (), (self.n_worlds, self.n_entities, self.n_channels))
 
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
-    def summary_begin(self, extrema: bool, thresholds: Sequence = ()) -> None:
-        """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
-        up to 8 (entity row, plane 0..24 or 25 + channel, above, value) tuples, each firing on value > bound (above) or < bound."""
-        ts = list(thresholds)
-        arr = (_lib.Threshold * max(len(ts), 1))()
-        for i, (entity, plane, above, value) in enumerate(ts):
+    @staticmethod
+    def _conditions(rows: Sequence):
+        """(entity row, plane, above, value) tuples -> a Threshold array (at least one element) and its length."""
+        rows = list(rows)
+        arr = (_lib.Threshold * max(len(rows), 1))()
+        for i, (entity, plane, above, value) in enumerate(rows):
             arr[i] = _lib.Threshold(int(entity), int(plane), 1 if above else 0, float(value))
-        _lib.check(self._L.b200_sixdof_summary_begin(self._h, 1 if extrema else 0, arr, len(ts)))
-        self._n_thresholds = len(ts)
+        return arr, len(rows)
+
+    def summary_begin(self, extrema: bool, thresholds: Sequence = (), moments: Sequence = (), dwells: Sequence = ()) -> None:
+        """Start (or start over) the run summaries: `extrema` keeps per-(world, entity, plane) extrema; `thresholds` =
+        up to 8 (entity row, plane 0..24 or 25 + channel, above, value) tuples, each firing on value > bound (above) or < bound;
+        `moments` = distinct planes (0..24 or 25 + channel) whose run count, mean and m2 are kept per (world, entity);
+        `dwells` = up to 8 tuples as `thresholds`, each counting the rows beyond its bound.  Without moments and dwells
+        this is b200_sixdof_summary_begin, else b200_sixdof_summary_start."""
+        thr, n_thr = self._conditions(thresholds)
+        mom = np.ascontiguousarray(np.asarray(list(moments), dtype=np.uint32).ravel())
+        dwl, n_dwl = self._conditions(dwells)
+        if mom.size == 0 and n_dwl == 0:
+            _lib.check(self._L.b200_sixdof_summary_begin(self._h, 1 if extrema else 0, thr, n_thr))
+        else:
+            spec = _lib.SummarySpec(1 if extrema else 0, n_thr, thr, mom.size, n_dwl,
+                                    mom.ctypes.data_as(C.POINTER(C.c_uint32)), dwl)
+            _lib.check(self._L.b200_sixdof_summary_start(self._h, C.byref(spec)))
+        self._n_thresholds, self._n_moments, self._n_dwells = n_thr, mom.size, n_dwl
 
     def summary_add_state(self) -> None:
         """Fold the current device state as one row at the current tick."""
@@ -490,6 +506,20 @@ class B200Exec:
         entity's 25 planes at that row (NaN if it never fired)."""
         out = np.empty((self.n_worlds, getattr(self, "_n_thresholds", 0), 26))
         _lib.check(self._L.b200_sixdof_thresholds_download(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    def moments(self) -> np.ndarray:
+        """[n_worlds, n_entities, k, 3]: (n, mean, m2 = sum (x - mean)^2) over each world's finite rows of each of the k
+        planes of `moments`, in the order given (n = 0: NaN mean and m2; m2 = +inf where the sum of squares overflowed)."""
+        out = np.empty((self.n_worlds, self.n_entities, getattr(self, "_n_moments", 0), _lib.MOMENT_FIELDS))
+        _lib.check(self._L.b200_sixdof_moments_download(self._h, out.ctypes.data, out.nbytes))
+        return out
+
+    def dwells(self) -> np.ndarray:
+        """[n_worlds, n_dwells, 3]: (rows, first_tick, last_tick) of the rows beyond each dwell's bound (ticks -1 while
+        no row has counted)."""
+        out = np.empty((self.n_worlds, getattr(self, "_n_dwells", 0), _lib.DWELL_FIELDS))
+        _lib.check(self._L.b200_sixdof_dwells_download(self._h, out.ctypes.data, out.nbytes))
         return out
 
     # ---- plumbing ---------------------------------------------------------------

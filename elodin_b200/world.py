@@ -440,7 +440,8 @@ class World:
               thresholds: Optional[Sequence["Threshold"]] = None, quantiles: Optional[Sequence[float]] = None,
               covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
               groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
-              channels: Optional[Sequence["Channel"]] = None) -> "Exec":
+              channels: Optional[Sequence["Channel"]] = None, moments: Optional[Sequence] = None,
+              dwells: Optional[Sequence["Threshold"]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -464,7 +465,10 @@ class World:
         objects with distinct names) adds derived values computed on the device from each body's row -- speeds,
         distances, altitudes, pointing angles -- as the component "<entity>.channels" (channel k at index k, in the
         order given; `Exec.channels` lists the names), which every ensemble table, the extrema and the thresholds
-        cover like the sampled components."""
+        cover like the sampled components.  `moments` (a selection in the syntax of `covariance`, channels as
+        "channels") also keeps every world's run count, mean, spread and RMS of those components over its telemetry
+        rows (`Exec.moments`), and `dwells` (up to 8 `Threshold`s) every world's count of rows beyond each bound with
+        the first and last such tick (`Exec.dwell`), both folded on the device with the extrema."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -473,7 +477,7 @@ class World:
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
                     ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain,
-                    channels)
+                    channels, moments, dwells)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -570,11 +574,12 @@ def _quantile_levels(levels) -> np.ndarray:
     return np.array(out)
 
 
-def _covariance_planes(spec, channel_names=()):
+def _covariance_planes(spec, channel_names=(), option: str = "covariance", max_planes: int = _lib.MAX_COV_PLANES):
     """World.build(..., covariance=...) -> (planes of the 25-plane row layout, channel k at 25 + k, labels), selection
-    order kept; a channel's label is its name."""
+    order kept; a channel's label is its name.  `option` names the build option in the refusals (moments= takes the
+    same selection, up to `max_planes` planes)."""
     if isinstance(spec, (str, bytes)) or not isinstance(spec, Sequence):
-        raise TypeError(f"covariance takes a sequence of components or (component, indices) pairs, got {spec!r}")
+        raise TypeError(f"{option} takes a sequence of components or (component, indices) pairs, got {spec!r}")
     planes, labels = [], []
     for item in spec:
         if isinstance(item, str):
@@ -584,23 +589,23 @@ def _covariance_planes(spec, channel_names=()):
         else:
             comp, idx = None, None
         if not isinstance(comp, str):
-            raise TypeError(f"covariance item {item!r}: a component name or a (component, indices) pair")
+            raise TypeError(f"{option} item {item!r}: a component name or a (component, indices) pair")
         span = (_lib.ROW_PLANES, _lib.ROW_PLANES + len(channel_names)) if comp == _CHANNELS else _SAMPLED.get(comp)
         if span is None:
             raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
-                                      f"component not found: {comp} (ensemble covariance covers {', '.join(_SAMPLED)})")
+                                      f"component not found: {comp} (ensemble {option} covers {', '.join(_SAMPLED)})")
         for i in range(span[1] - span[0]) if idx is None else idx:
             if comp == _CHANNELS:
-                _sampled_plane(_CHANNEL_SPAN, i, f"covariance item {item!r}")
+                _sampled_plane(_CHANNEL_SPAN, i, f"{option} item {item!r}")
                 if i >= len(channel_names):
-                    raise ValueError(f"covariance item {item!r}: channel {int(i)}, this Exec has {len(channel_names)}")
-            plane = _sampled_plane(span, i, f"covariance item {item!r}")
+                    raise ValueError(f"{option} item {item!r}: channel {int(i)}, this Exec has {len(channel_names)}")
+            plane = _sampled_plane(span, i, f"{option} item {item!r}")
             if plane in planes:
-                raise ValueError(f"covariance selects {comp}[{int(i)}] twice")
+                raise ValueError(f"{option} selects {comp}[{int(i)}] twice")
             planes.append(plane)
             labels.append(channel_names[int(i)] if comp == _CHANNELS else f"{comp}[{int(i)}]")
-    if not 1 <= len(planes) <= _lib.MAX_COV_PLANES:
-        raise ValueError(f"covariance selects {len(planes)} planes: 1 to {_lib.MAX_COV_PLANES}")
+    if not 1 <= len(planes) <= max_planes:
+        raise ValueError(f"{option} selects {len(planes)} planes: 1 to {max_planes}")
     return planes, labels
 
 
@@ -873,7 +878,8 @@ class Exec:
                  thresholds: Optional[Sequence[Threshold]] = None, quantiles: Optional[Sequence[float]] = None,
                  covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
                  groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
-                 channels: Optional[Sequence[Channel]] = None):
+                 channels: Optional[Sequence[Channel]] = None, moments: Optional[Sequence] = None,
+                 dwells: Optional[Sequence[Threshold]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -929,19 +935,37 @@ class Exec:
         n_rows = _lib.ROW_PLANES + len(self._channels)  # planes of an ensemble row
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
-        self._threshold_rows = []  # (entity row, plane, above, bound) per threshold
-        for t in self._thresholds:
-            if not isinstance(t, Threshold):
-                raise TypeError(f"thresholds take el.Threshold objects, got {t!r}")
-            try:
-                ent = world.entity_by_name(t.entity)
-            except _lib.B200ValueError:
-                ent = None
-            if ent not in bodies:
-                raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
-            if t.plane >= n_rows:
-                raise ValueError(f"{t!r}: channel {t.index}, this Exec has {len(self._channels)}")
-            self._threshold_rows.append((bodies.index(ent), t.plane, t.above, t.value))
+
+        def condition_rows(conditions, option):  # (entity row, plane, above, bound) per Threshold
+            out = []
+            for t in conditions:
+                if not isinstance(t, Threshold):
+                    raise TypeError(f"{option} take el.Threshold objects, got {t!r}")
+                try:
+                    ent = world.entity_by_name(t.entity)
+                except _lib.B200ValueError:
+                    ent = None
+                if ent not in bodies:
+                    raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
+                if t.plane >= n_rows:
+                    raise ValueError(f"{t!r}: channel {t.index}, this Exec has {len(self._channels)}")
+                out.append((bodies.index(ent), t.plane, t.above, t.value))
+            return out
+
+        self._threshold_rows = condition_rows(self._thresholds, "thresholds")
+        # run moments and dwells (folded with the extrema): the same mode rule, then their own values
+        for name, on in (("moments", moments is not None), ("dwells", dwells is not None)):
+            if on and not ensemble:
+                raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{name}: need World.build(..., ensemble=True)")
+        self._moment_planes, self._moment_labels = ([], []) if moments is None else _covariance_planes(
+            moments, [c.name for c in self._channels], "moments", n_rows)
+        if dwells is not None and (isinstance(dwells, (str, bytes)) or not isinstance(dwells, Sequence)):
+            raise TypeError(f"dwells take a sequence of el.Threshold objects, got {dwells!r}")
+        self._dwells = list(dwells or [])
+        if len(self._dwells) > _lib.MAX_DWELLS:
+            raise ValueError(f"{len(self._dwells)} dwells: at most {_lib.MAX_DWELLS}")
+        self._dwell_rows = condition_rows(self._dwells, "dwells")
+        self._summaries = bool(self._extrema or self._thresholds or self._moment_planes or self._dwells)
         # ensemble rows, per kind of table: the arguments of B200Exec.trajectory_<kind> / state_<kind>, and the blocks
         # of rows recorded so far ([k, n_entities, ...] each)
         self._ens_args: Dict[str, tuple] = {"stats": ()} if ensemble else {}
@@ -1023,7 +1047,9 @@ class Exec:
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._channels:  # before summary_begin, which fixes the row width
             self.backend.set_channels([c._record() for c in self._channels])
-        if self._extrema or self._thresholds:
+        if self._moment_planes or self._dwell_rows:
+            self.backend.summary_begin(self._extrema, self._threshold_rows, self._moment_planes, self._dwell_rows)
+        elif self._summaries:
             self.backend.summary_begin(self._extrema, self._threshold_rows)
         if self.groups is not None:
             self.backend.set_world_groups(self.groups)
@@ -1116,7 +1142,7 @@ class Exec:
         for kind, args in self._ens_args.items():
             rows = getattr(be, f"trajectory_{kind}")(*args) if ring else getattr(be, f"state_{kind}")(*args)[None]
             self._ens_rows[kind].append(rows)
-        if self._extrema or self._thresholds:
+        if self._summaries:
             (be.summary_add_trajectory if ring else be.summary_add_state)()
             self._summary_tables.clear()
         k, tpt = rows.shape[0], self.ticks_per_telemetry
@@ -1493,7 +1519,7 @@ class Exec:
         return col.row_of(ent_id), span
 
     def _summary_table(self, name: str) -> np.ndarray:
-        """The backend's extrema / thresholds table, downloaded once per fold."""
+        """The backend's extrema / thresholds / moments / dwells table, downloaded once per fold."""
         if name not in self._summary_tables:
             self._summary_tables[name] = getattr(self.backend, name)()
         return self._summary_tables[name]
@@ -1528,6 +1554,41 @@ class Exec:
         for name, (lo, hi) in _SAMPLED.items():
             out[name] = np.ascontiguousarray(t[:, 1 + lo:1 + hi])
         return out
+
+    def moments(self, pair: str) -> Dict[str, np.ndarray]:
+        """`exec.moments("rocket.channels")` -> {"index": the selected indices of the component, ascending, "count"
+        int64 [n_worlds, k], "mean", "std", "rms" [n_worlds, k]}: over each world's telemetry rows (row 0 = the initial
+        state) whose value is finite, the number of rows, the mean, the spread (numpy's ddof=0) and the root mean square,
+        for the components of World.build(..., moments=...).  NaN where count = 0; std and rms are +inf where the sum
+        of squares overflowed."""
+        if not self._moment_planes:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "moments(): build the Exec with World.build(..., ensemble=True, moments=[...])")
+        row, (lo, hi) = self._sampled_row(pair, "moments")
+        cols = sorted((p, j) for j, p in enumerate(self._moment_planes) if lo <= p < hi)
+        if not cols:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 f"moments({pair!r}): no index of it is selected by World.build(..., moments=[...])")
+        t = self._summary_table("moments")[:, row, [j for _, j in cols], :]  # [n_worlds, k, 3]
+        n, mean, m2 = t[..., 0], t[..., 1], t[..., 2]
+        with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+            var = m2 / n
+            out = {"index": np.array([p - lo for p, _ in cols], dtype=np.int64), "count": n.astype(np.int64),
+                   "mean": np.ascontiguousarray(mean), "std": np.sqrt(var), "rms": np.sqrt(mean * mean + var)}
+        return out
+
+    def dwell(self, i: int) -> Dict[str, np.ndarray]:
+        """`exec.dwell(i)` -> {"rows", "first_tick", "last_tick"}, each int64 [n_worlds]: for dwell i of World.build(...,
+        dwells=[...]), the number of each world's telemetry rows (row 0 = the initial state) beyond its bound, and the
+        ticks of the first and last of them (-1 where none).  `last_tick` of an error norm above a tolerance is the
+        settling time.  Counts are rows, not seconds: a partial last cycle makes the rows unevenly spaced."""
+        if not self._dwells:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 "dwell(): build the Exec with World.build(..., ensemble=True, dwells=[...])")
+        if not 0 <= i < len(self._dwells):
+            raise IndexError(f"dwell {i}: this Exec has {len(self._dwells)}")
+        t = self._summary_table("dwells")[:, i, :]  # [n_worlds, 3]
+        return {k: t[:, f].astype(np.int64) for f, k in enumerate(("rows", "first_tick", "last_tick"))}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

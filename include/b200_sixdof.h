@@ -507,6 +507,42 @@ int b200_sixdof_thresholds_download(b200_sixdof *h, void *dst, uint64_t bytes);
 /* Both downloads take host or device dst, return once it is filled, need `bytes` to match exactly (else
  * B200_ERR_VALUE_SIZE_MISMATCH) and count their launches in timings.kernel_launches, as the statistics entries do. */
 
+/* Run scores, folded by the same two entries in the same launch as the extrema (each plane a fold needs is read once):
+ * Moments, per (world, entity, selected plane): over the rows whose value is finite, in the order they are folded,
+ *   the first finite value sets K, then for each finite x:  y = x - K;  S1 = S1 + y;  S2 = S2 + y*y;  n = n + 1
+ *   (each operation correctly rounded, the product never contracted, in both math modes).  The table record is
+ *   (n, mean = K + S1 / n, m2 = S2 - S1 * (S1 / n) clamped at 0), with m2 = +inf where S2 overflowed and NaN mean and
+ *   m2 while n = 0.  The bits depend only on the sequence of finite rows folded, so any ring size gives the same table;
+ *   unlike the extrema, folding a row twice counts it twice.
+ * Dwells, per (world, dwell), 3 f64: rows = the number of rows folded whose value of (entity, plane) is strictly below
+ *   (above = 0) or above (above != 0) `value` (NaN never counts), first_tick / last_tick = the smallest / largest tick
+ *   of such a row (-1 while none).  first_tick is the tick of a threshold on the same condition; last_tick of an error
+ *   norm above a tolerance is the settling time.  Folding a row twice counts it twice. */
+#define B200_MOMENT_FIELDS 3u    /* n, mean, m2 */
+#define B200_DWELL_FIELDS 3u     /* rows, first_tick, last_tick */
+#define B200_MAX_DWELLS 8u
+typedef struct b200_summary_spec {
+    uint32_t extrema;                     /* != 0: keep the extrema table                                */
+    uint32_t n_thresholds;                /* 0 .. B200_MAX_THRESHOLDS                                    */
+    const b200_threshold *thresholds;
+    uint32_t n_moments;                   /* 0 .. R distinct planes (< R), in table order                */
+    uint32_t n_dwells;                    /* 0 .. B200_MAX_DWELLS                                        */
+    const uint32_t *moments;
+    const b200_threshold *dwells;         /* the condition of a threshold: entity, plane < R, above, value */
+} b200_summary_spec;
+/* Start (or start over) every run summary of *spec.  b200_sixdof_summary_begin(h, e, t, n) is this entry with no
+ * moments and no dwells, with the same launches and bits.  Allocates the moment accumulators (32 B per body and
+ * selected plane) and dwell records (24 B per world and dwell) on first use and clears them.
+ * B200_ERR_INVALID_ARGUMENT, with the summary started before left in force: a null spec, nothing requested, more than
+ * B200_MAX_THRESHOLDS thresholds or B200_MAX_DWELLS dwells, a null list with a count, an entity >= n_entities, a plane
+ * >= R, duplicate moment planes, or a NaN bound. */
+int b200_sixdof_summary_start(b200_sixdof *h, const b200_summary_spec *spec);
+/* dst = [n_worlds][n_entities][n_moments][3] f64 (n, mean, m2); refused when the summary has no moments */
+int b200_sixdof_moments_download(b200_sixdof *h, void *dst, uint64_t bytes);
+/* dst = [n_worlds][n_dwells][3] f64 (rows, first_tick, last_tick); refused when the summary has no dwells */
+int b200_sixdof_dwells_download(b200_sixdof *h, void *dst, uint64_t bytes);
+/* Both take host or device dst and count their launches like the extrema and threshold downloads. */
+
 /* ---- derived channels: per-body quantities computed on the device from a body's 25-plane row (B200_TRAJ_FULL layout)
  * and reduced like the state components.  With n_c channels set, channel k is plane 25 + k of the row every ensemble
  * entry reduces, ring and state alike, so a row is R = 25 + n_c planes wide in: the statistics and quantiles (plain and
