@@ -733,9 +733,9 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->sum_thr) cudaFree(h->sum_thr);
     if (h->sum_mom) cudaFree(h->sum_mom);
     if (h->sum_dwell) cudaFree(h->sum_dwell);
-    for (void *t : {(void *)h->all_table_dev, (void *)h->group_table_dev, (void *)h->all_cov_dev, (void *)h->group_cov_dev,
-                    (void *)h->all_order_dev, (void *)h->group_order_dev})
-        if (t) cudaFree(t);
+    for (const auto &t : h->tables)
+        for (void *p : {(void *)t.stats_dev, (void *)t.cov_dev, (void *)t.order_dev})
+            if (p) cudaFree(p);
     for (auto &e : h->chunk_in) if (e) cudaEventDestroy(e);
     for (auto &e : h->chunk_out) if (e) cudaEventDestroy(e);
     if (h->host_pack) cudaFreeHost(h->host_pack);
@@ -1150,20 +1150,26 @@ static bool device_destination(const b200_sixdof *h, const void *dst)
     return is_device_pointer(dst, &device) && device == h->device;
 }
 
-// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu) into dst, `bytes` already
-// checked.  A device destination takes the table straight from the kernel; any other gets it through the staging
-// buffer, after the `scratch` bytes the reduction needs.  launch(out, scratch, &launches) enqueues the reduction on the
-// handle's stream.
+static int refresh_channels(b200_sixdof *h, bool ring);
+
+// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu, hist_kernels.cu) of the rows
+// of the ring (ring) or of the state into dst, `bytes` already checked.  When it reads a channel plane (`channels`), the
+// channel planes are recomputed first, on the handle's stream.  A device destination takes the table straight from the
+// kernel; any other gets it through the staging buffer, after the `scratch` bytes the reduction needs.
+// launch(out, scratch, &launches) enqueues the reduction on the handle's stream.
 extern "C++" {
 template <class Launch>
-static int run_world_reduction(b200_sixdof *h, uint64_t scratch, void *dst, uint64_t bytes, Launch launch)
+static int run_world_reduction(b200_sixdof *h, bool ring, bool channels, uint64_t scratch, void *dst, uint64_t bytes,
+                               Launch launch)
 {
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (bytes == 0) return B200_OK;
     if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    int rc = channels ? refresh_channels(h, ring) : B200_OK;
+    if (rc) return rc;
     const bool direct = device_destination(h, dst);
     scratch = (scratch + 7) / 8 * 8;
-    int rc = ensure_staging(h, std::max<uint64_t>(scratch + (direct ? 0 : bytes), 8));
+    rc = ensure_staging(h, std::max<uint64_t>(scratch + (direct ? 0 : bytes), 8));
     if (rc) return rc;
     double *out = direct ? (double *)dst : (double *)((char *)h->staging + scratch);
     int launches = 0;
@@ -1328,19 +1334,13 @@ static int upload_group_table(b200_sixdof *h, const void *t, uint64_t bytes, voi
 // quantiles' route order over it and the covariance's group table; the grouped entries' tables, else the all-worlds ones.
 static int build_group_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped)
 {
-    std::vector<WorldGroup> &stats = grouped ? h->group_table : h->all_table, &cov = grouped ? h->group_cov : h->all_cov;
-    std::vector<uint32_t> &order = grouped ? h->group_order : h->all_order;
-    stats = world_group_table(sizes, n_groups, h->desc.n_entities);
-    cov = cov_group_table(sizes, n_groups, h->desc.n_entities);
-    order = quantile_order(stats);
-    int rc = upload_group_table(h, stats.data(), stats.size() * sizeof(WorldGroup),
-                                (void **)(grouped ? &h->group_table_dev : &h->all_table_dev));
-    if (!rc)
-        rc = upload_group_table(h, cov.data(), cov.size() * sizeof(WorldGroup),
-                                (void **)(grouped ? &h->group_cov_dev : &h->all_cov_dev));
-    if (!rc)
-        rc = upload_group_table(h, order.data(), order.size() * sizeof(uint32_t),
-                                (void **)(grouped ? &h->group_order_dev : &h->all_order_dev));
+    b200_sixdof::GroupTables &t = h->tables[grouped];
+    t.stats = world_group_table(sizes, n_groups, h->desc.n_entities);
+    t.cov = cov_group_table(sizes, n_groups, h->desc.n_entities);
+    t.order = quantile_order(t.stats);
+    int rc = upload_group_table(h, t.stats.data(), t.stats.size() * sizeof(WorldGroup), (void **)&t.stats_dev);
+    if (!rc) rc = upload_group_table(h, t.cov.data(), t.cov.size() * sizeof(WorldGroup), (void **)&t.cov_dev);
+    if (!rc) rc = upload_group_table(h, t.order.data(), t.order.size() * sizeof(uint32_t), (void **)&t.order_dev);
     return rc;
 }
 
@@ -1391,16 +1391,11 @@ static int run_world_stats(b200_sixdof *h, bool ring, bool grouped, void *dst, u
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s statistics are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    const std::vector<WorldGroup> &table = grouped ? h->group_table : h->all_table;
-    const WorldGroup *groups = grouped ? h->group_table_dev : h->all_table_dev;
-    const uint64_t scratch = bytes && h->status == B200_OK ? world_stats_scratch_doubles(S, table) * 8ull : 0;
-    if (bytes && h->status == B200_OK && dst) {
-        const int rc = refresh_channels(h, ring);
-        if (rc) return rc;
-    }
-    return run_world_reduction(h, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
+    const b200_sixdof::GroupTables &t = h->tables[grouped];
+    const uint64_t scratch = bytes && h->status == B200_OK ? world_stats_scratch_doubles(S, t.stats) * 8ull : 0;
+    return run_world_reduction(h, ring, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
-        return launch_world_stats(S, groups, table, (double *)scr, n, h->stream);
+        return launch_world_stats(S, t.stats_dev, t.stats, (double *)scr, n, h->stream);
     });
 }
 
@@ -1440,8 +1435,7 @@ static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *
     if (!q) return fail(B200_ERR_INVALID_ARGUMENT, "null quantile levels");
     for (uint32_t l = 0; l < n_q; ++l)
         if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
-    const std::vector<WorldGroup> &table = grouped ? h->group_table : h->all_table;
-    const std::vector<uint32_t> &order = grouped ? h->group_order : h->all_order;
+    const b200_sixdof::GroupTables &t = h->tables[grouped];
     const uint64_t G = reduction_groups(h, grouped).size();
     const uint64_t want = S.n_planes * G * S.n_entities * n_q * 8ull;
     if (bytes != want)
@@ -1449,18 +1443,15 @@ static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *
                     (unsigned long long)bytes);
     S.n_q = n_q;
     for (uint32_t l = 0; l < n_q; ++l) S.q[l] = q[l];
-    S.groups = grouped ? h->group_table_dev : h->all_table_dev;
-    S.order = grouped ? h->group_order_dev : h->all_order_dev;
+    S.groups = t.stats_dev;
+    S.order = t.order_dev;
     S.n_groups = G;
     const uint64_t triples = S.n_planes * G * S.n_entities;
     h->quantile_read_sum = triples;  // the small-group routes read every triple once
-    if (bytes && dst) {
-        const int rc = refresh_channels(h, ring);
-        if (rc) return rc;
-    }
-    int rc = run_world_reduction(h, quantile_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
+    const uint64_t scratch = quantile_scratch_bytes(S, t.stats);
+    int rc = run_world_reduction(h, ring, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
-        return launch_quantiles(S, table, order, scratch, n, &h->quantile_read_sum, h->stream);
+        return launch_quantiles(S, t.stats, t.order, scr, n, &h->quantile_read_sum, h->stream);
     });
     h->quantile_reads = rc == B200_OK && bytes && triples ? (double)h->quantile_read_sum / (double)triples : 0.0;
     return rc;
@@ -1520,15 +1511,10 @@ static int run_covariance(b200_sixdof *h, bool ring, bool grouped, const uint32_
                     (unsigned long long)bytes);
     S.n_p = n_p;
     for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
-    const std::vector<WorldGroup> &table = grouped ? h->group_cov : h->all_cov;
-    const WorldGroup *groups = grouped ? h->group_cov_dev : h->all_cov_dev;
-    if (channel && bytes && dst) {
-        const int rc = refresh_channels(h, ring);
-        if (rc) return rc;
-    }
-    return run_world_reduction(h, cov_scratch_bytes(S, table), dst, bytes, [&](double *out, void *scratch, int *n) {
+    const b200_sixdof::GroupTables &t = h->tables[grouped];
+    return run_world_reduction(h, ring, channel, cov_scratch_bytes(S, t.cov), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
-        return launch_covariance(S, groups, table, scratch, n, h->stream);
+        return launch_covariance(S, t.cov_dev, t.cov, scratch, n, h->stream);
     });
 }
 
@@ -1644,11 +1630,7 @@ static int run_histograms(b200_sixdof *h, bool ring, bool grouped, const b200_hi
     const uint64_t edge_bytes = edges.size() * 8ull, table_bytes = table.size() * sizeof(WorldGroup);
     edges.resize(edges.size() + table_bytes / 8);  // one copy to the device: the edges, then the group table
     std::memcpy(edges.data() + edge_bytes / 8, table.data(), table_bytes);
-    if (channel && bytes && dst) {
-        const int rc = refresh_channels(h, ring);
-        if (rc) return rc;
-    }
-    return run_world_reduction(h, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
+    return run_world_reduction(h, ring, channel, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
         cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes + table_bytes, cudaMemcpyHostToDevice, h->stream);
         if (e != cudaSuccess) return e;
         P.out = out;

@@ -60,14 +60,18 @@ struct b200_sixdof {
     uint64_t staging_bytes = 0;
     double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
-    // statistics group tables (stats_kernels.cu): all worlds as one group (built at creation) and the groups of
-    // b200_sixdof_set_world_groups (sizes empty = none set), each with its device copy; the quantiles read the same
-    // tables' worlds, in the route order of quantile_order (quantile_kernels.cu), and the covariance has its own
-    // chunking (cov_group_table, cov_kernels.cu), both built at the same two points
-    std::vector<b200::WorldGroup> all_table, group_table, all_cov, group_cov;
-    b200::WorldGroup *all_table_dev = nullptr, *group_table_dev = nullptr, *all_cov_dev = nullptr, *group_cov_dev = nullptr;
-    std::vector<uint32_t> all_order, group_order;
-    uint32_t *all_order_dev = nullptr, *group_order_dev = nullptr;
+    // the group tables of one split of the worlds, each with its device copy: the statistics' (stats_kernels.cu), the
+    // quantiles' route order over the same worlds (quantile_order, quantile_kernels.cu) and the covariance's own
+    // chunking (cov_group_table, cov_kernels.cu)
+    struct GroupTables {
+        std::vector<b200::WorldGroup> stats, cov;
+        std::vector<uint32_t> order;
+        b200::WorldGroup *stats_dev = nullptr, *cov_dev = nullptr;
+        uint32_t *order_dev = nullptr;
+    };
+    // indexed by `grouped`: all worlds as one group (built at creation), then the groups of b200_sixdof_set_world_groups
+    // (sizes empty = none set)
+    GroupTables tables[2];
     std::vector<uint64_t> group_sizes;
     // trajectory
     double *traj = nullptr;

@@ -558,6 +558,30 @@ def _sampled_plane(span, index, where: str) -> int:
     return span[0] + int(index)
 
 
+def _channel_plane(plane: int, n_channels: int, where: str) -> int:
+    """`plane` of an ensemble row (25 planes, then channel k at 25 + k); ValueError, prefixed by `where`, if it is a
+    channel beyond the `n_channels` of the Exec."""
+    if plane >= _lib.ROW_PLANES + n_channels:
+        raise ValueError(f"{where}: channel {plane - _lib.ROW_PLANES}, this Exec has {n_channels}")
+    return plane
+
+
+# the tables of ensemble mode, by kind, and the World.build option, after ensemble=True, that records each.  stats,
+# quantiles, covariance and histograms are reduced over the worlds per telemetry row (B200Exec.trajectory_<kind> /
+# state_<kind>; with groups=[...] also group_<kind>, per group of worlds); the others are run summaries, folded per
+# world (B200Exec.summary_begin) and downloaded by B200Exec.<kind>().
+_OPTIONS = {"stats": (), "quantiles": ("quantiles=[...]",), "covariance": ("covariance=[...]",),
+            "histograms": ("histograms=[...]",), "extrema": ("extrema=True",), "thresholds": ("thresholds=[...]",),
+            "moments": ("moments=[...]",), "dwells": ("dwells=[...]",)}
+_SUMMARIES = ("extrema", "thresholds", "moments", "dwells")
+
+
+def _build_with(what: str, *options: str) -> "_lib.B200Error":
+    """The refusal (ERR_INVALID_ARGUMENT) of `what` by an Exec built without World.build(..., ensemble=True, *options)."""
+    return _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                          f"{what}: build the Exec with World.build(..., {', '.join(('ensemble=True',) + options)})")
+
+
 def _quantile_levels(levels) -> np.ndarray:
     """World.build(..., quantiles=...): 1 to MAX_QUANTILES real levels in [0, 1], order and duplicates kept."""
     if isinstance(levels, (str, bytes)) or not isinstance(levels, Sequence) and not isinstance(levels, np.ndarray):
@@ -590,16 +614,14 @@ def _covariance_planes(spec, channel_names=(), option: str = "covariance", max_p
             comp, idx = None, None
         if not isinstance(comp, str):
             raise TypeError(f"{option} item {item!r}: a component name or a (component, indices) pair")
-        span = (_lib.ROW_PLANES, _lib.ROW_PLANES + len(channel_names)) if comp == _CHANNELS else _SAMPLED.get(comp)
+        span = _CHANNEL_SPAN if comp == _CHANNELS else _SAMPLED.get(comp)
         if span is None:
             raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
                                       f"component not found: {comp} (ensemble {option} covers {', '.join(_SAMPLED)})")
-        for i in range(span[1] - span[0]) if idx is None else idx:
-            if comp == _CHANNELS:
-                _sampled_plane(_CHANNEL_SPAN, i, f"{option} item {item!r}")
-                if i >= len(channel_names):
-                    raise ValueError(f"{option} item {item!r}: channel {int(i)}, this Exec has {len(channel_names)}")
-            plane = _sampled_plane(span, i, f"{option} item {item!r}")
+        width = len(channel_names) if comp == _CHANNELS else span[1] - span[0]
+        for i in range(width) if idx is None else idx:
+            where = f"{option} item {item!r}"
+            plane = _channel_plane(_sampled_plane(span, i, where), len(channel_names), where)
             if plane in planes:
                 raise ValueError(f"{option} selects {comp}[{int(i)}] twice")
             planes.append(plane)
@@ -916,23 +938,19 @@ class Exec:
             if col is None or col.entity_ids != bodies:
                 raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {cname}")
         # ensemble-mode options: checked here, before any device call, the mode before any option's own values
+        given = [name for name, value in (("extrema", extrema or None), ("thresholds", thresholds or None),
+                                          ("quantiles", quantiles), ("covariance", covariance), ("histograms", histograms),
+                                          ("groups", groups), ("retain", retain), ("channels", channels),
+                                          ("moments", moments), ("dwells", dwells)) if value is not None]
+        if given and not ensemble:
+            msg = f"{', '.join(given)}: need World.build(..., ensemble=True)"
+            raise ValueError(msg) if given == ["groups"] else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, msg)
+        self.groups = _world_groups(groups, self.n_worlds) if groups is not None else None
+        self._retain = _retained_worlds(retain, self.n_worlds, len(bodies)) if retain is not None else None
+        self._channels = _channel_list(channels) if channels is not None else []
+        n_c = len(self._channels)  # channel k is plane 25 + k of an ensemble row
         self._extrema = bool(extrema)
         self._thresholds = list(thresholds or [])
-        given = [name for name, on in (("extrema", self._extrema), ("thresholds", self._thresholds),
-                                       ("quantiles", quantiles is not None), ("covariance", covariance is not None),
-                                       ("histograms", histograms is not None)) if on]
-        if given and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{', '.join(given)}: need World.build(..., ensemble=True)")
-        if groups is not None and not ensemble:
-            raise ValueError("groups: need World.build(..., ensemble=True)")
-        self.groups = _world_groups(groups, self.n_worlds) if groups is not None else None
-        if retain is not None and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "retain: need World.build(..., ensemble=True)")
-        self._retain = _retained_worlds(retain, self.n_worlds, len(bodies)) if retain is not None else None
-        if channels is not None and not ensemble:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "channels: need World.build(..., ensemble=True)")
-        self._channels = _channel_list(channels) if channels is not None else []
-        n_rows = _lib.ROW_PLANES + len(self._channels)  # planes of an ensemble row
         if len(self._thresholds) > _lib.MAX_THRESHOLDS:
             raise ValueError(f"{len(self._thresholds)} thresholds: at most {_lib.MAX_THRESHOLDS}")
 
@@ -941,59 +959,41 @@ class Exec:
             for t in conditions:
                 if not isinstance(t, Threshold):
                     raise TypeError(f"{option} take el.Threshold objects, got {t!r}")
-                try:
-                    ent = world.entity_by_name(t.entity)
-                except _lib.B200ValueError:
-                    ent = None
-                if ent not in bodies:
-                    raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {t.pair}")
-                if t.plane >= n_rows:
-                    raise ValueError(f"{t!r}: channel {t.index}, this Exec has {len(self._channels)}")
-                out.append((bodies.index(ent), t.plane, t.above, t.value))
+                out.append((self._body_row(t.entity, t.pair), _channel_plane(t.plane, n_c, repr(t)), t.above, t.value))
             return out
 
         self._threshold_rows = condition_rows(self._thresholds, "thresholds")
-        # run moments and dwells (folded with the extrema): the same mode rule, then their own values
-        for name, on in (("moments", moments is not None), ("dwells", dwells is not None)):
-            if on and not ensemble:
-                raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{name}: need World.build(..., ensemble=True)")
         self._moment_planes, self._moment_labels = ([], []) if moments is None else _covariance_planes(
-            moments, [c.name for c in self._channels], "moments", n_rows)
+            moments, self.channels, "moments", _lib.ROW_PLANES + n_c)
         if dwells is not None and (isinstance(dwells, (str, bytes)) or not isinstance(dwells, Sequence)):
             raise TypeError(f"dwells take a sequence of el.Threshold objects, got {dwells!r}")
         self._dwells = list(dwells or [])
         if len(self._dwells) > _lib.MAX_DWELLS:
             raise ValueError(f"{len(self._dwells)} dwells: at most {_lib.MAX_DWELLS}")
         self._dwell_rows = condition_rows(self._dwells, "dwells")
-        self._summaries = bool(self._extrema or self._thresholds or self._moment_planes or self._dwells)
-        # ensemble rows, per kind of table: the arguments of B200Exec.trajectory_<kind> / state_<kind>, and the blocks
-        # of rows recorded so far ([k, n_entities, ...] each)
+        # the run summaries this Exec folds (kinds of _OPTIONS)
+        self._summaries = tuple(kind for kind, on in zip(_SUMMARIES, (self._extrema, self._thresholds,
+                                                                      self._moment_planes, self._dwells)) if on)
+        # the tables reduced per telemetry row: the arguments of B200Exec.trajectory_<kind> / state_<kind> per kind of
+        # _OPTIONS, and per table this Exec records (the kind, or group_<kind> for its per-group table, in the order
+        # they are reduced) the blocks of rows recorded so far ([k, ...] each)
         self._ens_args: Dict[str, tuple] = {"stats": ()} if ensemble else {}
         if quantiles is not None:
             self._ens_args["quantiles"] = (_quantile_levels(quantiles),)
         if covariance is not None:
-            planes, self._cov_labels = _covariance_planes(covariance, [c.name for c in self._channels])
+            planes, self._cov_labels = _covariance_planes(covariance, self.channels)
             self._ens_args["covariance"] = (planes,)
         if histograms is not None:
             self._histograms = _histogram_specs(histograms)
             specs = []
-            for h in self._histograms:  # the entity resolved against the Body entities, as for thresholds
-                try:
-                    ent = world.entity_by_name(h.entity)
-                except _lib.B200ValueError:
-                    ent = None
-                if ent not in bodies:
-                    raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {h.pair}")
-                if max(h.planes) >= n_rows:
-                    raise ValueError(f"Histogram({h.pair!r}, ...): a channel index, this Exec has {len(self._channels)}")
-                specs.append(h._spec(bodies.index(ent)))
+            for h in self._histograms:
+                specs.append(h._spec(self._body_row(h.entity, h.pair)))
+                for p in h.planes:
+                    _channel_plane(p, n_c, repr(h))
             self._ens_args["histograms"] = (specs,)
-        if self.groups is not None:  # the same tables per group of worlds
-            self._ens_args["group_stats"] = ()
-            for kind in ("histograms", "quantiles", "covariance"):
-                if kind in self._ens_args:
-                    self._ens_args[f"group_{kind}"] = self._ens_args[kind]
-        self._ens_rows: Dict[str, List[np.ndarray]] = {kind: [] for kind in self._ens_args}
+        grouped = [f"group_{kind}" for kind in ("stats", "histograms", "quantiles", "covariance")
+                   if kind in self._ens_args and self.groups is not None]
+        self._ens_rows: Dict[str, List[np.ndarray]] = {name: [] for name in [*self._ens_args, *grouped]}
         # Query join (query.rs:672-710): an effector only runs on the entities that own its input
         # component.  Full membership -> no mask; partial (order-preserving) membership -> entity mask +
         # a body-row-expanded copy of the column for the device; no members / foreign order -> error.
@@ -1027,7 +1027,7 @@ class Exec:
             # Ensemble mode: the state never leaves the device between the initial upload and the end of run();
             # each ring-full of telemetry samples is reduced over the worlds in place, then the ring is reset.
             ld = (n_bodies + 127) // 128 * 128
-            cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max(n_rows * ld * 8, 1)
+            cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max((_lib.ROW_PLANES + n_c) * ld * 8, 1)
             self._ring_cap = int(max(1, min(4096, cap)))
         elif resident and n_bodies:
             ld = (n_bodies + 127) // 128 * 128
@@ -1047,10 +1047,9 @@ class Exec:
         self._summary_tables: Dict[str, np.ndarray] = {}  # run summaries downloaded since the last fold
         if self._channels:  # before summary_begin, which fixes the row width
             self.backend.set_channels([c._record() for c in self._channels])
-        if self._moment_planes or self._dwell_rows:
-            self.backend.summary_begin(self._extrema, self._threshold_rows, self._moment_planes, self._dwell_rows)
-        elif self._summaries:
-            self.backend.summary_begin(self._extrema, self._threshold_rows)
+        if self._summaries:  # moments and dwells are optional keywords of B200Exec.summary_begin: passed when asked for
+            self.backend.summary_begin(self._extrema, self._threshold_rows, **{
+                k: v for k, v in (("moments", self._moment_planes), ("dwells", self._dwell_rows)) if v})
         if self.groups is not None:
             self.backend.set_world_groups(self.groups)
         if self._ensemble:
@@ -1139,9 +1138,10 @@ class Exec:
         records, folds the run summaries, records the retained worlds' rows (from the host columns when `host_rows`)
         and appends the rows' globals."""
         be = self.backend
-        for kind, args in self._ens_args.items():
-            rows = getattr(be, f"trajectory_{kind}")(*args) if ring else getattr(be, f"state_{kind}")(*args)[None]
-            self._ens_rows[kind].append(rows)
+        for name, blocks in self._ens_rows.items():
+            args = self._ens_args[name.removeprefix("group_")]
+            rows = getattr(be, f"trajectory_{name}")(*args) if ring else getattr(be, f"state_{name}")(*args)[None]
+            blocks.append(rows)
         if self._summaries:
             (be.summary_add_trajectory if ring else be.summary_add_state)()
             self._summary_tables.clear()
@@ -1164,13 +1164,18 @@ class Exec:
             for cid, col in self.world.columns.items():
                 self._history[cid].append(col.buffer[idx])
             return
-        rows = be.trajectory_worlds(idx) if ring else be.state_worlds(idx)[None]  # [k, R, n_entities, 25]
+        self._extend_history(be.trajectory_worlds(idx) if ring else be.state_worlds(idx)[None], idx)
+
+    def _extend_history(self, rows: np.ndarray, worlds: Optional[List[int]] = None) -> None:
+        """Append the k history rows of a [k, worlds, n_entities, 25] block of samples: the sampled components cut from
+        its planes (one contiguous block per column, the rows are views), every column six_dof() does not write passed
+        through from the host columns (at `worlds`, or every world)."""
         for name, (lo, hi) in _SAMPLED.items():
             self._history[component_id(name)].extend(np.ascontiguousarray(rows[..., lo:hi]))
         sampled = {component_id(name) for name in _SAMPLED}
         for cid, col in self.world.columns.items():
-            if cid not in sampled:                                    # pass-through, as on the resident route
-                self._history[cid].extend([col.buffer[idx]] * rows.shape[0])
+            if cid not in sampled:
+                self._history[cid].extend([col.buffer.copy() if worlds is None else col.buffer[worlds]] * rows.shape[0])
 
     def _run_ensemble(self, ticks: int, is_canceled, pre_step, post_step) -> None:
         """Ensemble mode: one row of world-axis statistics per telemetry cycle, reduced on the device from the
@@ -1272,8 +1277,6 @@ class Exec:
         t0 = time.perf_counter()
         self._upload_inputs()
         upload_ms = (time.perf_counter() - t0) * 1e3
-        body_cols = [(component_id(name), lo, hi) for name, (lo, hi) in _SAMPLED.items()]
-        sampled = {cid for cid, _, _ in body_cols}
         while cycles > 0:
             c = min(cycles, self._ring_cap)
             t0 = time.perf_counter()
@@ -1283,15 +1286,11 @@ class Exec:
             run_ms = (time.perf_counter() - t0) * 1e3 + upload_ms
             upload_ms = 0.0
             t_hist = time.perf_counter()
-            for cid, lo, hi in body_cols:                            # one contiguous block per column, rows are views
-                self._history[cid].extend(np.ascontiguousarray(traj[:, :, :, lo:hi]))
-            for cid, col in self.world.columns.items():
-                if cid not in sampled:                               # not written by six_dof(): pass-through
-                    self._history[cid].extend([col.buffer.copy()] * c)
+            self._extend_history(traj)
             self._globals_hist.extend((self.tick + (k + 1) * tpt, self.sim_time_step) for k in range(c))
             self.tick += c * tpt
-            for cid, lo, hi in body_cols:
-                np.copyto(self.world.columns[cid].buffer, traj[-1, :, :, lo:hi])
+            for name, (lo, hi) in _SAMPLED.items():
+                np.copyto(self.world.columns[component_id(name)].buffer, traj[-1, :, :, lo:hi])
             if getattr(self, "_db", None) is not None:
                 self._db.flush()  # the c cycles of this ring read-back, each with its own timestamp
             hist_ms = (time.perf_counter() - t_hist) * 1e3
@@ -1414,11 +1413,9 @@ class Exec:
         where no world is finite.  Needs World.build(..., ensemble=True); the sampled components are world_pos,
         world_vel, world_accel and force.  With groups=True (World.build(..., groups=[...])) each is [rows, G, width],
         taken over the worlds of each group."""
-        if groups:
-            t = self._ensemble_rows("group_stats", pair, "ensemble statistics", "ensemble(groups=True)", ", groups=[...]",
-                                    grouped=True)  # [rows, G, width, 5]
-        else:
-            t = self._ensemble_rows("stats", pair, "ensemble statistics", "ensemble()", "")  # [rows, width, 5]
+        t = self._table("ensemble", "stats", groups)
+        row, (lo, hi) = self._sampled_row(pair, "ensemble statistics")
+        t = t[..., row, lo:hi, :]  # [rows, (G,) width, 5]
         count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
             std = np.sqrt(t[..., 2] / count)
@@ -1432,12 +1429,9 @@ class Exec:
         world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates.
         With groups=True (World.build(..., groups=[...])) -> [rows, G, n_q, width], over the worlds of each group.
         Quantile tables do not merge across the ranks of a world-sharded campaign: each rank has its own."""
-        if groups:
-            t = self._ensemble_rows("group_quantiles", pair, "ensemble quantiles", "quantiles(groups=True)",
-                                    ", quantiles=[...], groups=[...]", grouped=True)  # [rows, G, width, n_q]
-            return np.ascontiguousarray(t.transpose(0, 1, 3, 2))
-        t = self._ensemble_rows("quantiles", pair, "ensemble quantiles", "quantiles()", ", quantiles=[...]")  # [rows, width, n_q]
-        return np.ascontiguousarray(t.transpose(0, 2, 1))
+        t = self._table("quantiles", "quantiles", groups)
+        row, (lo, hi) = self._sampled_row(pair, "ensemble quantiles")
+        return np.ascontiguousarray(np.swapaxes(t[..., row, lo:hi, :], -1, -2))  # from [rows, (G,) width, n_q]
 
     def covariance(self, entity: str, groups: bool = False) -> Dict[str, object]:
         """`exec.covariance("rocket")` -> {"count" [rows], "mean" [rows, p], "cov" [rows, p, p], "planes" [p] labels such
@@ -1447,13 +1441,7 @@ class Exec:
         (numpy's ddof=0, as Exec.ensemble's std), exactly symmetric, NaN where count = 0.  With groups=True
         (World.build(..., groups=[...])) a group axis follows the row axis: count [rows, G], mean [rows, G, p], cov
         [rows, G, p, p], over the worlds of each group."""
-        if groups:
-            t = self._ensemble_rows("group_covariance", f"{entity}.world_pos", "ensemble covariance",
-                                    "covariance(groups=True)", ", covariance=[...], groups=[...]", per_plane=False,
-                                    grouped=True)  # [rows, G, 1 + p + p*p]
-        else:
-            t = self._ensemble_rows("covariance", f"{entity}.world_pos", "ensemble covariance", "covariance()",
-                                    ", covariance=[...]", per_plane=False)  # [rows, 1 + p + p*p]
+        t = self._table("covariance", "covariance", groups)[..., self._body_row(entity, entity), :]  # [rows, (G,) 1 + p + p*p]
         p = len(self._cov_labels)
         count = np.ascontiguousarray(t[..., 0])
         with np.errstate(invalid="ignore", divide="ignore"):
@@ -1468,40 +1456,46 @@ class Exec:
         of range), and "edges" (np.linspace's; a pair for 2D).  Every world is counted once per row.  With groups=True
         (World.build(..., groups=[...])) a group axis follows the row axis: [rows, G, ...], over the worlds of each
         group."""
-        kind = "group_histograms" if groups else "histograms"
-        if kind not in self._ens_rows:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 f"histogram({'groups=True' if groups else ''}): build the Exec with World.build(..., "
-                                 f"ensemble=True, histograms=[...]{', groups=[...]' if groups else ''})")
+        t = self._table("histogram", "histograms", groups)
         if not 0 <= i < len(self._histograms):
             raise IndexError(f"histogram {i}: this Exec has {len(self._histograms)}")
         h = self._histograms[i]
         off = sum(x.record_len for x in self._histograms[:i])
-        t = np.concatenate(self._ens_rows[kind])[..., off:off + h.record_len].astype(np.int64)
+        t = t[..., off:off + h.record_len].astype(np.int64)
         if len(h.bins) == 1:
             return {"counts": np.ascontiguousarray(t[..., 3:]), "nonfinite": t[..., 0].copy(), "below": t[..., 1].copy(),
                     "above": t[..., 2].copy(), "edges": h.edges}
         return {"counts": np.ascontiguousarray(t[..., 2:]).reshape(*t.shape[:-1], *h.bins), "nonfinite": t[..., 0].copy(),
                 "outside": t[..., 1].copy(), "edges": h.edges}
 
-    def _ensemble_rows(self, kind: str, pair: str, what: str, method: str, option: str, per_plane: bool = True,
-                       grouped: bool = False):
-        """The recorded rows of table `kind` for the entity of `pair` (after the group axis when the table is
-        `grouped`), sliced to the planes of its component when the table is `per_plane`; refused (ERR_INVALID_ARGUMENT)
-        by `method` if this Exec was not built with `option`."""
-        if kind not in self._ens_rows:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{method}: build the Exec with World.build(..., ensemble=True{option})")
-        row, (lo, hi) = self._sampled_row(pair, what)
-        t = np.concatenate(self._ens_rows[kind])
-        if grouped:
-            return t[:, :, row, lo:hi] if per_plane else t[:, :, row]
-        t = t[:, row]
-        return t[:, lo:hi] if per_plane else t
+    def _table(self, accessor: str, kind: str, groups: bool = False) -> np.ndarray:
+        """Table `kind` of _OPTIONS (its per-group table with `groups`): the rows recorded so far, or the run summary,
+        downloaded once per fold; refused by `accessor` if this Exec does not record it."""
+        name = f"group_{kind}" if groups else kind
+        if name in self._ens_rows:
+            return np.concatenate(self._ens_rows[name])
+        if name not in _SUMMARIES or name not in self._summaries:
+            raise _build_with(f"{accessor}({'groups=True' if groups else ''})", *_OPTIONS[kind],
+                              *(("groups=[...]",) if groups else ()))
+        if name not in self._summary_tables:
+            self._summary_tables[name] = getattr(self.backend, name)()
+        return self._summary_tables[name]
 
     @property
     def channels(self) -> List[str]:
         """The names of the channels of World.build(..., channels=[...]), in order: index k of "<entity>.channels"."""
         return [c.name for c in self._channels]
+
+    def _body_row(self, entity: str, pair: str) -> int:
+        """The Body row of entity `entity`; ERR_COMPONENT_NOT_FOUND, naming `pair`, if it is not a Body entity."""
+        bodies = self.world.body_entities()
+        try:
+            ent = self.world.entity_by_name(entity)
+        except _lib.B200ValueError:
+            ent = None
+        if ent not in bodies:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
+        return bodies.index(ent)
 
     def _sampled_row(self, pair: str, what: str):
         """`<entity>.<component>` -> (Body row of the entity, plane span of the component in an ensemble row: 25 planes,
@@ -1509,20 +1503,9 @@ class Exec:
         ent, span = _sampled_span(pair, what)
         if span == _CHANNEL_SPAN:
             if not self._channels:
-                raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                     f"{pair}: build the Exec with World.build(..., ensemble=True, channels=[...])")
+                raise _build_with(pair, "channels=[...]")
             span = (span[0], span[0] + len(self._channels))
-        ent_id = self.world.entity_by_name(ent)
-        col = self.world.columns[component_id("world_pos")]
-        if ent_id not in col.entity_ids:
-            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair}")
-        return col.row_of(ent_id), span
-
-    def _summary_table(self, name: str) -> np.ndarray:
-        """The backend's extrema / thresholds / moments / dwells table, downloaded once per fold."""
-        if name not in self._summary_tables:
-            self._summary_tables[name] = getattr(self.backend, name)()
-        return self._summary_tables[name]
+        return self._body_row(ent, pair), span
 
     def extrema(self, pair: str) -> Dict[str, np.ndarray]:
         """`exec.extrema("rocket.world_pos")` -> {"min", "max", "min_tick", "max_tick", "first_nonfinite_tick"}, each
@@ -1530,11 +1513,9 @@ class Exec:
         finite values (NaN if none), the tick of the row that holds them (the earliest on ties) and the tick of the first
         NaN / inf row; ticks are int64, -1 where they never applied.  Needs World.build(..., ensemble=True,
         extrema=True)."""
-        if not self._extrema:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "extrema(): build the Exec with World.build(..., ensemble=True, extrema=True)")
+        t = self._table("extrema", "extrema")
         row, span = self._sampled_row(pair, "extrema")
-        t = self._summary_table("extrema")[:, row, span[0]:span[1], :]  # [n_worlds, width, 5]
+        t = t[:, row, span[0]:span[1], :]  # [n_worlds, width, 5]
         out = {k: np.ascontiguousarray(t[..., f]) for f, k in enumerate(("min", "max"))}
         for f, k in enumerate(("min_tick", "max_tick", "first_nonfinite_tick"), start=2):
             out[k] = t[..., f].astype(np.int64)
@@ -1544,12 +1525,10 @@ class Exec:
         """`exec.threshold(i)` -> {"tick": int64 [n_worlds], "world_pos": [n_worlds, 7], "world_vel", "world_accel",
         "force"}: for threshold i of World.build(..., thresholds=[...]), the tick of each world's first telemetry row
         that meets it (-1 = never) and the entity's state at that row (NaN where it never fired)."""
-        if not self._thresholds:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "threshold(): build the Exec with World.build(..., ensemble=True, thresholds=[...])")
+        t = self._table("threshold", "thresholds")
         if not 0 <= i < len(self._thresholds):
             raise IndexError(f"threshold {i}: this Exec has {len(self._thresholds)}")
-        t = self._summary_table("thresholds")[:, i, :]  # [n_worlds, 26]
+        t = t[:, i, :]  # [n_worlds, 26]
         out = {"tick": t[:, 0].astype(np.int64)}
         for name, (lo, hi) in _SAMPLED.items():
             out[name] = np.ascontiguousarray(t[:, 1 + lo:1 + hi])
@@ -1561,15 +1540,13 @@ class Exec:
         state) whose value is finite, the number of rows, the mean, the spread (numpy's ddof=0) and the root mean square,
         for the components of World.build(..., moments=...).  NaN where count = 0; std and rms are +inf where the sum
         of squares overflowed."""
-        if not self._moment_planes:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "moments(): build the Exec with World.build(..., ensemble=True, moments=[...])")
+        t = self._table("moments", "moments")
         row, (lo, hi) = self._sampled_row(pair, "moments")
         cols = sorted((p, j) for j, p in enumerate(self._moment_planes) if lo <= p < hi)
         if not cols:
             raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
                                  f"moments({pair!r}): no index of it is selected by World.build(..., moments=[...])")
-        t = self._summary_table("moments")[:, row, [j for _, j in cols], :]  # [n_worlds, k, 3]
+        t = t[:, row, [j for _, j in cols], :]  # [n_worlds, k, 3]
         n, mean, m2 = t[..., 0], t[..., 1], t[..., 2]
         with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
             var = m2 / n
@@ -1582,13 +1559,10 @@ class Exec:
         dwells=[...]), the number of each world's telemetry rows (row 0 = the initial state) beyond its bound, and the
         ticks of the first and last of them (-1 where none).  `last_tick` of an error norm above a tolerance is the
         settling time.  Counts are rows, not seconds: a partial last cycle makes the rows unevenly spaced."""
-        if not self._dwells:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                 "dwell(): build the Exec with World.build(..., ensemble=True, dwells=[...])")
+        t = self._table("dwell", "dwells")
         if not 0 <= i < len(self._dwells):
             raise IndexError(f"dwell {i}: this Exec has {len(self._dwells)}")
-        t = self._summary_table("dwells")[:, i, :]  # [n_worlds, 3]
-        return {k: t[:, f].astype(np.int64) for f, k in enumerate(("rows", "first_tick", "last_tick"))}
+        return {k: t[:, i, f].astype(np.int64) for f, k in enumerate(("rows", "first_tick", "last_tick"))}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

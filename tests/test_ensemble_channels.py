@@ -21,6 +21,7 @@ from tests.ensemble_util import (ROCKET, handle, need_gpu, no_device, rocket_wor
                                  sampled_state, two_body_world)
 from tests.test_ensemble_histograms import state_handle
 from tests.test_ensemble_retained import _EnsembleFake
+from tests.test_host_logic import _FakeBackend
 
 MODES = ("exact", "fast")
 ATAN2_ULP = 2  # CUDA Math API: maximum ulp error of double atan2(y, x)
@@ -325,6 +326,213 @@ def test_channels_need_channels_to_be_addressed(monkeypatch):
     assert ex.channels == []
     with pytest.raises(el.B200Error, match=r"rocket.channels: build the Exec with .*channels=\[...\]"):
         ex.ensemble("rocket.channels")
+
+
+# every table a fake reduction or run summary returns, and the code its values start with
+_CODES = {k: i + 1 for i, k in enumerate(("stats", "quantiles", "covariance", "histograms", "group_stats",
+                                          "group_quantiles", "group_covariance", "group_histograms",
+                                          "extrema", "thresholds", "moments", "dwells"))}
+
+
+def _named(kind, rows, tail):
+    """[len(rows), *tail]: 1e8 * the kind's code + 1e5 * the row + the flat index of the value within the row."""
+    n = int(np.prod(tail))
+    t = _CODES[kind] * 1e8 + np.asarray(rows, dtype=np.float64)[:, None] * 1e5 + np.arange(n, dtype=np.float64)
+    return t.reshape((len(rows),) + tuple(tail))
+
+
+class _RecordingFake(_ChannelFake):
+    """The channel fake with every ensemble call of an Exec recorded with its arguments, and tables from _named: the
+    ensemble tables numbered by telemetry row, per kind; the run summaries as row 0."""
+
+    def __init__(self, *a, **kw):
+        super().__init__(*a, **kw)
+        self.rows_seen, self.n_groups = {}, 0
+
+    @staticmethod
+    def _log(*call):
+        _FakeBackend.calls.append(call)
+
+    def set_channels(self, recs):
+        super().set_channels(recs)
+        self._log("set_channels", [(r.kind, r.n) for r in recs])
+
+    def summary_begin(self, extrema, thresholds=(), moments=(), dwells=()):
+        self.summary = (extrema, list(thresholds), list(moments), list(dwells))
+        self._log("summary_begin", *self.summary)
+
+    def set_world_groups(self, sizes):
+        self.n_groups = len(sizes)
+        self._log("set_world_groups", list(sizes))
+
+    def summary_add_state(self):
+        self._log("summary_add_state")
+
+    def summary_add_trajectory(self):
+        self._log("summary_add_trajectory")
+
+    def state_worlds(self, worlds):
+        self._log("state_worlds", list(worlds))
+        return super().state_worlds(worlds)
+
+    def trajectory_worlds(self, worlds):
+        self._log("trajectory_worlds", list(worlds))
+        return super().trajectory_worlds(worlds)
+
+    def download(self, cid, out):
+        self._log("download", cid)
+        super().download(cid, out)
+
+    def _reduce(self, kind, ring, arg):
+        self._log(f"{'trajectory' if ring else 'state'}_{kind}", *[list(np.asarray(a).tolist()) if isinstance(a, np.ndarray)
+                                                                 else a for a in arg])
+        E, R = self.n_entities, 25 + len(self.channel_records)
+        base = kind.removeprefix("group_")
+        if base == "stats":
+            tail = (E, R, 5)
+        elif base == "quantiles":
+            tail = (E, R, len(arg[0]))
+        elif base == "covariance":
+            tail = (E, 1 + len(arg[0]) + len(arg[0]) ** 2)
+        else:
+            tail = (sum((2 if len(planes) == 2 else 3) + int(np.prod(bins)) for _, planes, bins, _, _ in arg[0]),)
+        tail = (self.n_groups,) + tail if kind != base else tail
+        k = len(self.samples) if ring else 1
+        r0 = self.rows_seen.get(kind, 0)
+        self.rows_seen[kind] = r0 + k
+        t = _named(kind, range(r0, r0 + k), tail)
+        return t if ring else t[0]
+
+    def extrema(self):
+        return _named("extrema", [0], (self.n_worlds, self.n_entities, 25 + len(self.channel_records), 5))[0]
+
+    def thresholds(self):
+        return _named("thresholds", [0], (self.n_worlds, len(self.summary[1]), 26))[0]
+
+    def moments(self):
+        return _named("moments", [0], (self.n_worlds, self.n_entities, len(self.summary[2]), 3))[0]
+
+    def dwells(self):
+        return _named("dwells", [0], (self.n_worlds, len(self.summary[3]), 3))[0]
+
+
+def _reduction(kind, ring):
+    return lambda self, *arg: self._reduce(kind, ring, arg)
+
+
+for _kind in _CODES:
+    if _kind not in ("extrema", "thresholds", "moments", "dwells"):
+        setattr(_RecordingFake, f"state_{_kind}", _reduction(_kind, False))
+        setattr(_RecordingFake, f"trajectory_{_kind}", _reduction(_kind, True))
+
+
+@pytest.mark.parametrize("route", ["resident", "host"])
+def test_every_ensemble_option_at_once_with_a_fake_backend(monkeypatch, route):
+    """One Exec with every ensemble option, on the resident route (ring-fulls of 2, 2 and 1 cycles, then a partial
+    cycle) and on the invoke_batch route of a host system (two whole cycles, then a partial one): the exact sequence
+    of backend calls, and every accessor's slice of tables whose values name their position."""
+    from elodin_b200 import world as W
+
+    monkeypatch.setattr(W, "B200Exec", _RecordingFake)
+    chans = [SPEED, el.Norm("range", "world_pos", (4, 5)), el.AxisAngle("pitch", (-1, 0, 0), (0, 0, 1))]
+    levels = [0.1, 0.5, 0.9]
+    hists = [el.Histogram("ball.world_vel", 3, (-1.0, 1.0), 4),
+             el.Histogram("rocket.channels", (0, 1), ((0.0, 1.0), (0.0, 2.0)), (2, 3))]
+    M, E, R, G = 5, 2, 28, 3
+    sys_ = el.six_dof() if route == "resident" else el.six_dof() | el.host_system(lambda ctx: None)
+    ex = two_body_world().build(
+        sys_, simulation_rate=120.0, telemetry_rate=40.0, n_worlds=M, ensemble=True, ensemble_ring=2, channels=chans,
+        extrema=True, thresholds=[el.Threshold("rocket.channels", 1, below=0.0), el.Threshold("ball.world_pos", 4, above=1.0)],
+        quantiles=levels, covariance=[("channels", (2, 0)), ("world_pos", (4,))], histograms=hists, groups=[2, 0, 3],
+        retain=[4, 1], moments=[("world_pos", (6,)), ("channels", (1,))],
+        dwells=[el.Threshold("rocket.world_pos", 6, below=2.0)])
+    be = ex.backend
+    ticks = 16 if route == "resident" else 8
+    ex.run(ticks)
+
+    hist_specs = [(1, (10,), (4,), (-1.0,), (1.0,)), (0, (25, 26), (2, 3), (0.0, 0.0), (1.0, 2.0))]
+    args = {"stats": (), "quantiles": (levels,), "covariance": ([27, 25, 4],), "histograms": (hist_specs,)}
+    order = ("stats", "quantiles", "covariance", "histograms", "group_stats", "group_histograms", "group_quantiles",
+             "group_covariance")
+
+    def rows(ring, worlds=True):
+        src = "trajectory" if ring else "state"
+        calls = [(f"{src}_{k}", *args[k.removeprefix("group_")]) for k in order]
+        return calls + [(f"summary_add_{src}",)] + ([(f"{src}_worlds", [4, 1])] if worlds else [])
+
+    uploads = [("upload", cid) for cid in be.input_ids]
+    want = [("set_channels", [(1, 3), (1, 2), (2, 0)]),
+            ("summary_begin", True, [(0, 26, False, 0.0), (1, 4, True, 1.0)], [6, 26], [(0, 6, False, 2.0)]),
+            ("set_world_groups", [2, 0, 3])] + uploads + rows(False)
+    if route == "resident":                                  # 5 whole cycles of 3 ticks, then one tick
+        want += uploads
+        for c in (2, 2, 1):
+            want += [("reset",), ("step", 3 * c)] + rows(True)
+        want += [("step", 1)] + rows(False)
+        want += [("download", el.component_id(n)) for n in ("world_pos", "world_vel", "world_accel", "force")]
+        n_rows = 7
+    else:
+        for n in (3, 3, 2):
+            want += [("reset",)] + [("invoke", 1), ("step", 1)] * n + rows(n == 3, worlds=False)
+        n_rows = 4
+    assert _FakeBackend.calls == want
+    assert ex.tick == ticks
+
+    rows_ = np.arange(n_rows)
+    for pair, e, lo, hi in (("ball.world_vel", 1, 7, 13), ("rocket.channels", 0, 25, 28), ("rocket.world_pos", 0, 0, 7)):
+        t = _named("stats", rows_, (E, R, 5))[:, e, lo:hi]
+        g = _named("group_stats", rows_, (G, E, R, 5))[:, :, e, lo:hi]
+        for got, tab in ((ex.ensemble(pair), t), (ex.ensemble(pair, groups=True), g)):
+            assert np.array_equal(got["count"], tab[..., 0]) and np.array_equal(got["mean"], tab[..., 1])
+            assert np.array_equal(got["std"], np.sqrt(tab[..., 2] / tab[..., 0]))
+            assert np.array_equal(got["min"], tab[..., 3]) and np.array_equal(got["max"], tab[..., 4])
+        q = _named("quantiles", rows_, (E, R, 3))[:, e, lo:hi]
+        assert np.array_equal(ex.quantiles(pair), q.transpose(0, 2, 1))
+        q = _named("group_quantiles", rows_, (G, E, R, 3))[:, :, e, lo:hi]
+        assert np.array_equal(ex.quantiles(pair, groups=True), q.transpose(0, 1, 3, 2))
+        x = _named("extrema", [0], (M, E, R, 5))[0][:, e, lo:hi]
+        got = ex.extrema(pair)
+        assert np.array_equal(got["min"], x[..., 0]) and np.array_equal(got["max"], x[..., 1])
+        for f, k in enumerate(("min_tick", "max_tick", "first_nonfinite_tick"), start=2):
+            assert got[k].dtype == np.int64 and np.array_equal(got[k], x[..., f].astype(np.int64))
+    for entity, e in (("rocket", 0), ("ball", 1)):
+        for got, t in ((ex.covariance(entity), _named("covariance", rows_, (E, 13))[:, e]),
+                       (ex.covariance(entity, groups=True), _named("group_covariance", rows_, (G, E, 13))[:, :, e])):
+            assert got["planes"] == ["pitch", "speed", "world_pos[4]"]
+            assert np.array_equal(got["count"], t[..., 0]) and np.array_equal(got["mean"], t[..., 1:4])
+            assert np.array_equal(got["cov"], t[..., 4:].reshape(t.shape[:-1] + (3, 3)) / t[..., 0, None, None])
+    for got, t in ((ex.histogram(0), _named("histograms", rows_, (15,))),
+                   (ex.histogram(0, groups=True), _named("group_histograms", rows_, (G, 15)))):
+        t = t.astype(np.int64)
+        assert np.array_equal(got["counts"], t[..., 3:7]) and np.array_equal(got["nonfinite"], t[..., 0])
+        assert np.array_equal(got["below"], t[..., 1]) and np.array_equal(got["above"], t[..., 2])
+        assert np.array_equal(got["edges"], hists[0].edges)
+    for got, t in ((ex.histogram(1), _named("histograms", rows_, (15,))),
+                   (ex.histogram(1, groups=True), _named("group_histograms", rows_, (G, 15)))):
+        t = t.astype(np.int64)
+        assert np.array_equal(got["counts"], t[..., 9:15].reshape(t.shape[:-1] + (2, 3)))
+        assert np.array_equal(got["nonfinite"], t[..., 7]) and np.array_equal(got["outside"], t[..., 8])
+        assert all(np.array_equal(a, b) for a, b in zip(got["edges"], hists[1].edges))
+    thr = _named("thresholds", [0], (M, 2, 26))[0]
+    for i in range(2):
+        got = ex.threshold(i)
+        assert got["tick"].dtype == np.int64 and np.array_equal(got["tick"], thr[:, i, 0].astype(np.int64))
+        for name, (lo, hi) in (("world_pos", (0, 7)), ("world_vel", (7, 13)), ("world_accel", (13, 19)), ("force", (19, 25))):
+            assert np.array_equal(got[name], thr[:, i, 1 + lo:1 + hi])
+    mom = _named("moments", [0], (M, E, 2, 3))[0]
+    for pair, e, j, index in (("rocket.world_pos", 0, 0, 6), ("ball.channels", 1, 1, 1)):
+        got = ex.moments(pair)
+        n, mean, m2 = mom[:, e, [j], 0], mom[:, e, [j], 1], mom[:, e, [j], 2]
+        assert list(got["index"]) == [index] and got["count"].dtype == np.int64
+        assert np.array_equal(got["count"], n.astype(np.int64)) and np.array_equal(got["mean"], mean)
+        assert np.array_equal(got["std"], np.sqrt(m2 / n)) and np.array_equal(got["rms"], np.sqrt(mean * mean + m2 / n))
+    dw = _named("dwells", [0], (M, 1, 3))[0]
+    got = ex.dwell(0)
+    for f, k in enumerate(("rows", "first_tick", "last_tick")):
+        assert got[k].dtype == np.int64 and np.array_equal(got[k], dw[:, 0, f].astype(np.int64))
+    assert ex.retained == (4, 1) and ex.history_worlds("ball.world_pos").shape == (n_rows, 2, 7)
+    assert ex.history_worlds("ball.inertia").shape == (n_rows, 2, 7)
+    assert [r[0] for r in ex._globals_hist] == ([0, 3, 6, 9, 12, 15, 16] if route == "resident" else [0, 3, 6, 8])
 
 
 # --------------------------------------------------------------------------- GPU helpers
