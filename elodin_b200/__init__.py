@@ -21,7 +21,7 @@ from .effectors import (DragQuadratic, GravityConst, GravityEGM08, GravityEdges,
                         TorqueBodyFold, WrenchBody, WrenchWorld, all_pairs_edges)
 from .executor import B200Exec, device_count, merge_covariance, merge_histograms, merge_stats, pinned_empty, pinned_free
 from .world import (Annotated, Archetype, AxisAngle, Body, Channel, Component, ComponentType, Edge, EntityId, Exec, Force, Histogram,
-                    HostSystem, Inertia, Integrator, Norm, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
+                    HostSystem, Inertia, Integrator, Norm, Outcome, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
                     SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, Threshold, World, WorldAccel,
                     WorldPos, WorldVel, dataclass, host_system, quantised_time_step, six_dof, ticks_per_telemetry)
 

@@ -72,6 +72,10 @@ SYMBOLS = [
     "b200_sixdof_trajectory_download_worlds", "b200_sixdof_state_download_worlds",
     "b200_sixdof_set_channels", "b200_sixdof_channels", "b200_sixdof_trajectory_channels", "b200_sixdof_state_channels",
     "b200_sixdof_summary_start", "b200_sixdof_moments_download", "b200_sixdof_dwells_download",
+    "b200_sixdof_set_outcomes", "b200_sixdof_outcomes", "b200_sixdof_outcome_values", "b200_sixdof_outcome_stats",
+    "b200_sixdof_outcome_group_stats", "b200_sixdof_outcome_quantiles", "b200_sixdof_outcome_group_quantiles",
+    "b200_sixdof_outcome_covariance", "b200_sixdof_outcome_group_covariance", "b200_sixdof_outcome_histograms",
+    "b200_sixdof_outcome_group_histograms",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -92,6 +96,15 @@ MAX_CHANNELS = 8
 CHANNEL_NORM = 1
 CHANNEL_AXIS_ANGLE = 2
 ROW_PLANES = 25  # planes of a B200_TRAJ_FULL row; channel k is plane ROW_PLANES + k of an ensemble table
+# outcomes (b200_sixdof_set_outcomes): one f64 per world from a run summary, a device column or host values, reduced over
+# the worlds like a state of one entity
+MAX_OUTCOMES = 25
+OUTCOME_EXTREMA = 1
+OUTCOME_THRESHOLD = 2
+OUTCOME_MOMENT = 3
+OUTCOME_DWELL = 4
+OUTCOME_COLUMN = 5
+OUTCOME_VALUES = 6
 COMM_ID_BYTES = 128
 
 
@@ -187,6 +200,18 @@ class Channel(C.Structure):
         ("c", C.c_double * 3),
         ("d", C.c_double * 3),
         ("r0", C.c_double),
+    ]
+
+
+class Outcome(C.Structure):
+    _fields_ = [
+        ("kind", C.c_uint32),
+        ("field", C.c_uint32),
+        ("index", C.c_uint32),
+        ("reserved", C.c_uint32),
+        ("entity", C.c_uint64),
+        ("column", C.c_uint64),
+        ("values", C.POINTER(C.c_double)),
     ]
 
 
@@ -307,6 +332,18 @@ def lib():
     L.b200_sixdof_channels.restype = u32
     L.b200_sixdof_trajectory_channels.argtypes = [vp, vp, u64]
     L.b200_sixdof_state_channels.argtypes = [vp, vp, u64]
+    L.b200_sixdof_set_outcomes.argtypes = [vp, C.POINTER(Outcome), u32]
+    L.b200_sixdof_outcomes.argtypes = [vp]
+    L.b200_sixdof_outcomes.restype = u32
+    L.b200_sixdof_outcome_values.argtypes = [vp, vp, u64]
+    L.b200_sixdof_outcome_stats.argtypes = [vp, vp, u64]
+    L.b200_sixdof_outcome_group_stats.argtypes = [vp, vp, u64]
+    L.b200_sixdof_outcome_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_outcome_group_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_outcome_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_outcome_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_outcome_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_outcome_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

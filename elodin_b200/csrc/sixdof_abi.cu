@@ -733,9 +733,11 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->sum_thr) cudaFree(h->sum_thr);
     if (h->sum_mom) cudaFree(h->sum_mom);
     if (h->sum_dwell) cudaFree(h->sum_dwell);
-    for (const auto &t : h->tables)
-        for (void *p : {(void *)t.stats_dev, (void *)t.cov_dev, (void *)t.order_dev})
-            if (p) cudaFree(p);
+    if (h->out_planes) cudaFree(h->out_planes);
+    for (const auto *ts : {h->tables, h->out_tables})
+        for (int g = 0; g < 2; ++g)
+            for (void *p : {(void *)ts[g].stats_dev, (void *)ts[g].cov_dev, (void *)ts[g].order_dev})
+                if (p) cudaFree(p);
     for (auto &e : h->chunk_in) if (e) cudaEventDestroy(e);
     for (auto &e : h->chunk_out) if (e) cudaEventDestroy(e);
     if (h->host_pack) cudaFreeHost(h->host_pack);
@@ -1151,21 +1153,26 @@ static bool device_destination(const b200_sixdof *h, const void *dst)
 }
 
 static int refresh_channels(b200_sixdof *h, bool ring);
+static int write_outcomes(b200_sixdof *h);
 
-// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu, hist_kernels.cu) of the rows
-// of the ring (ring) or of the state into dst, `bytes` already checked.  When it reads a channel plane (`channels`), the
-// channel planes are recomputed first, on the handle's stream.  A device destination takes the table straight from the
-// kernel; any other gets it through the staging buffer, after the `scratch` bytes the reduction needs.
+// What a reduction over the world axis reads: the rows of the state or of the ring's samples (ensemble_rows), or the
+// outcome planes (b200_sixdof_set_outcomes), reduced as the state of a handle with one entity.
+enum class Rows { state, ring, outcomes };
+
+// A reduction over the world axis (stats_kernels.cu, quantile_kernels.cu, cov_kernels.cu, hist_kernels.cu) of `src` into
+// dst, `bytes` already checked.  When it reads a channel plane (`channels`), the channel planes are recomputed first, on
+// the handle's stream; the outcome planes are always rewritten first.  A device destination takes the table straight
+// from the kernel; any other gets it through the staging buffer, after the `scratch` bytes the reduction needs.
 // launch(out, scratch, &launches) enqueues the reduction on the handle's stream.
 extern "C++" {
 template <class Launch>
-static int run_world_reduction(b200_sixdof *h, bool ring, bool channels, uint64_t scratch, void *dst, uint64_t bytes,
+static int run_world_reduction(b200_sixdof *h, Rows src, bool channels, uint64_t scratch, void *dst, uint64_t bytes,
                                Launch launch)
 {
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (bytes == 0) return B200_OK;
     if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
-    int rc = channels ? refresh_channels(h, ring) : B200_OK;
+    int rc = src == Rows::outcomes ? write_outcomes(h) : channels ? refresh_channels(h, src == Rows::ring) : B200_OK;
     if (rc) return rc;
     const bool direct = device_destination(h, dst);
     scratch = (scratch + 7) / 8 * 8;
@@ -1330,18 +1337,34 @@ static int upload_group_table(b200_sixdof *h, const void *t, uint64_t bytes, voi
     return B200_OK;
 }
 
-// The tables of consecutive groups of sizes[0 .. n_groups), each with its device copy: the statistics' group table, the
-// quantiles' route order over it and the covariance's group table; the grouped entries' tables, else the all-worlds ones.
-static int build_group_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped)
+// The tables of consecutive groups of sizes[0 .. n_groups) of worlds of n_entities entities into t, each with its
+// device copy: the statistics' group table, the quantiles' route order over it and the covariance's group table.
+static int fill_group_tables(b200_sixdof *h, b200_sixdof::GroupTables &t, const uint64_t *sizes, uint32_t n_groups,
+                             uint64_t n_entities)
 {
-    b200_sixdof::GroupTables &t = h->tables[grouped];
-    t.stats = world_group_table(sizes, n_groups, h->desc.n_entities);
-    t.cov = cov_group_table(sizes, n_groups, h->desc.n_entities);
+    t.stats = world_group_table(sizes, n_groups, n_entities);
+    t.cov = cov_group_table(sizes, n_groups, n_entities);
     t.order = quantile_order(t.stats);
     int rc = upload_group_table(h, t.stats.data(), t.stats.size() * sizeof(WorldGroup), (void **)&t.stats_dev);
     if (!rc) rc = upload_group_table(h, t.cov.data(), t.cov.size() * sizeof(WorldGroup), (void **)&t.cov_dev);
     if (!rc) rc = upload_group_table(h, t.order.data(), t.order.size() * sizeof(uint32_t), (void **)&t.order_dev);
     return rc;
+}
+
+// The outcome entries' tables of one entity over the same worlds as h->tables[grouped], where n_entities != 1 (with one
+// entity they share `tables`).  Built only once outcomes are set (set_outcomes builds both), so that a handle without
+// outcomes allocates and uploads exactly what it did before outcomes existed.
+static int build_outcome_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped)
+{
+    if (h->desc.n_entities == 1 || h->outcomes.empty()) return B200_OK;
+    return fill_group_tables(h, h->out_tables[grouped], sizes, n_groups, 1);
+}
+
+// The grouped entries' tables, else the all-worlds ones, and the outcome entries' over the same worlds.
+static int build_group_tables(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups, bool grouped)
+{
+    const int rc = fill_group_tables(h, h->tables[grouped], sizes, n_groups, h->desc.n_entities);
+    return rc ? rc : build_outcome_tables(h, sizes, n_groups, grouped);
 }
 
 int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t n_groups)
@@ -1378,22 +1401,59 @@ static int no_groups(const char *what)
     return fail(B200_ERR_INVALID_ARGUMENT, "grouped %s: call b200_sixdof_set_world_groups first", what);
 }
 
-// Statistics of the planes over the worlds, per group when `grouped` (stats_kernels.cu), into dst: the groups checked,
-// then `bytes`, then the handle's status.
-static int run_world_stats(b200_sixdof *h, bool ring, bool grouped, void *dst, uint64_t bytes, const char *what)
+static int check_outcomes(const b200_sixdof *h);
+
+// The planes a reduction reads (Rows), their width (what a plane index is checked against) and its group tables.
+static StatsParams reduction_rows(const b200_sixdof *h, Rows src)
+{
+    if (src != Rows::outcomes) return ensemble_rows(h, src == Rows::ring);
+    const uint64_t P = h->outcomes.size();
+    StatsParams S{};
+    S.seg[0] = {h->out_planes, P, P * h->ld_o};
+    S.n_segs = 1;
+    S.planes_per_sample = (uint32_t)P;
+    S.n_planes = P;
+    S.ld = h->ld_o;
+    S.n_worlds = h->desc.n_worlds;
+    S.n_entities = 1;
+    return S;
+}
+
+static uint32_t reduction_width(const b200_sixdof *h, Rows src)
+{
+    return src == Rows::outcomes ? (uint32_t)h->outcomes.size() : row_width(h, src == Rows::ring);
+}
+
+static const b200_sixdof::GroupTables &reduction_tables(const b200_sixdof *h, Rows src, bool grouped)
+{
+    return src == Rows::outcomes && h->desc.n_entities != 1 ? h->out_tables[grouped] : h->tables[grouped];
+}
+
+// The checks every reduction makes first: a null handle, groups for a grouped one, and for the outcome entries an
+// outcome set that the summary in force still has.
+static int reduction_ready(const b200_sixdof *h, Rows src, bool grouped, const char *what)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     if (grouped && h->group_sizes.empty()) return no_groups(what);
+    return src == Rows::outcomes ? check_outcomes(h) : B200_OK;
+}
+
+// Statistics of the planes over the worlds, per group when `grouped` (stats_kernels.cu), into dst: the groups checked,
+// then `bytes`, then the handle's status.
+static int run_world_stats(b200_sixdof *h, Rows src, bool grouped, void *dst, uint64_t bytes, const char *what)
+{
+    int rc = reduction_ready(h, src, grouped, what);
+    if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
-    StatsParams S = ensemble_rows(h, ring);
+    StatsParams S = reduction_rows(h, src);
     const uint64_t G = grouped ? h->group_sizes.size() : 1;
     const uint64_t want = S.n_planes * G * S.n_entities * 5ull * 8ull;
     if (bytes != want)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s statistics are %llu bytes, got %llu", what, (unsigned long long)want,
                     (unsigned long long)bytes);
-    const b200_sixdof::GroupTables &t = h->tables[grouped];
+    const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped);
     const uint64_t scratch = bytes && h->status == B200_OK ? world_stats_scratch_doubles(S, t.stats) * 8ull : 0;
-    return run_world_reduction(h, ring, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
+    return run_world_reduction(h, src, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
         return launch_world_stats(S, t.stats_dev, t.stats, (double *)scr, n, h->stream);
     });
@@ -1401,41 +1461,41 @@ static int run_world_stats(b200_sixdof *h, bool ring, bool grouped, void *dst, u
 
 int b200_sixdof_trajectory_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, true, false, dst, bytes, "trajectory");
+    return run_world_stats(h, Rows::ring, false, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, false, false, dst, bytes, "state");
+    return run_world_stats(h, Rows::state, false, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, true, true, dst, bytes, "trajectory");
+    return run_world_stats(h, Rows::ring, true, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
 {
-    return run_world_stats(h, false, true, dst, bytes, "state");
+    return run_world_stats(h, Rows::state, true, dst, bytes, "state");
 }
 
 // Quantiles of the planes over the worlds, per group when `grouped` (quantile_kernels.cu), into dst: the groups checked,
 // then the handle's status, then the levels, then `bytes`.
-static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *q, uint32_t n_q, void *dst,
+static int run_quantiles(b200_sixdof *h, Rows src, bool grouped, const double *q, uint32_t n_q, void *dst,
                          uint64_t bytes, const char *what)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    if (grouped && h->group_sizes.empty()) return no_groups(what);
+    int rc = reduction_ready(h, src, grouped, what);
+    if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
     QuantileParams S{};
-    static_cast<StatsParams &>(S) = ensemble_rows(h, ring);
+    static_cast<StatsParams &>(S) = reduction_rows(h, src);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_q == 0 || n_q > B200_MAX_QUANTILES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u quantile levels: 1 to %u", n_q, B200_MAX_QUANTILES);
     if (!q) return fail(B200_ERR_INVALID_ARGUMENT, "null quantile levels");
     for (uint32_t l = 0; l < n_q; ++l)
         if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
-    const b200_sixdof::GroupTables &t = h->tables[grouped];
+    const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped);
     const uint64_t G = reduction_groups(h, grouped).size();
     const uint64_t want = S.n_planes * G * S.n_entities * n_q * 8ull;
     if (bytes != want)
@@ -1449,7 +1509,7 @@ static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *
     const uint64_t triples = S.n_planes * G * S.n_entities;
     h->quantile_read_sum = triples;  // the small-group routes read every triple once
     const uint64_t scratch = quantile_scratch_bytes(S, t.stats);
-    int rc = run_world_reduction(h, ring, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
+    rc = run_world_reduction(h, src, true, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
         S.out = out;
         return launch_quantiles(S, t.stats, t.order, scr, n, &h->quantile_read_sum, h->stream);
     });
@@ -1459,37 +1519,37 @@ static int run_quantiles(b200_sixdof *h, bool ring, bool grouped, const double *
 
 int b200_sixdof_trajectory_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, true, false, q, n_q, dst, bytes, "trajectory");
+    return run_quantiles(h, Rows::ring, false, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, false, false, q, n_q, dst, bytes, "state");
+    return run_quantiles(h, Rows::state, false, q, n_q, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, true, true, q, n_q, dst, bytes, "trajectory");
+    return run_quantiles(h, Rows::ring, true, q, n_q, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
 {
-    return run_quantiles(h, false, true, q, n_q, dst, bytes, "state");
+    return run_quantiles(h, Rows::state, true, q, n_q, dst, bytes, "state");
 }
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
 
 // Covariance of the selection `planes` (each < width) of every sample over the worlds, per group when `grouped`
 // (cov_kernels.cu), into dst: the groups checked, then the handle's status, then the selection, then `bytes`.
-static int run_covariance(b200_sixdof *h, bool ring, bool grouped, const uint32_t *planes, uint32_t n_p, void *dst,
+static int run_covariance(b200_sixdof *h, Rows src, bool grouped, const uint32_t *planes, uint32_t n_p, void *dst,
                           uint64_t bytes, const char *what)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    if (grouped && h->group_sizes.empty()) return no_groups(what);
+    int rc = reduction_ready(h, src, grouped, what);
+    if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
     CovParams S{};
-    static_cast<StatsParams &>(S) = ensemble_rows(h, ring);
-    const uint32_t width = row_width(h, ring);
+    static_cast<StatsParams &>(S) = reduction_rows(h, src);
+    const uint32_t width = reduction_width(h, src);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_p == 0 || n_p > B200_MAX_COV_PLANES)
         return fail(B200_ERR_INVALID_ARGUMENT, "%u covariance planes: 1 to %u", n_p, B200_MAX_COV_PLANES);
@@ -1511,8 +1571,8 @@ static int run_covariance(b200_sixdof *h, bool ring, bool grouped, const uint32_
                     (unsigned long long)bytes);
     S.n_p = n_p;
     for (uint32_t k = 0; k < n_p; ++k) S.planes[k] = planes[k];
-    const b200_sixdof::GroupTables &t = h->tables[grouped];
-    return run_world_reduction(h, ring, channel, cov_scratch_bytes(S, t.cov), dst, bytes, [&](double *out, void *scratch, int *n) {
+    const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped);
+    return run_world_reduction(h, src, channel, cov_scratch_bytes(S, t.cov), dst, bytes, [&](double *out, void *scratch, int *n) {
         S.out = out;
         return launch_covariance(S, t.cov_dev, t.cov, scratch, n, h->stream);
     });
@@ -1521,23 +1581,23 @@ static int run_covariance(b200_sixdof *h, bool ring, bool grouped, const uint32_
 // The ring's width (row_width), not its planes per sample: a handle without a ring refuses every plane.
 int b200_sixdof_trajectory_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, true, false, planes, n_p, dst, bytes, "trajectory");
+    return run_covariance(h, Rows::ring, false, planes, n_p, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, false, false, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, Rows::state, false, planes, n_p, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
                                             uint64_t bytes)
 {
-    return run_covariance(h, true, true, planes, n_p, dst, bytes, "trajectory");
+    return run_covariance(h, Rows::ring, true, planes, n_p, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
 {
-    return run_covariance(h, false, true, planes, n_p, dst, bytes, "state");
+    return run_covariance(h, Rows::state, true, planes, n_p, dst, bytes, "state");
 }
 
 // np.linspace(lo, hi, n + 1) into e[0 .. n]: i * step + lo, the product rounded before the sum (never an fma), e[n] = hi.
@@ -1561,15 +1621,15 @@ static int linspace_edges(double lo, double hi, uint32_t n, double *e)
 // Histograms of the specs over the worlds, per group when `grouped` (hist_kernels.cu), into dst: the groups checked,
 // then the handle's status, then the specs (each plane < width), then `bytes`.  The edges and the group table are
 // computed here and copied to the device ahead of the launch.
-static int run_histograms(b200_sixdof *h, bool ring, bool grouped, const b200_histogram *specs, uint32_t n_specs,
+static int run_histograms(b200_sixdof *h, Rows src, bool grouped, const b200_histogram *specs, uint32_t n_specs,
                           void *dst, uint64_t bytes, const char *what)
 {
-    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
-    if (grouped && h->group_sizes.empty()) return no_groups(what);
+    int rc = reduction_ready(h, src, grouped, what);
+    if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
     HistParams P{};
-    static_cast<StatsParams &>(P) = ensemble_rows(h, ring);
-    const uint32_t width = row_width(h, ring);
+    static_cast<StatsParams &>(P) = reduction_rows(h, src);
+    const uint32_t width = reduction_width(h, src);
     bool channel = false;
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_specs == 0 || n_specs > B200_MAX_HISTOGRAMS)
@@ -1630,7 +1690,7 @@ static int run_histograms(b200_sixdof *h, bool ring, bool grouped, const b200_hi
     const uint64_t edge_bytes = edges.size() * 8ull, table_bytes = table.size() * sizeof(WorldGroup);
     edges.resize(edges.size() + table_bytes / 8);  // one copy to the device: the edges, then the group table
     std::memcpy(edges.data() + edge_bytes / 8, table.data(), table_bytes);
-    return run_world_reduction(h, ring, channel, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
+    return run_world_reduction(h, src, channel, edge_bytes + table_bytes, dst, bytes, [&](double *out, void *scratch, int *n) {
         cudaError_t e = cudaMemcpyAsync(scratch, edges.data(), edge_bytes + table_bytes, cudaMemcpyHostToDevice, h->stream);
         if (e != cudaSuccess) return e;
         P.out = out;
@@ -1642,24 +1702,24 @@ static int run_histograms(b200_sixdof *h, bool ring, bool grouped, const b200_hi
 int b200_sixdof_trajectory_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                       uint64_t bytes)
 {
-    return run_histograms(h, true, false, specs, n_specs, dst, bytes, "trajectory");
+    return run_histograms(h, Rows::ring, false, specs, n_specs, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst, uint64_t bytes)
 {
-    return run_histograms(h, false, false, specs, n_specs, dst, bytes, "state");
+    return run_histograms(h, Rows::state, false, specs, n_specs, dst, bytes, "state");
 }
 
 int b200_sixdof_trajectory_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                             uint64_t bytes)
 {
-    return run_histograms(h, true, true, specs, n_specs, dst, bytes, "trajectory");
+    return run_histograms(h, Rows::ring, true, specs, n_specs, dst, bytes, "trajectory");
 }
 
 int b200_sixdof_state_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                        uint64_t bytes)
 {
-    return run_histograms(h, false, true, specs, n_specs, dst, bytes, "state");
+    return run_histograms(h, Rows::state, true, specs, n_specs, dst, bytes, "state");
 }
 
 // Host-only, like b200_stats_merge: parts folded left to right with the kernels' cov_merge, entry by entry.
@@ -2099,6 +2159,226 @@ int b200_sixdof_trajectory_channels(b200_sixdof *h, void *dst, uint64_t bytes)
 int b200_sixdof_state_channels(b200_sixdof *h, void *dst, uint64_t bytes)
 {
     return download_channels(h, false, dst, bytes, "state");
+}
+
+// ---- outcomes (outcome_kernels.cu)
+
+// outcome k of the set: 0 when it names a record the handle has now (the summary in force, a device column), else the
+// refusal.  Every outcome entry repeats it: a later summary_start may have dropped what an outcome names.
+static int check_outcome(const b200_sixdof *h, const b200_outcome &o, uint32_t k)
+{
+    const uint64_t E = h->desc.n_entities;
+    if (o.reserved != 0) return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: reserved field is not 0", k);
+    const bool per_entity = o.kind == B200_OUTCOME_EXTREMA || o.kind == B200_OUTCOME_MOMENT || o.kind == B200_OUTCOME_COLUMN;
+    if (per_entity ? o.entity >= E : o.entity != 0)
+        return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: entity row %llu, %s", k, (unsigned long long)o.entity,
+                    per_entity ? "beyond the world's entities" : "its kind takes none (0)");
+    if (o.kind != B200_OUTCOME_COLUMN && o.column != 0)
+        return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: column 0x%016llx, its kind takes none (0)", k,
+                    (unsigned long long)o.column);
+    auto bad_field = [&](uint32_t n) {
+        return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: field %u, kind %u has fields 0 to %u", k, o.field, o.kind, n - 1);
+    };
+    auto past = [&](const char *what, size_t have) {
+        return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: %s %u, the summary in force has %zu", k, what, o.index, have);
+    };
+    switch (o.kind) {
+    case B200_OUTCOME_EXTREMA:
+        if (o.field >= B200_EXTREMA_FIELDS) return bad_field(B200_EXTREMA_FIELDS);
+        if (!h->sum_begun || !h->sum_extrema)
+            return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: the summary in force has no extrema", k);
+        if (o.index >= row_width(h, false))
+            return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: extrema plane %u, a row has %u", k, o.index, row_width(h, false));
+        return B200_OK;
+    case B200_OUTCOME_THRESHOLD:
+        if (o.field > 25) return bad_field(26);
+        if (o.index >= (h->sum_begun ? h->sum_thr_list.size() : 0)) return past("threshold", h->sum_begun ? h->sum_thr_list.size() : 0);
+        return B200_OK;
+    case B200_OUTCOME_MOMENT:
+        if (o.field >= 4) return bad_field(4);
+        if (o.index >= (h->sum_begun ? h->sum_mom_planes.size() : 0)) return past("moment slot", h->sum_begun ? h->sum_mom_planes.size() : 0);
+        return B200_OK;
+    case B200_OUTCOME_DWELL:
+        if (o.field >= B200_DWELL_FIELDS) return bad_field(B200_DWELL_FIELDS);
+        if (o.index >= (h->sum_begun ? h->sum_dwell_list.size() : 0)) return past("dwell", h->sum_begun ? h->sum_dwell_list.size() : 0);
+        return B200_OK;
+    case B200_OUTCOME_COLUMN: {
+        if (o.index != 0) return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: index %u, a column outcome takes 0", k, o.index);
+        const Column *c = h->find(o.column);
+        if (!c) return fail(B200_ERR_COMPONENT_NOT_FOUND, "outcome %u: component 0x%016llx not found", k, (unsigned long long)o.column);
+        if (c->global)
+            return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: column 0x%016llx is global, not per body", k, (unsigned long long)o.column);
+        if (o.field >= c->width)
+            return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: plane %u, the column has %u", k, o.field, c->width);
+        return B200_OK;
+    }
+    case B200_OUTCOME_VALUES:
+        if (o.field != 0) return bad_field(1);
+        if (o.index != 0) return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: index %u, a values outcome takes 0", k, o.index);
+        return B200_OK;
+    default:
+        return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: unknown kind %u", k, o.kind);
+    }
+}
+
+static int check_outcomes(const b200_sixdof *h)
+{
+    if (h->outcomes.empty()) return fail(B200_ERR_INVALID_ARGUMENT, "no outcomes: call b200_sixdof_set_outcomes first");
+    for (uint32_t k = 0; k < h->outcomes.size(); ++k) {
+        const int rc = check_outcome(h, h->outcomes[k], k);
+        if (rc) return rc;
+    }
+    return B200_OK;
+}
+
+// The outcome pass of the set in force (checked by check_outcomes): each outcome resolved to its record, the pointers
+// taken from the handle now (summary_start may have moved the accumulators).
+static OutcomeParams outcome_params(const b200_sixdof *h)
+{
+    OutcomeParams P{};
+    const uint64_t E = h->desc.n_entities, ld = h->ld;
+    for (uint32_t k = 0; k < h->outcomes.size(); ++k) {
+        const b200_outcome &o = h->outcomes[k];
+        OutcomeParams::Src s{nullptr, E, kOutCopy, k};
+        switch (o.kind) {
+        case B200_OUTCOME_EXTREMA:  // SoA: plane p * 5 + f of ld, body w * E + e
+            s.src = h->sum_ext + ((uint64_t)o.index * B200_EXTREMA_FIELDS + o.field) * ld + o.entity;
+            s.op = o.field >= 2 ? kOutTick : kOutCopy;
+            break;
+        case B200_OUTCOME_THRESHOLD:  // [w][n_thr][26]
+            s.src = h->sum_thr + (uint64_t)o.index * 26 + o.field;
+            s.stride = h->sum_thr_list.size() * 26;
+            s.op = o.field == 0 ? kOutTick : kOutCopy;
+            break;
+        case B200_OUTCOME_MOMENT:  // SoA: (n, K, S1, S2) at plane j * 4 + f of ld
+            s.src = h->sum_mom + (uint64_t)o.index * 4 * ld + o.entity;
+            s.op = kOutCount + o.field;
+            break;
+        case B200_OUTCOME_DWELL:  // [w][n_dwell][3]
+            s.src = h->sum_dwell + (uint64_t)o.index * B200_DWELL_FIELDS + o.field;
+            s.stride = h->sum_dwell_list.size() * B200_DWELL_FIELDS;
+            s.op = o.field == 0 ? kOutCopy : kOutTick;
+            break;
+        case B200_OUTCOME_COLUMN:
+            s.src = h->find(o.column)->dev + (uint64_t)o.field * ld + o.entity;
+            break;
+        default:  // VALUES: written by set_outcomes
+            continue;
+        }
+        P.o[P.n_src++] = s;
+    }
+    P.out = h->out_planes;
+    P.ld_o = h->ld_o;
+    P.ld = ld;
+    P.n_worlds = h->desc.n_worlds;
+    return P;
+}
+
+// The outcome planes of every source, written on the handle's stream (one launch; none with only VALUES outcomes).
+// Never cached: the summaries fold, and b200_sixdof_device_plane hands out writable columns.
+static int write_outcomes(b200_sixdof *h)
+{
+    int launches = 0;
+    CU(h, launch_outcomes(outcome_params(h), &launches, h->stream));
+    h->timings.kernel_launches += (uint64_t)launches;
+    return B200_OK;
+}
+
+int b200_sixdof_set_outcomes(b200_sixdof *h, const b200_outcome *o, uint32_t n)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (n > B200_MAX_OUTCOMES) return fail(B200_ERR_INVALID_ARGUMENT, "%u outcomes: at most %u", n, B200_MAX_OUTCOMES);
+    if (n && !o) return fail(B200_ERR_INVALID_ARGUMENT, "null outcomes");
+    for (uint32_t k = 0; k < n; ++k) {
+        const int rc = check_outcome(h, o[k], k);
+        if (rc) return rc;
+        if ((o[k].kind == B200_OUTCOME_VALUES) != (o[k].values != nullptr))
+            return fail(B200_ERR_INVALID_ARGUMENT, "outcome %u: %s", k,
+                        o[k].values ? "values given, its kind takes none (NULL)" : "null values");
+    }
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaStreamSynchronize(h->stream));  // no reduction in flight still reads the planes replaced here
+    const uint64_t ld_o = round_up(std::max<uint64_t>(h->desc.n_worlds, 1), 128);
+    double *planes = nullptr;
+    if (n) {
+        cudaError_t e = cudaMalloc(&planes, (uint64_t)n * ld_o * 8ull);
+        if (e != cudaSuccess) return cuda_fail(h, e, "cudaMalloc(outcome planes)");
+        for (uint32_t k = 0; k < n && e == cudaSuccess; ++k)
+            if (o[k].kind == B200_OUTCOME_VALUES)
+                e = cudaMemcpy(planes + k * ld_o, o[k].values, h->desc.n_worlds * 8ull, cudaMemcpyDefault);
+        if (e != cudaSuccess) {
+            cudaFree(planes);
+            return cuda_fail(h, e, "cudaMemcpy(outcome values)");
+        }
+    }
+    if (h->out_planes) CU(h, cudaFree(h->out_planes));
+    h->out_planes = planes;
+    h->ld_o = ld_o;
+    h->outcomes.assign(o, o + n);
+    for (auto &x : h->outcomes) x.values = nullptr;
+    int rc = build_outcome_tables(h, &h->desc.n_worlds, 1, false);
+    if (!rc) rc = build_outcome_tables(h, h->group_sizes.data(), (uint32_t)h->group_sizes.size(), true);
+    return rc;
+}
+
+uint32_t b200_sixdof_outcomes(const b200_sixdof *h) { return h ? (uint32_t)h->outcomes.size() : 0; }
+
+// [n_worlds][P]: the outcome planes written, then turned into world-major rows (the layout kernel of the columns)
+int b200_sixdof_outcome_values(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    int rc = reduction_ready(h, Rows::outcomes, false, "outcome");
+    if (rc) return rc;
+    CU(h, cudaSetDevice(h->device));
+    const uint64_t P = h->outcomes.size(), want = h->desc.n_worlds * P * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome values are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    return run_world_reduction(h, Rows::outcomes, false, 0, dst, bytes, [&](double *out, void *, int *n) {
+        *n = 1;
+        return launch_soa_to_aos(h->out_planes, out, h->desc.n_worlds, (uint32_t)P, h->ld_o, h->stream);
+    });
+}
+
+int b200_sixdof_outcome_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return run_world_stats(h, Rows::outcomes, false, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    return run_world_stats(h, Rows::outcomes, true, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    return run_quantiles(h, Rows::outcomes, false, q, n_q, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes)
+{
+    return run_quantiles(h, Rows::outcomes, true, q, n_q, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_covariance(h, Rows::outcomes, false, planes, n_p, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_covariance(h, Rows::outcomes, true, planes, n_p, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                   uint64_t bytes)
+{
+    return run_histograms(h, Rows::outcomes, false, specs, n_specs, dst, bytes, "outcome");
+}
+
+int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                         uint64_t bytes)
+{
+    return run_histograms(h, Rows::outcomes, true, specs, n_specs, dst, bytes, "outcome");
 }
 
 int b200_sixdof_trajectory_reset(b200_sixdof *h)

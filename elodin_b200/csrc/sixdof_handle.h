@@ -80,6 +80,14 @@ struct b200_sixdof {
     // [n_c][ld] for the state, recomputed by every entry that reads them (channel_kernels.cu)
     std::vector<b200_channel> channels;
     double *chan_ring = nullptr, *chan_state = nullptr;
+    // outcomes (b200_sixdof_set_outcomes): the set (values pointers cleared) and its planes, P of ld_o f64 (VALUES planes
+    // written once by set_outcomes, the others by every outcome entry, outcome_kernels.cu); with n_entities != 1 the
+    // outcome entries reduce over group tables of one entity of their own, indexed like `tables` and built only once
+    // outcomes are set
+    std::vector<b200_outcome> outcomes;
+    double *out_planes = nullptr;
+    uint64_t ld_o = 0;
+    GroupTables out_tables[2];
     // run summaries (b200_sixdof_summary_*): device accumulators, allocated on first use, kept across begins
     bool sum_begun = false;
     bool sum_ever = false;           // summary_begin has been called: the channel set (the row width) is fixed

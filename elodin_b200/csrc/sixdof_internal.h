@@ -1,6 +1,7 @@
 // Host<->kernel parameter blocks of libb200_sixdof (internal; the public surface
 // is include/b200_sixdof.h).
 #pragma once
+#include <cfloat>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include <vector>
@@ -375,6 +376,22 @@ cudaError_t launch_summary_fold(const SummaryParams &S, int *launches, cudaStrea
 // extrema accumulators of rows of R planes, bodies [b0, b0 + nb) -> out[nb][5 R] (the public table's rows)
 cudaError_t launch_extrema_table(const double *ext, uint64_t ld, uint32_t R, uint64_t b0, uint64_t nb, double *out,
                                  cudaStream_t s);
+// Field f (0 = n, 1 = mean, 2 = m2) of the moment record of the accumulator at a (n, K, S1, S2 at a[0], a[ld],
+// a[2 ld], a[3 ld]): mean = K + S1 / n, m2 = S2 - S1 * (S1 / n) clamped at 0, +inf where S2 overflowed, NaN mean and m2
+// while n = 0; each operation correctly rounded in both math modes, so that the host can restate it bit for bit.  The
+// public moment table (moment_table_kernel) and the moment outcomes (outcome_kernel) both take their values from here.
+__device__ __forceinline__ double moment_field(const double *a, uint64_t ld, uint32_t f)
+{
+    const double n = a[0];
+    if (f != 0 && n == 0.0) return __longlong_as_double(0x7ff8000000000000ll);
+    if (f == 1) return __dadd_rn(a[ld], __ddiv_rn(a[2 * ld], n));
+    if (f == 2) {
+        const double S1 = a[2 * ld], S2 = a[3 * ld];
+        const double d = __dsub_rn(S2, __dmul_rn(S1, __ddiv_rn(S1, n)));
+        return S2 > DBL_MAX ? S2 : d < 0.0 ? 0.0 : d;
+    }
+    return n;
+}
 // moment accumulators of k selected planes, bodies [b0, b0 + nb) -> out[nb][k][3] (n, mean, m2: the public table's rows)
 cudaError_t launch_moment_table(const double *mom, uint64_t ld, uint32_t k, uint64_t b0, uint64_t nb, double *out,
                                 cudaStream_t s);
@@ -393,5 +410,28 @@ struct ChannelParams {
 };
 // one launch on s (*launches = 1; 0 without samples, bodies or channels)
 cudaError_t launch_channels(const ChannelParams &P, int *launches, cudaStream_t s);
+
+// Outcome values (outcome_kernels.cu, include/b200_sixdof.h b200_outcome): source k gives world w < n_worlds the value
+// out[plane * ld_o + w], read at src + w * stride (sixdof_abi.cu:outcome_params resolves every outcome to its record):
+//   kCopy  the f64 at src, its bits;   kTick  the f64 at src, NaN where it is -1;
+//   kCount, kMean, kStd, kRms  of the moment accumulator at src (planes of ld, moment_field).
+// VALUES outcomes have no source: set_outcomes wrote their planes once.
+enum : uint32_t { kOutCopy = 0, kOutTick = 1, kOutCount = 2, kOutMean = 3, kOutStd = 4, kOutRms = 5 };
+struct OutcomeParams {
+    struct Src {
+        const double *src;
+        uint64_t stride;
+        uint32_t op;
+        uint32_t plane;
+    } o[B200_MAX_OUTCOMES];
+    uint32_t n_src;
+    uint32_t pad;
+    double *out;
+    uint64_t ld_o;   // f64 per outcome plane
+    uint64_t ld;     // f64 per moment accumulator plane
+    uint64_t n_worlds;
+};
+// one launch on s (*launches = 1; 0 without sources or worlds)
+cudaError_t launch_outcomes(const OutcomeParams &P, int *launches, cudaStream_t s);
 
 } // namespace b200

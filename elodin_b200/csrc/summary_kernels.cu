@@ -190,28 +190,13 @@ __global__ void __launch_bounds__(kSumThreads) scores_clear_kernel(double *mom, 
     }
 }
 
-// (n, mean = K + S1 / n, m2 = S2 - S1 * (S1 / n) clamped at 0, +inf where S2 overflowed; NaN mean and m2 while n = 0),
-// each operation correctly rounded in both math modes so that the host can restate it bit for bit
+// the public table's (n, mean, m2) records (moment_field)
 __global__ void __launch_bounds__(kSumThreads) moment_table_kernel(const double *__restrict__ mom, uint64_t ld, uint32_t k,
                                                                    uint64_t b0, uint64_t nb, double *__restrict__ out)
 {
     const uint64_t F = 3ull * k;
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nb * F; i += (uint64_t)gridDim.x * blockDim.x) {
-        const uint64_t f = i % 3;
-        const double *a = mom + (i % F) / 3 * 4 * ld + b0 + i / F;
-        const double n = a[0];
-        double v = n;
-        if (f != 0 && n == 0.0) {
-            v = nan_value();
-        } else if (f == 1) {
-            v = __dadd_rn(a[ld], __ddiv_rn(a[2 * ld], n));
-        } else if (f == 2) {
-            const double S1 = a[2 * ld], S2 = a[3 * ld];
-            const double d = __dsub_rn(S2, __dmul_rn(S1, __ddiv_rn(S1, n)));
-            v = S2 > DBL_MAX ? S2 : d < 0.0 ? 0.0 : d;
-        }
-        out[i] = v;
-    }
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < nb * F; i += (uint64_t)gridDim.x * blockDim.x)
+        out[i] = moment_field(mom + (i % F) / 3 * 4 * ld + b0 + i / F, ld, (uint32_t)(i % 3));
 }
 
 __global__ void __launch_bounds__(kSumThreads) extrema_table_kernel(const double *__restrict__ ext, uint64_t ld, uint32_t R,

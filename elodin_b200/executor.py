@@ -270,11 +270,13 @@ class B200Exec:
                                      nbytes)
 
     # ---- ensemble statistics (reductions over the world axis, on the device) ------------------------------------
-    def _reduce(self, kind: str, ring: bool, args: tuple, shape, out_ptr: Optional[int] = None,
+    def _reduce(self, kind: str, ring, args: tuple, shape, out_ptr: Optional[int] = None,
                 nbytes: Optional[int] = None) -> Optional[np.ndarray]:
-        """b200_sixdof_{trajectory|state}_{kind}(h, *args, dst, bytes): into `out_ptr` (`nbytes`, by default those of
-        `shape`), returning nothing, or into a new [shape] f64 array, returned."""
-        fn = getattr(self._L, f"b200_sixdof_{'trajectory' if ring else 'state'}_{kind}")
+        """b200_sixdof_{trajectory|state}_{kind}(h, *args, dst, bytes) (`ring` True | False; "outcome" for
+        b200_sixdof_outcome_{kind}): into `out_ptr` (`nbytes`, by default those of `shape`), returning nothing, or into
+        a new [shape] f64 array, returned."""
+        source = ring if isinstance(ring, str) else "trajectory" if ring else "state"
+        fn = getattr(self._L, f"b200_sixdof_{source}_{kind}")
         out = None if out_ptr is not None else np.empty(shape)
         ptr = out_ptr if out is None else out.ctypes.data
         _lib.check(fn(self._h, *args, C.c_void_p(ptr), int(np.prod(shape)) * 8 if nbytes is None else nbytes))
@@ -457,6 +459,75 @@ class B200Exec:
     def state_channels(self) -> np.ndarray:
         """The channels of the current state: [n_worlds, n_entities, n_c]."""
         return self._reduce("channels", False, (), (self.n_worlds, self.n_entities, self.n_channels))
+
+    # ---- outcomes (one value per world, from the run summaries, a column or host values, reduced over the worlds)
+    def set_outcomes(self, outcomes: Sequence) -> None:
+        """Replace the outcome set with `outcomes` (at most MAX_OUTCOMES _lib.Outcome records, or tuples (kind, field,
+        index, entity, column, values) with the trailing items optional: column a component name or id, values
+        n_worlds f64 for OUTCOME_VALUES); an empty set clears it.  Outcomes name summaries of the summary in force:
+        call it after summary_begin."""
+        outs = list(outcomes)
+        arr = (_lib.Outcome * max(len(outs), 1))()
+        keep = []  # the values arrays, alive for the call (the library copies them)
+        for k, o in enumerate(outs):
+            if isinstance(o, _lib.Outcome):
+                arr[k] = o
+                continue
+            kind, field, index, entity, column, values = tuple(o) + (0, 0, 0, None)[len(o) - 2:]
+            r = arr[k]
+            r.kind, r.field, r.index, r.entity = int(kind), int(field), int(index), int(entity)
+            r.column = _cid(column) if column else 0
+            if values is not None:
+                keep.append(np.ascontiguousarray(np.asarray(values, dtype=np.float64).ravel()))
+                r.values = keep[-1].ctypes.data_as(C.POINTER(C.c_double))
+        _lib.check(self._L.b200_sixdof_set_outcomes(self._h, arr, len(outs)))
+
+    @property
+    def n_outcomes(self) -> int:
+        """The number of outcomes set, 0 = none."""
+        return int(self._L.b200_sixdof_outcomes(self._h))
+
+    def outcome_values(self) -> np.ndarray:
+        """[n_worlds, P]: every outcome's value of every world, written on the device now (-1 ticks as NaN)."""
+        return self._reduce("values", "outcome", (), (self.n_worlds, self.n_outcomes))
+
+    def outcome_stats(self) -> np.ndarray:
+        """[P, 5]: state_stats()'s fields of every outcome over the worlds."""
+        return self._reduce("stats", "outcome", (), (self.n_outcomes, _lib.STATS_FIELDS))
+
+    def outcome_group_stats(self) -> np.ndarray:
+        """[G, P, 5]: outcome_stats() per group of set_world_groups."""
+        return self._reduce("group_stats", "outcome", (), (self.world_groups, self.n_outcomes, _lib.STATS_FIELDS))
+
+    def outcome_quantiles(self, q) -> np.ndarray:
+        """[P, n_q]: state_quantiles()'s levels of every outcome over the worlds whose value is finite."""
+        lv = self._levels(q)
+        return self._reduce("quantiles", "outcome", lv, (self.n_outcomes, lv[1]))
+
+    def outcome_group_quantiles(self, q) -> np.ndarray:
+        """[G, P, n_q]: outcome_quantiles(q) per group."""
+        lv = self._levels(q)
+        return self._reduce("group_quantiles", "outcome", lv, (self.world_groups, self.n_outcomes, lv[1]))
+
+    def outcome_covariance(self, planes) -> np.ndarray:
+        """[1 + p + p*p]: the covariance record of the outcomes `planes` (indices below P), as state_covariance()."""
+        sel = self._selection(planes)
+        return self._reduce("covariance", "outcome", sel, (1 + sel[1] + sel[1] ** 2,))
+
+    def outcome_group_covariance(self, planes) -> np.ndarray:
+        """[G, 1 + p + p*p]: outcome_covariance(planes) per group."""
+        sel = self._selection(planes)
+        return self._reduce("group_covariance", "outcome", sel, (self.world_groups, 1 + sel[1] + sel[1] ** 2))
+
+    def outcome_histograms(self, specs) -> np.ndarray:
+        """[sum of the record lengths]: state_histograms(specs) of the outcomes (entity row 0, planes below P)."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("histograms", "outcome", args, (row,))
+
+    def outcome_group_histograms(self, specs) -> np.ndarray:
+        """[G, sum of the record lengths]: outcome_histograms(specs) per group."""
+        args, row = self._hist_specs(specs)
+        return self._reduce("group_histograms", "outcome", args, (self.world_groups, row))
 
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     @staticmethod

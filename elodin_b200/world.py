@@ -441,7 +441,7 @@ class World:
               covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
               groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
               channels: Optional[Sequence["Channel"]] = None, moments: Optional[Sequence] = None,
-              dwells: Optional[Sequence["Threshold"]] = None) -> "Exec":
+              dwells: Optional[Sequence["Threshold"]] = None, outcomes: Optional[Sequence["Outcome"]] = None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -468,7 +468,12 @@ class World:
         cover like the sampled components.  `moments` (a selection in the syntax of `covariance`, channels as
         "channels") also keeps every world's run count, mean, spread and RMS of those components over its telemetry
         rows (`Exec.moments`), and `dwells` (up to 8 `Threshold`s) every world's count of rows beyond each bound with
-        the first and last such tick (`Exec.dwell`), both folded on the device with the extrema."""
+        the first and last such tick (`Exec.dwell`), both folded on the device with the extrema.  `outcomes` (1 to 25
+        `Outcome`s with distinct names) takes one value per world from those run summaries, a device column (a dispersed
+        input or the final state) or host values, and reduces it over the worlds on the device when asked
+        (`Exec.outcome_stats`, `outcome_quantiles`, `outcome_covariance`, `outcome_histogram`, each per group with
+        `groups=True`): apogee percentiles per sweep point, an impact ellipse, an event probability, input-to-outcome
+        correlations, without a per-world table reaching the host."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -477,7 +482,7 @@ class World:
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
                     ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain,
-                    channels, moments, dwells)
+                    channels, moments, dwells, outcomes)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -829,7 +834,13 @@ class Histogram:
         if two and len(index) != 2:
             raise ValueError(f"{where}: one index (1D) or a pair of indices (2D)")
         idx = tuple(index) if two else (index,)
-        self.planes = tuple(_sampled_plane(span, i, where) for i in idx)  # in the 25-plane row layout
+        self._axes(where, tuple(_sampled_plane(span, i, where) for i in idx), range, bins)  # 25-plane row layout
+        self.pair, self.index = pair, tuple(int(i) for i in idx) if two else int(index)
+
+    def _axes(self, where: str, planes: tuple, range, bins) -> None:
+        """The planes (one or two), bins, ranges, edges and record length, checked; refusals prefixed by `where`."""
+        two, idx = len(planes) == 2, planes
+        self.planes = planes
         if two and self.planes[0] == self.planes[1]:
             raise ValueError(f"{where}: the same component on both axes")
         bins_t = tuple(bins) if isinstance(bins, (tuple, list)) else (bins,) * len(idx)
@@ -857,7 +868,6 @@ class Histogram:
             self.range.append((lo, hi))
             self._edges.append(e)
         self.range = tuple(self.range)
-        self.pair, self.index = pair, tuple(int(i) for i in idx) if two else int(index)
         self.record_len = (2 if two else 3) + cells  # f64 of its record in a row of the table
 
     @property
@@ -875,6 +885,131 @@ class Histogram:
         r = self.range[0] if len(self.range) == 1 else self.range
         b = self.bins[0] if len(self.bins) == 1 else self.bins
         return f"Histogram({self.pair!r}, {self.index!r}, range={r!r}, bins={b!r})"
+
+
+def _histogram_record(h: Histogram, t: np.ndarray) -> Dict[str, object]:
+    """The records of histogram `h` ([..., record_len] f64) -> Exec.histogram's dict of int64 counts and edges."""
+    t = t.astype(np.int64)
+    if len(h.bins) == 1:
+        return {"counts": np.ascontiguousarray(t[..., 3:]), "nonfinite": t[..., 0].copy(), "below": t[..., 1].copy(),
+                "above": t[..., 2].copy(), "edges": h.edges}
+    return {"counts": np.ascontiguousarray(t[..., 2:]).reshape(*t.shape[:-1], *h.bins), "nonfinite": t[..., 0].copy(),
+            "outside": t[..., 1].copy(), "edges": h.edges}
+
+
+_EXTREMA_FIELDS = ("min", "max", "min_tick", "max_tick", "first_nonfinite_tick")
+_MOMENT_FIELDS = ("count", "mean", "std", "rms")
+_DWELL_FIELDS = ("rows", "first_tick", "last_tick")
+# the Body columns on the device besides the effector inputs: what a column outcome may read
+_BODY_COLUMNS = ("world_pos", "world_vel", "world_accel", "force", "inertia")
+
+
+class Outcome:
+    """One value per world for `World.build(..., ensemble=True, outcomes=[...])`, reduced over the worlds on the device
+    by `Exec.outcome_stats`, `outcome_quantiles`, `outcome_covariance` and `outcome_histogram`:
+
+    - `Outcome(name, "rocket.world_pos", 6, "max")`: a field of the extrema of component 6 (min, max, min_tick,
+      max_tick, first_nonfinite_tick; needs extrema=True); `Outcome(name, "rocket.channels", 1, "rms")`: a field of the
+      run moments of a component (count, mean, std, rms; needs moments= to select it).
+    - `Outcome(name, "rocket.inertia", 6)`, with no field: the current device value of component 6 of a Body column --
+      a dispersed input (inertia 6 = mass, an effector's input column) or, after a run, the final state.
+    - `Outcome.threshold(name, i, "tick")` / `Outcome.threshold(name, i, "world_pos", 4)`: threshold i's record;
+      `Outcome.dwell(name, i, "last_tick")`: dwell i's record.
+    - `Outcome.values(name, array)`: [n_worlds] values from the host, e.g. a plan parameter no device column holds.
+      In a world-sharded campaign each rank passes its own slice (`sharding.shard_worlds`).
+
+    A tick that never happened (-1) is NaN, so the reductions leave those worlds out: the count of a threshold's tick
+    is the number of worlds where it fired."""
+
+    def __init__(self, name: str, pair: str, index, field: Optional[str] = None):
+        where = f"Outcome({name!r}, {pair!r}, {index!r}{'' if field is None else f', {field!r}'})"
+        self._name(name, where)
+        self.name = name
+        ent, _, comp = pair.rpartition(".") if isinstance(pair, str) else ("", "", "")
+        if field is None:  # a device column: the width is known once the world is (World.build)
+            if not ent or not comp:
+                raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND, f"component not found: {pair!r}")
+            if isinstance(index, (bool, np.bool_)) or not isinstance(index, (int, np.integer)) or index < 0:
+                raise ValueError(f"{where}: index {index!r} is not a non-negative integer")
+            self.kind, self.entity, self.component, self.index, self.field = _lib.OUTCOME_COLUMN, ent, comp, int(index), 0
+            return
+        self.entity, span = _sampled_span(pair, "outcomes")
+        self.plane = _sampled_plane(span, index, where)  # of the ensemble row: 25 planes, then the channels
+        if field in _EXTREMA_FIELDS:
+            self.kind, self.field = _lib.OUTCOME_EXTREMA, _EXTREMA_FIELDS.index(field)
+        elif field in _MOMENT_FIELDS:
+            self.kind, self.field = _lib.OUTCOME_MOMENT, _MOMENT_FIELDS.index(field)
+        else:
+            raise ValueError(f"{where}: field {field!r} is none of {', '.join(_EXTREMA_FIELDS + _MOMENT_FIELDS)}")
+        self.pair, self.index = pair, int(index)
+
+    @staticmethod
+    def _name(name, where: str) -> None:
+        if not isinstance(name, str) or not name:
+            raise ValueError(f"{where}: the name must be a non-empty string")
+
+    @classmethod
+    def _record_of(cls, kind: int, name: str, i, field: int, where: str) -> "Outcome":
+        cls._name(name, where)
+        if isinstance(i, (bool, np.bool_)) or not isinstance(i, (int, np.integer)) or i < 0:
+            raise ValueError(f"{where}: index {i!r} is not a non-negative integer")
+        o = cls.__new__(cls)
+        o.name, o.kind, o.index, o.field = name, kind, int(i), field
+        return o
+
+    @classmethod
+    def threshold(cls, name: str, i: int, component: str, index=None) -> "Outcome":
+        """Threshold i's record of each world: "tick" (NaN where it never fired), or component `index` of the entity's
+        state at that row (world_pos, world_vel, world_accel or force)."""
+        where = f"Outcome.threshold({name!r}, {i!r}, {component!r}{'' if index is None else f', {index!r}'})"
+        if component == "tick" and index is None:
+            field = 0
+        elif component in _SAMPLED and index is not None:
+            field = 1 + _sampled_plane(_SAMPLED[component], index, where)
+        else:
+            raise ValueError(f"{where}: \"tick\", or one of {', '.join(_SAMPLED)} with an index")
+        return cls._record_of(_lib.OUTCOME_THRESHOLD, name, i, field, where)
+
+    @classmethod
+    def dwell(cls, name: str, i: int, field: str) -> "Outcome":
+        """Dwell i's record of each world: "rows", "first_tick" or "last_tick" (ticks NaN where no row counted)."""
+        where = f"Outcome.dwell({name!r}, {i!r}, {field!r})"
+        if field not in _DWELL_FIELDS:
+            raise ValueError(f"{where}: field {field!r} is none of {', '.join(_DWELL_FIELDS)}")
+        return cls._record_of(_lib.OUTCOME_DWELL, name, i, _DWELL_FIELDS.index(field), where)
+
+    @classmethod
+    def values(cls, name: str, values) -> "Outcome":
+        """`values` [n_worlds] f64 from the host, copied to the device once when the Exec is built."""
+        where = f"Outcome.values({name!r})"
+        cls._name(name, where)
+        v = np.asarray(values)
+        if v.ndim != 1 or not (np.issubdtype(v.dtype, np.floating) or np.issubdtype(v.dtype, np.integer)):
+            raise ValueError(f"{where}: values must be a 1-D array of numbers, got {v.dtype} {v.shape}")
+        o = cls._record_of(_lib.OUTCOME_VALUES, name, 0, 0, where)
+        o.array = np.ascontiguousarray(v, dtype=np.float64)
+        return o
+
+    def __repr__(self) -> str:
+        kind = {_lib.OUTCOME_EXTREMA: "extrema", _lib.OUTCOME_MOMENT: "moment", _lib.OUTCOME_COLUMN: "column",
+                _lib.OUTCOME_THRESHOLD: "threshold", _lib.OUTCOME_DWELL: "dwell", _lib.OUTCOME_VALUES: "values"}[self.kind]
+        return f"Outcome({self.name!r}, {kind}, index={self.index}, field={self.field})"
+
+
+def _outcome_list(outcomes) -> List[Outcome]:
+    """World.build(..., outcomes=...): 1 to MAX_OUTCOMES el.Outcome objects with distinct names."""
+    if isinstance(outcomes, (str, bytes)) or not isinstance(outcomes, Sequence):
+        raise TypeError(f"outcomes take a sequence of el.Outcome objects, got {outcomes!r}")
+    for o in outcomes:
+        if not isinstance(o, Outcome):
+            raise TypeError(f"outcomes take el.Outcome objects, got {o!r}")
+    if not 1 <= len(outcomes) <= _lib.MAX_OUTCOMES:
+        raise ValueError(f"{len(outcomes)} outcomes: 1 to {_lib.MAX_OUTCOMES}")
+    names = [o.name for o in outcomes]
+    for n in names:
+        if names.count(n) > 1:
+            raise ValueError(f"outcomes: the name {n!r} is used twice")
+    return list(outcomes)
 
 
 class _Row(np.ndarray):
@@ -901,7 +1036,7 @@ class Exec:
                  covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
                  groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
                  channels: Optional[Sequence[Channel]] = None, moments: Optional[Sequence] = None,
-                 dwells: Optional[Sequence[Threshold]] = None):
+                 dwells: Optional[Sequence[Threshold]] = None, outcomes: Optional[Sequence[Outcome]] = None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -941,7 +1076,8 @@ class Exec:
         given = [name for name, value in (("extrema", extrema or None), ("thresholds", thresholds or None),
                                           ("quantiles", quantiles), ("covariance", covariance), ("histograms", histograms),
                                           ("groups", groups), ("retain", retain), ("channels", channels),
-                                          ("moments", moments), ("dwells", dwells)) if value is not None]
+                                          ("moments", moments), ("dwells", dwells), ("outcomes", outcomes))
+                 if value is not None]
         if given and not ensemble:
             msg = f"{', '.join(given)}: need World.build(..., ensemble=True)"
             raise ValueError(msg) if given == ["groups"] else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, msg)
@@ -971,6 +1107,8 @@ class Exec:
         if len(self._dwells) > _lib.MAX_DWELLS:
             raise ValueError(f"{len(self._dwells)} dwells: at most {_lib.MAX_DWELLS}")
         self._dwell_rows = condition_rows(self._dwells, "dwells")
+        self._outcomes = _outcome_list(outcomes) if outcomes is not None else []
+        self._outcome_records = [self._outcome_record(o, n_c) for o in self._outcomes]
         # the run summaries this Exec folds (kinds of _OPTIONS)
         self._summaries = tuple(kind for kind, on in zip(_SUMMARIES, (self._extrema, self._thresholds,
                                                                       self._moment_planes, self._dwells)) if on)
@@ -1050,6 +1188,8 @@ class Exec:
         if self._summaries:  # moments and dwells are optional keywords of B200Exec.summary_begin: passed when asked for
             self.backend.summary_begin(self._extrema, self._threshold_rows, **{
                 k: v for k, v in (("moments", self._moment_planes), ("dwells", self._dwell_rows)) if v})
+        if self._outcome_records:  # after summary_begin: outcomes name the summaries in force
+            self.backend.set_outcomes(self._outcome_records)
         if self.groups is not None:
             self.backend.set_world_groups(self.groups)
         if self._ensemble:
@@ -1461,12 +1601,7 @@ class Exec:
             raise IndexError(f"histogram {i}: this Exec has {len(self._histograms)}")
         h = self._histograms[i]
         off = sum(x.record_len for x in self._histograms[:i])
-        t = t[..., off:off + h.record_len].astype(np.int64)
-        if len(h.bins) == 1:
-            return {"counts": np.ascontiguousarray(t[..., 3:]), "nonfinite": t[..., 0].copy(), "below": t[..., 1].copy(),
-                    "above": t[..., 2].copy(), "edges": h.edges}
-        return {"counts": np.ascontiguousarray(t[..., 2:]).reshape(*t.shape[:-1], *h.bins), "nonfinite": t[..., 0].copy(),
-                "outside": t[..., 1].copy(), "edges": h.edges}
+        return _histogram_record(h, t[..., off:off + h.record_len])
 
     def _table(self, accessor: str, kind: str, groups: bool = False) -> np.ndarray:
         """Table `kind` of _OPTIONS (its per-group table with `groups`): the rows recorded so far, or the run summary,
@@ -1563,6 +1698,114 @@ class Exec:
         if not 0 <= i < len(self._dwells):
             raise IndexError(f"dwell {i}: this Exec has {len(self._dwells)}")
         return {k: t[:, i, f].astype(np.int64) for f, k in enumerate(("rows", "first_tick", "last_tick"))}
+
+    def _outcome_record(self, o: Outcome, n_c: int) -> tuple:
+        """Outcome `o` -> its B200Exec.set_outcomes tuple (kind, field, index, entity row, column id, values), checked
+        against this Exec's options and world before the handle exists."""
+        where = repr(o)
+        if o.kind in (_lib.OUTCOME_EXTREMA, _lib.OUTCOME_MOMENT):
+            row = self._body_row(o.entity, o.pair)
+            plane = _channel_plane(o.plane, n_c, where)
+            if o.kind == _lib.OUTCOME_EXTREMA:
+                if not self._extrema:
+                    raise _build_with(where, "extrema=True")
+                return (o.kind, o.field, plane, row)
+            if plane not in self._moment_planes:
+                raise _build_with(where, f"moments=[...] selecting {o.pair}[{o.index}]")
+            return (o.kind, o.field, self._moment_planes.index(plane), row)
+        if o.kind == _lib.OUTCOME_COLUMN:
+            pair = f"{o.entity}.{o.component}"
+            inputs = [e.column_name() for e in self._effectors if e.column_name()]
+            if o.component not in _BODY_COLUMNS + tuple(inputs):
+                raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                          f"component not found: {pair} (outcomes read the device columns: "
+                                          f"{', '.join(_BODY_COLUMNS + tuple(inputs))})")
+            row = self._body_row(o.entity, pair)
+            width = self.world.columns[component_id(o.component)].width
+            if o.index >= width:
+                raise ValueError(f"{where}: index {o.index}, {pair} has {width} components")
+            return (o.kind, o.index, 0, row, o.component)
+        if o.kind == _lib.OUTCOME_VALUES:
+            if o.array.shape != (self.n_worlds,):
+                raise ValueError(f"{where}: {o.array.shape[0]} values, this Exec has {self.n_worlds} worlds")
+            return (o.kind, 0, 0, 0, 0, o.array)
+        have, option = ((len(self._thresholds), "thresholds") if o.kind == _lib.OUTCOME_THRESHOLD
+                        else (len(self._dwells), "dwells"))
+        if o.index >= have:
+            raise ValueError(f"{where}: {option[:-1]} {o.index}, this Exec has {have}")
+        return (o.kind, o.field, o.index)
+
+    @property
+    def outcomes(self) -> List[str]:
+        """The names of World.build(..., outcomes=[...]), in order: the outcome axis of every outcome table."""
+        return [o.name for o in self._outcomes]
+
+    def _outcome_ready(self, accessor: str, groups: bool) -> None:
+        if not self._outcomes or (groups and self.groups is None):
+            raise _build_with(f"{accessor}({'groups=True' if groups else ''})", "outcomes=[...]",
+                              *(("groups=[...]",) if groups else ()))
+
+    def _outcome_plane(self, name: str) -> int:
+        if name not in self.outcomes:
+            raise _lib.B200ValueError(_lib.ERR_COMPONENT_NOT_FOUND,
+                                      f"outcome not found: {name!r} (this Exec has {', '.join(self.outcomes)})")
+        return self.outcomes.index(name)
+
+    def outcome_values(self) -> Dict[str, np.ndarray]:
+        """{name: [n_worlds]}: every outcome's value of every world, from the summaries as folded so far (ticks that
+        never happened are NaN).  It downloads per-world values: meant for small campaigns and tests."""
+        self._outcome_ready("outcome_values", False)
+        t = self.backend.outcome_values()
+        return {n: np.ascontiguousarray(t[:, k]) for k, n in enumerate(self.outcomes)}
+
+    def outcome_stats(self, groups: bool = False) -> Dict[str, np.ndarray]:
+        """{"count", "mean", "std", "min", "max"}, each [P] (or [G, P] with groups=True) in the order of `outcomes`:
+        over the worlds whose value is finite, as Exec.ensemble.  Computed on the device now, from the summaries as
+        folded so far.  The tables of world-sharded ranks merge with executor.merge_stats."""
+        self._outcome_ready("outcome_stats", groups)
+        t = self.backend.outcome_group_stats() if groups else self.backend.outcome_stats()
+        count = np.ascontiguousarray(t[..., 0])
+        with np.errstate(invalid="ignore", divide="ignore"):
+            std = np.sqrt(t[..., 2] / count)
+        return {"count": count, "mean": np.ascontiguousarray(t[..., 1]), "std": std,
+                "min": np.ascontiguousarray(t[..., 3]), "max": np.ascontiguousarray(t[..., 4])}
+
+    def outcome_quantiles(self, q, groups: bool = False) -> np.ndarray:
+        """[n_q, P] (or [G, n_q, P] with groups=True): numpy's linear quantiles at the levels `q` of every outcome
+        over the worlds whose value is finite, exact.  Quantile tables do not merge across ranks."""
+        self._outcome_ready("outcome_quantiles", groups)
+        lv = _quantile_levels(list(np.atleast_1d(q)))
+        t = self.backend.outcome_group_quantiles(lv) if groups else self.backend.outcome_quantiles(lv)
+        return np.ascontiguousarray(np.swapaxes(t, -1, -2))
+
+    def outcome_covariance(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, object]:
+        """{"count", "mean" [p], "cov" [p, p], "planes" (the names)} of the outcomes `names` (default: all), in
+        Exec.covariance's layout (a group axis first with groups=True): over the worlds whose p values are all finite.
+        The tables of world-sharded ranks merge with executor.merge_covariance."""
+        self._outcome_ready("outcome_covariance", groups)
+        names = list(self.outcomes if names is None else names)
+        planes = [self._outcome_plane(n) for n in names]
+        t = self.backend.outcome_group_covariance(planes) if groups else self.backend.outcome_covariance(planes)
+        p = len(planes)
+        count = np.array(t[..., 0])  # a scalar without groups
+        with np.errstate(invalid="ignore", divide="ignore"):
+            cov = t[..., 1 + p:].reshape(*t.shape[:-1], p, p) / count[..., None, None]
+        return {"count": count, "mean": np.ascontiguousarray(t[..., 1:1 + p]), "cov": cov, "planes": names}
+
+    def outcome_histogram(self, name, range, bins=10, groups: bool = False) -> Dict[str, object]:
+        """The histogram of outcome `name` (1D) or of a pair of names (2D) over the worlds, in Exec.histogram's dict
+        ("counts", "nonfinite", "below" / "above" or "outside", "edges"), with el.Histogram's range and bins rules (a
+        group axis first with groups=True).  The tables of world-sharded ranks add up (executor.merge_histograms)."""
+        self._outcome_ready("outcome_histogram", groups)
+        two = isinstance(name, (tuple, list))
+        where = f"outcome_histogram({name!r})"
+        if two and len(name) != 2:
+            raise ValueError(f"{where}: one name (1D) or a pair of names (2D)")
+        h = Histogram.__new__(Histogram)
+        h._axes(where, tuple(self._outcome_plane(n) for n in (name if two else (name,))), range, bins)
+        spec = [h._spec(0)]
+        t = self.backend.outcome_group_histograms(spec) if groups else self.backend.outcome_histograms(spec)
+        return _histogram_record(h, t)
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

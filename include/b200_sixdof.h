@@ -592,6 +592,74 @@ int b200_sixdof_trajectory_channels(b200_sixdof *h, void *dst, uint64_t bytes);
 /* the channels of the current state: dst = [n_worlds][n_entities][n_c] f64 (host or device) */
 int b200_sixdof_state_channels(b200_sixdof *h, void *dst, uint64_t bytes);
 
+/* ---- outcomes: one f64 per world, taken from the run summaries, a device column or host values, and reduced over the
+ * worlds by the ensemble reductions above.  This joins the two families: the apogee percentiles per sweep point, the
+ * impact-point covariance, the probability that a threshold fired or a settling-time histogram, without a per-world
+ * table reaching the host.
+ *   kind       field                                       value of world w
+ *   EXTREMA    0..4: min, max, min_tick, max_tick,         the extrema record of (w, entity, plane `index` < R)
+ *              first_nonfinite_tick
+ *   THRESHOLD  0: tick; 1 + p: plane p (0..24) of the row  threshold `index`'s record of w
+ *   MOMENT     0..3: count, mean, std, rms                 moment slot `index` (the spec's order) of (w, entity)
+ *   DWELL      0..2: rows, first_tick, last_tick           dwell `index`'s record of w
+ *   COLUMN     a plane of the column (< its width)         the column's current device value for (w, entity): a
+ *                                                          dispersed input (inertia plane 6 = mass) or the final state
+ *   VALUES     0                                           values[w], copied by set_outcomes
+ * Value rules: a tick field that holds -1 ("never") is NaN, so the reductions, which drop non-finite values, leave out
+ * the worlds where the event never happened (the count of a threshold's tick is the number of worlds that fired, and
+ * count / n_worlds the event probability; a histogram counts them in `nonfinite`).  Every other field keeps its bits,
+ * except the moments: count, mean and m2 are those of b200_sixdof_moments_download, then std = sqrt(m2 / n) and
+ * rms = sqrt(mean * mean + m2 / n), each operation correctly rounded (numpy's bits for the same expression).
+ * Every outcome entry first writes the outcome planes, P planes of n_worlds values, with one launch on the handle's
+ * stream (counted in timings.kernel_launches; never cached: the summaries and columns change under it), then runs the
+ * reduction on them as on a state of one entity: the tables have the layout and the bits of the state_* entries of a
+ * handle with n_entities = 1 whose first P state planes hold the outcome values (E = 1 below).  Grouped entries use the
+ * groups of b200_sixdof_set_world_groups.  Every entry checks the outcome set against the summary in force (a later
+ * summary_start can drop what an outcome names) and refuses it, naming the outcome, with B200_ERR_INVALID_ARGUMENT, as
+ * it refuses a handle without outcomes; then it checks what the state_* entry checks, in the same order. ---- */
+#define B200_MAX_OUTCOMES 25u   /* = B200_MAX_COV_PLANES: one covariance call takes every outcome */
+enum { B200_OUTCOME_EXTREMA = 1, B200_OUTCOME_THRESHOLD = 2, B200_OUTCOME_MOMENT = 3,
+       B200_OUTCOME_DWELL = 4, B200_OUTCOME_COLUMN = 5, B200_OUTCOME_VALUES = 6 };
+typedef struct b200_outcome {
+    uint32_t kind;        /* B200_OUTCOME_*                                                  */
+    uint32_t field;       /* see the table above                                             */
+    uint32_t index;       /* EXTREMA: plane < R; THRESHOLD / DWELL: which one; MOMENT: slot  */
+    uint32_t reserved;    /* must be 0                                                       */
+    uint64_t entity;      /* EXTREMA, MOMENT, COLUMN: entity row (< n_entities); else 0      */
+    uint64_t column;      /* COLUMN: component id; else 0                                    */
+    const double *values; /* VALUES: n_worlds f64, copied by set_outcomes; else NULL         */
+} b200_outcome;
+/* o[0 .. n) replaces the outcome set; n = 0 clears it.  B200_ERR_INVALID_ARGUMENT, with the previous set left in force,
+ * for: a null handle, n > B200_MAX_OUTCOMES, null o with n > 0, an unknown kind, a bad field, index or entity, a
+ * non-zero reserved field, entity or column set where the kind takes none, a summary the summary in force does not have
+ * (no extrema, a threshold, dwell or moment slot past its count, an extrema plane >= R), a global column (tick, time
+ * step), a column plane >= its width, or null values; B200_ERR_COMPONENT_NOT_FOUND for an unknown column id.  Allocates
+ * P * ld_o f64, ld_o = n_worlds rounded up to 128. */
+int b200_sixdof_set_outcomes(b200_sixdof *h, const b200_outcome *o, uint32_t n);
+/* the number of outcomes set (0 for a null handle) */
+uint32_t b200_sixdof_outcomes(const b200_sixdof *h);
+/* dst = [n_worlds][P] f64: the outcome values themselves (host or device; for small campaigns and tests) */
+int b200_sixdof_outcome_values(b200_sixdof *h, void *dst, uint64_t bytes);
+/* dst = [P][5] f64, the state statistics' fields */
+int b200_sixdof_outcome_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* dst = [G][P][5] f64 */
+int b200_sixdof_outcome_group_stats(b200_sixdof *h, void *dst, uint64_t bytes);
+/* dst = [P][n_q] f64 */
+int b200_sixdof_outcome_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* dst = [G][P][n_q] f64 */
+int b200_sixdof_outcome_group_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, void *dst, uint64_t bytes);
+/* planes < P: dst = [1 + n_p + n_p^2] f64 */
+int b200_sixdof_outcome_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* dst = [G][1 + n_p + n_p^2] f64 */
+int b200_sixdof_outcome_group_covariance(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
+                                         uint64_t bytes);
+/* spec.entity = 0, planes < P: dst = [sum of the record lengths] f64 */
+int b200_sixdof_outcome_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                   uint64_t bytes);
+/* dst = [G][sum of the record lengths] f64 */
+int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
+                                         uint64_t bytes);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
