@@ -366,10 +366,17 @@ int do_upload(b200_sixdof *h, uint64_t id, const void *src, uint64_t bytes)
         return fail(B200_ERR_VALUE_SIZE_MISMATCH, "component value had wrong size: 0x%016llx has %llu bytes, got %llu",
                     (unsigned long long)id, (unsigned long long)column_bytes(h, *c), (unsigned long long)bytes);
     if (!src) return fail(B200_ERR_INVALID_ARGUMENT, "null source buffer");
+    const bool device = is_device_pointer(src);
     if (c->global) {
-        // the two globals are 8-byte host scalars (Globals entity, world.rs:174-191)
+        // the two globals are 8-byte scalars the handle keeps on the host (Globals entity, world.rs:174-191); a device
+        // buffer is read on the handle's stream, after the work already queued there
         uint64_t raw;
-        std::memcpy(&raw, src, 8);
+        if (device) {
+            CU(h, cudaMemcpyAsync(&raw, src, 8, cudaMemcpyDefault, h->stream));
+            CU(h, cudaStreamSynchronize(h->stream));
+        } else {
+            std::memcpy(&raw, src, 8);
+        }
         if (id == B200_ID_TICK) h->tick = raw;
         else std::memcpy(&h->sim_time_step, &raw, 8);
         return B200_OK;
@@ -381,6 +388,8 @@ int do_upload(b200_sixdof *h, uint64_t id, const void *src, uint64_t bytes)
     CU(h, cudaMemcpyAsync(h->staging, src, bytes, cudaMemcpyDefault, h->stream));
     CU(h, launch_aos_to_soa(h->staging, c->dev, h->n_bodies, c->width, h->ld, h->stream));
     h->timings.kernel_launches++;
+    // a host source is the caller's again when this returns: the copy out of it must have happened
+    if (!device) CU(h, cudaStreamSynchronize(h->stream));
     return B200_OK;
 }
 
@@ -396,7 +405,12 @@ int do_download(b200_sixdof *h, uint64_t id, void *dst, uint64_t bytes)
         uint64_t raw;
         if (id == B200_ID_TICK) raw = h->tick;
         else std::memcpy(&raw, &h->sim_time_step, 8);
-        std::memcpy(dst, &raw, 8);
+        if (is_device_pointer(dst)) { // written on the handle's stream, after the work already queued there
+            CU(h, cudaMemcpyAsync(dst, &raw, 8, cudaMemcpyDefault, h->stream));
+            CU(h, cudaStreamSynchronize(h->stream));
+        } else {
+            std::memcpy(dst, &raw, 8);
+        }
         return B200_OK;
     }
     if (bytes == 0) return B200_OK;
@@ -958,6 +972,17 @@ static int invoke_pipelined(b200_sixdof *h, const BatchPlan &plan, uint64_t n_ti
         h->chunk_out.push_back(b);
     }
     int rc;
+    // whole-batch AoS staging: an UPLOAD / DOWNLOAD column lives at its plan offset (doubles)
+    if ((rc = grow_device(h, &h->stage_in, &h->stage_in_bytes, plan.in_total * 8))) return rc;
+    if ((rc = grow_device(h, &h->stage_out, &h->stage_out_bytes, plan.out_total * 8))) return rc;
+    // globals first (scalars the handle keeps on the host)
+    for (const BatchPlan::Col &c : plan.in)
+        if (c.role == BatchPlan::GLOBAL && (rc = do_upload(h, c.col->id, c.src, 8))) return rc;
+    // the copy streams must not run ahead of work already queued on the compute stream (a caller's stream may still
+    // write an input or read an output the copies below touch)
+    CU(h, cudaEventRecord(h->ev[2], h->stream));
+    CU(h, cudaStreamWaitEvent(h->copy_in, h->ev[2], 0));
+    CU(h, cudaStreamWaitEvent(h->copy_out, h->ev[2], 0));
     // the pass-through outputs whose input is here: by the copy engine when either side is device memory, else
     // host-to-host on a few worker threads, while the PCIe link carries the columns that did change
     std::vector<std::thread> fillers;
@@ -975,16 +1000,6 @@ static int invoke_pipelined(b200_sixdof *h, const BatchPlan &plan, uint64_t n_ti
             fillers.emplace_back([dst = c.dst, src = c.src, o0, o1] { std::memcpy(dst + o0, src + o0, o1 - o0); });
         }
     }
-    // whole-batch AoS staging: an UPLOAD / DOWNLOAD column lives at its plan offset (doubles)
-    if ((rc = grow_device(h, &h->stage_in, &h->stage_in_bytes, plan.in_total * 8))) return rc;
-    if ((rc = grow_device(h, &h->stage_out, &h->stage_out_bytes, plan.out_total * 8))) return rc;
-    // globals first (host-resident scalars)
-    for (const BatchPlan::Col &c : plan.in)
-        if (c.role == BatchPlan::GLOBAL && (rc = do_upload(h, c.col->id, c.src, 8))) return rc;
-    // the copy streams must not run ahead of work already queued on the compute stream
-    CU(h, cudaEventRecord(h->ev[2], h->stream));
-    CU(h, cudaStreamWaitEvent(h->copy_in, h->ev[2], 0));
-    CU(h, cudaStreamWaitEvent(h->copy_out, h->ev[2], 0));
     CU(h, cudaEventRecord(h->ev[0], h->copy_in));
 
     host_loop0 = host_ms();

@@ -238,7 +238,12 @@ uint64_t b200_sixdof_column_bytes(const b200_sixdof *h, uint64_t component_id);
 
 /* Host (or device: the copy direction is inferred, cudaMemcpyDefault) AoS column
  * -> device SoA planes, and back.  `bytes` must equal b200_sixdof_column_bytes
- * (else B200_ERR_VALUE_SIZE_MISMATCH, as cranelift_exec.rs:175-177,188-190). */
+ * (else B200_ERR_VALUE_SIZE_MISMATCH, as cranelift_exec.rs:175-177,188-190).
+ * Either buffer may be device memory on the handle's GPU, the two globals' 8-byte
+ * buffers included.  Both run on the handle's stream, after the work already queued
+ * there.  upload returns once a host source has been read (the caller may reuse it);
+ * from a device source it returns at once, the copy stream-ordered.  download
+ * returns with the data in `dst`. */
 int b200_sixdof_upload(b200_sixdof *h, uint64_t component_id, const void *src, uint64_t bytes);
 int b200_sixdof_download(b200_sixdof *h, uint64_t component_id, void *dst, uint64_t bytes);
 
@@ -256,7 +261,11 @@ int b200_sixdof_sync(b200_sixdof *h);
  *   in_cols[i]  == NULL: the column is not dirty — the host has not modified it since the previous call
  *                        (World::dirty_components, libs/nox-py/src/world.rs:43,249-252) — the device copy stands;
  *   out_cols[j] == NULL: the caller does not read that column after this batch (e.g. WorldAccel / Force between
- *                        telemetry cycles, pass-through Inertia): it is neither downloaded nor filled. */
+ *                        telemetry cycles, pass-through Inertia): it is neither downloaded nor filled.
+ * Any buffer may be device memory on the handle's GPU (tick and simulation_time_step included); a call with
+ * a device buffer other than the two globals runs on the pipelined world ranges.  Every copy out of an input
+ * and into an output is ordered after the work already queued on the handle's stream, and the call returns
+ * with every output written. */
 int b200_sixdof_invoke_batch(b200_sixdof *h, const uint8_t *const *in_cols,
                              uint8_t *const *out_cols, uint64_t n_ticks);
 
@@ -664,7 +673,14 @@ int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *s
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
  * the legacy default stream, e.g. torch.cuda.current_stream().cuda_stream), or, with
- * use_own_stream != 0, go back to the handle's private non-blocking stream. */
+ * use_own_stream != 0, go back to the handle's private non-blocking stream.  Waits for
+ * the work queued on the stream it leaves.  On a caller stream, every entry is ordered
+ * after the work already queued on that stream, and the caller's later work on it sees
+ * what the entry did (b200_sixdof_step: the new state, e.g. through
+ * b200_sixdof_device_plane, with no sync in between).  Entries that return data
+ * (downloads, invoke_batch, reductions) return with it complete.  The private stream
+ * has no ordering with any other stream: a caller that shares buffers with the handle
+ * there synchronises first. */
 int b200_sixdof_set_stream(b200_sixdof *h, void *cuda_stream, int use_own_stream);
 int b200_sixdof_timings(const b200_sixdof *h, b200_timings *out);
 int b200_sixdof_status(const b200_sixdof *h);                  /* sticky status of the handle */
