@@ -76,6 +76,7 @@ SYMBOLS = [
     "b200_sixdof_outcome_group_stats", "b200_sixdof_outcome_quantiles", "b200_sixdof_outcome_group_quantiles",
     "b200_sixdof_outcome_covariance", "b200_sixdof_outcome_group_covariance", "b200_sixdof_outcome_histograms",
     "b200_sixdof_outcome_group_histograms",
+    "b200_sixdof_sharded_quantiles_begin", "b200_sixdof_sharded_quantiles_round", "b200_sixdof_sharded_quantiles_end",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -84,6 +85,7 @@ MOMENT_FIELDS = 3  # n, mean, m2 = sum (x - mean)^2 over a world's finite rows
 MAX_DWELLS = 8
 DWELL_FIELDS = 3  # rows, first_tick, last_tick of the rows beyond a dwell's bound
 MAX_QUANTILES = 16  # levels per quantile call
+QUANTILE_SOURCES = {"ring": 0, "state": 1, "outcomes": 2}  # b200_sixdof_sharded_quantiles_begin's source
 MAX_COV_PLANES = 25  # planes per covariance selection
 MAX_HISTOGRAMS = 8  # specs per histogram call
 MAX_HISTOGRAM_CELLS = 4096  # bins of one spec (na * nb for 2D)
@@ -340,6 +342,9 @@ def lib():
     L.b200_sixdof_outcome_group_stats.argtypes = [vp, vp, u64]
     L.b200_sixdof_outcome_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
     L.b200_sixdof_outcome_group_quantiles.argtypes = [vp, C.POINTER(C.c_double), u32, vp, u64]
+    L.b200_sixdof_sharded_quantiles_begin.argtypes = [vp, u32, C.c_int, C.POINTER(C.c_double), u32, C.POINTER(u64)]
+    L.b200_sixdof_sharded_quantiles_round.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64)]
+    L.b200_sixdof_sharded_quantiles_end.argtypes = [vp, vp, u64]
     L.b200_sixdof_outcome_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_outcome_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_outcome_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]

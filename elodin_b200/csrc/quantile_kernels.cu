@@ -88,7 +88,14 @@ struct Layout {
     const QRow *rows;             // [nr] the slice's rows
     QGroup *grp;                  // [G]
     uint32_t *hist;               // [G][kBins]
-    unsigned long long *area;     // [G][kGroupCap]
+    unsigned long long *area;     // [G][area_stride]: kGroupCap, or kSlots when sharded (right after hist)
+    uint64_t area_stride;
+    // sharded (a rank's part of a world-sharded call, b200_sixdof_sharded_quantiles_*): pass 0 counts into cnt[G], the
+    // plans start from the whole key range and compact only ranges of one key, and every plan adds its groups' todo
+    // flags to *todo
+    bool sharded;
+    uint32_t *cnt;
+    uint32_t *todo;
 };
 
 __device__ __forceinline__ unsigned long long order_key(double x)
@@ -302,7 +309,7 @@ __global__ void __launch_bounds__(kPassThreads) quantile_count_kernel(QuantilePa
         }
         if (live && n) {
             QGroup &G = L.grp[il * sl.ne + e];
-            atomicAdd(&G.n, n);
+            atomicAdd(L.sharded ? &L.cnt[il * sl.ne + e] : &G.n, n);
             atomicMin(&G.kmin, mn);
             atomicMax(&G.kmax, mx);
         }
@@ -342,7 +349,7 @@ __global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantilePar
         }
         if (live && G.todo) {
             uint32_t *hist = L.hist + g * kBins;
-            unsigned long long *area = L.area + g * kGroupCap;
+            unsigned long long *area = L.area + g * L.area_stride;
             const double *p = stats_plane(S, r.i) + sl.e0 + e;
             const uint64_t w1 = r.o + min((c + 1) * r.Wc, (uint64_t)r.n);
             const unsigned long long kmin = G.kmin, kmax = G.kmax;
@@ -390,13 +397,17 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_plan_kernel(QuantilePar
     constexpr uint32_t kItems = kBins / kPlanThreads;
     QGroup &G = L.grp[blockIdx.x];
     uint32_t *hist = L.hist + (uint64_t)blockIdx.x * kBins;
+    unsigned long long *area = L.area + blockIdx.x * L.area_stride;
     const uint32_t t = threadIdx.x;
     if (t == 0) dirty = level == 0 || (G.todo && G.n_refine);
     if (level == 0) {
         if (t == 0) {
+            // sharded: n is the ranks' sum, and min / max do not add, so every rank starts from the whole key range
+            if (L.sharded) G.n = L.cnt[blockIdx.x];
+            const unsigned long long lo = L.sharded ? 0 : G.kmin, hi = L.sharded ? ~0ull : G.kmax;
             for (uint32_t s = 0; s < kSlots; ++s) {
                 QSlot &q = G.slot[s];
-                q = QSlot{G.kmin, G.kmax, 0, G.n, kUnused, s, 0, 0, 0, 0};
+                q = QSlot{lo, hi, 0, G.n, kUnused, s, 0, 0, 0, 0};
                 if (G.n == 0 || s / 2 >= S.n_q) continue;
                 uint32_t r0, r1;
                 bool two;
@@ -451,6 +462,10 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_plan_kernel(QuantilePar
         uint32_t n_refine = 0;
         for (uint32_t s = 0; s < kSlots; ++s) {
             QSlot &q = G.slot[s];
+            if (q.state == kCompact && L.sharded) {  // a range of one key: the ranks' summed area words are that key
+                q.lo = q.hi = area[G.slot[q.owner].cofs];
+                q.state = kDone;
+            }
             if (q.state == kCompact) q.state = kCompacted;  // the pass that just ran copied it
             if (q.state != 5 && q.state != kRefine) continue;
             q.state = kRefine;
@@ -466,7 +481,7 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_plan_kernel(QuantilePar
             if (q.owner != s) continue;
             if (q.lo == q.hi) {
                 q.state = kDone;
-            } else if (!last && q.count <= kBucketCap && G.used + q.count <= kGroupCap) {
+            } else if (!last && (L.sharded ? q.count == 1 : q.count <= kBucketCap && G.used + q.count <= kGroupCap)) {
                 q.state = kCompact;
                 q.cofs = G.used;
                 q.fill = 0;
@@ -492,10 +507,13 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_plan_kernel(QuantilePar
         const uint32_t todo = n_act > 0;
         G.todo = todo;
         atomicAdd(L.reads, (unsigned long long)(todo + (level == 0)));  // level 0: pass 0 read the group too
+        if (L.sharded && todo) atomicAdd(L.todo, 1u);
     }
     __syncthreads();
     if (dirty)
         for (uint32_t b = t; b < kBins; b += blockDim.x) hist[b] = 0;
+    // sharded: the keys read off above are in the slots now; a rank that does not hold the next pass's keys sends zeros
+    if (L.sharded && t < kSlots) area[t] = 0;
 }
 
 // finish: one block per group sorts each compacted range in shared memory, then writes the group's quantiles
@@ -504,7 +522,7 @@ __global__ void __launch_bounds__(kPlanThreads) quantile_finish_kernel(QuantileP
     extern __shared__ unsigned long long keys[];  // kBucketCap
     __shared__ unsigned long long rank_key[kSlots];
     QGroup &G = L.grp[blockIdx.x];
-    const unsigned long long *area = L.area + (uint64_t)blockIdx.x * kGroupCap;
+    const unsigned long long *area = L.area + blockIdx.x * L.area_stride;
     const uint32_t t = threadIdx.x;
     if (t < kSlots) rank_key[t] = G.slot[t].lo;  // a finished range holds one key
     __syncthreads();
@@ -535,12 +553,20 @@ constexpr uint64_t kSliceGroups = (kScratchCap - 256) / kGroupBytes;  // about 1
 constexpr uint64_t kRowBytes = kSliceGroups * sizeof(QRow);           // a slice has at most kSliceGroups rows
 static_assert(256 + kRowBytes + kSliceGroups * kGroupBytes <= kScratchCap, "a slice's scratch must fit in kScratchCap");
 
-inline Layout layout_of(uint64_t G, void *scratch)
+// The scratch of a slice of G triples: a 256-byte header (the reads counter, then the sharded todo counter), the row
+// table, then per triple its plan, histogram and compaction area; a sharded slice's areas (kSlots keys: it compacts
+// ranges of one key only) follow the histograms directly, so a round's counters and keys are one run of u32 words, and
+// its pass 0 counts follow them.
+constexpr uint64_t kExchangeBytes = kBins * 4ull + kSlots * 8ull;  // a sharded triple's words of a histogram round
+constexpr uint64_t kShardGroupBytes = (sizeof(QGroup) + 7) / 8 * 8 + kExchangeBytes + 4;
+
+inline Layout layout_of(uint64_t G, void *scratch, bool sharded)
 {
     Layout L;
     L.G = G;
     char *p = (char *)scratch;
     L.reads = (unsigned long long *)p;
+    L.todo = sharded ? (uint32_t *)(p + 8) : nullptr;
     p += 256;
     L.rows = (const QRow *)p;
     p += kRowBytes;
@@ -549,6 +575,10 @@ inline Layout layout_of(uint64_t G, void *scratch)
     L.hist = (uint32_t *)p;
     p += G * kBins * sizeof(uint32_t);
     L.area = (unsigned long long *)p;
+    L.area_stride = sharded ? kSlots : kGroupCap;
+    p += G * L.area_stride * 8;
+    L.sharded = sharded;
+    L.cnt = sharded ? (uint32_t *)p : nullptr;
     return L;
 }
 
@@ -564,6 +594,7 @@ __global__ void quantile_init_kernel(Layout L, bool first, unsigned long long re
         L.grp[g].used = 0;
         L.grp[g].n_act = 0;
         L.grp[g].n_refine = 0;
+        if (L.sharded) L.cnt[g] = 0;
     }
 }
 
@@ -587,6 +618,88 @@ inline Routes routes_of(const std::vector<WorldGroup> &table, const std::vector<
         r.block += table[g].n <= kSmallMax;
     }
     return r;
+}
+
+// One slice of the radix sequence over the large groups large[0 .. n_large) of a table (slice_shape; row slices
+// outermost, then entity slices): its triples, row table, scratch layout and pass launch shape.
+struct SliceRun {
+    Slice sl;
+    Layout L;
+    PassShape sp;
+    unsigned grid;
+    size_t hist_smem;
+    std::vector<QRow> rows;
+};
+
+constexpr uint64_t kGridCap = 64ull * kNumSMs * 8;
+
+inline uint64_t slices_of(const QuantileParams &S, uint64_t n_large)
+{
+    const Slice sh = slice_shape(S.n_entities);
+    const uint64_t n_rows = n_large * S.n_planes;
+    return (n_rows + sh.nr - 1) / sh.nr * ((S.n_entities + sh.ne - 1) / sh.ne);
+}
+
+SliceRun slice_run(const QuantileParams &S, const std::vector<WorldGroup> &table, const uint32_t *large,
+                   uint64_t n_large, uint64_t k, void *scratch, bool sharded)
+{
+    const Slice sh = slice_shape(S.n_entities);
+    const uint64_t n_rows = n_large * S.n_planes, n_e = (S.n_entities + sh.ne - 1) / sh.ne;
+    const uint64_t r0 = k / n_e * sh.nr, e0 = k % n_e * sh.ne;
+    SliceRun run;
+    Slice &sl = run.sl;
+    sl = Slice{r0, std::min(sh.nr, n_rows - r0), e0, std::min(sh.ne, S.n_entities - e0), 0, 0};
+    for (uint64_t r = r0; r < r0 + sl.nr; ++r) {
+        const uint32_t g = large[r / S.n_planes];
+        const WorldGroup &wg = table[g];
+        const PassShape sp = pass_shape(wg.n, sl.ne, sl.nr);
+        run.rows.push_back(QRow{(uint32_t)wg.o, (uint32_t)wg.n, (uint32_t)sp.Wc, (uint32_t)sp.C, (uint32_t)sl.K, g,
+                                (uint32_t)(r % S.n_planes), 0});
+        sl.K += sp.C;
+        sl.Cu = r == r0 || sl.Cu == sp.C ? sp.C : 0;
+    }
+    run.L = layout_of(sl.nr * sl.ne, scratch, sharded);
+    run.sp = pass_shape(0, sl.ne, sl.nr);  // the tiles (Et, J, T): the slice's entities alone
+    run.grid = (unsigned)std::min(sl.K * run.sp.T, kGridCap);
+    run.hist_smem = sl.ne == 1 ? kBins * 4ull : 0;
+    return run;
+}
+
+cudaError_t radix_attributes()
+{
+    cudaError_t e = cudaFuncSetAttribute(quantile_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(quantile_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(quantile_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBucketCap * 8));
+    return e;
+}
+
+// The slice's row table, copied in stream order into the scratch the previous slice is done with, then its init and
+// pass 0 (no pass 0 launch when no row of the slice holds a world: a sharded rank's empty groups)
+cudaError_t launch_open(const QuantileParams &S, const SliceRun &r, bool first, unsigned long long reads0, cudaStream_t s)
+{
+    const cudaError_t e = cudaMemcpyAsync((void *)r.L.rows, r.rows.data(), r.rows.size() * sizeof(QRow),
+                                          cudaMemcpyHostToDevice, s);
+    if (e != cudaSuccess) return e;
+    quantile_init_kernel<<<(unsigned)std::min((r.L.G + 255) / 256, kGridCap), 256, 0, s>>>(r.L, first, reads0);
+    if (r.grid) quantile_count_kernel<<<r.grid, kPassThreads, 0, s>>>(S, r.sl, r.sp, r.L);
+    return cudaSuccess;
+}
+
+void launch_plan(const QuantileParams &S, const SliceRun &r, int level, cudaStream_t s)
+{
+    quantile_plan_kernel<<<(unsigned)r.L.G, kPlanThreads, kBins * 4, s>>>(S, r.L, level);
+}
+
+void launch_pass(const QuantileParams &S, const SliceRun &r, cudaStream_t s)
+{
+    if (r.grid) quantile_pass_kernel<<<r.grid, kPassThreads, r.hist_smem, s>>>(S, r.sl, r.sp, r.L);
+}
+
+void launch_finish(const QuantileParams &S, const SliceRun &r, cudaStream_t s)
+{
+    quantile_finish_kernel<<<(unsigned)r.L.G, kPlanThreads, kBucketCap * 8, s>>>(S, r.sl, r.L);
 }
 
 } // namespace
@@ -618,11 +731,10 @@ cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGro
     *launches = 0;
     if (S.n_planes == 0 || S.n_entities == 0) return cudaSuccess;
     const uint64_t PE = S.n_planes * S.n_entities;
-    const uint64_t cap = 64ull * kNumSMs * 8;
     const Routes rt = routes_of(table, order);
     cudaError_t e = cudaSuccess;
     if (rt.warp > 0) {
-        quantile_warp_kernel<<<(unsigned)std::min((rt.warp * PE + 7) / 8, cap), 256, 0, s>>>(S, 0, rt.warp);
+        quantile_warp_kernel<<<(unsigned)std::min((rt.warp * PE + 7) / 8, kGridCap), 256, 0, s>>>(S, 0, rt.warp);
         *launches += 1;
     }
     if (rt.block > rt.warp) {
@@ -633,65 +745,116 @@ cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGro
         const size_t smem = P * 8ull;
         e = cudaFuncSetAttribute(quantile_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
-        quantile_block_kernel<<<(unsigned)std::min((rt.block - rt.warp) * PE, cap), 512, smem, s>>>(S, rt.warp,
-                                                                                                    rt.block - rt.warp);
+        quantile_block_kernel<<<(unsigned)std::min((rt.block - rt.warp) * PE, kGridCap), 512, smem, s>>>(S, rt.warp,
+                                                                                                         rt.block - rt.warp);
         *launches += 1;
     }
     const uint64_t large = order.size() - rt.block;
     if (large == 0) return cudaGetLastError();
-    e = cudaFuncSetAttribute(quantile_pass_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(quantile_plan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBins * 4));
-    if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(quantile_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kBucketCap * 8));
+    e = radix_attributes();
     if (e != cudaSuccess) return e;
-    const Slice sh = slice_shape(S.n_entities);
-    const Layout L0 = layout_of(0, scratch);
-    const uint64_t n_rows = large * S.n_planes;
-    std::vector<QRow> rows;
-    bool first = true;
     // The same fixed sequence on every slice (one slice unless the triples need more than kScratchCap of scratch);
-    // each plan clears the histograms it leaves for the next pass, so the scratch needs no clearing in between.  The
-    // slice's row table is copied ahead of its launches, in stream order, into the scratch the previous slice is done
-    // with.
-    for (uint64_t r0 = 0; r0 < n_rows; r0 += sh.nr) {
-        for (uint64_t e0 = 0; e0 < S.n_entities; e0 += sh.ne) {
-            Slice sl{r0, std::min(sh.nr, n_rows - r0), e0, std::min(sh.ne, S.n_entities - e0), 0, 0};
-            rows.clear();
-            for (uint64_t r = r0; r < r0 + sl.nr; ++r) {
-                const uint32_t g = order[rt.block + r / S.n_planes];
-                const WorldGroup &wg = table[g];
-                const PassShape sp = pass_shape(wg.n, sl.ne, sl.nr);
-                rows.push_back(QRow{(uint32_t)wg.o, (uint32_t)wg.n, (uint32_t)sp.Wc, (uint32_t)sp.C, (uint32_t)sl.K, g,
-                                    (uint32_t)(r % S.n_planes), 0});
-                sl.K += sp.C;
-                sl.Cu = r == r0 || sl.Cu == sp.C ? sp.C : 0;
-            }
-            const uint64_t Gs = sl.nr * sl.ne;
-            const Layout L = layout_of(Gs, scratch);
-            const PassShape sp = pass_shape(0, sl.ne, sl.nr);  // the tiles (Et, J, T): the slice's entities alone
-            const unsigned grid = (unsigned)std::min(sl.K * sp.T, cap);
-            const size_t hist_smem = sl.ne == 1 ? kBins * 4ull : 0;
-            e = cudaMemcpyAsync((void *)L.rows, rows.data(), rows.size() * sizeof(QRow), cudaMemcpyHostToDevice, s);
-            if (e != cudaSuccess) return e;
-            quantile_init_kernel<<<(unsigned)std::min((Gs + 255) / 256, cap), 256, 0, s>>>(L, first, rt.block * PE);
-            quantile_count_kernel<<<grid, kPassThreads, 0, s>>>(S, sl, sp, L);
-            quantile_plan_kernel<<<(unsigned)Gs, kPlanThreads, kBins * 4, s>>>(S, L, 0);
-            *launches += 3;
-            for (int level = 1; level <= kLevels; ++level) {
-                quantile_pass_kernel<<<grid, kPassThreads, hist_smem, s>>>(S, sl, sp, L);
-                quantile_plan_kernel<<<(unsigned)Gs, kPlanThreads, kBins * 4, s>>>(S, L, level);
-                *launches += 2;
-            }
-            quantile_finish_kernel<<<(unsigned)Gs, kPlanThreads, kBucketCap * 8, s>>>(S, sl, L);
-            *launches += 1;
-            first = false;
+    // each plan clears the histograms it leaves for the next pass, so the scratch needs no clearing in between.
+    const uint64_t n_slices = slices_of(S, large);
+    for (uint64_t k = 0; k < n_slices; ++k) {
+        const SliceRun r = slice_run(S, table, order.data() + rt.block, large, k, scratch, false);
+        e = launch_open(S, r, k == 0, rt.block * PE, s);
+        if (e != cudaSuccess) return e;
+        launch_plan(S, r, 0, s);
+        *launches += 3;
+        for (int level = 1; level <= kLevels; ++level) {
+            launch_pass(S, r, s);
+            launch_plan(S, r, level, s);
+            *launches += 2;
         }
+        launch_finish(S, r, s);
+        *launches += 1;
     }
     e = cudaGetLastError();
     // the reads counter, 8 bytes, lands before the caller's stream synchronise
-    if (e == cudaSuccess) e = cudaMemcpyAsync(reads, L0.reads, sizeof *reads, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(reads, layout_of(0, scratch, false).reads, sizeof *reads, cudaMemcpyDeviceToHost, s);
     return e;
+}
+
+// ---- world-sharded calls ---------------------------------------------------------------------------------------------
+// Every group takes the radix route (the route would follow the global world count, which no rank knows before the count
+// round) and every slice runs the launch sequence above with the sharded layout, a round between a pass and its plan:
+//   count round   open the slice; out: the pass 0 counts cnt[G]; in: their sums, then plan 0 from the whole key range
+//   pass round k  pass k; out: the slice's histograms and compaction keys; in: their sums, then plan k
+// A plan whose slice has nothing left to do ends the slice (finish) and opens the next one.  Every rank plans from the
+// same sums, so every rank makes the same rounds and ends on the same order statistics: those of the union of the
+// worlds.  A range whose global count is 1 is compacted: the one rank that holds its key copies it to the cleared area
+// and the others send zeros, so the summed words are the key; larger ranges are refined down to one key.
+
+uint64_t sharded_quantile_scratch_bytes(const QuantileParams &S, uint64_t n_groups)
+{
+    if (S.n_planes == 0 || S.n_entities == 0 || n_groups == 0) return 0;
+    const Slice sh = slice_shape(S.n_entities);
+    return (256 + kRowBytes + std::min(sh.nr, n_groups * S.n_planes) * sh.ne * kShardGroupBytes + 255) / 256 * 256;
+}
+
+uint64_t sharded_quantile_round_bytes(const QuantileParams &S, uint64_t n_groups)
+{
+    if (S.n_planes == 0 || S.n_entities == 0 || n_groups == 0) return 0;
+    const Slice sh = slice_shape(S.n_entities);
+    return std::min(sh.nr, n_groups * S.n_planes) * sh.ne * kExchangeBytes;
+}
+
+cudaError_t sharded_quantile_round(QuantileShard &Q, const void *reduced, void *partial, uint64_t *partial_bytes,
+                                   int *launches, cudaStream_t s)
+{
+#define QTRY(call)                                   \
+    do {                                             \
+        const cudaError_t e_ = (call);               \
+        if (e_ != cudaSuccess) return e_;            \
+    } while (0)
+    *partial_bytes = 0;
+    *launches = 0;
+    const QuantileParams &S = Q.S;
+    const uint64_t n_groups = Q.table.size();
+    const uint64_t n_slices = S.n_planes && S.n_entities ? slices_of(S, n_groups) : 0;
+    std::vector<uint32_t> all(n_groups);
+    for (uint32_t g = 0; g < n_groups; ++g) all[g] = g;
+    QTRY(radix_attributes());
+    if (Q.level >= 0) {  // the sums of the last round's words, then the plan of the pass they count
+        const SliceRun r = slice_run(S, Q.table, all.data(), n_groups, Q.slice, Q.scratch, true);
+        const uint64_t G = r.L.G;
+        QTRY(cudaMemcpyAsync(Q.level == 0 ? (void *)r.L.cnt : (void *)r.L.hist, reduced,
+                             Q.level == 0 ? G * 4 : G * kExchangeBytes, cudaMemcpyDefault, s));
+        QTRY(cudaMemsetAsync(r.L.todo, 0, 4, s));
+        launch_plan(S, r, Q.level, s);
+        uint32_t todo = 0;
+        QTRY(cudaMemcpyAsync(&todo, r.L.todo, 4, cudaMemcpyDeviceToHost, s));
+        QTRY(cudaStreamSynchronize(s));
+        *launches += 1;
+        if (todo && Q.level < kLevels) {
+            launch_pass(S, r, s);
+            ++Q.level;
+            *launches += 1;
+            QTRY(cudaMemcpyAsync(partial, r.L.hist, G * kExchangeBytes, cudaMemcpyDefault, s));
+            QTRY(cudaStreamSynchronize(s));
+            *partial_bytes = G * kExchangeBytes;
+            return cudaGetLastError();
+        }
+        launch_finish(S, r, s);
+        *launches += 1;
+        ++Q.slice;
+        Q.level = -1;
+    }
+    if (Q.slice < n_slices) {
+        const SliceRun r = slice_run(S, Q.table, all.data(), n_groups, Q.slice, Q.scratch, true);
+        QTRY(launch_open(S, r, Q.slice == 0, 0, s));
+        *launches += r.grid ? 2 : 1;
+        Q.level = 0;
+        QTRY(cudaMemcpyAsync(partial, r.L.cnt, r.L.G * 4, cudaMemcpyDefault, s));
+        QTRY(cudaStreamSynchronize(s));
+        *partial_bytes = r.L.G * 4;
+        return cudaGetLastError();
+    }
+    if (n_slices) QTRY(cudaMemcpyAsync(&Q.reads, layout_of(0, Q.scratch, true).reads, 8, cudaMemcpyDeviceToHost, s));
+    QTRY(cudaStreamSynchronize(s));
+    return cudaGetLastError();
+#undef QTRY
 }
 
 } // namespace b200

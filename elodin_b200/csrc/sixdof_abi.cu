@@ -360,6 +360,7 @@ int clear_mass_class(b200_sixdof *h, uint64_t b0, uint64_t n)
 
 int do_upload(b200_sixdof *h, uint64_t id, const void *src, uint64_t bytes)
 {
+    ++h->rows_gen;
     Column *c = h->find(id);
     if (!c) return fail(B200_ERR_COMPONENT_NOT_FOUND, "component not found: 0x%016llx", (unsigned long long)id);
     if (bytes != column_bytes(h, *c))
@@ -738,6 +739,7 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->pos_alt) cudaFree(h->pos_alt);
     if (h->vel_alt) cudaFree(h->vel_alt);
     if (h->staging) cudaFree(h->staging);
+    if (h->sq_scratch) cudaFree(h->sq_scratch);
     if (h->stage_in) cudaFree(h->stage_in);
     if (h->stage_out) cudaFree(h->stage_out);
     if (h->traj) cudaFree(h->traj);
@@ -1082,6 +1084,7 @@ static int invoke_pipelined(b200_sixdof *h, const BatchPlan &plan, uint64_t n_ti
 int b200_sixdof_invoke_batch(b200_sixdof *h, const uint8_t *const *in_cols, uint8_t *const *out_cols, uint64_t n_ticks)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    ++h->rows_gen;
     if (!in_cols || !out_cols) return fail(B200_ERR_INVALID_ARGUMENT, "null column tables");
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     CU(h, cudaSetDevice(h->device));
@@ -1399,6 +1402,7 @@ int b200_sixdof_set_world_groups(b200_sixdof *h, const uint64_t *sizes, uint32_t
         return fail(B200_ERR_INVALID_ARGUMENT, "world group sizes sum to %llu, not to the %llu worlds", (unsigned long long)sum,
                     (unsigned long long)h->desc.n_worlds);
     CU(h, cudaSetDevice(h->device));
+    ++h->rows_gen;
     h->group_sizes.assign(sizes, sizes + n_groups);
     return build_group_tables(h, sizes, n_groups, true);
 }
@@ -1494,15 +1498,14 @@ int b200_sixdof_state_group_stats(b200_sixdof *h, void *dst, uint64_t bytes)
     return run_world_stats(h, Rows::state, true, dst, bytes, "state");
 }
 
-// Quantiles of the planes over the worlds, per group when `grouped` (quantile_kernels.cu), into dst: the groups checked,
-// then the handle's status, then the levels, then `bytes`.
-static int run_quantiles(b200_sixdof *h, Rows src, bool grouped, const double *q, uint32_t n_q, void *dst,
-                         uint64_t bytes, const char *what)
+// The checks of a quantile call, in order: the groups, then the handle's status, then the levels.  Fills S with the
+// rows, the levels and the group table of the call.
+static int quantile_params(b200_sixdof *h, Rows src, bool grouped, const double *q, uint32_t n_q, const char *what,
+                           QuantileParams &S)
 {
     int rc = reduction_ready(h, src, grouped, what);
     if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
-    QuantileParams S{};
     static_cast<StatsParams &>(S) = reduction_rows(h, src);
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (n_q == 0 || n_q > B200_MAX_QUANTILES)
@@ -1511,16 +1514,28 @@ static int run_quantiles(b200_sixdof *h, Rows src, bool grouped, const double *q
     for (uint32_t l = 0; l < n_q; ++l)
         if (!(q[l] >= 0.0 && q[l] <= 1.0)) return fail(B200_ERR_INVALID_ARGUMENT, "quantile level %u is %g, not in [0, 1]", l, q[l]);
     const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped);
-    const uint64_t G = reduction_groups(h, grouped).size();
-    const uint64_t want = S.n_planes * G * S.n_entities * n_q * 8ull;
-    if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s quantiles are %llu bytes, got %llu", what, (unsigned long long)want,
-                    (unsigned long long)bytes);
     S.n_q = n_q;
     for (uint32_t l = 0; l < n_q; ++l) S.q[l] = q[l];
     S.groups = t.stats_dev;
     S.order = t.order_dev;
-    S.n_groups = G;
+    S.n_groups = reduction_groups(h, grouped).size();
+    return B200_OK;
+}
+
+// Quantiles of the planes over the worlds, per group when `grouped` (quantile_kernels.cu), into dst: the groups checked,
+// then the handle's status, then the levels, then `bytes`.
+static int run_quantiles(b200_sixdof *h, Rows src, bool grouped, const double *q, uint32_t n_q, void *dst,
+                         uint64_t bytes, const char *what)
+{
+    QuantileParams S{};
+    int rc = quantile_params(h, src, grouped, q, n_q, what, S);
+    if (rc) return rc;
+    const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped);
+    const uint64_t G = S.n_groups;
+    const uint64_t want = S.n_planes * G * S.n_entities * n_q * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "%s quantiles are %llu bytes, got %llu", what, (unsigned long long)want,
+                    (unsigned long long)bytes);
     const uint64_t triples = S.n_planes * G * S.n_entities;
     h->quantile_read_sum = triples;  // the small-group routes read every triple once
     const uint64_t scratch = quantile_scratch_bytes(S, t.stats);
@@ -1553,6 +1568,117 @@ int b200_sixdof_state_group_quantiles(b200_sixdof *h, const double *q, uint32_t 
 }
 
 double b200_sixdof_quantile_reads(const b200_sixdof *h) { return h ? h->quantile_reads : 0.0; }
+
+// ---- world-sharded quantiles (quantile_kernels.cu: sharded_quantile_round) ----
+
+// The write generation of what a sharded call over `outcomes` (else the ring or state rows) reads: the outcome planes
+// are rewritten from the run summaries by every outcome entry, so a summary start or fold changes them too.
+static uint64_t rows_generation(const b200_sixdof *h, bool outcomes)
+{
+    return h->rows_gen + (outcomes ? h->sum_gen : 0);
+}
+
+int b200_sixdof_sharded_quantiles_begin(b200_sixdof *h, uint32_t source, int grouped, const double *q, uint32_t n_q,
+                                        uint64_t *max_round_bytes)
+{
+    static const char *const names[3] = {"trajectory", "state", "outcome"};
+    static const Rows rows[3] = {Rows::ring, Rows::state, Rows::outcomes};
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (source > B200_QUANTILE_OUTCOMES)
+        return fail(B200_ERR_INVALID_ARGUMENT, "quantile source %u: B200_QUANTILE_RING, _STATE or _OUTCOMES", source);
+    if (!max_round_bytes) return fail(B200_ERR_INVALID_ARGUMENT, "null max_round_bytes");
+    h->sq.active = false;  // a call still pending is discarded
+    const Rows src = rows[source];
+    QuantileParams S{};
+    int rc = quantile_params(h, src, grouped != 0, q, n_q, names[source], S);
+    if (rc) return rc;
+    const b200_sixdof::GroupTables &t = reduction_tables(h, src, grouped != 0);
+    const uint64_t table_bytes = S.n_planes * S.n_groups * S.n_entities * n_q * 8ull;
+    const uint64_t scratch = sharded_quantile_scratch_bytes(S, S.n_groups);
+    rc = src == Rows::outcomes ? write_outcomes(h) : refresh_channels(h, src == Rows::ring);
+    if (!rc) rc = grow_device(h, &h->sq_scratch, &h->sq_scratch_bytes, std::max<uint64_t>(scratch + table_bytes, 8));
+    if (rc) return rc;
+    b200_sixdof::ShardedQuantiles &c = h->sq;
+    c.Q.S = S;
+    c.Q.S.out = (double *)((char *)h->sq_scratch + scratch);
+    c.Q.table = t.stats;
+    c.Q.scratch = h->sq_scratch;
+    c.Q.slice = 0;
+    c.Q.level = -1;
+    c.Q.reads = 0;
+    c.outcomes = src == Rows::outcomes;
+    c.gen = rows_generation(h, c.outcomes);
+    c.partial_bytes = 0;
+    c.max_round = sharded_quantile_round_bytes(S, S.n_groups);
+    c.table_bytes = table_bytes;
+    c.triples = S.n_planes * S.n_groups * S.n_entities;
+    c.ready = false;
+    c.active = true;
+    *max_round_bytes = c.max_round;
+    return B200_OK;
+}
+
+// the checks every round and end make first: a call begun, on the rows it began on
+static int sharded_quantiles_pending(b200_sixdof *h, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (!h->sq.active) return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles %s without a begin", what);
+    if (h->sq.gen != rows_generation(h, h->sq.outcomes)) {
+        h->sq.active = false;
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles %s: the handle's rows changed since the begin", what);
+    }
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    return B200_OK;
+}
+
+int b200_sixdof_sharded_quantiles_round(b200_sixdof *h, const void *reduced, uint64_t reduced_bytes, void *partial,
+                                        uint64_t partial_cap, uint64_t *partial_bytes)
+{
+    int rc = sharded_quantiles_pending(h, "round");
+    if (rc) return rc;
+    b200_sixdof::ShardedQuantiles &c = h->sq;
+    if (c.ready) return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles: the table is ready, call the end");
+    if (reduced_bytes != c.partial_bytes)
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles: %llu reduced bytes, the last round sent %llu",
+                    (unsigned long long)reduced_bytes, (unsigned long long)c.partial_bytes);
+    if (reduced_bytes && !reduced) return fail(B200_ERR_INVALID_ARGUMENT, "null reduced words");
+    if (!partial_bytes) return fail(B200_ERR_INVALID_ARGUMENT, "null partial_bytes");
+    if (partial_cap < c.max_round || (c.max_round && !partial))
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles: a partial of %llu bytes, the begin asked for %llu",
+                    (unsigned long long)partial_cap, (unsigned long long)c.max_round);
+    CU(h, cudaSetDevice(h->device));
+    int launches = 0;
+    uint64_t out = 0;
+    const cudaError_t e = sharded_quantile_round(c.Q, reduced, partial, &out, &launches, h->stream);
+    h->timings.kernel_launches += (uint64_t)launches;
+    if (e != cudaSuccess) {
+        c.active = false;
+        return cuda_fail(h, e, "sharded_quantile_round");
+    }
+    c.partial_bytes = *partial_bytes = out;
+    c.ready = out == 0;
+    return B200_OK;
+}
+
+int b200_sixdof_sharded_quantiles_end(b200_sixdof *h, void *dst, uint64_t bytes)
+{
+    int rc = sharded_quantiles_pending(h, "end");
+    if (rc) return rc;
+    b200_sixdof::ShardedQuantiles &c = h->sq;
+    if (!c.ready) return fail(B200_ERR_INVALID_ARGUMENT, "sharded quantiles: end before the last round");
+    if (bytes != c.table_bytes)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "sharded quantiles are %llu bytes, got %llu",
+                    (unsigned long long)c.table_bytes, (unsigned long long)bytes);
+    if (bytes && !dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    CU(h, cudaSetDevice(h->device));
+    if (bytes) {
+        CU(h, cudaMemcpyAsync(dst, c.Q.S.out, bytes, cudaMemcpyDefault, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+    }
+    h->quantile_reads = bytes && c.triples ? (double)c.Q.reads / (double)c.triples : 0.0;
+    c.active = false;
+    return B200_OK;
+}
 
 // Covariance of the selection `planes` (each < width) of every sample over the worlds, per group when `grouped`
 // (cov_kernels.cu), into dst: the groups checked, then the handle's status, then the selection, then `bytes`.
@@ -1846,6 +1972,7 @@ static int summary_ready(b200_sixdof *h, const char *what)
 // recomputed first where the fold reads one: with extrema, or a threshold, moment or dwell on a channel plane.
 static int run_summary_fold(b200_sixdof *h, bool ring, uint64_t tick0, uint64_t tick_step)
 {
+    ++h->sum_gen;
     SummaryParams S = summary_params(h);
     const StatsParams P = ensemble_rows(h, ring);
     bool channel = false;
@@ -1885,6 +2012,7 @@ static int check_condition(const b200_sixdof *h, const b200_threshold &t, const 
 // handle's stream.
 static int summary_start(b200_sixdof *h, const b200_summary_spec &sp, const char *nothing)
 {
+    ++h->sum_gen;
     CU(h, cudaSetDevice(h->device));
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (sp.n_thresholds > B200_MAX_THRESHOLDS)
@@ -2132,6 +2260,7 @@ int b200_sixdof_set_channels(b200_sixdof *h, const b200_channel *c, uint32_t n)
     h->chan_ring = ring;
     h->chan_state = state;
     h->channels.assign(c, c + n);
+    ++h->rows_gen;
     return B200_OK;
 }
 
@@ -2326,6 +2455,7 @@ int b200_sixdof_set_outcomes(b200_sixdof *h, const b200_outcome *o, uint32_t n)
             return cuda_fail(h, e, "cudaMemcpy(outcome values)");
         }
     }
+    ++h->rows_gen;
     if (h->out_planes) CU(h, cudaFree(h->out_planes));
     h->out_planes = planes;
     h->ld_o = ld_o;
@@ -2400,6 +2530,7 @@ int b200_sixdof_trajectory_reset(b200_sixdof *h)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
     h->ticks_done = 0;
+    ++h->rows_gen;
     return B200_OK;
 }
 

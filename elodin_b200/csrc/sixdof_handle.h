@@ -60,6 +60,18 @@ struct b200_sixdof {
     uint64_t staging_bytes = 0;
     double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
+    // a world-sharded quantile call (b200_sixdof_sharded_quantiles_*) between begin and end: its state, the write
+    // generation of the rows at begin (rows_gen: bumped by every entry that changes what a reduction reads), and its own
+    // device scratch (not the staging buffer, which the other reductions reuse between its rounds)
+    struct ShardedQuantiles {
+        bool active = false, ready = false, outcomes = false;
+        uint64_t gen = 0, partial_bytes = 0, max_round = 0, table_bytes = 0, triples = 0;
+        b200::QuantileShard Q;
+    } sq;
+    uint64_t rows_gen = 0;
+    uint64_t sum_gen = 0;  // bumped by every summary start and fold: what the outcome planes are computed from
+    double *sq_scratch = nullptr;
+    uint64_t sq_scratch_bytes = 0;
     // the group tables of one split of the worlds, each with its device copy: the statistics' (stats_kernels.cu), the
     // quantiles' route order over the same worlds (quantile_order, quantile_kernels.cu) and the covariance's own
     // chunking (cov_group_table, cov_kernels.cu)
@@ -174,6 +186,7 @@ inline bool is_device_pointer(const void *p, int *device = nullptr)
 // n ticks happened: the trajectory slot base, the Tick column and the tick counter of the timings.
 inline void advance_ticks(b200_sixdof *h, uint64_t n)
 {
+    ++h->rows_gen;
     h->ticks_done += n;
     h->tick += n;
     h->timings.ticks += n;

@@ -257,6 +257,24 @@ uint64_t quantile_scratch_bytes(const QuantileParams &S, const std::vector<World
 cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGroup> &table,
                              const std::vector<uint32_t> &order, void *scratch, int *launches,
                              unsigned long long *reads, cudaStream_t s);
+// A rank's part of a world-sharded quantile call between its rounds (b200_sixdof_sharded_quantiles_*): the radix select
+// over every group of `table`, slice by slice, each pass's counters summed over the ranks before its plan runs.
+struct QuantileShard {
+    QuantileParams S;               // S.out: the whole table, in device memory
+    std::vector<WorldGroup> table;  // the rank's part of every group (only o and n are read)
+    void *scratch = nullptr;        // sharded_quantile_scratch_bytes(S, table.size())
+    uint64_t slice = 0;             // the slice the rounds are in
+    int level = -1;                 // the pass whose words the last round sent (0: the counts), -1: none
+    unsigned long long reads = 0;   // reads of the planes summed over the triples, once the last round is made
+};
+// device scratch of a sharded call over n_groups groups (0 without a triple), and its largest round in bytes
+uint64_t sharded_quantile_scratch_bytes(const QuantileParams &S, uint64_t n_groups);
+uint64_t sharded_quantile_round_bytes(const QuantileParams &S, uint64_t n_groups);
+// One round on s, returning once the round's words are in `partial` (host or device memory): the sums of the last
+// round's words from `reduced` (nothing before the first round), then the launches up to the next round's words
+// (*partial_bytes; 0 once S.out holds the table).  *launches: the kernels it launched.
+cudaError_t sharded_quantile_round(QuantileShard &Q, const void *reduced, void *partial, uint64_t *partial_bytes,
+                                   int *launches, cudaStream_t s);
 
 // Ensemble covariance over the world axis (cov_kernels.cu).  One entry (a, b) of a group over a set of worlds: the
 // count n, the means of planes a and b, and the co-moment m = sum (x_a - mean_a)(x_b - mean_b); while n = 0 the other

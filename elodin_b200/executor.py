@@ -325,6 +325,63 @@ class B200Exec:
         """Reads of the reduced planes the last quantile call made, averaged over its groups."""
         return float(self._L.b200_sixdof_quantile_reads(self._h))
 
+    # ---- world-sharded quantiles: the quantile tables of the union of every rank's worlds, in rounds -------------
+    @staticmethod
+    def _words(buf) -> tuple:
+        """A host (numpy) or device (torch) buffer, or None -> (pointer, bytes)."""
+        if buf is None:
+            return None, 0
+        if isinstance(buf, np.ndarray):
+            if not buf.flags.c_contiguous:
+                raise ValueError("sharded quantile words: a C-contiguous buffer")
+            return buf.ctypes.data, buf.nbytes
+        return int(buf.data_ptr()), int(buf.numel()) * int(buf.element_size())
+
+    def sharded_quantiles_shape(self, q, source: str = "ring", groups: bool = False) -> tuple:
+        """The shape of the table b200_sixdof_sharded_quantiles_end writes: that of trajectory_ / state_ /
+        outcome_[group_]quantiles(q) (`source` "ring", "state" or "outcomes")."""
+        n_q = np.atleast_1d(np.asarray(q, dtype=np.float64)).size
+        G = (self.world_groups,) if groups else ()
+        if source == "ring":
+            n, E, W = self._rows(ring=True)
+            return (n,) + G + (E, W, n_q)
+        if source == "state":
+            return G + self._rows(ring=False) + (n_q,)
+        if source == "outcomes":
+            return G + (self.n_outcomes, n_q)
+        raise ValueError(f"quantile source {source!r}: 'ring', 'state' or 'outcomes'")
+
+    def sharded_quantiles_begin(self, q, source: str = "ring", groups: bool = False) -> int:
+        """Begin this rank's part of a world-sharded quantile call (b200_sixdof_sharded_quantiles_begin): the source,
+        grouping and levels are fixed here.  Returns the largest round in bytes (the partial buffer's least size)."""
+        if source not in _lib.QUANTILE_SOURCES:
+            raise ValueError(f"quantile source {source!r}: 'ring', 'state' or 'outcomes'")
+        lv = self._levels(q)
+        mx = C.c_uint64(0)
+        _lib.check(self._L.b200_sixdof_sharded_quantiles_begin(self._h, _lib.QUANTILE_SOURCES[source], int(bool(groups)),
+                                                                lv[0], lv[1], C.byref(mx)))
+        self._sq_shape = self.sharded_quantiles_shape(q, source, groups)
+        return int(mx.value)
+
+    def sharded_quantiles_round(self, reduced, reduced_bytes: int, partial) -> int:
+        """One round: `reduced` holds the ranks' u32 sum of this rank's last partial (None, 0 on the first round),
+        `partial` (at least the begin's bytes; numpy or a torch CUDA tensor) receives this round's words.  Returns their
+        size in bytes; 0: the table is ready (sharded_quantiles_end)."""
+        rp, _ = self._words(reduced)
+        pp, pcap = self._words(partial)
+        out = C.c_uint64(0)
+        _lib.check(self._L.b200_sixdof_sharded_quantiles_round(self._h, C.c_void_p(rp), int(reduced_bytes),
+                                                                C.c_void_p(pp), pcap, C.byref(out)))
+        return int(out.value)
+
+    def sharded_quantiles_end(self) -> np.ndarray:
+        """The table of the call, with the shape and bits of the unsharded entry on one handle holding every rank's
+        worlds in rank order."""
+        shape = getattr(self, "_sq_shape", ())
+        out = np.empty(shape)
+        _lib.check(self._L.b200_sixdof_sharded_quantiles_end(self._h, C.c_void_p(out.ctypes.data), out.nbytes))
+        return out
+
     # ---- ensemble covariance (co-moments of a plane selection over the world axis, on the device) --------------
     @staticmethod
     def _selection(planes) -> tuple:
@@ -409,8 +466,8 @@ class B200Exec:
 
     def trajectory_group_quantiles(self, q) -> np.ndarray:
         """trajectory_quantiles(q) per group: [samples, G, n_entities, width, n_q]; group g's quantiles have the bits of
-        trajectory_quantiles(q) on a batch of exactly its worlds (NaN for an empty group).  Like the ungrouped tables,
-        they do not merge across the ranks of a world-sharded campaign: each rank gets its own."""
+        trajectory_quantiles(q) on a batch of exactly its worlds (NaN for an empty group).  A world-sharded campaign
+        reduces them over every rank's worlds with sharding.gather_quantiles(ex, q, "ring", groups=True)."""
         lv = self._levels(q)
         n, E, W = self._rows(ring=True)
         return self._reduce("group_quantiles", True, lv, (n, self.world_groups, E, W, lv[1]))

@@ -115,6 +115,123 @@ def gather_histograms(table, group=None) -> np.ndarray:
     return merge_histograms(_all_gather_tables(table, group))
 
 
+def all_reduce_min(value: int, group=None) -> int:
+    """The least of every rank's integer `value` (on a CUDA tensor for NCCL groups, host memory for gloo)."""
+    import torch
+    import torch.distributed as dist
+
+    t = torch.tensor([int(value)], dtype=torch.int64, device="cuda" if dist.get_backend(group) == "nccl" else "cpu")
+    dist.all_reduce(t, op=dist.ReduceOp.MIN, group=group)
+    return int(t.item())
+
+
+_ARGUMENT_ERROR = -1  # the status a rank sends for a source or levels it cannot use
+
+
+def _quantile_descriptor(ex, levels: np.ndarray, source: str, groups: bool, status: int) -> List[int]:
+    """What every rank of a sharded quantile call must agree on, as int64 words: source, grouping, the table's shape
+    (groups, entities, width, samples, outcomes, levels), the levels' bits; then the rank's worlds and begin's status."""
+    from . import _lib
+
+    try:
+        shape = list(ex.sharded_quantiles_shape(levels, source, groups))
+    except Exception:  # noqa: BLE001 - a rank that cannot even describe its table differs from the others
+        shape = []
+    shape = (shape + [-1] * 6)[:6]
+    bits = np.zeros(_lib.MAX_QUANTILES, dtype=np.float64)
+    bits[: min(levels.size, _lib.MAX_QUANTILES)] = levels[: _lib.MAX_QUANTILES]
+    return ([(_lib.QUANTILE_SOURCES.get(source, -1) if isinstance(source, str) else -1), int(bool(groups)), int(levels.size)] + shape
+            + [int(b) for b in bits.view(np.int64)] + [int(ex.n_worlds), int(status)])
+
+
+def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=None) -> np.ndarray:
+    """Quantile tables of a world-sharded campaign, exact over every rank's worlds: every rank passes its executor (its
+    own worlds; with `groups`, the global groups cut to them by shard_groups), the same levels `q` and the same source
+    ("ring", "state" or "outcomes"); the ranks run b200_sixdof_sharded_quantiles_* in lockstep, summing each round's
+    u32 words with one all-reduce (on a CUDA buffer for NCCL groups, host memory for gloo).  Every rank returns the table
+    of trajectory_ / state_ / outcome_[group_]quantiles(q) on one executor holding every rank's worlds in rank order,
+    bit for bit.  Before the first round the ranks all-gather a descriptor of their calls; a disagreement, a global
+    world count of 2^32 or more, or any rank's failure (then or in a later round) raises the same error on every
+    rank."""
+    import torch.distributed as dist
+
+    from . import _lib
+
+    # An argument this rank cannot use still goes through the descriptor exchange as a failed status, so that a rank
+    # whose arguments differ from the others' raises with them instead of leaving them waiting.
+    arg_err, levels = None, np.zeros(0)
+    try:
+        if source not in _lib.QUANTILE_SOURCES:
+            raise ValueError(f"quantile source {source!r}: 'ring', 'state' or 'outcomes'")
+        levels = np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
+    except (TypeError, ValueError) as e:
+        arg_err = e
+    if not (dist.is_available() and dist.is_initialized()):
+        if arg_err is not None:
+            raise arg_err
+        raise RuntimeError("sharding.gather_quantiles needs an initialized torch.distributed process group")
+    import torch
+
+    cuda = dist.get_backend(group) == "nccl"
+    dev = "cuda" if cuda else "cpu"
+    status, err, max_round = (_ARGUMENT_ERROR, arg_err, 0) if arg_err is not None else (0, None, 0)
+    if arg_err is None:
+        try:
+            max_round = ex.sharded_quantiles_begin(levels, source, groups)
+        except _lib.B200Error as e:
+            status, err = int(e.code), e
+    mine = torch.tensor(_quantile_descriptor(ex, levels, source, groups, status), dtype=torch.int64, device=dev)
+    every = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(every, mine, group=group)
+    every = [d.cpu().numpy() for d in every]
+    failed = [r for r, d in enumerate(every) if d[-1] != 0]
+    if failed:
+        if err is not None:
+            raise err
+        r, code = failed[0], int(every[failed[0]][-1])
+        if code == _ARGUMENT_ERROR:
+            raise ValueError(f"sharded quantiles: rank {r} passed a source or levels it cannot use")
+        raise _lib.B200Error(code, f"sharded quantiles: rank {r} could not begin (code {code})")
+    differ = [r for r, d in enumerate(every) if not np.array_equal(d[:-2], every[0][:-2])]
+    if differ:
+        raise ValueError(f"sharded quantiles: rank {differ[0]} differs from rank 0 in source, grouping, levels or table "
+                         f"shape (descriptors {every[0][:9].tolist()} and {every[differ[0]][:9].tolist()})")
+    n_worlds = sum(int(d[-2]) for d in every)
+    if n_worlds >= 1 << 32:
+        raise ValueError(f"sharded quantiles: {n_worlds} worlds in all, at most 2^32 - 1")
+
+    def settle():
+        # NCCL works on its own stream and only orders torch's current stream after it; the library reads and writes
+        # the buffer on the handle's stream, so the host waits for the buffer before every round call
+        if cuda:
+            torch.cuda.current_stream().synchronize()
+
+    # int32 words: a two's-complement sum wraps exactly as the u32 sum the rounds are defined by
+    partial = torch.zeros(max(max_round // 4, 1), dtype=torch.int32, device=dev)
+    settle()
+    nbytes = 0
+    while True:
+        ok = 1
+        try:
+            nbytes = ex.sharded_quantiles_round(partial if nbytes else None, nbytes, partial)
+        except _lib.B200Error as e:
+            ok, err = 0, e
+        # status and round size in one collective: a failure, or ranks whose rounds differ, raise on every rank
+        word = torch.tensor([ok, nbytes, -nbytes], dtype=torch.int64, device=dev)
+        dist.all_reduce(word, op=dist.ReduceOp.MIN, group=group)
+        ok_all, least, most = int(word[0].item()), int(word[1].item()), -int(word[2].item())
+        if not ok_all:
+            raise err if err is not None else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                                             "sharded quantiles: a round failed on another rank")
+        if least != most:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"sharded quantiles: the ranks' rounds differ ({least} to "
+                                 f"{most} bytes): their rows or arguments are not those of one campaign")
+        if nbytes == 0:
+            return ex.sharded_quantiles_end()
+        dist.all_reduce(partial[: nbytes // 4], op=dist.ReduceOp.SUM, group=group)
+        settle()
+
+
 def total_entity_steps(local_entity_steps: int, group=None) -> int:
     import torch
     import torch.distributed as dist

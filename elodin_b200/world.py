@@ -441,7 +441,8 @@ class World:
               covariance: Optional[Sequence] = None, histograms: Optional[Sequence["Histogram"]] = None,
               groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
               channels: Optional[Sequence["Channel"]] = None, moments: Optional[Sequence] = None,
-              dwells: Optional[Sequence["Threshold"]] = None, outcomes: Optional[Sequence["Outcome"]] = None) -> "Exec":
+              dwells: Optional[Sequence["Threshold"]] = None, outcomes: Optional[Sequence["Outcome"]] = None,
+              process_group=None) -> "Exec":
         """`ensemble=True` records statistics over the world axis instead of per-world rows (see `Exec.ensemble`):
         the run stays on the device at any batch size.  `ensemble_ring` = telemetry samples the device ring holds
         between two reductions (default: as many as fit in 256 MiB, at least one).  With ensemble=True, `extrema=True`
@@ -473,7 +474,13 @@ class World:
         input or the final state) or host values, and reduces it over the worlds on the device when asked
         (`Exec.outcome_stats`, `outcome_quantiles`, `outcome_covariance`, `outcome_histogram`, each per group with
         `groups=True`): apogee percentiles per sweep point, an impact ellipse, an event probability, input-to-outcome
-        correlations, without a per-world table reaching the host."""
+        correlations, without a per-world table reaching the host.  `process_group` (a torch.distributed group, with
+        ensemble=True and quantiles or outcomes) makes this Exec one rank of a world-sharded campaign whose quantile
+        tables are collective: every rank builds over its own worlds (`sharding.shard_worlds`, its groups cut by
+        `sharding.shard_groups`) and `Exec.quantiles` (grouped or not, row 0 included) and `Exec.outcome_quantiles` are
+        reduced over every rank's worlds (`sharding.gather_quantiles`), exact, the same on every rank; every rank must
+        then record and ask for them together.  The ring capacity becomes the ranks' least, so that every rank reduces at
+        the same ticks.  The other tables stay per rank, merged with the other gather helpers of `sharding`."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
             raise _lib.B200Error(
                 _lib.ERR_UNSUPPORTED,
@@ -482,7 +489,7 @@ class World:
             math = "fast"
         return Exec(self, system, simulation_rate, telemetry_rate, max_ticks, math, n_worlds, device, world_params, resident,
                     ensemble, ensemble_ring, extrema, thresholds, quantiles, covariance, histograms, groups, retain,
-                    channels, moments, dwells, outcomes)
+                    channels, moments, dwells, outcomes, process_group)
 
     def run(self, system: System, simulation_rate: float = 120.0, generate_real_time: bool = False,
             telemetry_rate: Optional[float] = None, default_playback_speed: float = 1.0,
@@ -1028,6 +1035,8 @@ class _Series(np.ndarray):
 class Exec:
     """`PyExec` (libs/nox-py/src/exec.rs:96-173): owns the world + a B200Exec."""
 
+    _pg = None  # World.build(..., process_group=): the group the quantile tables are reduced over, None = this rank
+
     def __init__(self, world: World, system: System, simulation_rate: float, telemetry_rate: Optional[float],
                  max_ticks: Optional[int], math: str, n_worlds: int, device: int,
                  world_params: Optional[Dict[str, np.ndarray]], resident: Optional[bool] = None,
@@ -1036,7 +1045,8 @@ class Exec:
                  covariance: Optional[Sequence] = None, histograms: Optional[Sequence[Histogram]] = None,
                  groups: Optional[Sequence[int]] = None, retain: Optional[Sequence[int]] = None,
                  channels: Optional[Sequence[Channel]] = None, moments: Optional[Sequence] = None,
-                 dwells: Optional[Sequence[Threshold]] = None, outcomes: Optional[Sequence[Outcome]] = None):
+                 dwells: Optional[Sequence[Threshold]] = None, outcomes: Optional[Sequence[Outcome]] = None,
+                 process_group=None):
         systems = _flatten(system)
         six = [s for s in systems if isinstance(s, SixDof)]
         if len(six) != 1:
@@ -1076,11 +1086,16 @@ class Exec:
         given = [name for name, value in (("extrema", extrema or None), ("thresholds", thresholds or None),
                                           ("quantiles", quantiles), ("covariance", covariance), ("histograms", histograms),
                                           ("groups", groups), ("retain", retain), ("channels", channels),
-                                          ("moments", moments), ("dwells", dwells), ("outcomes", outcomes))
+                                          ("moments", moments), ("dwells", dwells), ("outcomes", outcomes),
+                                          ("process_group", process_group))
                  if value is not None]
         if given and not ensemble:
             msg = f"{', '.join(given)}: need World.build(..., ensemble=True)"
             raise ValueError(msg) if given == ["groups"] else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, msg)
+        if process_group is not None and quantiles is None and outcomes is None:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "process_group makes the quantile tables collective: build "
+                                 "with World.build(..., ensemble=True, quantiles=[...]) or outcomes=[...]")
+        self._pg = process_group
         self.groups = _world_groups(groups, self.n_worlds) if groups is not None else None
         self._retain = _retained_worlds(retain, self.n_worlds, len(bodies)) if retain is not None else None
         self._channels = _channel_list(channels) if channels is not None else []
@@ -1167,6 +1182,10 @@ class Exec:
             ld = (n_bodies + 127) // 128 * 128
             cap = ensemble_ring if ensemble_ring is not None else _ENSEMBLE_RING_BYTES // max((_lib.ROW_PLANES + n_c) * ld * 8, 1)
             self._ring_cap = int(max(1, min(4096, cap)))
+            if self._pg is not None:  # every rank reduces at the same ticks: the ranks' least capacity
+                from .sharding import all_reduce_min
+
+                self._ring_cap = all_reduce_min(self._ring_cap, self._pg)
         elif resident and n_bodies:
             ld = (n_bodies + 127) // 128 * 128
             self._ring_cap = int(max(1, min(4096, (64 << 20) // (25 * ld * 8))))
@@ -1280,7 +1299,13 @@ class Exec:
         be = self.backend
         for name, blocks in self._ens_rows.items():
             args = self._ens_args[name.removeprefix("group_")]
-            rows = getattr(be, f"trajectory_{name}")(*args) if ring else getattr(be, f"state_{name}")(*args)[None]
+            if self._pg is not None and name.endswith("quantiles"):  # collective: over every rank's worlds
+                from .sharding import gather_quantiles
+
+                rows = gather_quantiles(be, *args, "ring" if ring else "state", name == "group_quantiles", self._pg)
+                rows = rows if ring else rows[None]
+            else:
+                rows = getattr(be, f"trajectory_{name}")(*args) if ring else getattr(be, f"state_{name}")(*args)[None]
             blocks.append(rows)
         if self._summaries:
             (be.summary_add_trajectory if ring else be.summary_add_state)()
@@ -1568,7 +1593,7 @@ class Exec:
         quantiles=...) in the order given -- the layout of np.quantile(rows_k, q, axis=0) stacked over rows.  NaN where no
         world is finite.  The values are order statistics of the worlds (and one fixed lerp): exact, not estimates.
         With groups=True (World.build(..., groups=[...])) -> [rows, G, n_q, width], over the worlds of each group.
-        Quantile tables do not merge across the ranks of a world-sharded campaign: each rank has its own."""
+        Built with a `process_group`, the rows are over every rank's worlds (World.build)."""
         t = self._table("quantiles", "quantiles", groups)
         row, (lo, hi) = self._sampled_row(pair, "ensemble quantiles")
         return np.ascontiguousarray(np.swapaxes(t[..., row, lo:hi, :], -1, -2))  # from [rows, (G,) width, n_q]
@@ -1772,10 +1797,16 @@ class Exec:
 
     def outcome_quantiles(self, q, groups: bool = False) -> np.ndarray:
         """[n_q, P] (or [G, n_q, P] with groups=True): numpy's linear quantiles at the levels `q` of every outcome
-        over the worlds whose value is finite, exact.  Quantile tables do not merge across ranks."""
+        over the worlds whose value is finite, exact.  Built with a `process_group`, over every rank's worlds (a
+        collective: every rank calls it with the same levels)."""
         self._outcome_ready("outcome_quantiles", groups)
         lv = _quantile_levels(list(np.atleast_1d(q)))
-        t = self.backend.outcome_group_quantiles(lv) if groups else self.backend.outcome_quantiles(lv)
+        if self._pg is not None:
+            from .sharding import gather_quantiles
+
+            t = gather_quantiles(self.backend, lv, "outcomes", groups, self._pg)
+        else:
+            t = self.backend.outcome_group_quantiles(lv) if groups else self.backend.outcome_quantiles(lv)
         return np.ascontiguousarray(np.swapaxes(t, -1, -2))
 
     def outcome_covariance(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, object]:

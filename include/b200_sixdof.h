@@ -337,8 +337,9 @@ int b200_stats_merge(const double *parts, uint32_t n_parts, uint64_t n_groups, d
  * Route: up to 8192 worlds each group is sorted in shared memory (one read of the planes, no scratch); above that, a
  * radix select reads the planes at most 8 times on any data (3 on continuous data).  It needs about 198 KB of device
  * scratch per group and runs the groups in slices of about 1350 (a fixed launch sequence per slice), so the scratch,
- * which lives in the handle's staging buffer, is at most 256 MiB whatever the ring or entity count.  Quantile tables do NOT merge across
- * ranks (unlike b200_stats_merge): a world-sharded campaign gets one table per rank.
+ * which lives in the handle's staging buffer, is at most 256 MiB whatever the ring or entity count.  Quantile tables
+ * cannot be merged after the fact (unlike b200_stats_merge): a world-sharded campaign reduces them together, in rounds,
+ * with b200_sixdof_sharded_quantiles_begin / _round / _end below.
  * Both entries return the handle's sticky status if it has failed; they take 1 .. B200_MAX_QUANTILES levels
  * q[0 .. n_q) (any order, duplicates allowed; NaN or outside [0, 1]: B200_ERR_INVALID_ARGUMENT), run on the handle's
  * stream, return once dst is filled, take host or device dst, count their launches in timings.kernel_launches (1 below
@@ -352,6 +353,52 @@ int b200_sixdof_state_quantiles(b200_sixdof *h, const double *q, uint32_t n_q, v
 /* reads of the reduced planes the last quantile call (grouped or not) made, averaged over its (world group, plane,
  * entity) triples (1 on the shared-memory routes) */
 double b200_sixdof_quantile_reads(const b200_sixdof *h);
+
+/* ---- world-sharded quantiles: the quantile tables above (ring, state or outcomes, grouped or not) of a campaign whose
+ * worlds are split over several handles ("ranks", usually one per GPU), exact, over the union of their worlds.  Every
+ * group takes the radix select (quantile_kernels.cu); its passes count keys into integer histograms, which add exactly
+ * across ranks, and its plan is a function of those counts alone.  So the host drives rounds: each rank sends the u32
+ * words of a round (`partial`), the host sums them elementwise over the ranks with one all-reduce (SUM of unsigned 32-bit
+ * words, over any channel: NCCL, gloo, MPI, or a test adding arrays), and hands each rank the sums (`reduced`) in its next
+ * round call.  Every rank plans from the same sums, so every rank makes the same rounds, with the same sizes, and ends on
+ * the same order statistics: the table equals, bit for bit (the sign of a zero included: totalOrder keys), the matching
+ * unsharded entry on one handle holding the ranks' worlds in rank order, for any rank count >= 1 and any split.
+ *   Rounds.  The groups run in the unsharded entries' slices (the 256 MiB scratch cap) inside the round sequence.  A
+ *   slice takes at most 8 rounds: a count round (one u32 per triple of the slice), then at most 7 histogram rounds (per
+ *   triple of the slice 2^14 u32 counters and 32 u64 keys, as 64 u32 words), fewer where every rank of a slice is
+ *   finished early; a range whose global count is 1 is finished by copying its key (the rank that holds it) into words
+ *   the other ranks leave 0.  b200_sixdof_quantile_reads, set by the end, counts per triple the count pass and every
+ *   pass with work for it.
+ *   Preconditions (a C host checks them itself; sharding.gather_quantiles does): every rank passes the same source,
+ *   grouping, levels, entity count, ring length and outcome count, a rank's groups are the global groups cut to its
+ *   worlds (the same G on every rank; a group may be empty on a rank), and the global world count is below 2^32.
+ *   Between begin and end the handle's rows must not change: a step, upload, invoke_batch, trajectory_reset,
+ *   set_channels, set_outcomes or set_world_groups (and for B200_QUANTILE_OUTCOMES a summary begin, start or add, which
+ *   the outcome planes are computed from) makes the next round or end fail with B200_ERR_INVALID_ARGUMENT (and discards
+ *   the call); any other reduction may run between rounds.  Writes through a b200_sixdof_device_plane pointer are not
+ *   seen by the handle: a host that writes planes that way between rounds gets a table of mixed rows.  The call's device scratch is its own, not the
+ *   staging buffer: about 66 KB per triple of the largest slice (at most about 90 MiB) plus the table. ---- */
+enum { B200_QUANTILE_RING = 0, B200_QUANTILE_STATE = 1, B200_QUANTILE_OUTCOMES = 2 };
+/* Checks what the matching quantile entry checks, in the same order (the groups when grouped, the outcomes for
+ * B200_QUANTILE_OUTCOMES, the sticky status, the levels), after B200_ERR_INVALID_ARGUMENT for a null handle, a source
+ * that is none of the three or a null max_round_bytes; discards a call still pending; fixes the source, grouping and
+ * levels of the call and writes its largest round in bytes (0: no triple, the first round ends the call). */
+int b200_sixdof_sharded_quantiles_begin(b200_sixdof *h, uint32_t source, int grouped, const double *q, uint32_t n_q,
+                                        uint64_t *max_round_bytes);
+/* One round: `reduced` = the ranks' elementwise sum of this rank's previous partial (NULL, 0 on the first call), host or
+ * device memory; writes the next round's words to `partial` (host or device memory, partial_cap >= begin's
+ * max_round_bytes) and their size to *partial_bytes, and returns once they are there (reduced and partial may be the
+ * same buffer: the sums are read first); *partial_bytes == 0: the table is ready.  The sums are read on the handle's
+ * stream, which is not ordered after other streams: a device `reduced` written by another stream (an NCCL all-reduce)
+ * must be complete before the call.  B200_ERR_INVALID_ARGUMENT, with the call left as it was, for reduced_bytes that is
+ * not the previous partial_bytes, a too small partial or a round after the last one; and, discarding it, for a round
+ * without a begin or after the rows changed. */
+int b200_sixdof_sharded_quantiles_round(b200_sixdof *h, const void *reduced, uint64_t reduced_bytes, void *partial,
+                                        uint64_t partial_cap, uint64_t *partial_bytes);
+/* dst (host or device): exactly the layout and size of the matching unsharded entry (trajectory_ / state_ /
+ * outcome_[group_]quantiles; else B200_ERR_VALUE_SIZE_MISMATCH).  B200_ERR_INVALID_ARGUMENT for an end without a begin,
+ * before the last round, or after the rows changed.  Ends the call. */
+int b200_sixdof_sharded_quantiles_end(b200_sixdof *h, void *dst, uint64_t bytes);
 
 /* ---- ensemble covariance: the joint spread of chosen components over the worlds, on the device.  A selection is
  * planes[0 .. n_p) of the B200_TRAJ_FULL sample layout (world_pos 0-6, world_vel 7-12, world_accel 13-18, force 19-24),
@@ -439,7 +486,8 @@ int b200_sixdof_state_histograms(b200_sixdof *h, const b200_histogram *specs, ui
  * block sort, above that the radix select.  A call launches once per sort route that has groups, plus 18 launches per
  * slice of the large groups' (group, plane, entity) triples (at most about 1350 triples a slice, whole (group, plane)
  * rows or entity ranges of one row); b200_sixdof_quantile_reads averages the reads over every (group, plane, entity).
- * An empty group gives NaN at every level.  Grouped quantile tables do not merge across ranks, as the ungrouped ones.
+ * An empty group gives NaN at every level.  Grouped quantile tables of a world-sharded campaign, with each rank's groups
+ * cut to its worlds, are reduced together with b200_sixdof_sharded_quantiles_begin (grouped = 1), as the ungrouped ones.
  * Covariance: group g is chunked as a batch of sizes[g] worlds would be, and an empty group is one chunk of no worlds,
  * with n = 0 and NaN after it.  A call launches one chunk launch, plus a merge launch where a group of the slice has
  * more than one chunk, per slice of groups and samples, slices keeping the chunk partials at most 256 MiB.  Grouped
