@@ -82,11 +82,16 @@ struct b200_comm {
         uint64_t owner_serial = 0, ld = 0;     // the handle the window was sized for (address + creation serial)
         double *base[B200_MAX_PEERS] = {};  // rank r's window as mapped here ([rank] = the local allocation)
         unsigned *ctr = nullptr;            // block counter of the push kernel (local)
+        // ticks exchanged through this window since attach: picks the parity half, is the value a push releases and
+        // what the waits compare against.  The window owns it, so that nothing done to the handle between calls (a
+        // trajectory reset sets ticks_done back to 0) can leave the delivery counters ahead of the count.
+        uint64_t seq = 0;
     } win;
 };
 
-// Layout of a peer window: X[2][6][ld] doubles (parity of the tick count; planes x y z vx vy vz of every row of
-// the world), then B200_MAX_PEERS uint64 delivery counters: flags[r] = ticks whose rows rank r has delivered here.
+// Layout of a peer window: X[2][6][ld] doubles (parity of the window's tick count `seq`; planes x y z vx vy vz of
+// every row of the world), then B200_MAX_PEERS uint64 delivery counters: flags[r] = the window tick count whose rows
+// rank r has delivered here.
 static inline uint64_t win_doubles(uint64_t ld) { return 2ull * 6ull * ld; }
 static inline size_t win_bytes(uint64_t ld) { return (size_t)(win_doubles(ld) * 8ull + B200_MAX_PEERS * 8ull + 64); }
 
@@ -401,6 +406,7 @@ int b200_comm_peer_attach(b200_comm *c, b200_sixdof *h)
     }
     w.owner = h;
     w.owner_serial = h->serial;
+    w.seq = 0; // the counters were zeroed with the window
     return B200_OK;
 }
 
@@ -430,6 +436,7 @@ void b200_comm_peer_detach(b200_comm *c)
     c->win.base[c->rank] = nullptr;
     c->win.ctr = nullptr;
     c->win.owner = nullptr;
+    c->win.seq = 0;
     (void)cudaGetLastError();
 }
 
@@ -439,7 +446,8 @@ void b200_comm_peer_detach(b200_comm *c)
 // other ranks' gravity needs — are exchanged with an in-place ncclAllGather per plane (one NCCL group per tick,
 // 6 planes x N/R doubles per rank over NVLink); the last tick of the call gathers every plane of WorldPos, WorldVel,
 // WorldAccel and Force so that each rank ends with the complete world.  Stage positions depend on the tick's input
-// state only (rk4.rs:85-111), so one exchange per tick suffices.
+// state only (rk4.rs:85-111), so one exchange per tick suffices.  The body launch samples the trajectory ring for
+// this rank's rows only and the ring is never gathered, so with R > 1 a handle with a ring is refused.
 int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
 {
     if (!h || !c) return fail(B200_ERR_INVALID_ARGUMENT, "null argument");
@@ -449,6 +457,9 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
         return fail(B200_ERR_UNSUPPORTED, "row sharding applies to one world with dense (all-pairs) edge_fold gravity (and no EGM08 effector)");
     const uint64_t N = h->desc.n_entities, R = (uint64_t)c->n_ranks;
     if (N % R != 0) return fail(B200_ERR_UNSUPPORTED, "row sharding needs n_entities (%llu) divisible by the rank count (%llu)", (unsigned long long)N, (unsigned long long)R);
+    if (R > 1 && h->traj)
+        return fail(B200_ERR_UNSUPPORTED, "row sharding over %llu ranks cannot keep a trajectory ring: each rank samples its own rows "
+                    "only; create the handle without a ring (trajectory_capacity = 0)", (unsigned long long)R);
     CU(h, cudaSetDevice(h->device));
     const uint64_t rows = N / R, i0 = rows * (uint64_t)c->rank;
     const bool exact = h->desc.math_mode == B200_MATH_EXACT;
@@ -461,7 +472,7 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
     unsigned long long *const flags = peer ? (unsigned long long *)(c->win.base[c->rank] + win_doubles(h->ld)) : nullptr;
     if (peer) {
         // the window's current-parity half <- the local world (covers uploads and non-sharded steps since the last call)
-        const unsigned long long T = h->ticks_done;
+        const unsigned long long T = c->win.seq;
         peer_fill_kernel<<<(unsigned)((N + 255) / 256), 256, 0, h->stream>>>(pos, vel, c->win.base[c->rank] + (T & 1ull) * 6ull * h->ld, flags,
                                                                              h->ld, (uint32_t)N, (int)R, T);
         CU(h, cudaGetLastError());
@@ -477,7 +488,7 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
     P.n_ticks = 1;
     for (uint64_t t = 0; t < n_ticks; ++t) {
         const bool last = t + 1 == n_ticks;
-        const unsigned long long T = h->ticks_done + t;
+        const unsigned long long T = c->win.seq; // window tick count (peer route only); the ring slot counts ticks_done
         if (peer) {
             // gravity reads every row's x, v from the window half of this tick count (the fold kernels touch planes
             // 4..6 of pos and 3..5 of vel only), once every rank's rows of that count have landed
@@ -490,7 +501,7 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
             }
         }
         CU(h, launch_graph_force(G, (int)h->desc.math_mode, true, h->stream));
-        P.tick0 = T;
+        P.tick0 = h->ticks_done + t;
         P.write_fa = (exact || last) ? 1u : 0u;
         CU(h, launch_body_step(P, (int)h->desc.integrator, (int)h->desc.math_mode, h->stream));
         h->timings.kernel_launches += 2;
@@ -507,6 +518,7 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
             peer_push_kernel<<<dim3((unsigned)((rows + 127) / 128), 6), 128, 0, h->stream>>>(a);
             CU(h, cudaGetLastError());
             h->timings.kernel_launches++;
+            ++c->win.seq; // per pushed tick: the counters never run ahead of the count, even if a later launch fails
             if (!last) continue;
         }
         // exchange over NCCL: in-place all-gather of the row slices, plane by plane (every tick without a peer window;

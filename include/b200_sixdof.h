@@ -766,7 +766,10 @@ int b200_sixdof_trajectory_allgather(b200_sixdof *h, b200_comm *c, const uint64_
 /* ONE world, source rows split over the ranks (SURVEY §8e second case; needs dense edge_fold gravity, n_worlds = 1,
  * n_entities divisible by the rank count).  Every rank creates the same handle and uploads the same initial state,
  * then calls this instead of b200_sixdof_step: per tick it folds and integrates its own rows and all-gathers the
- * rows' new position / velocity planes over NCCL; after the call every rank holds the complete world.
+ * rows' new position / velocity planes over NCCL; after the call every rank holds the complete world (WorldPos,
+ * WorldVel, WorldAccel, Force).  Each rank's tick samples the trajectory ring for its own rows only, and the ring is not
+ * gathered: with more than one rank, a handle with a trajectory ring is refused (B200_ERR_UNSUPPORTED); with one rank
+ * the ring is complete.  Any other entry (step, upload, invoke_batch, trajectory_reset) may run between two calls.
  * At N = 1024 replicas (every GPU integrates the whole world, no exchange) are faster — the tick is a ~10 us
  * latency chain and the exchange adds to it; row shards pay off for worlds of several thousand bodies
  * (DESIGN.md §7, measured by bench.py `multi_gpu.nbody_1024_single_world`). */
@@ -778,7 +781,8 @@ int b200_sixdof_step_row_sharded(b200_sixdof *h, b200_comm *c, uint64_t n_ticks)
  * attached, b200_sixdof_step_row_sharded runs per tick: wait until every rank's rows of this tick count have landed
  * here -> gravity from the window -> integrate own rows -> store the rows' new x, v straight into every rank's window
  * over NVLink and release each counter.  Only the call's last tick still all-gathers (attitude, WorldAccel, Force of
- * the other ranks' rows).  Results are bit-identical to the NCCL route and to replicas.
+ * the other ranks' rows).  Results are bit-identical to the NCCL route and to replicas.  The window counts its own
+ * ticks (zeroed by attach), so a trajectory reset or any other operation on the handle between calls is safe.
  * Collective: every rank of `c` calls attach (and detach / b200_comm_destroy) with handles of the same shape; one
  * window per communicator.  Returns B200_ERR_UNSUPPORTED on every rank if any rank cannot map the windows (no IPC
  * between the processes) — the NCCL route keeps working.  B200_ROW_PEER=0 ignores an attached window. */
