@@ -19,7 +19,8 @@ from . import _lib, effectors
 from ._lib import B200Error, B200ValueError, component_id
 from .effectors import (DragQuadratic, GravityConst, GravityEGM08, GravityEdges, GravityFrame, GravityJ2, Pipe, System, ThrustBody,
                         TorqueBodyFold, WrenchBody, WrenchWorld, all_pairs_edges)
-from .executor import B200Exec, device_count, merge_covariance, merge_histograms, merge_stats, pinned_empty, pinned_free
+from .executor import (B200Exec, device_count, merge_covariance, merge_histograms, merge_stats, merge_top_worlds, pinned_empty,
+                       pinned_free)
 from .world import (Annotated, Archetype, AxisAngle, Body, Channel, Component, ComponentType, Edge, EntityId, Exec, Force, Histogram,
                     HostSystem, Inertia, Integrator, Norm, Outcome, PrimitiveType, Quaternion, Seed, SimulationTick, SimulationTimeStep,
                     SpatialForce, SpatialInertia, SpatialMotion, SpatialTransform, StepContext, Threshold, World, WorldAccel,

@@ -75,7 +75,8 @@ SYMBOLS = [
     "b200_sixdof_set_outcomes", "b200_sixdof_outcomes", "b200_sixdof_outcome_values", "b200_sixdof_outcome_stats",
     "b200_sixdof_outcome_group_stats", "b200_sixdof_outcome_quantiles", "b200_sixdof_outcome_group_quantiles",
     "b200_sixdof_outcome_covariance", "b200_sixdof_outcome_group_covariance", "b200_sixdof_outcome_histograms",
-    "b200_sixdof_outcome_group_histograms",
+    "b200_sixdof_outcome_group_histograms", "b200_sixdof_outcome_top_worlds", "b200_sixdof_outcome_group_top_worlds",
+    "b200_sixdof_top_worlds_reads",
     "b200_sixdof_sharded_quantiles_begin", "b200_sixdof_sharded_quantiles_round", "b200_sixdof_sharded_quantiles_end",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
@@ -107,6 +108,7 @@ OUTCOME_MOMENT = 3
 OUTCOME_DWELL = 4
 OUTCOME_COLUMN = 5
 OUTCOME_VALUES = 6
+MAX_TOP_WORLDS = 1024  # worlds per record of the worst-worlds entries (b200_sixdof_outcome_top_worlds)
 COMM_ID_BYTES = 128
 
 
@@ -349,6 +351,10 @@ def lib():
     L.b200_sixdof_outcome_group_covariance.argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_outcome_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
     L.b200_sixdof_outcome_group_histograms.argtypes = [vp, C.POINTER(Histogram), u32, vp, u64]
+    L.b200_sixdof_outcome_top_worlds.argtypes = [vp, C.POINTER(u32), u32, u32, C.c_int, vp, u64]
+    L.b200_sixdof_outcome_group_top_worlds.argtypes = [vp, C.POINTER(u32), u32, u32, C.c_int, vp, u64]
+    L.b200_sixdof_top_worlds_reads.argtypes = [vp]
+    L.b200_sixdof_top_worlds_reads.restype = C.c_double
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -2526,6 +2526,67 @@ int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *s
     return run_histograms(h, Rows::outcomes, true, specs, n_specs, dst, bytes, "outcome");
 }
 
+// The k worst worlds of the selected outcome planes, per group when `grouped` (topk_kernels.cu), into dst: the outcome
+// set and groups checked, then the selection, k, largest and `bytes`; the handle's status in run_world_reduction.
+static int run_top_worlds(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
+                          void *dst, uint64_t bytes)
+{
+    int rc = reduction_ready(h, Rows::outcomes, grouped, "outcome top worlds");
+    if (rc) return rc;
+    CU(h, cudaSetDevice(h->device));
+    const uint32_t P = (uint32_t)h->outcomes.size();
+    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null top-worlds planes");
+    if (n_p == 0 || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u top-worlds planes: 1 to %u", n_p, P);
+    uint64_t seen = 0;
+    for (uint32_t j = 0; j < n_p; ++j) {
+        if (planes[j] >= P)
+            return fail(B200_ERR_INVALID_ARGUMENT, "top-worlds plane %u is %u: the outcome has %u planes", j, planes[j], P);
+        if (seen & (1ull << planes[j])) return fail(B200_ERR_INVALID_ARGUMENT, "top-worlds plane %u listed twice", planes[j]);
+        seen |= 1ull << planes[j];
+    }
+    if (k == 0 || k > B200_MAX_TOP_WORLDS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "top worlds k = %u: 1 to %u", k, B200_MAX_TOP_WORLDS);
+    if (largest != 0 && largest != 1) return fail(B200_ERR_INVALID_ARGUMENT, "top worlds largest = %d: 0 or 1", largest);
+    const uint64_t G = reduction_groups(h, grouped).size();
+    const uint64_t want = G * n_p * (1ull + 2ull * k) * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome top worlds are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    TopkParams S{};
+    S.planes = h->out_planes;
+    S.ld = h->ld_o;
+    S.n_p = n_p;
+    S.k = k;
+    S.largest = largest;
+    for (uint32_t j = 0; j < n_p; ++j) S.plane[j] = planes[j];
+    const b200_sixdof::GroupTables &t = reduction_tables(h, Rows::outcomes, grouped);
+    S.groups = t.stats_dev;
+    S.order = t.order_dev;
+    const uint64_t tasks = G * n_p;
+    h->topk_read_sum = tasks;  // the small-group routes read every task once
+    rc = run_world_reduction(h, Rows::outcomes, false, topk_scratch_bytes(S, t.stats), dst, bytes,
+                             [&](double *out, void *scratch, int *n) {
+                                 S.out = out;
+                                 return launch_top_worlds(S, t.stats, t.order, scratch, n, &h->topk_read_sum, h->stream);
+                             });
+    h->topk_reads = rc == B200_OK ? (double)h->topk_read_sum / (double)tasks : 0.0;
+    return rc;
+}
+
+int b200_sixdof_outcome_top_worlds(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
+                                   void *dst, uint64_t bytes)
+{
+    return run_top_worlds(h, false, planes, n_p, k, largest, dst, bytes);
+}
+
+int b200_sixdof_outcome_group_top_worlds(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
+                                         void *dst, uint64_t bytes)
+{
+    return run_top_worlds(h, true, planes, n_p, k, largest, dst, bytes);
+}
+
+double b200_sixdof_top_worlds_reads(const b200_sixdof *h) { return h ? h->topk_reads : 0.0; }
+
 int b200_sixdof_trajectory_reset(b200_sixdof *h)
 {
     if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");

@@ -60,6 +60,8 @@ struct b200_sixdof {
     uint64_t staging_bytes = 0;
     double quantile_reads = 0.0;            // reads of the planes by the last quantile call, per group
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
+    double topk_reads = 0.0;                // reads of the planes by the last top-worlds call, per task
+    unsigned long long topk_read_sum = 0;   // the same, summed over the tasks (written by the stream)
     // a world-sharded quantile call (b200_sixdof_sharded_quantiles_*) between begin and end: its state, the write
     // generation of the rows at begin (rows_gen: bumped by every entry that changes what a reduction reads), and its own
     // device scratch (not the staging buffer, which the other reductions reuse between its rounds)

@@ -452,4 +452,27 @@ struct OutcomeParams {
 // one launch on s (*launches = 1; 0 without sources or worlds)
 cudaError_t launch_outcomes(const OutcomeParams &P, int *launches, cudaStream_t s);
 
+// Worst worlds of the outcome planes (topk_kernels.cu, include/b200_sixdof.h b200_sixdof_outcome_top_worlds): for
+// group g of the table and selected plane j, the first min(k, count) finite worlds in totalOrder (descending when
+// `largest`), ties by ascending world, into out[(g * n_p + j) * (1 + 2k) ..] = [count, values[k], worlds[k]].
+struct TopkParams {
+    const double *planes;  // outcome plane 0; plane p at planes + p * ld, world w at [w]
+    uint64_t ld;
+    uint32_t n_p, k;       // selected planes, 1 <= k <= B200_MAX_TOP_WORLDS
+    int32_t largest;
+    uint32_t plane[B200_MAX_OUTCOMES];
+    const WorldGroup *groups;  // the group table, in device memory
+    const uint32_t *order;     // quantile_order(table), in device memory
+    double *out;
+};
+// bytes of device scratch the call over the groups of `table` needs: 0 without a group above 8192 worlds, else at most
+// 256 MiB
+uint64_t topk_scratch_bytes(const TopkParams &S, const std::vector<WorldGroup> &table);
+// one launch per small route that has groups, and a fixed launch sequence per slice of the large groups' tasks
+// (*launches); `scratch` holds topk_scratch_bytes(S, table).  With a large group *reads (host memory) receives, once the
+// stream reaches it, the reads of the planes summed over every task; it is left alone otherwise (one read per task).
+cudaError_t launch_top_worlds(const TopkParams &S, const std::vector<WorldGroup> &table,
+                              const std::vector<uint32_t> &order, void *scratch, int *launches,
+                              unsigned long long *reads, cudaStream_t s);
+
 } // namespace b200

@@ -586,6 +586,23 @@ class B200Exec:
         args, row = self._hist_specs(specs)
         return self._reduce("group_histograms", "outcome", args, (self.world_groups, row))
 
+    def outcome_top_worlds(self, planes, k: int, largest) -> np.ndarray:
+        """[p, 1 + 2k]: per outcome of `planes` (distinct indices below P) the record [count, values[k], worlds[k]] of
+        the first min(k, count) worlds whose value is finite, ordered by value (IEEE totalOrder, -0 < +0; descending
+        when `largest`), ties by ascending world index; slots past count hold NaN and -1."""
+        sel = self._selection(planes)
+        return self._reduce("top_worlds", "outcome", sel + (int(k), int(largest)), (sel[1], 1 + 2 * int(k)))
+
+    def outcome_group_top_worlds(self, planes, k: int, largest) -> np.ndarray:
+        """[G, p, 1 + 2k]: outcome_top_worlds(planes, k, largest) per group; worlds are the handle's world indices."""
+        sel = self._selection(planes)
+        return self._reduce("group_top_worlds", "outcome", sel + (int(k), int(largest)),
+                            (self.world_groups, sel[1], 1 + 2 * int(k)))
+
+    def top_worlds_reads(self) -> float:
+        """Reads of the outcome planes the last top-worlds call made, averaged over its (group, plane) tasks."""
+        return float(self._L.b200_sixdof_top_worlds_reads(self._h))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     @staticmethod
     def _conditions(rows: Sequence):
@@ -723,6 +740,42 @@ def merge_histograms(tables: Sequence[np.ndarray]) -> np.ndarray:
     if np.any(out > 2.0 ** 53):
         raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, "merge_histograms: a count exceeds 2^53")
     return out
+
+
+def top_world_keys(values, largest) -> np.ndarray:
+    """The sort keys of the worst-worlds order: the IEEE totalOrder key of each f64 value (-0 < +0) as uint64,
+    complemented when `largest`, so that ascending (key, world) is the order of b200_sixdof_outcome_top_worlds."""
+    u = np.ascontiguousarray(values, dtype=np.float64).view(np.uint64)
+    key = np.where(u >> np.uint64(63), ~u, u | np.uint64(1 << 63))
+    return ~key if largest else key
+
+
+def merge_top_worlds(tables: Sequence[np.ndarray], offsets: Sequence[int], largest) -> np.ndarray:
+    """Merge worst-worlds tables of the same shape [..., 1 + 2k] (one per rank of a world-sharded campaign, in rank
+    order, or per handle): table r's worlds are shifted by offsets[r] (its first world in the campaign), the candidates
+    of every table re-ordered by (key, world) and the first k kept; the counts add up.  Exact: the ranks hold contiguous
+    world ranges in rank order, so each rank's tie order by local index is the campaign's."""
+    stacked = _stack(tables, "merge_top_worlds", "1 + 2k", lambda rec: rec >= 3 and rec % 2 == 1)
+    if len(offsets) != len(stacked):
+        raise ValueError(f"merge_top_worlds: {len(stacked)} tables and {len(offsets)} offsets")
+    k = (stacked.shape[-1] - 1) // 2
+    flat = stacked.reshape(len(stacked), -1, 1 + 2 * k)
+    out = np.empty(flat.shape[1:])
+    for t in range(flat.shape[1]):
+        vals, worlds = [], []
+        for r, rec in enumerate(flat[:, t]):
+            n = min(int(rec[0]), k)
+            vals.append(rec[1:1 + n])
+            worlds.append(rec[1 + k:1 + k + n] + float(offsets[r]))
+        v, w = np.concatenate(vals), np.concatenate(worlds)
+        top = np.lexsort((w, top_world_keys(v, largest)))[:k]
+        n = top.size
+        out[t, 0] = flat[:, t, 0].sum()
+        out[t, 1:1 + k] = np.nan
+        out[t, 1 + k:] = -1.0
+        out[t, 1:1 + n] = v[top]
+        out[t, 1 + k:1 + k + n] = w[top]
+    return out.reshape(stacked.shape[1:])
 
 
 def math_nan() -> float:

@@ -232,6 +232,68 @@ def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=No
         settle()
 
 
+def _top_worlds_descriptor(planes, k, largest, groups, shape, n_worlds: int, status: int) -> List[int]:
+    """What every rank of a sharded worst-worlds call must agree on, as int64 words: the planes (padded with -1), their
+    count, k, largest, grouping and the table's shape; then the rank's worlds and its local call's status."""
+    from . import _lib
+
+    sel = [int(p) for p in planes][: _lib.MAX_OUTCOMES] if planes is not None else []
+    shape = (list(shape) + [-1] * 3)[:3]
+    return (sel + [-1] * (_lib.MAX_OUTCOMES - len(sel)) + [len(sel), int(k), int(bool(largest)), int(bool(groups))] + shape
+            + [int(n_worlds), int(status)])
+
+
+def gather_top_worlds(ex, planes, k: int, largest: bool, groups: bool = False, group=None) -> np.ndarray:
+    """Worst worlds of a world-sharded campaign, exact over every rank's worlds: every rank passes its executor (its
+    own worlds; with `groups`, the global groups cut to them by shard_groups) and the same planes, k and direction.
+    Each rank computes its own records (B200Exec.outcome_[group_]top_worlds), the ranks all-gather a descriptor of
+    their calls and then the records (1 + 2k f64 per task), and merge them with merge_top_worlds, offsetting each
+    rank's worlds by the worlds of the ranks before it.  Every rank returns the table of the same call on one executor
+    holding every rank's worlds in rank order, with campaign world indices.  A disagreement in the arguments or the
+    table shape, or any rank's failure, raises on every rank."""
+    import torch
+    import torch.distributed as dist
+
+    from . import _lib
+    from .executor import merge_top_worlds
+
+    if not (dist.is_available() and dist.is_initialized()):
+        raise RuntimeError("sharding.gather_top_worlds needs an initialized torch.distributed process group")
+    dev = "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+    status, err, table, sel = 0, None, None, None
+    try:
+        sel = [int(p) for p in np.atleast_1d(np.asarray(planes)).ravel()]
+        table = ex.outcome_group_top_worlds(sel, k, largest) if groups else ex.outcome_top_worlds(sel, k, largest)
+    except _lib.B200Error as e:
+        status, err = int(e.code), e
+    except (TypeError, ValueError) as e:
+        status, err = _ARGUMENT_ERROR, e
+    shape = table.shape if table is not None else ()
+    try:
+        words = _top_worlds_descriptor(sel, k, largest, groups, shape if groups else (1,) + tuple(shape), ex.n_worlds, status)
+    except (TypeError, ValueError) as e:  # a k or flag that is not a number: this rank differs from the others
+        status, err = _ARGUMENT_ERROR, err or e
+        words = _top_worlds_descriptor(None, -1, False, groups, (), ex.n_worlds, status)
+    mine = torch.tensor(words, dtype=torch.int64, device=dev)
+    every = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(every, mine, group=group)
+    every = [d.cpu().numpy() for d in every]
+    failed = [r for r, d in enumerate(every) if d[-1] != 0]
+    if failed:
+        if err is not None:
+            raise err
+        r, code = failed[0], int(every[failed[0]][-1])
+        if code == _ARGUMENT_ERROR:
+            raise ValueError(f"sharded top worlds: rank {r} passed planes, k or largest it cannot use")
+        raise _lib.B200Error(code, f"sharded top worlds: rank {r} failed (code {code})")
+    differ = [r for r, d in enumerate(every) if not np.array_equal(d[:-2], every[0][:-2])]
+    if differ:
+        raise ValueError(f"sharded top worlds: rank {differ[0]} differs from rank 0 in planes, k, largest, grouping or "
+                         f"table shape")
+    offsets = np.concatenate([[0], np.cumsum([int(d[-2]) for d in every])[:-1]])
+    return merge_top_worlds(_all_gather_tables(table, group), offsets, largest)
+
+
 def total_entity_steps(local_entity_steps: int, group=None) -> int:
     import torch
     import torch.distributed as dist

@@ -474,11 +474,14 @@ class World:
         input or the final state) or host values, and reduces it over the worlds on the device when asked
         (`Exec.outcome_stats`, `outcome_quantiles`, `outcome_covariance`, `outcome_histogram`, each per group with
         `groups=True`): apogee percentiles per sweep point, an impact ellipse, an event probability, input-to-outcome
-        correlations, without a per-world table reaching the host.  `process_group` (a torch.distributed group, with
+        correlations, without a per-world table reaching the host; `Exec.outcome_top_worlds` names the worst runs
+        themselves (the k worlds with the largest or smallest value of each outcome), for `retain=` and per-run
+        databases.  `process_group` (a torch.distributed group, with
         ensemble=True and quantiles or outcomes) makes this Exec one rank of a world-sharded campaign whose quantile
         tables are collective: every rank builds over its own worlds (`sharding.shard_worlds`, its groups cut by
         `sharding.shard_groups`) and `Exec.quantiles` (grouped or not, row 0 included) and `Exec.outcome_quantiles` are
-        reduced over every rank's worlds (`sharding.gather_quantiles`), exact, the same on every rank; every rank must
+        reduced over every rank's worlds (`sharding.gather_quantiles`), and `Exec.outcome_top_worlds` merged over them
+        with campaign world indices (`sharding.gather_top_worlds`), exact, the same on every rank; every rank must
         then record and ask for them together.  The ring capacity becomes the ranks' least, so that every rank reduces at
         the same ticks.  The other tables stay per rank, merged with the other gather helpers of `sharding`."""
         if backend not in ("b200", "b200-exact", "b200-fast"):
@@ -1837,6 +1840,34 @@ class Exec:
         spec = [h._spec(0)]
         t = self.backend.outcome_group_histograms(spec) if groups else self.backend.outcome_histograms(spec)
         return _histogram_record(h, t)
+
+    def outcome_top_worlds(self, k: int, names: Optional[Sequence[str]] = None, largest: bool = True,
+                           groups: bool = False) -> Dict[str, object]:
+        """The worst runs: for each outcome of `names` (default: all), the k worlds with the largest (`largest`) or
+        smallest finite value, found on the device.  {"count" [p] (the finite worlds), "value" [p, k], "world" [p, k]
+        (int64 world indices, ready for World.build(..., retain=...) and monte_carlo.write_run_databases), "names"},
+        with a group axis first with groups=True.  Ordered by value (IEEE totalOrder: -0 < +0), ties by ascending world
+        index; slots past the count hold NaN and -1.  Built with a `process_group`, over every rank's worlds with
+        campaign world indices (a collective: every rank calls it with the same arguments)."""
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= _lib.MAX_TOP_WORLDS:
+            raise ValueError(f"outcome_top_worlds: k = {k!r}, an int in [1, {_lib.MAX_TOP_WORLDS}]")
+        if not isinstance(largest, (bool, np.bool_)):
+            raise TypeError(f"outcome_top_worlds: largest = {largest!r}, a bool")
+        self._outcome_ready("outcome_top_worlds", groups)
+        names = list(self.outcomes if names is None else ([names] if isinstance(names, str) else names))
+        if not names or len(set(names)) != len(names):
+            raise ValueError(f"outcome_top_worlds: names {names!r}, one or more distinct outcome names")
+        planes = [self._outcome_plane(n) for n in names]
+        k, largest = int(k), bool(largest)
+        if self._pg is not None:
+            from .sharding import gather_top_worlds
+
+            t = gather_top_worlds(self.backend, planes, k, largest, groups, self._pg)
+        else:
+            t = (self.backend.outcome_group_top_worlds(planes, k, largest) if groups
+                 else self.backend.outcome_top_worlds(planes, k, largest))
+        return {"count": np.ascontiguousarray(t[..., 0]), "value": np.ascontiguousarray(t[..., 1:1 + k]),
+                "world": t[..., 1 + k:].astype(np.int64), "names": names}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

@@ -717,6 +717,43 @@ int b200_sixdof_outcome_histograms(b200_sixdof *h, const b200_histogram *specs, 
 int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *specs, uint32_t n_specs, void *dst,
                                          uint64_t bytes);
 
+/* ---- worst worlds: the k worlds with the largest or smallest value of each selected outcome, per group of worlds,
+ * found on the device; their world indices feed retained rows (World.build(..., retain=)) and per-run databases.
+ *   Contract  for a task (group g, selected outcome p) the candidates are the worlds w of the group whose outcome value
+ *             x_w is finite (NaN and +-inf are dropped, as by every reduction: a tick that never happened is never a
+ *             worst run; to find diverged worlds, ask a threshold's tick with largest = 0, the earliest firing);
+ *             count = the number of candidates.
+ *   Order     the IEEE totalOrder key of the quantile entries (-0 < +0), ascending for largest = 0 and descending for
+ *             largest = 1; ties are always broken by ascending world index.  The record holds the first min(k, count)
+ *             candidates in that order: a function of the data alone, whatever the route, launch shape or slicing.
+ *             numpy: u = x.view(uint64), key = where(u >> 63, ~u, u | 1 << 63), complemented for largest, then
+ *             np.lexsort((world, key))[:k] over the finite worlds.
+ *   Record    per task 1 + 2k f64: [count, value_0 .. value_{k-1}, world_0 .. world_{k-1}]; values keep their bits,
+ *             worlds are the handle's world indices (not indices within the group), exact as f64 below 2^53; slots past
+ *             count hold NaN and -1.
+ *   Bound     groups of at most 8192 worlds are sorted in shared memory after one read of the planes.  Larger ones
+ *             take a radix select of the composite key (value key, world index) with a fixed launch sequence: a count
+ *             pass, at most 8 histogram passes of 2^14 bins (5 over the value keys, 3 more over the world indices of
+ *             one value key tied more than 8192 times) and one gather: at most 10 reads of the planes on any data, 3 on
+ *             continuous data.  b200_sixdof_top_worlds_reads reports the reads of the last call, averaged over its
+ *             tasks.
+ *   Memory    device scratch of at most 256 MiB (the large tasks run in slices), in the staging buffer; a host
+ *             destination takes the table through the staging buffer after the scratch.
+ * Each entry checks, in this order: what every outcome entry checks (the outcome set, naming a refused outcome; the
+ * groups for the grouped entry); null planes, n_p of 0 or more than P, a plane >= P or listed twice; k of 0 or more
+ * than B200_MAX_TOP_WORLDS; largest not 0 or 1 (all B200_ERR_INVALID_ARGUMENT); then the byte count
+ * (B200_ERR_VALUE_SIZE_MISMATCH) and the sticky status.  Like every outcome entry it first writes the outcome planes
+ * and is never cached. ---- */
+#define B200_MAX_TOP_WORLDS 1024u
+/* dst = [n_p][1 + 2k] f64 (host or device) */
+int b200_sixdof_outcome_top_worlds(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
+                                   void *dst, uint64_t bytes);
+/* dst = [G][n_p][1 + 2k] f64, groups of b200_sixdof_set_world_groups */
+int b200_sixdof_outcome_group_top_worlds(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
+                                         void *dst, uint64_t bytes);
+/* average plane reads per task of the last top-worlds call (0 for a null handle or before any call) */
+double b200_sixdof_top_worlds_reads(const b200_sixdof *h);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
