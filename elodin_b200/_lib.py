@@ -76,7 +76,8 @@ SYMBOLS = [
     "b200_sixdof_outcome_group_stats", "b200_sixdof_outcome_quantiles", "b200_sixdof_outcome_group_quantiles",
     "b200_sixdof_outcome_covariance", "b200_sixdof_outcome_group_covariance", "b200_sixdof_outcome_histograms",
     "b200_sixdof_outcome_group_histograms", "b200_sixdof_outcome_top_worlds", "b200_sixdof_outcome_group_top_worlds",
-    "b200_sixdof_top_worlds_reads",
+    "b200_sixdof_top_worlds_reads", "b200_sixdof_outcome_ranks", "b200_sixdof_outcome_group_ranks",
+    "b200_sixdof_outcome_rank_correlation", "b200_sixdof_outcome_group_rank_correlation", "b200_sixdof_rank_reads",
     "b200_sixdof_sharded_quantiles_begin", "b200_sixdof_sharded_quantiles_round", "b200_sixdof_sharded_quantiles_end",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
@@ -355,6 +356,10 @@ def lib():
     L.b200_sixdof_outcome_group_top_worlds.argtypes = [vp, C.POINTER(u32), u32, u32, C.c_int, vp, u64]
     L.b200_sixdof_top_worlds_reads.argtypes = [vp]
     L.b200_sixdof_top_worlds_reads.restype = C.c_double
+    for name in ("ranks", "group_ranks", "rank_correlation", "group_rank_correlation"):
+        getattr(L, f"b200_sixdof_outcome_{name}").argtypes = [vp, C.POINTER(u32), u32, vp, u64]
+    L.b200_sixdof_rank_reads.argtypes = [vp]
+    L.b200_sixdof_rank_reads.restype = C.c_double
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

@@ -750,6 +750,7 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->sum_mom) cudaFree(h->sum_mom);
     if (h->sum_dwell) cudaFree(h->sum_dwell);
     if (h->out_planes) cudaFree(h->out_planes);
+    if (h->rank_planes) cudaFree(h->rank_planes);
     for (const auto *ts : {h->tables, h->out_tables})
         for (int g = 0; g < 2; ++g)
             for (void *p : {(void *)ts[g].stats_dev, (void *)ts[g].cov_dev, (void *)ts[g].order_dev})
@@ -2458,6 +2459,9 @@ int b200_sixdof_set_outcomes(b200_sixdof *h, const b200_outcome *o, uint32_t n)
     ++h->rows_gen;
     if (h->out_planes) CU(h, cudaFree(h->out_planes));
     h->out_planes = planes;
+    if (h->rank_planes) CU(h, cudaFree(h->rank_planes));  // the next rank call allocates for the new set
+    h->rank_planes = nullptr;
+    h->rank_bytes = 0;
     h->ld_o = ld_o;
     h->outcomes.assign(o, o + n);
     for (auto &x : h->outcomes) x.values = nullptr;
@@ -2586,6 +2590,106 @@ int b200_sixdof_outcome_group_top_worlds(b200_sixdof *h, const uint32_t *planes,
 }
 
 double b200_sixdof_top_worlds_reads(const b200_sixdof *h) { return h ? h->topk_reads : 0.0; }
+
+// Midranks of the selected outcome planes within each group (rank_kernels.cu) into the handle's rank planes, then into
+// dst: as [n_worlds][n_p] rows, or (corr) as the rank correlation records, the covariance of the rank planes (the
+// covariance kernels, unchanged) turned into [n, rho].  The outcome set and groups checked, then the selection, then
+// `bytes`, then the handle's status.  The outcome planes are only read.
+static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *planes, uint32_t n_p, void *dst,
+                     uint64_t bytes)
+{
+    int rc = reduction_ready(h, Rows::outcomes, grouped, corr ? "outcome rank correlation" : "outcome ranks");
+    if (rc) return rc;
+    CU(h, cudaSetDevice(h->device));
+    const uint32_t P = (uint32_t)h->outcomes.size(), least = corr ? 2 : 1;
+    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null rank planes");
+    if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u rank planes: %u to %u", n_p, least, P);
+    uint64_t seen = 0;
+    for (uint32_t j = 0; j < n_p; ++j) {
+        if (planes[j] >= P)
+            return fail(B200_ERR_INVALID_ARGUMENT, "rank plane %u is %u: the outcome has %u planes", j, planes[j], P);
+        if (seen & (1ull << planes[j])) return fail(B200_ERR_INVALID_ARGUMENT, "rank plane %u listed twice", planes[j]);
+        seen |= 1ull << planes[j];
+    }
+    const uint64_t G = reduction_groups(h, grouped).size(), W = h->desc.n_worlds;
+    const uint64_t want = corr ? G * (1ull + (uint64_t)n_p * n_p) * 8ull : W * n_p * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome %s %llu bytes, got %llu", corr ? "rank correlation is" : "ranks are",
+                    (unsigned long long)want, (unsigned long long)bytes);
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (bytes == 0) return B200_OK;
+    const uint64_t ld = h->ld_o;
+    if ((rc = grow_device(h, &h->rank_planes, &h->rank_bytes, n_p * ld * 8ull + ld))) return rc;
+    const b200_sixdof::GroupTables &t = reduction_tables(h, Rows::outcomes, grouped);
+    RankParams S{};
+    S.planes = h->out_planes;
+    S.ld = ld;
+    S.n_p = n_p;
+    for (uint32_t j = 0; j < n_p; ++j) S.plane[j] = planes[j];
+    S.groups = t.stats_dev;
+    S.order = t.order_dev;
+    S.ranks = h->rank_planes;
+    S.mask = (uint8_t *)(h->rank_planes + n_p * ld);
+    const uint64_t tasks = G * n_p, rank_scratch = rank_scratch_bytes(S, t.stats, t.order);
+    h->rank_read_sum = tasks;  // the small-group routes read every task once
+    if (!corr) {
+        rc = run_world_reduction(h, Rows::outcomes, false, rank_scratch, dst, bytes, [&](double *out, void *scratch, int *n) {
+            cudaError_t e = launch_ranks(S, W, t.stats, t.order, scratch, n, &h->rank_read_sum, h->stream);
+            if (e != cudaSuccess) return e;
+            *n += 1;
+            return launch_soa_to_aos(h->rank_planes, out, W, n_p, ld, h->stream);
+        });
+    } else {
+        // the covariance of the rank planes as the state of a handle with one entity, its table before the scratch
+        CovParams C{};
+        C.seg[0] = {h->rank_planes, n_p, n_p * ld};
+        C.n_segs = 1;
+        C.planes_per_sample = n_p;
+        C.n_planes = n_p;
+        C.ld = ld;
+        C.n_worlds = W;
+        C.n_entities = 1;
+        C.n_p = n_p;
+        for (uint32_t j = 0; j < n_p; ++j) C.planes[j] = j;
+        const uint64_t table = G * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
+        const uint64_t scratch = table + std::max(rank_scratch, cov_scratch_bytes(C, t.cov));
+        rc = run_world_reduction(h, Rows::outcomes, false, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
+            int a = 0, b = 0, c = 0;
+            void *rest = (char *)scr + table;
+            cudaError_t e = launch_ranks(S, W, t.stats, t.order, rest, &a, &h->rank_read_sum, h->stream);
+            C.out = (double *)scr;
+            if (e == cudaSuccess) e = launch_covariance(C, t.cov_dev, t.cov, rest, &b, h->stream);
+            if (e == cudaSuccess) e = launch_rank_correlation((const double *)scr, out, G, n_p, &c, h->stream);
+            *n = a + b + c;
+            return e;
+        });
+    }
+    h->rank_reads = rc == B200_OK ? (double)h->rank_read_sum / (double)tasks : 0.0;
+    return rc;
+}
+
+int b200_sixdof_outcome_ranks(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_ranks(h, false, false, planes, n_p, dst, bytes);
+}
+
+int b200_sixdof_outcome_group_ranks(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_ranks(h, true, false, planes, n_p, dst, bytes);
+}
+
+int b200_sixdof_outcome_rank_correlation(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes)
+{
+    return run_ranks(h, false, true, planes, n_p, dst, bytes);
+}
+
+int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
+                                               uint64_t bytes)
+{
+    return run_ranks(h, true, true, planes, n_p, dst, bytes);
+}
+
+double b200_sixdof_rank_reads(const b200_sixdof *h) { return h ? h->rank_reads : 0.0; }
 
 int b200_sixdof_trajectory_reset(b200_sixdof *h)
 {

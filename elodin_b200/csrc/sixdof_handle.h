@@ -62,6 +62,12 @@ struct b200_sixdof {
     unsigned long long quantile_read_sum = 0;  // the same, summed over the groups (written by the stream)
     double topk_reads = 0.0;                // reads of the planes by the last top-worlds call, per task
     unsigned long long topk_read_sum = 0;   // the same, summed over the tasks (written by the stream)
+    double rank_reads = 0.0;                // reads of the planes by the last rank call, per task
+    unsigned long long rank_read_sum = 0;   // the same, summed over the tasks (written by the stream)
+    // the rank planes of the last rank call (n_p x ld_o f64, then ld_o bytes of completeness mask): allocated by the
+    // first rank call, freed by set_outcomes and destroy
+    double *rank_planes = nullptr;
+    uint64_t rank_bytes = 0;
     // a world-sharded quantile call (b200_sixdof_sharded_quantiles_*) between begin and end: its state, the write
     // generation of the rows at begin (rows_gen: bumped by every entry that changes what a reduction reads), and its own
     // device scratch (not the staging buffer, which the other reductions reuse between its rounds)

@@ -475,4 +475,33 @@ cudaError_t launch_top_worlds(const TopkParams &S, const std::vector<WorldGroup>
                               const std::vector<uint32_t> &order, void *scratch, int *launches,
                               unsigned long long *reads, cudaStream_t s);
 
+// Midranks of the outcome planes (rank_kernels.cu, include/b200_sixdof.h b200_sixdof_outcome_ranks): for group g of the
+// table and selected plane j, every complete world's midrank within the group (scipy.stats.rankdata(method="average")
+// over the worlds whose n_p selected values are all finite, -0 == +0) into rank plane j, NaN for the other worlds.
+struct RankParams {
+    const double *planes;  // outcome plane 0; plane p at planes + p * ld, world w at [w]
+    uint64_t ld;
+    uint32_t n_p;          // selected planes
+    uint32_t plane[B200_MAX_OUTCOMES];
+    const WorldGroup *groups;  // the group table, in device memory
+    const uint32_t *order;     // quantile_order(table), in device memory
+    double *ranks;             // rank plane j at ranks + j * ld
+    uint8_t *mask;             // n_worlds bytes: world complete
+};
+// bytes of device scratch the call over the groups of `table` needs: 0 without a group above 8192 worlds, else at most
+// 256 MiB unless one (group, plane) task alone needs more (about 42 bytes per world)
+uint64_t rank_scratch_bytes(const RankParams &S, const std::vector<WorldGroup> &table, const std::vector<uint32_t> &order);
+// the mask launch, one launch per small route that has groups, and a fixed launch sequence per slice of the large
+// groups' tasks (*launches; none without worlds); `scratch` holds rank_scratch_bytes(S, table, order).  With a large
+// group *reads (host memory) receives, once the stream reaches it, the reads of the planes summed over every task; it
+// is left alone otherwise (one read per task).
+cudaError_t launch_ranks(const RankParams &S, uint64_t n_worlds, const std::vector<WorldGroup> &table,
+                         const std::vector<uint32_t> &order, void *scratch, int *launches, unsigned long long *reads,
+                         cudaStream_t s);
+// G covariance records [n, mean[n_p], M[n_p][n_p]] (cov, device) into G records [n, rho[n_p][n_p]] (out, device):
+// rho = M[a][b] / sqrt(M[a][a] * M[b][b]), each operation correctly rounded, NaN where n < 2 or M[a][a] or M[b][b] is
+// not > 0.  One launch (*launches = 1).
+cudaError_t launch_rank_correlation(const double *cov, double *out, uint64_t G, uint32_t n_p, int *launches,
+                                    cudaStream_t s);
+
 } // namespace b200

@@ -603,6 +603,34 @@ class B200Exec:
         """Reads of the outcome planes the last top-worlds call made, averaged over its (group, plane) tasks."""
         return float(self._L.b200_sixdof_top_worlds_reads(self._h))
 
+    def outcome_ranks(self, planes) -> np.ndarray:
+        """[n_worlds, p]: the midrank of every world in each outcome of `planes` (distinct indices below P) among the
+        worlds whose p selected values are all finite (scipy.stats.rankdata(method="average"), -0 == +0); NaN for the
+        other worlds."""
+        sel = self._selection(planes)
+        return self._reduce("ranks", "outcome", sel, (self.n_worlds, sel[1]))
+
+    def outcome_group_ranks(self, planes) -> np.ndarray:
+        """[n_worlds, p]: outcome_ranks(planes) within each group of set_world_groups."""
+        sel = self._selection(planes)
+        return self._reduce("group_ranks", "outcome", sel, (self.n_worlds, sel[1]))
+
+    def outcome_rank_correlation(self, planes) -> np.ndarray:
+        """[1 + p*p]: [n, rho[p][p]], the Spearman correlation of the outcomes `planes` (p >= 2) over the worlds whose p
+        values are all finite: the covariance record of their ranks, rho = M[a][b] / sqrt(M[a][a] * M[b][b]), NaN in
+        the row and column of a constant plane and everywhere when n < 2."""
+        sel = self._selection(planes)
+        return self._reduce("rank_correlation", "outcome", sel, (1 + sel[1] ** 2,))
+
+    def outcome_group_rank_correlation(self, planes) -> np.ndarray:
+        """[G, 1 + p*p]: outcome_rank_correlation(planes) per group."""
+        sel = self._selection(planes)
+        return self._reduce("group_rank_correlation", "outcome", sel, (self.world_groups, 1 + sel[1] ** 2))
+
+    def rank_reads(self) -> float:
+        """Reads of the outcome planes the last rank call made, averaged over its (group, plane) tasks."""
+        return float(self._L.b200_sixdof_rank_reads(self._h))
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     @staticmethod
     def _conditions(rows: Sequence):
@@ -776,6 +804,45 @@ def merge_top_worlds(tables: Sequence[np.ndarray], offsets: Sequence[int], large
         out[t, 1:1 + n] = v[top]
         out[t, 1 + k:1 + k + n] = w[top]
     return out.reshape(stacked.shape[1:])
+
+
+def rank_correlation(cov: np.ndarray, p: int) -> np.ndarray:
+    """The rank correlation records [..., 1 + p*p] of covariance records [..., 1 + p + p*p] of rank planes, as the
+    device computes them: rho[a][b] = M[a][b] / sqrt(M[a][a] * M[b][b]) (each operation correctly rounded, so the
+    same bits), NaN where n < 2 or M[a][a] or M[b][b] is not > 0."""
+    cov = np.asarray(cov, dtype=np.float64)
+    n = cov[..., :1]
+    M = cov[..., 1 + p:].reshape(*cov.shape[:-1], p, p)
+    d = np.diagonal(M, axis1=-2, axis2=-1)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        rho = M / np.sqrt(d[..., :, None] * d[..., None, :])
+    ok = (n[..., None] >= 2) & (d[..., :, None] > 0) & (d[..., None, :] > 0)
+    rho = np.where(ok, rho, np.nan)
+    return np.concatenate([n, rho.reshape(*cov.shape[:-1], p * p)], axis=-1)
+
+
+def partial_rank_correlation(R: np.ndarray) -> np.ndarray:
+    """PRCC from a rank correlation matrix R [..., n_in + 1, n_in + 1] whose last row and column are the output:
+    [..., n_in], prcc_i = -P[i, y] / sqrt(P[i, i] * P[y, y]) with P = inv(R); NaN where R holds a NaN, R is singular
+    or a diagonal of P is not > 0."""
+    R = np.asarray(R, dtype=np.float64)
+    k = R.shape[-1]
+    flat = R.reshape(-1, k, k)
+    out = np.full((flat.shape[0], k - 1), np.nan)
+    for t, r in enumerate(flat):
+        if not np.all(np.isfinite(r)):
+            continue
+        try:
+            P = np.linalg.inv(r)
+        except np.linalg.LinAlgError:
+            continue
+        if not np.all(np.isfinite(P)) or np.linalg.cond(r) > 1e12:
+            continue
+        d = np.diagonal(P)
+        if not np.all(d > 0):
+            continue
+        out[t] = -P[:-1, -1] / np.sqrt(d[:-1] * d[-1])
+    return out.reshape(*R.shape[:-2], k - 1)
 
 
 def math_nan() -> float:

@@ -30,7 +30,7 @@ import numpy as np
 from . import _lib
 from ._lib import component_id
 from .effectors import Effector, System, _flatten
-from .executor import B200Exec
+from .executor import B200Exec, partial_rank_correlation
 
 # --------------------------------------------------------------------------- value types
 
@@ -1868,6 +1868,65 @@ class Exec:
                  else self.backend.outcome_top_worlds(planes, k, largest))
         return {"count": np.ascontiguousarray(t[..., 0]), "value": np.ascontiguousarray(t[..., 1:1 + k]),
                 "world": t[..., 1 + k:].astype(np.int64), "names": names}
+
+    def _rank_planes(self, accessor: str, names, groups: bool, least: int) -> List[int]:
+        """The planes of `names` for a rank method, every refusal made before any backend call."""
+        self._outcome_ready(accessor, groups)
+        if self._pg is not None:
+            raise _lib.B200Error(_lib.ERR_UNSUPPORTED,
+                                 f"{accessor}: ranks over the worlds of a world-sharded campaign are not supported; "
+                                 "build without process_group to rank one handle's worlds")
+        names = list(names)
+        if len(names) < least or len(set(names)) != len(names):
+            raise ValueError(f"{accessor}: names {names!r}, {least} or more distinct outcome names")
+        return [self._outcome_plane(n) for n in names]
+
+    def outcome_ranks(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, np.ndarray]:
+        """{name: [n_worlds]}: the midrank of every world in each outcome of `names` (default: all), computed on the
+        device among the worlds whose selected values are all finite (scipy.stats.rankdata(method="average"); -0 and
+        +0 are one value), within its group with groups=True; NaN for the other worlds.  It downloads per-world values:
+        meant for small campaigns and tests."""
+        names = list(self.outcomes if names is None else ([names] if isinstance(names, str) else names))
+        planes = self._rank_planes("outcome_ranks", names, groups, 1)
+        t = self.backend.outcome_group_ranks(planes) if groups else self.backend.outcome_ranks(planes)
+        return {n: np.ascontiguousarray(t[:, k]) for k, n in enumerate(names)}
+
+    def outcome_rank_correlation(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, object]:
+        """Spearman rank correlation of the outcomes `names` (default: all; two or more), on the device: {"count",
+        "rho" [p, p], "names"}, a group axis first with groups=True.  Over the worlds whose p values are all finite,
+        ranked with midranks; NaN in the row and column of an outcome constant over them, and everywhere below 2
+        worlds (as scipy.stats.spearmanr)."""
+        names = list(self.outcomes if names is None else names)
+        planes = self._rank_planes("outcome_rank_correlation", names, groups, 2)
+        t = self.backend.outcome_group_rank_correlation(planes) if groups else self.backend.outcome_rank_correlation(planes)
+        p = len(planes)
+        return {"count": np.array(t[..., 0]), "rho": t[..., 1:].reshape(*t.shape[:-1], p, p), "names": names}
+
+    def outcome_sensitivity(self, inputs: Sequence[str], outputs: Sequence[str], groups: bool = False) -> Dict[str, object]:
+        """How much each dispersed input drives each output: {"count", "rho" [n_out, n_in] (Spearman), "prcc"
+        [n_out, n_in] (partial rank correlation: the correlation of the ranks of output y and input i once the ranks
+        of the other inputs are regressed out), "inputs", "outputs"}, a group axis first with groups=True.  One device
+        rank correlation over inputs + outputs; the PRCC of output y comes from the inverse of the rank correlation
+        matrix of the inputs and y (executor.partial_rank_correlation), NaN where that matrix holds a NaN or is
+        singular.  Every output shares one set of complete worlds, those whose inputs and outputs are all finite: to
+        rank an output over only its own finite worlds, call it separately."""
+        inputs = [inputs] if isinstance(inputs, str) else list(inputs)
+        outputs = [outputs] if isinstance(outputs, str) else list(outputs)
+        if not inputs or not outputs or set(inputs) & set(outputs):
+            raise ValueError(f"outcome_sensitivity: inputs {inputs!r} and outputs {outputs!r}, non-empty and disjoint")
+        if len(inputs) + len(outputs) > _lib.MAX_OUTCOMES:
+            raise ValueError(f"outcome_sensitivity: {len(inputs) + len(outputs)} names, at most {_lib.MAX_OUTCOMES}")
+        names = inputs + outputs
+        planes = self._rank_planes("outcome_sensitivity", names, groups, 2)
+        t = self.backend.outcome_group_rank_correlation(planes) if groups else self.backend.outcome_rank_correlation(planes)
+        p, n_in = len(names), len(inputs)
+        R = t[..., 1:].reshape(*t.shape[:-1], p, p)
+        rho = np.ascontiguousarray(R[..., n_in:, :n_in])
+        prcc = np.empty_like(rho)
+        for y in range(len(outputs)):
+            sub = list(range(n_in)) + [n_in + y]
+            prcc[..., y, :] = partial_rank_correlation(R[..., sub, :][..., :, sub])
+        return {"count": np.array(t[..., 0]), "rho": rho, "prcc": prcc, "inputs": inputs, "outputs": outputs}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

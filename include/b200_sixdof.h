@@ -754,6 +754,56 @@ int b200_sixdof_outcome_group_top_worlds(b200_sixdof *h, const uint32_t *planes,
 /* average plane reads per task of the last top-worlds call (0 for a null handle or before any call) */
 double b200_sixdof_top_worlds_reads(const b200_sixdof *h);
 
+/* ---- rank correlation: midranks of chosen outcomes within each group of worlds, and the Spearman correlation of
+ * those ranks, computed on the device; with partial rank correlation (Exec.outcome_sensitivity) the measure of how much
+ * each dispersed input drives an outcome, robust to ties, non-linearity and single huge values.
+ *   Task      (group g, selected outcome j) over a selection of n_p distinct outcome planes; the ungrouped entries
+ *             treat all worlds as one group.
+ *   Complete  the worlds of group g whose n_p selected values are all finite (listwise deletion, as for the
+ *             covariance); n_g = their count.
+ *   Midrank   of a complete world w in plane j: less + (eq + 1) / 2, less = the complete worlds of the group with a
+ *             smaller value, eq = those with an equal value, w included (scipy.stats.rankdata(x, method="average")
+ *             over the complete worlds).  Values compare numerically: -0 and +0 are one value (unlike the totalOrder
+ *             key of the quantile and top-worlds entries).  Every midrank is a half-integer, exact in f64; a world
+ *             that is not complete gets NaN.  Nothing breaks ties, so the ranks are a function of the data alone,
+ *             whatever the route, launch shape or slicing.
+ *   Rho       the covariance record of the rank planes (the outcome covariance kernels, unchanged) turned into
+ *             rho[a][b] = M[a][b] / sqrt(M[a][a] * M[b][b]), each operation correctly rounded (numpy's bits for the
+ *             same expression); exactly 1 on the diagonal of a plane that varies; NaN in the row and column of a plane
+ *             that is constant over the complete worlds (M[a][a] = 0, as scipy.stats.spearmanr), and everywhere when
+ *             n < 2.
+ *   Record    per group 1 + n_p^2 f64: [n, rho[n_p][n_p] row-major].
+ *   Bound     the selected planes are read once per call for completeness (a byte per world in the handle's rank
+ *             buffer).  Groups of at most 8192 worlds are then sorted in shared memory after one read.  Larger ones
+ *             take an MSD bucket pass over the value keys: a count pass, at most 5 histogram levels of 2^14 bins (a bin
+ *             one key wide is one tie run, ranked with no sort; a bin of at most 8192 worlds is a bucket, sorted in
+ *             shared memory; a larger one refines at the next level) and one scatter: at most 7 reads of a task's plane
+ *             on any data, 3 where the first level leaves no bin above 8192 worlds (values of one sign over a few
+ *             binades), plus one read of the bucket area.  b200_sixdof_rank_reads reports the reads of the last call,
+ *             averaged over its tasks (the completeness read not counted).
+ *   Memory    the rank planes, n_p * ld_o f64 and ld_o bytes, are allocated by the first rank call (grown by a later
+ *             one with more planes) and freed by set_outcomes and destroy: a handle that never asks for ranks
+ *             allocates nothing more.  The outcome planes are only read.  Device scratch (in the staging buffer) of
+ *             about 42 bytes per world of a large group's task, at most 256 MiB (the large tasks run in slices) unless
+ *             one task alone needs more.
+ * Each entry checks, in this order: what every outcome entry checks (the outcome set, naming a refused outcome; the
+ * groups for the grouped entries); null planes, n_p of 0 (ranks) or below 2 (correlation), n_p above P, a plane >= P
+ * or listed twice (all B200_ERR_INVALID_ARGUMENT); then the byte count (B200_ERR_VALUE_SIZE_MISMATCH) and the sticky
+ * status.  Like every outcome entry it first writes the outcome planes of the summaries and columns (never the VALUES
+ * planes) and is never cached; it runs on the handle's stream, returns once dst (host or device) is filled and counts
+ * its launches in timings.kernel_launches. ---- */
+/* dst = [n_worlds][n_p] f64 midranks (host or device; for small campaigns and tests, like outcome_values) */
+int b200_sixdof_outcome_ranks(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* dst = [n_worlds][n_p] f64 midranks within each group of b200_sixdof_set_world_groups */
+int b200_sixdof_outcome_group_ranks(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* dst = [1 + n_p^2] f64 */
+int b200_sixdof_outcome_rank_correlation(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst, uint64_t bytes);
+/* dst = [G][1 + n_p^2] f64 */
+int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, void *dst,
+                                               uint64_t bytes);
+/* average plane reads per task of the last rank call (0 for a null handle or before any call) */
+double b200_sixdof_rank_reads(const b200_sixdof *h);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
