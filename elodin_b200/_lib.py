@@ -79,6 +79,7 @@ SYMBOLS = [
     "b200_sixdof_top_worlds_reads", "b200_sixdof_outcome_ranks", "b200_sixdof_outcome_group_ranks",
     "b200_sixdof_outcome_rank_correlation", "b200_sixdof_outcome_group_rank_correlation", "b200_sixdof_rank_reads",
     "b200_sixdof_sharded_quantiles_begin", "b200_sixdof_sharded_quantiles_round", "b200_sixdof_sharded_quantiles_end",
+    "b200_sixdof_sharded_ranks_begin", "b200_sixdof_sharded_ranks_round", "b200_sixdof_sharded_ranks_end",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -360,6 +361,9 @@ def lib():
         getattr(L, f"b200_sixdof_outcome_{name}").argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_rank_reads.argtypes = [vp]
     L.b200_sixdof_rank_reads.restype = C.c_double
+    L.b200_sixdof_sharded_ranks_begin.argtypes = [vp, C.c_int, C.POINTER(u32), u32, u32, u32, C.POINTER(u64)]
+    L.b200_sixdof_sharded_ranks_round.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64)]
+    L.b200_sixdof_sharded_ranks_end.argtypes = [vp, vp, u64, vp, u64]
     L.b200_sixdof_tick_count.argtypes = [vp]
     L.b200_sixdof_tick_count.restype = u64
     L.b200_sixdof_set_stream.argtypes = [vp, vp, C.c_int]

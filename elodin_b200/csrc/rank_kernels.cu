@@ -31,6 +31,10 @@
 //    two worlds) and a bucket area slot (u64, u32): about 42 bytes per world.  The large tasks run in slices of at
 //    most kScratchCap = 256 MiB, the same launch sequence per slice; a task that alone needs more runs alone.
 //
+// A world-sharded call (sharded_rank_round, below) runs the same bucket pass over every task, in rounds whose u32 words
+// the ranks sum: the plan sees the summed counts, so every rank resolves the same ranges, tie runs and buckets, and the
+// buckets' keys travel summed too (each rank writes its own, the others leave those words 0).
+//
 // The order helpers and bitonic_pairs are duplicated from topk_kernels.cu (the top-worlds kernels keep their registers
 // and this file's rank key differs at zero).
 #include <algorithm>
@@ -548,6 +552,405 @@ __global__ void rank_corr_kernel(const double *cov, double *out, uint64_t G, uin
     }
 }
 
+// ---- world-sharded calls ----------------------------------------------------------------------------------------------
+
+using TaskState = RankShard::TaskState;
+constexpr uint32_t kNoBucket = 0xffffffffu;
+
+// One task of a sharded slice: the rank's worlds [o, o + n) of group g and selected plane j, in C chunks of Wc worlds
+// (k0 = the chunks of the slice's tasks before it); R ranges at most per level, from N, the group's complete worlds over
+// every rank; lcn of them on this rank; its area at `off` bytes into the slice's
+struct SRow {
+    uint64_t off;
+    uint32_t o, n, Wc, C, k0, j, R, N, lcn, pad;
+};
+
+// A piece (tie run or bucket) that holds worlds of this rank.  Only such pieces are kept, so a task keeps at most lcn.
+// base, count: its less and its worlds over every rank; a bucket's number b (kNoBucket: a tie run), where its keys
+// start in the task's key words (kb) and where this rank's start (ko), its worlds on this rank (lc) and where they start
+// in the rank's bucket list (lb), and the slots of the list filled so far
+struct Piece {
+    uint32_t base, count, b, kb, ko, lc, lb, fill;
+};
+
+// The area of one sharded task: the ranges of the two level parities (R each: a range holds more than kCap worlds over
+// every rank), then the rank's part: its pieces, its worlds' states and its bucket worlds and their keys.  The level
+// histograms live in the slice's pools, sized by the ranges that exist.
+struct SArea {
+    Range *rg0, *rg1;
+    Piece *pc;                  // [lcn]
+    uint32_t *wst;              // [n]
+    uint32_t *bi;               // [lcn]
+    unsigned long long *bkey;   // [lcn]
+};
+
+__host__ __device__ inline uint64_t shard_area_bytes(uint64_t R, uint64_t lcn, uint64_t n)
+{
+    return 2 * R * sizeof(Range) + lcn * sizeof(Piece) + align8(n * 4ull) + align8(lcn * 4ull) + lcn * 8ull;
+}
+
+__device__ inline SArea shard_area_of(void *base, const SRow &r)
+{
+    SArea A;
+    char *p = (char *)base + r.off;
+    A.rg0 = (Range *)p;
+    p += r.R * sizeof(Range);
+    A.rg1 = (Range *)p;
+    p += r.R * sizeof(Range);
+    A.pc = (Piece *)p;
+    p += r.lcn * sizeof(Piece);
+    A.wst = (uint32_t *)p;
+    p += align8(r.n * 4ull);
+    A.bi = (uint32_t *)p;
+    p += align8(r.lcn * 4ull);
+    A.bkey = (unsigned long long *)p;
+    return A;
+}
+
+__device__ __forceinline__ Range *srg_of(const SArea &A, int level) { return (level & 1) ? A.rg1 : A.rg0; }
+
+struct SLayout {
+    uint64_t T;                 // tasks of the slice
+    const SRow *rows;           // [T]
+    TaskState *st;              // [T]
+    const uint64_t *hoff0, *hoff1;  // [T] per level parity: where each task's histograms start in the pool (u32 words)
+    const uint64_t *xk;         // [T]: where each task's keys start in the slice's key words
+    void *base;                 // the tasks' areas, at rows[t].off
+    uint32_t *pool0, *pool1;    // per level parity: the level's histograms, [ranges][kBins] per task; then codes
+    uint32_t *x;                // the exchange
+    uint32_t rank, n_ranks;
+};
+
+__device__ __forceinline__ uint32_t *shist(const SLayout &L, int level, uint64_t t)
+{
+    // selected, not indexed: an indexed parameter array would be copied to the stack
+    return (level & 1) ? L.pool1 + L.hoff1[t] : L.pool0 + L.hoff0[t];
+}
+
+// the sizes: the complete worlds and the worlds of every group on this rank, into its slots
+// x[(g * n_ranks + rank) * 2 + {0, 1}] (x zeroed)
+__global__ void __launch_bounds__(256) shard_size_kernel(RankParams S, uint64_t G, uint32_t *x, uint32_t rank,
+                                                         uint32_t n_ranks)
+{
+    __shared__ uint32_t part[8];
+    for (uint64_t g = blockIdx.x; g < G; g += gridDim.x) {
+        const WorldGroup wg = S.groups[g];
+        uint32_t n = 0;
+        for (uint64_t w = threadIdx.x; w < wg.n; w += blockDim.x) n += S.mask[wg.o + w];
+        for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+        if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = n;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int k = 1; k < 8; ++k) n += part[k];
+            x[(g * n_ranks + rank) * 2] = n;
+            x[(g * n_ranks + rank) * 2 + 1] = (uint32_t)wg.n;
+        }
+        __syncthreads();
+    }
+}
+
+// every world's state: bin 0 of level 0, the task's one piece (a task of at most kCap worlds), or none
+__global__ void shard_init_kernel(SLayout L, const uint8_t *mask)
+{
+    const SRow r = L.rows[blockIdx.y];
+    const SArea A = shard_area_of(L.base, r);
+    const uint32_t first = r.N <= kCap ? kPiece : 0u;
+    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < r.n; w += (uint64_t)gridDim.x * blockDim.x)
+        A.wst[w] = mask[r.o + w] ? first : kNone;
+}
+
+// plan 0: one thread per task; the task whole, over the whole key range (min and max do not add over the ranks), is a
+// tie run of one world, a bucket, or the range of level 1
+__global__ void shard_plan0_kernel(SLayout L)
+{
+    const uint64_t ti = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (ti >= L.T) return;
+    const SRow r = L.rows[ti];
+    const SArea A = shard_area_of(L.base, r);
+    TaskState s{};
+    s.N = r.N;
+    s.lcn = r.lcn;
+    if (r.N <= kCap) {
+        const bool run = r.N == 1;
+        if (r.lcn) {
+            A.pc[0] = Piece{0, r.N, run ? kNoBucket : 0u, 0, 0, r.lcn, 0, 0};
+            s.n_pieces = 1;
+        }
+        if (!run) {
+            s.n_buckets = 1;
+            s.bucket_worlds = r.N;
+            s.local_worlds = r.lcn;
+        }
+    } else {
+        A.rg1[0] = Range{0ull, 64 - kBinBits, 0};
+        s.nr[1] = 1;
+    }
+    L.st[ti] = s;
+}
+
+__device__ inline uint32_t srow_of_chunk(const SRow *rows, uint64_t T, uint64_t k)
+{
+    uint64_t lo = 0, hi = T - 1;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi + 1) / 2;
+        if (rows[mid].k0 <= k) lo = mid;
+        else hi = mid - 1;
+    }
+    return (uint32_t)lo;
+}
+
+// pass l >= 1, as rank_pass_kernel: the rank's worlds of a task with ranges at level l leave their level l - 1 bin (at
+// level 1, the task's one range) for a piece or a level l bin, counted in the level's pool
+__global__ void __launch_bounds__(kPassThreads) shard_pass_kernel(RankParams S, uint64_t K, SLayout L, int level)
+{
+    const uint32_t t = threadIdx.x;
+    for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
+        const uint32_t ti = srow_of_chunk(L.rows, L.T, c);
+        const SRow r = L.rows[ti];
+        const SArea A = shard_area_of(L.base, r);
+        const uint32_t w0 = (uint32_t)(c - r.k0) * r.Wc, w1 = min(w0 + r.Wc, r.n);
+        const TaskState &ts = L.st[ti];
+        const uint32_t *code = level > 1 ? shist(L, level - 1, ti) : nullptr;
+        if (ts.nr[level] == 0) {  // uniform over the block
+            // a task whose last plan was l - 1: its worlds take their pieces now, before the pool of l - 1 is reused
+            if (level > 1 && ts.level == (uint32_t)(level - 1))
+                for (uint32_t w = w0 + t; w < w1; w += kPassThreads) {
+                    const uint32_t st = A.wst[w];
+                    if (!(st & kPiece)) A.wst[w] = code[st];
+                }
+            continue;
+        }
+        uint32_t *hist = shist(L, level, ti);
+        const Range *rg = srg_of(A, level);
+        const double *p = plane_of(S, r.j) + r.o;
+        for (uint32_t w = w0 + t; w < w1; w += kPassThreads) {
+            const uint32_t st = A.wst[w];
+            if (st & kPiece) continue;
+            const uint32_t cd = code ? code[st] : 0u;
+            if (cd & kPiece) {
+                A.wst[w] = cd;
+                continue;
+            }
+            const Range R = rg[cd];
+            const uint32_t b = cd * kBins + (uint32_t)((rank_key(p[w]) - R.lo) >> R.shift);
+            const cg::coalesced_group same = cg::labeled_partition(cg::coalesced_threads(), b);
+            if (same.thread_rank() == 0) atomicAdd(&hist[b], same.size());
+            A.wst[w] = b;
+        }
+    }
+}
+
+// Per-thread sums of a run of bins, scanned over the block: the less of the bins before it, and the buckets, their
+// worlds over every rank and on this one, and the ranges they hold.  Scanned as three primitive words (less | ranges,
+// bucket worlds | buckets, local bucket worlds): no half reaches 2^32 over a task of fewer than 2^31 worlds.
+struct PlanSum {
+    uint32_t less, nb, bw, lw, nr;
+};
+
+__device__ __forceinline__ PlanSum plan_add(const PlanSum &a, const PlanSum &b)
+{
+    return PlanSum{a.less + b.less, a.nb + b.nb, a.bw + b.bw, a.lw + b.lw, a.nr + b.nr};
+}
+
+constexpr unsigned kShardPlanThreads = 512;
+
+// plan l >= 1: a block per task with ranges at level l resolves its ranges in order, from the summed counts in the
+// exchange (laid out as the pool) and the local ones in the pool, writing the bins' codes over the local counts: every
+// rank numbers the next level's ranges and the buckets in the same order, so the ranks' words line up in the next
+// exchange.  Only the pieces that hold worlds of this rank are kept.
+__global__ void __launch_bounds__(kShardPlanThreads) shard_plan_kernel(SLayout L, int level)
+{
+    using Scan64 = cub::BlockScan<unsigned long long, kShardPlanThreads>;
+    using Scan32 = cub::BlockScan<uint32_t, kShardPlanThreads>;
+    __shared__ union {
+        typename Scan64::TempStorage s64;
+        typename Scan32::TempStorage s32;
+    } scan_tmp;
+    constexpr uint32_t kItems = kBins / kShardPlanThreads;
+    const uint64_t ti = blockIdx.y;
+    const SRow row = L.rows[ti];
+    const SArea A = shard_area_of(L.base, row);
+    TaskState &s = L.st[ti];
+    const uint32_t nr = s.nr[level], t = threadIdx.x;
+    if (nr == 0) return;  // the task is done: its codes stay for the scatter
+    const uint32_t next_level = level + 1;
+    PlanSum carry{0, s.n_buckets, s.bucket_worlds, s.local_worlds, 0};
+    const uint32_t *sums = L.x + ((level & 1) ? L.hoff1[ti] : L.hoff0[ti]);
+    for (uint32_t x = 0; x < nr; ++x) {
+        const Range R = srg_of(A, level)[x];
+        const uint32_t next_shift = R.shift > kBinBits ? R.shift - kBinBits : 0;
+        // the bins are read twice (the second time from cache) rather than held across the scan
+        const uint32_t *sum = sums + (uint64_t)x * kBins + t * kItems;
+        uint32_t *code = shist(L, level, ti) + (uint64_t)x * kBins + t * kItems;
+        PlanSum mine{0, 0, 0, 0, 0};
+        for (uint32_t k = 0; k < kItems; ++k) {
+            const uint32_t g = sum[k];
+            mine.less += g;
+            if (g <= 1 || R.shift == 0) continue;
+            if (g <= kCap) {
+                mine.nb += 1;
+                mine.bw += g;
+                mine.lw += code[k];
+            } else {
+                mine.nr += 1;
+            }
+        }
+        unsigned long long a0, a1, t0, t1;
+        uint32_t a2, t2;
+        Scan64(scan_tmp.s64).ExclusiveSum(mine.less | (unsigned long long)mine.nr << 32, a0, t0);
+        __syncthreads();
+        Scan64(scan_tmp.s64).ExclusiveSum(mine.bw | (unsigned long long)mine.nb << 32, a1, t1);
+        __syncthreads();
+        Scan32(scan_tmp.s32).ExclusiveSum(mine.lw, a2, t2);
+        const PlanSum total{(uint32_t)t0, (uint32_t)(t1 >> 32), (uint32_t)t1, t2, (uint32_t)(t0 >> 32)};
+        PlanSum at{(uint32_t)a0, (uint32_t)(a1 >> 32), (uint32_t)a1, a2, (uint32_t)(a0 >> 32)};
+        at = plan_add(carry, at);  // carry.less is 0: less restarts at every range's base
+        at.less += R.base;
+        for (uint32_t k = 0; k < kItems; ++k) {
+            const uint32_t g = sum[k];
+            if (g == 0) continue;
+            const uint32_t base = at.less, b = t * kItems + k, lc = code[k];
+            at.less += g;
+            if (g > kCap && R.shift != 0) {
+                srg_of(A, next_level)[at.nr] = Range{R.lo + ((unsigned long long)b << R.shift), next_shift, base};
+                code[k] = at.nr;
+                at.nr += 1;
+                continue;
+            }
+            const bool run = g == 1 || R.shift == 0;
+            if (lc) {
+                const uint32_t id = atomicAdd(&s.n_pieces, 1u);
+                A.pc[id] = run ? Piece{base, g, kNoBucket, 0, 0, lc, 0, 0} : Piece{base, g, at.nb, at.bw, at.bw, lc, at.lw, 0};
+                code[k] = kPiece | id;
+            }
+            if (!run) {
+                at.nb += 1;
+                at.bw += g;
+                at.lw += lc;
+            }
+        }
+        carry = plan_add(carry, total);
+        carry.less = 0;
+        __syncthreads();  // scan_tmp is reused
+    }
+    if (t == 0) {
+        s.level = level;
+        s.n_buckets = carry.nb;
+        s.bucket_worlds = carry.bw;
+        s.local_worlds = carry.lw;
+        s.nr[next_level] = carry.nr;
+    }
+}
+
+// scatter: every complete world of the rank takes its piece: a tie run's midrank, or its bucket's next slot in the
+// rank's bucket list, with its key
+__global__ void __launch_bounds__(kPassThreads) shard_scatter_kernel(RankParams S, uint64_t K, SLayout L)
+{
+    const uint32_t t = threadIdx.x;
+    for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
+        const uint32_t ti = srow_of_chunk(L.rows, L.T, c);
+        const SRow r = L.rows[ti];
+        const SArea A = shard_area_of(L.base, r);
+        const uint32_t level = L.st[ti].level;
+        const uint32_t *code = level ? shist(L, level, ti) : nullptr;
+        const double *p = plane_of(S, r.j) + r.o;
+        double *out = rank_plane(S, r.j) + r.o;
+        const uint32_t w0 = (uint32_t)(c - r.k0) * r.Wc, w1 = min(w0 + r.Wc, r.n);
+        for (uint32_t w = w0 + t; w < w1; w += kPassThreads) {
+            uint32_t st = A.wst[w];
+            if (st == kNone) continue;
+            if (!(st & kPiece)) st = code[st];
+            Piece &P = A.pc[st & ~kPiece];
+            if (P.b == kNoBucket) {
+                out[w] = (double)P.base + (double)(P.count + 1) * 0.5;
+                continue;
+            }
+            const uint32_t slot = atomicAdd(&P.fill, 1u);
+            A.bi[P.lb + slot] = w;
+            A.bkey[P.lb + slot] = rank_key(p[w]);
+        }
+    }
+}
+
+// is piece P a bucket whose keys start in the window [s0, s1) of the slice's key words (its task's from xk)?
+__device__ __forceinline__ bool in_window(const Piece &P, uint64_t xk, uint64_t s0, uint64_t s1)
+{
+    return P.b != kNoBucket && xk + P.kb >= s0 && xk + P.kb < s1;
+}
+
+// the window [s0, s1) of the buckets' keys: mode 0, every bucket's count on this rank into its slot
+// x[(its first key - s0) * n_ranks + rank] (x zeroed); mode 1, from the sums, where this rank's keys of the bucket go:
+// after those of the ranks before it; mode 2, this rank's keys there, from s0 on (x zeroed)
+__global__ void shard_window_kernel(SLayout L, uint64_t s0, uint64_t s1, int mode)
+{
+    const SArea A = shard_area_of(L.base, L.rows[blockIdx.y]);
+    const uint32_t np = L.st[blockIdx.y].n_pieces;
+    const uint64_t xk = L.xk[blockIdx.y];
+    unsigned long long *keys = (unsigned long long *)L.x;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < np; i += gridDim.x * blockDim.x) {
+        Piece &P = A.pc[i];
+        if (!in_window(P, xk, s0, s1)) continue;
+        const uint64_t slot = (xk + P.kb - s0) * L.n_ranks;
+        if (mode == 0) {
+            L.x[slot + L.rank] = P.lc;
+        } else if (mode == 1) {
+            uint32_t off = 0;
+            for (uint32_t r = 0; r < L.rank; ++r) off += L.x[slot + r];
+            P.ko = P.kb + off;
+        } else {
+            for (uint32_t k = 0; k < P.lc; ++k) keys[xk + P.ko - s0 + k] = A.bkey[P.lb + k];
+        }
+    }
+}
+
+// the midrank within the sorted keys a[0, n) of key k, which a holds: its tie run [s, e) from two binary searches
+__device__ __forceinline__ double midrank_of(const unsigned long long *a, uint32_t n, unsigned long long k)
+{
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t m = (lo + hi) / 2;
+        if (a[m] < k) lo = m + 1;
+        else hi = m;
+    }
+    const uint32_t s = lo;
+    hi = n;
+    while (lo < hi) {
+        const uint32_t m = (lo + hi) / 2;
+        if (a[m] <= k) lo = m + 1;
+        else hi = m;
+    }
+    return (double)(s + lo + 1) * 0.5;
+}
+
+// finish of the window [s0, s1): block (x, task y) sorts the task's buckets there that hold worlds of this rank (pieces
+// x, x + gridDim.x, ..) from every rank's keys in the summed exchange, and writes base + the in-bucket midrank of each
+// of the rank's worlds
+__global__ void __launch_bounds__(kPlanThreads) shard_finish_kernel(RankParams S, SLayout L, uint64_t s0, uint64_t s1)
+{
+    extern __shared__ unsigned long long keys[];  // kCap keys, then kCap slots for bitonic_pairs
+    uint32_t *idx = (uint32_t *)(keys + kCap);
+    const SRow r = L.rows[blockIdx.y];
+    const SArea A = shard_area_of(L.base, r);
+    const uint32_t np = L.st[blockIdx.y].n_pieces, t = threadIdx.x;
+    const uint64_t xk = L.xk[blockIdx.y];
+    const unsigned long long *x = (const unsigned long long *)L.x;
+    double *out = rank_plane(S, r.j) + r.o;
+    for (uint32_t i = blockIdx.x; i < np; i += gridDim.x) {
+        const Piece P = A.pc[i];
+        if (!in_window(P, xk, s0, s1)) continue;  // uniform over the block
+        const uint32_t n2 = pow2_at_least(P.count);
+        for (uint32_t k = t; k < n2; k += blockDim.x) {
+            keys[k] = k < P.count ? x[xk + P.kb - s0 + k] : ~0ull;
+            idx[k] = k;
+        }
+        __syncthreads();
+        bitonic_pairs(keys, idx, n2, t, blockDim.x, []() { __syncthreads(); });
+        for (uint32_t k = t; k < P.lc; k += blockDim.x)
+            out[A.bi[P.lb + k]] = (double)P.base + midrank_of(keys, P.count, A.bkey[P.lb + k]);
+        __syncthreads();
+    }
+}
+
 constexpr uint64_t kScratchCap = 256ull << 20;  // device scratch of a large-group call, unless one task needs more
 constexpr uint64_t kHeader = 256;               // the reads counter
 constexpr uint64_t kGridCap = 64ull * kNumSMs * 8;
@@ -689,5 +1092,373 @@ cudaError_t launch_rank_correlation(const double *cov, double *out, uint64_t G, 
     *launches = 1;
     return cudaGetLastError();
 }
+
+// ---- world-sharded calls ----------------------------------------------------------------------------------------------
+// Every (group, plane) task whose group holds a complete world on some rank takes the MSD bucket pass (the small routes
+// would see only this rank's worlds), in slices cut alike on every rank, with an exchange before every step that needs
+// the other ranks' counts or keys:
+//   sizes     once per call: every group's complete worlds and worlds, rank-slotted (G x n_ranks x 2 u32)
+//   open      per slice: the world states, then plan 0 from the global size alone
+//   hist l    pass l counts the rank's worlds into the level's pool; out: the pool (each task's counts of the level's
+//             ranges); in: their sums, then plan l
+//   scatter   after the last plan: tie runs' midranks, and the rank's bucket worlds with their keys in its bucket list
+//   windows   the buckets in windows of their first key in the slice's key words, so that no exchange passes kRoundCap:
+//             offsets  each bucket's count on this rank, rank-slotted: where this rank's keys of the bucket go
+//             keys     each rank's keys (u64) at the bucket's place plus its offset, the other ranks leaving those words
+//                      0; in: every key of the window's buckets, then the finish
+// A step that finds no work skips the exchange.  Every rank plans from the same sums, numbers ranges and buckets in the
+// same order and so makes the same exchanges, each of the same size.  The histograms are sent in rounds of at most
+// kRoundCap bytes.
+namespace {
+
+enum : int { kStart = 0, kSizes, kHist, kOffsets, kKeys, kDone };
+constexpr uint64_t kRoundCap = 32ull << 20;
+constexpr uint64_t kMaxSliceTasks = 65535;  // a slice's tasks are a grid's y extent
+
+// the slice's header: rows, task states, the pools' offsets of the two level parities and the key offsets, then the
+// tasks' areas
+struct SliceHeader {
+    uint64_t rows, st, hoff0, hoff1, xk, areas;
+};
+
+SliceHeader slice_header(uint64_t T)
+{
+    SliceHeader H;
+    H.rows = kHeader;
+    H.st = align8(H.rows + T * sizeof(SRow));
+    H.hoff0 = align8(H.st + T * sizeof(TaskState));
+    H.hoff1 = H.hoff0 + T * 8;
+    H.xk = H.hoff1 + T * 8;
+    H.areas = H.xk + T * 8;
+    return H;
+}
+
+// a task of at most kCap worlds over every rank is one piece: no ranges
+uint64_t shard_ranges(uint64_t N) { return N > kCap ? ranges_of(N) : 0; }
+
+// a task's bytes in a slice, for a rank with lcn complete worlds of n
+uint64_t task_bytes_of(uint64_t N, uint64_t lcn, uint64_t n)
+{
+    return sizeof(SRow) + sizeof(TaskState) + 24 + align8(shard_area_bytes(shard_ranges(N), lcn, n));
+}
+
+// the tasks (group << 32 | plane: the groups with complete worlds, in table order, then the selected planes), and the
+// slices: each the longest run of tasks that fit in kScratchCap on the rank holding the most of each group (at least
+// one task), from the rank-slotted sizes alone, so alike on every rank; Q.slices = their first tasks, then the count
+void cut_slices(RankShard &Q)
+{
+    Q.tasks.clear();
+    for (uint32_t g = 0; g < Q.n_global.size(); ++g)
+        if (Q.n_global[g])
+            for (uint32_t j = 0; j < Q.S.n_p; ++j) Q.tasks.push_back((uint64_t)g << 32 | j);
+    Q.slices.clear();
+    const auto most = [&](uint64_t t) {
+        const uint64_t g = Q.tasks[t] >> 32;
+        return task_bytes_of(Q.n_global[g], Q.l_most[g], Q.w_most[g]);
+    };
+    for (uint64_t t = 0; t < Q.tasks.size();) {
+        Q.slices.push_back(t);
+        uint64_t bytes = kHeader + most(t);
+        for (++t; t < Q.tasks.size(); ++t) {
+            if (bytes + most(t) > kScratchCap || t - Q.slices.back() == kMaxSliceTasks) break;
+            bytes += most(t);
+        }
+    }
+    Q.slices.push_back(Q.tasks.size());
+}
+
+// the rows of slice k (their areas: this rank's) and the slice's bytes of scratch
+std::vector<SRow> slice_rows(const RankShard &Q, uint64_t k, uint64_t *bytes)
+{
+    const uint64_t t0 = Q.slices[k], T = Q.slices[k + 1] - t0;
+    std::vector<SRow> rows(T);
+    uint64_t off = slice_header(T).areas, K = 0;
+    for (uint64_t i = 0; i < T; ++i) {
+        const uint32_t g = (uint32_t)(Q.tasks[t0 + i] >> 32), j = (uint32_t)Q.tasks[t0 + i];
+        const WorldGroup &wg = Q.table[g];
+        const uint64_t N = Q.n_global[g], R = shard_ranges(N), lcn = Q.n_local[g];
+        const uint32_t Wc = chunk_of(wg.n, T), C = (uint32_t)((wg.n + Wc - 1) / Wc);
+        rows[i] = SRow{off, (uint32_t)wg.o, (uint32_t)wg.n, Wc, C, (uint32_t)K, j, (uint32_t)R, (uint32_t)N,
+                       (uint32_t)lcn, 0};
+        off += align8(shard_area_bytes(R, lcn, wg.n));
+        K += C;
+    }
+    *bytes = off;
+    return rows;
+}
+
+struct SliceRun {
+    SLayout L;
+    uint64_t K;           // chunks of the rank's worlds
+    unsigned grid, per_task;
+    std::vector<SRow> rows;
+};
+
+SliceRun slice_run(const RankShard &Q)
+{
+    SliceRun r;
+    uint64_t bytes = 0;
+    r.rows = slice_rows(Q, Q.slice, &bytes);
+    const uint64_t T = r.rows.size();
+    const SliceHeader H = slice_header(T);
+    char *base = (char *)Q.area;
+    r.L = SLayout{T, (const SRow *)(base + H.rows), (TaskState *)(base + H.st),
+                  (const uint64_t *)(base + H.hoff0), (const uint64_t *)(base + H.hoff1),
+                  (const uint64_t *)(base + H.xk), base, Q.pool[0], Q.pool[1], Q.x, Q.rank, Q.n_ranks};
+    r.K = 0;
+    for (const SRow &row : r.rows) r.K += row.C;
+    r.grid = (unsigned)std::min(r.K, kGridCap);
+    r.per_task = (unsigned)std::max<uint64_t>(1, 8ull * kNumSMs / T);
+    return r;
+}
+
+#define RTRY(call)                        \
+    do {                                  \
+        const cudaError_t e_ = (call);    \
+        if (e_ != cudaSuccess) return e_; \
+    } while (0)
+
+// a grow-only buffer of at least `need` bytes, once the stream is done with the old one
+cudaError_t grow(void **p, uint64_t *have, uint64_t need, cudaStream_t s)
+{
+    if (*have >= need) return cudaSuccess;
+    RTRY(cudaStreamSynchronize(s));
+    if (*p) RTRY(cudaFree(*p));
+    *p = nullptr;
+    *have = 0;
+    RTRY(cudaMalloc(p, need));
+    *have = need;
+    return cudaSuccess;
+}
+
+// offsets packed in task order, words[t] each, into the header's array at `where`; their total
+uint64_t set_offsets(const RankShard &Q, uint64_t where, const std::vector<uint64_t> &words, cudaStream_t s,
+                     cudaError_t *e)
+{
+    std::vector<uint64_t> off(words.size());
+    uint64_t total = 0;
+    for (size_t t = 0; t < words.size(); ++t) {
+        off[t] = total;
+        total += words[t];
+    }
+    *e = cudaMemcpyAsync((char *)Q.area + where, off.data(), off.size() * 8, cudaMemcpyHostToDevice, s);
+    return total;
+}
+
+// start exchange `step` of `bytes` (> 0) whose words the stream is writing into Q.x: its first round
+cudaError_t start(RankShard &Q, int step, uint64_t bytes, void *partial, uint64_t *partial_bytes, cudaStream_t s)
+{
+    Q.step = step;
+    Q.xbytes = bytes;
+    Q.xpos = 0;
+    const uint64_t n = std::min(bytes, kRoundCap);
+    RTRY(cudaMemcpyAsync(partial, Q.x, n, cudaMemcpyDefault, s));
+    RTRY(cudaStreamSynchronize(s));
+    *partial_bytes = n;
+    return cudaGetLastError();
+}
+
+// the slice's task states, after a plan
+cudaError_t read_states(RankShard &Q, const SliceRun &r, cudaStream_t s)
+{
+    Q.st.resize(r.L.T);
+    RTRY(cudaMemcpyAsync(Q.st.data(), r.L.st, r.L.T * sizeof(TaskState), cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+}
+
+// the window of the slice's buckets whose first key is in [s0, s1) (keys <= kCap past s1): its offsets exchange
+cudaError_t open_window(RankShard &Q, void *partial, uint64_t *partial_bytes, int *launches, cudaStream_t s)
+{
+    const uint64_t s0 = Q.window * Q.wkeys, s1 = std::min(s0 + Q.wkeys, Q.keys);
+    const uint64_t bytes = (s1 - s0) * Q.n_ranks * 4;
+    // room for the keys exchange too: it follows in the same words, without a sync in between
+    RTRY(grow((void **)&Q.x, &Q.x_bytes, std::max(bytes, (std::min(s1 + kCap, Q.keys) - s0) * 8), s));
+    SliceRun r = slice_run(Q);
+    RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+    shard_window_kernel<<<dim3(r.per_task, (unsigned)r.L.T), 256, 0, s>>>(r.L, s0, s1, 0);
+    *launches += 1;
+    return start(Q, kOffsets, bytes, partial, partial_bytes, s);
+}
+
+// after plan `level` of the slice: the next level's histogram exchange, or the scatter and the windows of the buckets,
+// or the slice's end (Q.step = kDone)
+cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial_bytes, int *launches, cudaStream_t s)
+{
+    SliceRun r = slice_run(Q);
+    RTRY(read_states(Q, r, s));
+    const uint64_t T = r.L.T;
+    const SliceHeader H = slice_header(T);
+    std::vector<uint64_t> words(T);
+    uint64_t refine = 0, keys = 0;
+    for (uint64_t t = 0; t < T; ++t) {
+        refine += Q.st[t].nr[level + 1] > 0;
+        keys += Q.st[t].bucket_worlds;
+    }
+    cudaError_t e = cudaSuccess;
+    if (refine && level < kLevels) {
+        const int next = level + 1, p = next & 1;
+        for (uint64_t t = 0; t < T; ++t) words[t] = (uint64_t)Q.st[t].nr[next] * kBins;
+        const uint64_t total = set_offsets(Q, p ? H.hoff1 : H.hoff0, words, s, &e);
+        RTRY(e);
+        RTRY(grow((void **)&Q.pool[p], &Q.pool_bytes[p], total * 4, s));
+        RTRY(grow((void **)&Q.x, &Q.x_bytes, total * 4, s));
+        r = slice_run(Q);
+        RTRY(cudaMemsetAsync(Q.pool[p], 0, total * 4, s));
+        Q.reads += refine;
+        if (r.grid) {
+            shard_pass_kernel<<<r.grid, kPassThreads, 0, s>>>(Q.S, r.K, r.L, next);
+            *launches += 1;
+        }
+        RTRY(cudaMemcpyAsync(Q.x, Q.pool[p], total * 4, cudaMemcpyDeviceToDevice, s));
+        Q.level = next;
+        return start(Q, kHist, total * 4, partial, partial_bytes, s);
+    }
+    Q.reads += T;
+    if (r.grid) {
+        shard_scatter_kernel<<<r.grid, kPassThreads, 0, s>>>(Q.S, r.K, r.L);
+        *launches += 1;
+    }
+    if (keys) {
+        for (uint64_t t = 0; t < T; ++t) words[t] = Q.st[t].bucket_worlds;
+        Q.keys = set_offsets(Q, H.xk, words, s, &e);
+        RTRY(e);
+        // an offsets window of wkeys * n_ranks u32 and its keys (up to kCap past it) are both one round below the cap
+        Q.wkeys = std::max<uint64_t>(1, std::min((kRoundCap - kCap * 8ull) / 8, kRoundCap / (4ull * Q.n_ranks)) - 1);
+        Q.window = 0;
+        return open_window(Q, partial, partial_bytes, launches, s);
+    }
+    Q.step = kDone;  // the caller opens the next slice
+    return cudaGetLastError();
+}
+
+cudaError_t open_slice(RankShard &Q, void *partial, uint64_t *partial_bytes, int *launches, cudaStream_t s)
+{
+    const SliceRun r = slice_run(Q);
+    RTRY(cudaMemcpyAsync((void *)r.L.rows, r.rows.data(), r.rows.size() * sizeof(SRow), cudaMemcpyHostToDevice, s));
+    shard_init_kernel<<<dim3(r.per_task, (unsigned)r.L.T), 256, 0, s>>>(r.L, Q.S.mask);
+    shard_plan0_kernel<<<(unsigned)((r.L.T + 127) / 128), 128, 0, s>>>(r.L);
+    *launches += 2;
+    return after_plan(Q, 0, partial, partial_bytes, launches, s);
+}
+
+} // namespace
+
+uint64_t sharded_rank_round_bytes() { return kRoundCap; }
+
+// a world state names a bin of its task's ranges below the piece flag: R * kBins < 2^31
+uint64_t sharded_rank_max_worlds() { return (kPiece / kBins) * (kCap + 1ull) - 1; }
+
+void rank_shard_free(RankShard &Q)
+{
+    for (void *p : {Q.area, (void *)Q.x, (void *)Q.pool[0], (void *)Q.pool[1]})
+        if (p) cudaFree(p);
+    Q.area = nullptr;
+    Q.x = Q.pool[0] = Q.pool[1] = nullptr;
+    Q.area_bytes = Q.x_bytes = Q.pool_bytes[0] = Q.pool_bytes[1] = 0;
+}
+
+cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial, uint64_t *partial_bytes, int *launches,
+                               cudaStream_t s)
+{
+    *partial_bytes = 0;
+    *launches = 0;
+    const uint64_t G = Q.table.size();
+    if (Q.step == kStart) {  // the completeness mask, then the sizes
+        const uint64_t bytes = G * Q.n_ranks * 8;
+        RTRY(grow((void **)&Q.x, &Q.x_bytes, bytes, s));
+        RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+        uint64_t W = 0;
+        for (const WorldGroup &wg : Q.table) W = std::max(W, wg.o + wg.n);
+        if (W) {
+            rank_mask_kernel<<<(unsigned)std::min<uint64_t>((W + 255) / 256, kGridCap), 256, 0, s>>>(Q.S, W);
+            shard_size_kernel<<<(unsigned)std::min<uint64_t>(G, kGridCap), 256, 0, s>>>(Q.S, G, Q.x, Q.rank, Q.n_ranks);
+            *launches += 2;
+        }
+        return start(Q, kSizes, bytes, partial, partial_bytes, s);
+    }
+    if (Q.step == kDone) return cudaSuccess;
+    // the sums of the round last sent
+    const uint64_t n = std::min(Q.xbytes - Q.xpos, kRoundCap);
+    RTRY(cudaMemcpyAsync((char *)Q.x + Q.xpos, reduced, n, cudaMemcpyDefault, s));
+    Q.xpos += n;
+    if (Q.xpos < Q.xbytes) {  // the exchange's next round
+        const uint64_t m = std::min(Q.xbytes - Q.xpos, kRoundCap);
+        RTRY(cudaMemcpyAsync(partial, (char *)Q.x + Q.xpos, m, cudaMemcpyDefault, s));
+        RTRY(cudaStreamSynchronize(s));
+        *partial_bytes = m;
+        return cudaGetLastError();
+    }
+    if (Q.step == kSizes) {
+        std::vector<uint32_t> words(G * Q.n_ranks * 2);
+        RTRY(cudaMemcpyAsync(words.data(), Q.x, words.size() * 4, cudaMemcpyDeviceToHost, s));
+        RTRY(cudaStreamSynchronize(s));
+        Q.n_global.assign(G, 0);
+        Q.n_local.assign(G, 0);
+        Q.l_most.assign(G, 0);
+        Q.w_most.assign(G, 0);
+        for (uint64_t g = 0; g < G; ++g) {
+            for (uint32_t k = 0; k < Q.n_ranks; ++k) {
+                const uint32_t *w = &words[(g * Q.n_ranks + k) * 2];
+                Q.n_global[g] += w[0];
+                Q.l_most[g] = std::max<uint64_t>(Q.l_most[g], w[0]);
+                Q.w_most[g] = std::max<uint64_t>(Q.w_most[g], w[1]);
+            }
+            Q.n_local[g] = words[(g * Q.n_ranks + Q.rank) * 2];
+            if (Q.bad_group == ~0ull && Q.n_global[g] > sharded_rank_max_worlds()) Q.bad_group = g;
+        }
+        if (Q.bad_group != ~0ull) {
+            Q.step = kDone;
+            return cudaSuccess;
+        }
+        cut_slices(Q);
+        uint64_t most = 0;
+        for (Q.slice = 0; Q.slice + 1 < Q.slices.size(); ++Q.slice) {
+            uint64_t bytes = 0;
+            slice_rows(Q, Q.slice, &bytes);
+            most = std::max(most, bytes);
+        }
+        RTRY(grow(&Q.area, &Q.area_bytes, std::max<uint64_t>(most, 8), s));
+        Q.slice = 0;
+        Q.step = kDone;
+    } else {
+        SliceRun r = slice_run(Q);
+        const uint64_t T = r.L.T;
+        if (Q.step == kHist) {
+            shard_plan_kernel<<<dim3(1, (unsigned)T), kShardPlanThreads, 0, s>>>(r.L, Q.level);
+            *launches += 1;
+            RTRY(after_plan(Q, Q.level, partial, partial_bytes, launches, s));
+            if (Q.step != kDone) return cudaSuccess;
+        } else {
+            const uint64_t s0 = Q.window * Q.wkeys, s1 = std::min(s0 + Q.wkeys, Q.keys);
+            if (Q.step == kOffsets) {  // the offsets applied, then this rank's keys of the window
+                const uint64_t bytes = (std::min(s1 + kCap, Q.keys) - s0) * 8;
+                shard_window_kernel<<<dim3(r.per_task, (unsigned)T), 256, 0, s>>>(r.L, s0, s1, 1);
+                RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+                shard_window_kernel<<<dim3(r.per_task, (unsigned)T), 256, 0, s>>>(r.L, s0, s1, 2);
+                *launches += 2;
+                return start(Q, kKeys, bytes, partial, partial_bytes, s);
+            }
+            RTRY(cudaFuncSetAttribute(shard_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCap * 12)));
+            shard_finish_kernel<<<dim3(r.per_task, (unsigned)T), kPlanThreads, kCap * 12, s>>>(Q.S, r.L, s0, s1);
+            *launches += 1;
+            if (s1 < Q.keys) {
+                ++Q.window;
+                return open_window(Q, partial, partial_bytes, launches, s);
+            }
+        }
+        ++Q.slice;
+    }
+    // the slice just ended (or the sizes): open slices until one makes an exchange
+    while (Q.slice + 1 < Q.slices.size()) {
+        RTRY(open_slice(Q, partial, partial_bytes, launches, s));
+        if (Q.step != kDone) return cudaSuccess;
+        ++Q.slice;
+    }
+    Q.step = kDone;
+    RTRY(cudaStreamSynchronize(s));
+    return cudaGetLastError();
+}
+
+#undef RTRY
 
 } // namespace b200

@@ -751,6 +751,7 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->sum_dwell) cudaFree(h->sum_dwell);
     if (h->out_planes) cudaFree(h->out_planes);
     if (h->rank_planes) cudaFree(h->rank_planes);
+    rank_shard_free(h->sr.Q);
     for (const auto *ts : {h->tables, h->out_tables})
         for (int g = 0; g < 2; ++g)
             for (void *p : {(void *)ts[g].stats_dev, (void *)ts[g].cov_dev, (void *)ts[g].order_dev})
@@ -2595,13 +2596,14 @@ double b200_sixdof_top_worlds_reads(const b200_sixdof *h) { return h ? h->topk_r
 // dst: as [n_worlds][n_p] rows, or (corr) as the rank correlation records, the covariance of the rank planes (the
 // covariance kernels, unchanged) turned into [n, rho].  The outcome set and groups checked, then the selection, then
 // `bytes`, then the handle's status.  The outcome planes are only read.
-static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *planes, uint32_t n_p, void *dst,
-                     uint64_t bytes)
+// The checks of a rank call on the outcome set, groups and selection, in order (run_ranks); least: the fewest planes
+static int rank_selection(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t least,
+                          const char *what)
 {
-    int rc = reduction_ready(h, Rows::outcomes, grouped, corr ? "outcome rank correlation" : "outcome ranks");
+    int rc = reduction_ready(h, Rows::outcomes, grouped, what);
     if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
-    const uint32_t P = (uint32_t)h->outcomes.size(), least = corr ? 2 : 1;
+    const uint32_t P = (uint32_t)h->outcomes.size();
     if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null rank planes");
     if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u rank planes: %u to %u", n_p, least, P);
     uint64_t seen = 0;
@@ -2611,17 +2613,17 @@ static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *pl
         if (seen & (1ull << planes[j])) return fail(B200_ERR_INVALID_ARGUMENT, "rank plane %u listed twice", planes[j]);
         seen |= 1ull << planes[j];
     }
-    const uint64_t G = reduction_groups(h, grouped).size(), W = h->desc.n_worlds;
-    const uint64_t want = corr ? G * (1ull + (uint64_t)n_p * n_p) * 8ull : W * n_p * 8ull;
-    if (bytes != want)
-        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome %s %llu bytes, got %llu", corr ? "rank correlation is" : "ranks are",
-                    (unsigned long long)want, (unsigned long long)bytes);
-    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
-    if (bytes == 0) return B200_OK;
+    return B200_OK;
+}
+
+// The parameters of a rank call over the handle's rank planes (grown to n_p planes)
+static int rank_params(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, RankParams &S)
+{
     const uint64_t ld = h->ld_o;
-    if ((rc = grow_device(h, &h->rank_planes, &h->rank_bytes, n_p * ld * 8ull + ld))) return rc;
+    const int rc = grow_device(h, &h->rank_planes, &h->rank_bytes, n_p * ld * 8ull + ld);
+    if (rc) return rc;
     const b200_sixdof::GroupTables &t = reduction_tables(h, Rows::outcomes, grouped);
-    RankParams S{};
+    S = RankParams{};
     S.planes = h->out_planes;
     S.ld = ld;
     S.n_p = n_p;
@@ -2630,6 +2632,45 @@ static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *pl
     S.order = t.order_dev;
     S.ranks = h->rank_planes;
     S.mask = (uint8_t *)(h->rank_planes + n_p * ld);
+    return B200_OK;
+}
+
+// The covariance of the rank planes as the state of a handle with one entity
+static CovParams rank_cov_params(const b200_sixdof *h, uint32_t n_p)
+{
+    CovParams C{};
+    C.seg[0] = {h->rank_planes, n_p, n_p * h->ld_o};
+    C.n_segs = 1;
+    C.planes_per_sample = n_p;
+    C.n_planes = n_p;
+    C.ld = h->ld_o;
+    C.n_worlds = h->desc.n_worlds;
+    C.n_entities = 1;
+    C.n_p = n_p;
+    for (uint32_t j = 0; j < n_p; ++j) C.planes[j] = j;
+    return C;
+}
+
+static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *planes, uint32_t n_p, void *dst,
+                     uint64_t bytes)
+{
+    if (h) {  // it rewrites the rank planes a sharded call fills
+        h->sr.active = false;
+        rank_shard_free(h->sr.Q);
+    }
+    int rc = rank_selection(h, grouped, planes, n_p, corr ? 2 : 1, corr ? "outcome rank correlation" : "outcome ranks");
+    if (rc) return rc;
+    const uint64_t G = reduction_groups(h, grouped).size(), W = h->desc.n_worlds;
+    const uint64_t want = corr ? G * (1ull + (uint64_t)n_p * n_p) * 8ull : W * n_p * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome %s %llu bytes, got %llu", corr ? "rank correlation is" : "ranks are",
+                    (unsigned long long)want, (unsigned long long)bytes);
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (bytes == 0) return B200_OK;
+    const uint64_t ld = h->ld_o;
+    RankParams S;
+    if ((rc = rank_params(h, grouped, planes, n_p, S))) return rc;
+    const b200_sixdof::GroupTables &t = reduction_tables(h, Rows::outcomes, grouped);
     const uint64_t tasks = G * n_p, rank_scratch = rank_scratch_bytes(S, t.stats, t.order);
     h->rank_read_sum = tasks;  // the small-group routes read every task once
     if (!corr) {
@@ -2640,17 +2681,8 @@ static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *pl
             return launch_soa_to_aos(h->rank_planes, out, W, n_p, ld, h->stream);
         });
     } else {
-        // the covariance of the rank planes as the state of a handle with one entity, its table before the scratch
-        CovParams C{};
-        C.seg[0] = {h->rank_planes, n_p, n_p * ld};
-        C.n_segs = 1;
-        C.planes_per_sample = n_p;
-        C.n_planes = n_p;
-        C.ld = ld;
-        C.n_worlds = W;
-        C.n_entities = 1;
-        C.n_p = n_p;
-        for (uint32_t j = 0; j < n_p; ++j) C.planes[j] = j;
+        // the covariance of the rank planes, its table before the scratch
+        CovParams C = rank_cov_params(h, n_p);
         const uint64_t table = G * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
         const uint64_t scratch = table + std::max(rank_scratch, cov_scratch_bytes(C, t.cov));
         rc = run_world_reduction(h, Rows::outcomes, false, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
@@ -2690,6 +2722,139 @@ int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *p
 }
 
 double b200_sixdof_rank_reads(const b200_sixdof *h) { return h ? h->rank_reads : 0.0; }
+
+// ---- world-sharded ranks (rank_kernels.cu: sharded_rank_round) ----
+
+int b200_sixdof_sharded_ranks_begin(b200_sixdof *h, int grouped, const uint32_t *planes, uint32_t n_p, uint32_t rank,
+                                    uint32_t n_ranks, uint64_t *max_round_bytes)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (!max_round_bytes) return fail(B200_ERR_INVALID_ARGUMENT, "null max_round_bytes");
+    h->sr.active = false;  // a call still pending is discarded, and its scratch freed
+    rank_shard_free(h->sr.Q);
+    int rc = rank_selection(h, grouped != 0, planes, n_p, 1, "sharded outcome ranks");
+    if (rc) return rc;
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (rank >= n_ranks) return fail(B200_ERR_INVALID_ARGUMENT, "rank %u of %u ranks", rank, n_ranks);
+    RankParams S;
+    if ((rc = write_outcomes(h)) || (rc = rank_params(h, grouped != 0, planes, n_p, S))) return rc;
+    b200_sixdof::ShardedRanks &c = h->sr;
+    RankShard &Q = c.Q;
+    Q.S = S;
+    Q.table = reduction_tables(h, Rows::outcomes, grouped != 0).stats;
+    Q.rank = rank;
+    Q.n_ranks = n_ranks;
+    Q.step = 0;
+    Q.level = 0;
+    Q.xbytes = Q.xpos = 0;
+    Q.slices.clear();
+    Q.slice = 0;
+    Q.bad_group = ~0ull;
+    Q.reads = 0;
+    c.grouped = grouped != 0;
+    c.gen = rows_generation(h, true);
+    c.partial_bytes = 0;
+    c.tasks = Q.table.size() * n_p;
+    c.ready = false;
+    c.active = true;
+    *max_round_bytes = sharded_rank_round_bytes();
+    return B200_OK;
+}
+
+// the checks every round and end make first: a call begun, on the outcome planes it began on
+static int sharded_ranks_pending(b200_sixdof *h, const char *what)
+{
+    if (!h) return fail(B200_ERR_INVALID_ARGUMENT, "null handle");
+    if (!h->sr.active) return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks %s without a begin", what);
+    if (h->sr.gen != rows_generation(h, true)) {
+        h->sr.active = false;
+        rank_shard_free(h->sr.Q);
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks %s: the handle's outcomes changed since the begin", what);
+    }
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    return B200_OK;
+}
+
+int b200_sixdof_sharded_ranks_round(b200_sixdof *h, const void *reduced, uint64_t reduced_bytes, void *partial,
+                                    uint64_t partial_cap, uint64_t *partial_bytes)
+{
+    int rc = sharded_ranks_pending(h, "round");
+    if (rc) return rc;
+    b200_sixdof::ShardedRanks &c = h->sr;
+    if (c.ready) return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: the ranks are ready, call the end");
+    if (reduced_bytes != c.partial_bytes)
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: %llu reduced bytes, the last round sent %llu",
+                    (unsigned long long)reduced_bytes, (unsigned long long)c.partial_bytes);
+    if (reduced_bytes && !reduced) return fail(B200_ERR_INVALID_ARGUMENT, "null reduced words");
+    if (!partial_bytes) return fail(B200_ERR_INVALID_ARGUMENT, "null partial_bytes");
+    const uint64_t most = sharded_rank_round_bytes();
+    if (partial_cap < most || !partial)
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: a partial of %llu bytes, the begin asked for %llu",
+                    (unsigned long long)partial_cap, (unsigned long long)most);
+    CU(h, cudaSetDevice(h->device));
+    int launches = 0;
+    uint64_t out = 0;
+    const cudaError_t e = sharded_rank_round(c.Q, reduced, partial, &out, &launches, h->stream);
+    h->timings.kernel_launches += (uint64_t)launches;
+    if (e == cudaErrorMemoryAllocation) {  // not sticky: the call ends, the handle stays usable
+        (void)cudaGetLastError();
+        c.active = false;
+        rank_shard_free(c.Q);
+        return fail(B200_ERR_OUT_OF_MEMORY, "sharded ranks: out of device memory for the call's scratch");
+    }
+    if (e != cudaSuccess) {
+        c.active = false;
+        return cuda_fail(h, e, "sharded_rank_round");
+    }
+    if (c.Q.bad_group != ~0ull) {
+        c.active = false;
+        rank_shard_free(c.Q);
+        const uint64_t g = c.Q.bad_group;
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: group %llu holds %llu complete worlds over the ranks, above "
+                    "the %llu a task can index", (unsigned long long)g, (unsigned long long)c.Q.n_global[g],
+                    (unsigned long long)sharded_rank_max_worlds());
+    }
+    c.partial_bytes = *partial_bytes = out;
+    c.ready = out == 0;
+    return B200_OK;
+}
+
+int b200_sixdof_sharded_ranks_end(b200_sixdof *h, void *ranks_dst, uint64_t ranks_bytes, void *cov_dst,
+                                  uint64_t cov_bytes)
+{
+    int rc = sharded_ranks_pending(h, "end");
+    if (rc) return rc;
+    b200_sixdof::ShardedRanks &c = h->sr;
+    if (!c.ready) return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: end before the last round");
+    rank_shard_free(c.Q);  // the rank planes hold the result
+    const uint32_t n_p = c.Q.S.n_p;
+    const uint64_t W = h->desc.n_worlds, G = c.Q.table.size();
+    const uint64_t want_r = W * n_p * 8ull, want_c = G * (1ull + n_p + (uint64_t)n_p * n_p) * 8ull;
+    if (ranks_dst && ranks_bytes != want_r)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "sharded ranks are %llu bytes, got %llu", (unsigned long long)want_r,
+                    (unsigned long long)ranks_bytes);
+    if (cov_dst && cov_bytes != want_c)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "sharded rank covariance is %llu bytes, got %llu",
+                    (unsigned long long)want_c, (unsigned long long)cov_bytes);
+    if (ranks_dst)
+        rc = run_world_reduction(h, Rows::outcomes, false, 0, ranks_dst, ranks_bytes, [&](double *out, void *, int *n) {
+            *n = 1;
+            return launch_soa_to_aos(h->rank_planes, out, W, n_p, h->ld_o, h->stream);
+        });
+    if (!rc && cov_dst) {
+        const b200_sixdof::GroupTables &t = reduction_tables(h, Rows::outcomes, c.grouped);
+        CovParams C = rank_cov_params(h, n_p);
+        rc = run_world_reduction(h, Rows::outcomes, false, cov_scratch_bytes(C, t.cov), cov_dst, cov_bytes,
+                                 [&](double *out, void *scratch, int *n) {
+                                     C.out = out;
+                                     return launch_covariance(C, t.cov_dev, t.cov, scratch, n, h->stream);
+                                 });
+    }
+    if (rc) return rc;
+    h->rank_reads = c.tasks ? (double)c.Q.reads / (double)c.tasks : 0.0;
+    c.active = false;
+    return B200_OK;
+}
 
 int b200_sixdof_trajectory_reset(b200_sixdof *h)
 {

@@ -76,6 +76,14 @@ struct b200_sixdof {
         uint64_t gen = 0, partial_bytes = 0, max_round = 0, table_bytes = 0, triples = 0;
         b200::QuantileShard Q;
     } sq;
+    // a world-sharded rank call (b200_sixdof_sharded_ranks_*) between begin and end: its state (which owns its device
+    // scratch), the write generation of the outcome planes at begin; it fills the rank planes above, so an unsharded
+    // rank call discards it
+    struct ShardedRanks {
+        bool active = false, ready = false, grouped = false;
+        uint64_t gen = 0, partial_bytes = 0, tasks = 0;
+        b200::RankShard Q;
+    } sr;
     uint64_t rows_gen = 0;
     uint64_t sum_gen = 0;  // bumped by every summary start and fold: what the outcome planes are computed from
     double *sq_scratch = nullptr;

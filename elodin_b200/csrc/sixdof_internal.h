@@ -503,5 +503,56 @@ cudaError_t launch_ranks(const RankParams &S, uint64_t n_worlds, const std::vect
 // not > 0.  One launch (*launches = 1).
 cudaError_t launch_rank_correlation(const double *cov, double *out, uint64_t G, uint32_t n_p, int *launches,
                                     cudaStream_t s);
+// A rank's part of a world-sharded rank call between its rounds (b200_sixdof_sharded_ranks_*): the MSD bucket pass over
+// every (group, plane) task, slice by slice, each exchange's u32 words summed over the ranks before the step that reads
+// them.  The exchanges, in order: the group sizes (once per call), then per slice at most 5 histograms, then per window
+// of the slice's buckets their local counts and their keys; none passes sharded_rank_round_bytes() but the histograms,
+// which are sent in rounds of at most that many bytes.
+struct RankShard {
+    // one per task of the slice, in device scratch, copied back after every plan
+    struct TaskState {
+        uint32_t N;              // complete worlds over every rank
+        uint32_t lcn;            // complete worlds on this rank
+        uint32_t level;          // the level whose codes name the worlds' bins
+        uint32_t nr[7];          // ranges of each level
+        uint32_t n_buckets;      // buckets, numbered in the same order on every rank
+        uint32_t bucket_worlds;  // the buckets' worlds over every rank: the task's key words
+        uint32_t local_worlds;   // the buckets' worlds on this rank
+        uint32_t n_pieces;       // the pieces that hold worlds of this rank
+        uint32_t pad[2];
+    };
+    RankParams S;                   // S.ranks, S.mask: the handle's rank planes
+    std::vector<WorldGroup> table;  // the rank's part of every group (only o and n are read)
+    uint32_t rank = 0, n_ranks = 1;
+    // device buffers, grown during the call and freed by rank_shard_free: the slices' task areas, the two level pools
+    // of histograms and the words of the exchange in flight
+    void *area = nullptr;
+    uint64_t area_bytes = 0;
+    uint32_t *pool[2] = {nullptr, nullptr};
+    uint64_t pool_bytes[2] = {0, 0};
+    uint32_t *x = nullptr;
+    uint64_t x_bytes = 0;
+    int step = 0;                   // the exchange in flight (0: none yet)
+    int level = 0;                  // the histogram level of a histogram exchange
+    uint64_t xbytes = 0, xpos = 0;  // its size, and where the round last sent starts
+    // per group: complete worlds over every rank and on this one, and the most complete worlds and worlds one rank holds
+    std::vector<uint64_t> n_global, n_local, l_most, w_most;
+    std::vector<uint64_t> tasks;    // group << 32 | plane
+    std::vector<uint64_t> slices;   // the first task of every slice, then the task count
+    uint64_t slice = 0;
+    std::vector<TaskState> st;      // the slice's task states after the last plan
+    uint64_t keys = 0, wkeys = 0, window = 0;  // the slice's key words, a window's, the window in flight
+    uint64_t bad_group = ~0ull;     // a group of too many complete worlds over the ranks: the call fails
+    unsigned long long reads = 0;   // reads of the planes summed over the tasks
+};
+// the largest round of a sharded rank call in bytes, and the most complete worlds a group may hold over the ranks
+uint64_t sharded_rank_round_bytes();
+uint64_t sharded_rank_max_worlds();
+// One round on s, returning once the round's words are in `partial` (host or device memory): the sums of the last
+// round's words from `reduced` (nothing before the first round), then the launches up to the next round's words
+// (*partial_bytes; 0 once the rank planes hold the midranks of the rank's worlds, or once Q.bad_group is set).
+cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial, uint64_t *partial_bytes, int *launches,
+                               cudaStream_t s);
+void rank_shard_free(RankShard &Q);
 
 } // namespace b200

@@ -631,6 +631,39 @@ class B200Exec:
         """Reads of the outcome planes the last rank call made, averaged over its (group, plane) tasks."""
         return float(self._L.b200_sixdof_rank_reads(self._h))
 
+    # ---- world-sharded ranks: the midranks of the union of every rank's worlds, in rounds ----------------------------
+    def sharded_ranks_begin(self, planes, groups: bool, rank: int, n_ranks: int) -> int:
+        """Begin this rank's part of a world-sharded rank call (b200_sixdof_sharded_ranks_begin): the outcomes
+        `planes`, the grouping, this rank's index and the rank count are fixed here.  Returns the largest round in bytes
+        (the partial buffer's least size)."""
+        sel = self._selection(planes)
+        mx = C.c_uint64(0)
+        _lib.check(self._L.b200_sixdof_sharded_ranks_begin(self._h, int(bool(groups)), sel[0], sel[1], int(rank),
+                                                            int(n_ranks), C.byref(mx)))
+        self._sr_shape = (sel[1], self.world_groups if groups else 1)
+        return int(mx.value)
+
+    def sharded_ranks_round(self, reduced, reduced_bytes: int, partial) -> int:
+        """One round, as sharded_quantiles_round; 0: the ranks are ready (sharded_ranks_end)."""
+        rp, _ = self._words(reduced)
+        pp, pcap = self._words(partial)
+        out = C.c_uint64(0)
+        _lib.check(self._L.b200_sixdof_sharded_ranks_round(self._h, C.c_void_p(rp), int(reduced_bytes), C.c_void_p(pp),
+                                                            pcap, C.byref(out)))
+        return int(out.value)
+
+    def sharded_ranks_end(self, ranks: bool = True, covariance: bool = True) -> tuple:
+        """(ranks [n_worlds, p] or None, covariance [G or 1, 1 + p + p*p] or None): the campaign midranks of this
+        rank's worlds, with the bits of outcome_[group_]ranks on one handle holding every rank's worlds in rank order,
+        and the covariance records of this rank's rank planes (merge them over the ranks with merge_covariance)."""
+        p, G = getattr(self, "_sr_shape", (0, 1))
+        r = np.empty((self.n_worlds, p)) if ranks else None
+        c = np.empty((G, 1 + p + p * p)) if covariance else None
+        ptr = lambda a: C.c_void_p(a.ctypes.data if a is not None else None)
+        _lib.check(self._L.b200_sixdof_sharded_ranks_end(self._h, ptr(r), r.nbytes if ranks else 0, ptr(c),
+                                                          c.nbytes if covariance else 0))
+        return r, c
+
     # ---- run summaries (reductions over the time axis, per world, on the device) --------------------------------
     @staticmethod
     def _conditions(rows: Sequence):

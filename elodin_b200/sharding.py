@@ -144,32 +144,24 @@ def _quantile_descriptor(ex, levels: np.ndarray, source: str, groups: bool, stat
             + [int(b) for b in bits.view(np.int64)] + [int(ex.n_worlds), int(status)])
 
 
-def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=None) -> np.ndarray:
-    """Quantile tables of a world-sharded campaign, exact over every rank's worlds: every rank passes its executor (its
-    own worlds; with `groups`, the global groups cut to them by shard_groups), the same levels `q` and the same source
-    ("ring", "state" or "outcomes"); the ranks run b200_sixdof_sharded_quantiles_* in lockstep, summing each round's
-    u32 words with one all-reduce (on a CUDA buffer for NCCL groups, host memory for gloo).  Every rank returns the table
-    of trajectory_ / state_ / outcome_[group_]quantiles(q) on one executor holding every rank's worlds in rank order,
-    bit for bit.  Before the first round the ranks all-gather a descriptor of their calls; a disagreement, a global
-    world count of 2^32 or more, or any rank's failure (then or in a later round) raises the same error on every
-    rank."""
+def _sharded_call(what: str, args: str, fields: str, begin, descriptor, round_, end, arg_err, group,
+                  world_cap: Optional[int] = None):
+    """The lockstep protocol of a sharded call (b200_sixdof_sharded_quantiles_* / _ranks_*), on every rank: `begin()`
+    (returning the largest round in bytes; None when `arg_err`, an argument this rank cannot use, is set), then an
+    all-gather of `descriptor(status)` (int words, ending with the rank's worlds and its begin's status), then the
+    rounds of `round_(reduced, reduced_bytes, partial)` with their u32 words summed by one all-reduce each (on a CUDA
+    buffer for NCCL groups, host memory for gloo), then `end()`.  A disagreement in the descriptors, a global world
+    count of `world_cap` or more, or any rank's failure (at begin or in a later round) raises the same error on every
+    rank instead of leaving the others waiting.  `what` names the call, `args` its arguments and `fields` its descriptor in
+    the messages."""
     import torch.distributed as dist
 
     from . import _lib
 
-    # An argument this rank cannot use still goes through the descriptor exchange as a failed status, so that a rank
-    # whose arguments differ from the others' raises with them instead of leaving them waiting.
-    arg_err, levels = None, np.zeros(0)
-    try:
-        if source not in _lib.QUANTILE_SOURCES:
-            raise ValueError(f"quantile source {source!r}: 'ring', 'state' or 'outcomes'")
-        levels = np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
-    except (TypeError, ValueError) as e:
-        arg_err = e
     if not (dist.is_available() and dist.is_initialized()):
         if arg_err is not None:
             raise arg_err
-        raise RuntimeError("sharding.gather_quantiles needs an initialized torch.distributed process group")
+        raise RuntimeError(f"{what} needs an initialized torch.distributed process group")
     import torch
 
     cuda = dist.get_backend(group) == "nccl"
@@ -177,10 +169,10 @@ def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=No
     status, err, max_round = (_ARGUMENT_ERROR, arg_err, 0) if arg_err is not None else (0, None, 0)
     if arg_err is None:
         try:
-            max_round = ex.sharded_quantiles_begin(levels, source, groups)
+            max_round = begin()
         except _lib.B200Error as e:
             status, err = int(e.code), e
-    mine = torch.tensor(_quantile_descriptor(ex, levels, source, groups, status), dtype=torch.int64, device=dev)
+    mine = torch.tensor(descriptor(status), dtype=torch.int64, device=dev)
     every = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
     dist.all_gather(every, mine, group=group)
     every = [d.cpu().numpy() for d in every]
@@ -190,15 +182,15 @@ def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=No
             raise err
         r, code = failed[0], int(every[failed[0]][-1])
         if code == _ARGUMENT_ERROR:
-            raise ValueError(f"sharded quantiles: rank {r} passed a source or levels it cannot use")
-        raise _lib.B200Error(code, f"sharded quantiles: rank {r} could not begin (code {code})")
+            raise ValueError(f"{what}: rank {r} passed {args} it cannot use")
+        raise _lib.B200Error(code, f"{what}: rank {r} could not begin (code {code})")
     differ = [r for r, d in enumerate(every) if not np.array_equal(d[:-2], every[0][:-2])]
     if differ:
-        raise ValueError(f"sharded quantiles: rank {differ[0]} differs from rank 0 in source, grouping, levels or table "
-                         f"shape (descriptors {every[0][:9].tolist()} and {every[differ[0]][:9].tolist()})")
+        raise ValueError(f"{what}: rank {differ[0]} differs from rank 0 in {fields} (descriptors {every[0][:9].tolist()} "
+                         f"and {every[differ[0]][:9].tolist()})")
     n_worlds = sum(int(d[-2]) for d in every)
-    if n_worlds >= 1 << 32:
-        raise ValueError(f"sharded quantiles: {n_worlds} worlds in all, at most 2^32 - 1")
+    if world_cap is not None and n_worlds >= world_cap:
+        raise ValueError(f"{what}: {n_worlds} worlds in all, at most {world_cap - 1}")
 
     def settle():
         # NCCL works on its own stream and only orders torch's current stream after it; the library reads and writes
@@ -213,7 +205,7 @@ def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=No
     while True:
         ok = 1
         try:
-            nbytes = ex.sharded_quantiles_round(partial if nbytes else None, nbytes, partial)
+            nbytes = round_(partial if nbytes else None, nbytes, partial)
         except _lib.B200Error as e:
             ok, err = 0, e
         # status and round size in one collective: a failure, or ranks whose rounds differ, raise on every rank
@@ -222,14 +214,140 @@ def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=No
         ok_all, least, most = int(word[0].item()), int(word[1].item()), -int(word[2].item())
         if not ok_all:
             raise err if err is not None else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
-                                                             "sharded quantiles: a round failed on another rank")
+                                                             f"{what}: a round failed on another rank")
         if least != most:
-            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"sharded quantiles: the ranks' rounds differ ({least} to "
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{what}: the ranks' rounds differ ({least} to "
                                  f"{most} bytes): their rows or arguments are not those of one campaign")
         if nbytes == 0:
-            return ex.sharded_quantiles_end()
+            break
         dist.all_reduce(partial[: nbytes // 4], op=dist.ReduceOp.SUM, group=group)
         settle()
+    # the end's status too, so that a rank whose end fails (out of memory, say) raises on every rank before a caller's
+    # next collective
+    ok, out = 1, None
+    try:
+        out = end()
+    except _lib.B200Error as e:
+        ok, err = 0, e
+    word = torch.tensor([ok], dtype=torch.int64, device=dev)
+    dist.all_reduce(word, op=dist.ReduceOp.MIN, group=group)
+    if not int(word[0].item()):
+        raise err if not ok else _lib.B200Error(_lib.ERR_INVALID_ARGUMENT, f"{what}: the end failed on another rank")
+    return out
+
+
+def gather_quantiles(ex, q, source: str = "ring", groups: bool = False, group=None) -> np.ndarray:
+    """Quantile tables of a world-sharded campaign, exact over every rank's worlds: every rank passes its executor (its
+    own worlds; with `groups`, the global groups cut to them by shard_groups), the same levels `q` and the same source
+    ("ring", "state" or "outcomes"); the ranks run b200_sixdof_sharded_quantiles_* in lockstep, summing each round's
+    u32 words with one all-reduce (on a CUDA buffer for NCCL groups, host memory for gloo).  Every rank returns the table
+    of trajectory_ / state_ / outcome_[group_]quantiles(q) on one executor holding every rank's worlds in rank order,
+    bit for bit.  Before the first round the ranks all-gather a descriptor of their calls; a disagreement, a global
+    world count of 2^32 or more, or any rank's failure (then or in a later round) raises the same error on every
+    rank."""
+    from . import _lib
+
+    # An argument this rank cannot use still goes through the descriptor exchange as a failed status, so that a rank
+    # whose arguments differ from the others' raises with them instead of leaving them waiting.
+    arg_err, levels = None, np.zeros(0)
+    try:
+        if source not in _lib.QUANTILE_SOURCES:
+            raise ValueError(f"quantile source {source!r}: 'ring', 'state' or 'outcomes'")
+        levels = np.ascontiguousarray(np.atleast_1d(np.asarray(q, dtype=np.float64)).ravel())
+    except (TypeError, ValueError) as e:
+        arg_err = e
+    return _sharded_call("sharded quantiles", "a source or levels", "source, grouping, levels or table shape",
+                         lambda: ex.sharded_quantiles_begin(levels, source, groups),
+                         lambda status: _quantile_descriptor(ex, levels, source, groups, status),
+                         lambda *a: ex.sharded_quantiles_round(*a), lambda: ex.sharded_quantiles_end(), arg_err, group,
+                         world_cap=1 << 32)
+
+
+def _rank_descriptor(ex, sel: List[int], groups: bool, status: int) -> List[int]:
+    """What every rank of a sharded rank call must agree on, as int64 words: the planes (padded with -1), their count,
+    grouping, the group and outcome counts; then the rank's worlds and begin's status."""
+    from . import _lib
+
+    sel = sel[: _lib.MAX_OUTCOMES]
+    try:
+        shape = [int(ex.world_groups) if groups else 1, int(ex.n_outcomes)]
+    except Exception:  # noqa: BLE001 - a rank that cannot even describe its call differs from the others
+        shape = [-1, -1]
+    return sel + [-1] * (_lib.MAX_OUTCOMES - len(sel)) + [len(sel), int(bool(groups))] + shape + [int(ex.n_worlds), int(status)]
+
+
+def _rank_planes(planes, least: int = 1) -> List[int]:
+    sel = [int(p) for p in np.atleast_1d(np.asarray(planes)).ravel()]
+    if len(sel) < least or len(set(sel)) != len(sel) or min(sel, default=0) < 0:
+        raise ValueError(f"sharded ranks: planes {sel!r}, {least} or more distinct outcome planes")
+    return sel
+
+
+def _gather_rank_call(ex, planes, groups: bool, group, ranks: bool, covariance: bool):
+    """The sharded rank call (b200_sixdof_sharded_ranks_*) over every rank of `group`, with the checks of
+    gather_quantiles: this rank's (ranks, covariance records) of B200Exec.sharded_ranks_end."""
+    import torch.distributed as dist
+
+    arg_err, sel = None, []
+    try:
+        sel = _rank_planes(planes, 2 if covariance else 1)  # a correlation needs two planes, as the unsharded call
+    except (TypeError, ValueError) as e:
+        arg_err = e
+    rank = dist.get_rank(group) if dist.is_available() and dist.is_initialized() else 0
+    n_ranks = dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+    return _sharded_call("sharded ranks", "planes", "planes, grouping, group or outcome count",
+                         lambda: ex.sharded_ranks_begin(sel, groups, rank, n_ranks),
+                         lambda status: _rank_descriptor(ex, sel, groups, status), lambda *a: ex.sharded_ranks_round(*a),
+                         lambda: ex.sharded_ranks_end(ranks, covariance), arg_err, group)
+
+
+def gather_ranks(ex, planes, groups: bool = False, group=None) -> np.ndarray:
+    """Midranks of a world-sharded campaign: every rank passes its executor (its own worlds; with `groups`, the global
+    groups cut to them by shard_groups) and the same outcome `planes`; the ranks run b200_sixdof_sharded_ranks_* in
+    lockstep, as gather_quantiles does.  Every rank returns [its n_worlds, p]: the rows of its own worlds in
+    outcome_[group_]ranks(planes) on one executor holding every rank's worlds in rank order, bit for bit."""
+    return _gather_rank_call(ex, planes, groups, group, True, False)[0]
+
+
+def gather_rank_correlation(ex, planes, groups: bool = False, group=None) -> np.ndarray:
+    """Rank correlation of a world-sharded campaign: the sharded rank call of gather_ranks, then every rank's covariance
+    records of its rank planes, all-gathered and merged in rank order (merge_covariance), turned into
+    [1 + p*p] (or [G, 1 + p*p] with `groups`) records by executor.rank_correlation.  Every rank gets the same bits;
+    with one rank those of outcome_[group_]rank_correlation(planes)."""
+    from .executor import merge_covariance, rank_correlation
+
+    cov = _gather_rank_call(ex, planes, groups, group, False, True)[1]
+    merged = merge_covariance(_all_gather_tables(cov, group))
+    out = rank_correlation(merged, len(_rank_planes(planes, 2)))
+    return out if groups else out[0]
+
+
+def outcome_ranks(exec_, names=None, groups: bool = False) -> dict:
+    """Exec.outcome_ranks over every rank of a world-sharded campaign (World.build(..., process_group=pg)): a
+    collective, every rank passing the same names.  Returns this rank's dict, {name: [its n_worlds]} of campaign
+    midranks."""
+    from .world import _ranks_dict
+
+    names, planes = exec_._rank_names("outcome_ranks", names, groups, 1, sharded=True, one=True)
+    return _ranks_dict(names, gather_ranks(exec_.backend, planes, groups, exec_._pg))
+
+
+def outcome_rank_correlation(exec_, names=None, groups: bool = False) -> dict:
+    """Exec.outcome_rank_correlation over every rank of a world-sharded campaign: a collective; every rank gets the
+    same dict."""
+    from .world import _rank_correlation_dict
+
+    names, planes = exec_._rank_names("outcome_rank_correlation", names, groups, 2, sharded=True)
+    return _rank_correlation_dict(names, gather_rank_correlation(exec_.backend, planes, groups, exec_._pg))
+
+
+def outcome_sensitivity(exec_, inputs, outputs, groups: bool = False) -> dict:
+    """Exec.outcome_sensitivity over every rank of a world-sharded campaign: a collective; every rank gets the same
+    dict (rho and PRCC from the merged rank correlation)."""
+    from .world import _sensitivity_dict
+
+    inputs, outputs, planes = exec_._sensitivity_names(inputs, outputs, groups, sharded=True)
+    return _sensitivity_dict(inputs, outputs, gather_rank_correlation(exec_.backend, planes, groups, exec_._pg))
 
 
 def _top_worlds_descriptor(planes, k, largest, groups, shape, n_worlds: int, status: int) -> List[int]:

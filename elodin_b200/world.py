@@ -1869,38 +1869,59 @@ class Exec:
         return {"count": np.ascontiguousarray(t[..., 0]), "value": np.ascontiguousarray(t[..., 1:1 + k]),
                 "world": t[..., 1 + k:].astype(np.int64), "names": names}
 
-    def _rank_planes(self, accessor: str, names, groups: bool, least: int) -> List[int]:
-        """The planes of `names` for a rank method, every refusal made before any backend call."""
+    def _rank_planes(self, accessor: str, names, groups: bool, least: int, sharded: bool = False) -> List[int]:
+        """The planes of `names` for a rank method, every refusal made before any backend call.  The Exec methods rank
+        one handle's worlds and refuse a world-sharded Exec; the collectives of `sharding` (sharded=True) need one."""
         self._outcome_ready(accessor, groups)
-        if self._pg is not None:
+        if self._pg is not None and not sharded:
             raise _lib.B200Error(_lib.ERR_UNSUPPORTED,
                                  f"{accessor}: ranks over the worlds of a world-sharded campaign are not supported; "
-                                 "build without process_group to rank one handle's worlds")
+                                 "build without process_group to rank one handle's worlds (or call "
+                                 f"sharding.{accessor}(exec, ...) on every rank)")
+        if self._pg is None and sharded:
+            raise _lib.B200Error(_lib.ERR_INVALID_ARGUMENT,
+                                 f"sharding.{accessor}: a collective over the ranks of a world-sharded campaign; build "
+                                 "the Exec with World.build(..., process_group=...)")
         names = list(names)
         if len(names) < least or len(set(names)) != len(names):
             raise ValueError(f"{accessor}: names {names!r}, {least} or more distinct outcome names")
         return [self._outcome_plane(n) for n in names]
 
+    def _rank_names(self, accessor: str, names, groups: bool, least: int, sharded: bool = False,
+                    one: bool = False) -> tuple:
+        """(names, planes) of a rank method: `names` (default: every outcome; with `one`, a single name too) resolved
+        by _rank_planes."""
+        names = list(self.outcomes if names is None else ([names] if one and isinstance(names, str) else names))
+        return names, self._rank_planes(accessor, names, groups, least, sharded)
+
+    def _sensitivity_names(self, inputs, outputs, groups: bool, sharded: bool = False) -> tuple:
+        """(inputs, outputs, planes of inputs + outputs) of outcome_sensitivity, every refusal made before any backend
+        call."""
+        inputs = [inputs] if isinstance(inputs, str) else list(inputs)
+        outputs = [outputs] if isinstance(outputs, str) else list(outputs)
+        if not inputs or not outputs or set(inputs) & set(outputs):
+            raise ValueError(f"outcome_sensitivity: inputs {inputs!r} and outputs {outputs!r}, non-empty and disjoint")
+        if len(inputs) + len(outputs) > _lib.MAX_OUTCOMES:
+            raise ValueError(f"outcome_sensitivity: {len(inputs) + len(outputs)} names, at most {_lib.MAX_OUTCOMES}")
+        return inputs, outputs, self._rank_planes("outcome_sensitivity", inputs + outputs, groups, 2, sharded)
+
     def outcome_ranks(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, np.ndarray]:
         """{name: [n_worlds]}: the midrank of every world in each outcome of `names` (default: all), computed on the
         device among the worlds whose selected values are all finite (scipy.stats.rankdata(method="average"); -0 and
         +0 are one value), within its group with groups=True; NaN for the other worlds.  It downloads per-world values:
-        meant for small campaigns and tests."""
-        names = list(self.outcomes if names is None else ([names] if isinstance(names, str) else names))
-        planes = self._rank_planes("outcome_ranks", names, groups, 1)
-        t = self.backend.outcome_group_ranks(planes) if groups else self.backend.outcome_ranks(planes)
-        return {n: np.ascontiguousarray(t[:, k]) for k, n in enumerate(names)}
+        meant for small campaigns and tests.  A world-sharded Exec ranks over every rank's worlds with
+        sharding.outcome_ranks."""
+        names, planes = self._rank_names("outcome_ranks", names, groups, 1, one=True)
+        return _ranks_dict(names, self.backend.outcome_group_ranks(planes) if groups else self.backend.outcome_ranks(planes))
 
     def outcome_rank_correlation(self, names: Optional[Sequence[str]] = None, groups: bool = False) -> Dict[str, object]:
         """Spearman rank correlation of the outcomes `names` (default: all; two or more), on the device: {"count",
         "rho" [p, p], "names"}, a group axis first with groups=True.  Over the worlds whose p values are all finite,
         ranked with midranks; NaN in the row and column of an outcome constant over them, and everywhere below 2
-        worlds (as scipy.stats.spearmanr)."""
-        names = list(self.outcomes if names is None else names)
-        planes = self._rank_planes("outcome_rank_correlation", names, groups, 2)
+        worlds (as scipy.stats.spearmanr).  A world-sharded Exec uses sharding.outcome_rank_correlation."""
+        names, planes = self._rank_names("outcome_rank_correlation", names, groups, 2)
         t = self.backend.outcome_group_rank_correlation(planes) if groups else self.backend.outcome_rank_correlation(planes)
-        p = len(planes)
-        return {"count": np.array(t[..., 0]), "rho": t[..., 1:].reshape(*t.shape[:-1], p, p), "names": names}
+        return _rank_correlation_dict(names, t)
 
     def outcome_sensitivity(self, inputs: Sequence[str], outputs: Sequence[str], groups: bool = False) -> Dict[str, object]:
         """How much each dispersed input drives each output: {"count", "rho" [n_out, n_in] (Spearman), "prcc"
@@ -1909,24 +1930,11 @@ class Exec:
         rank correlation over inputs + outputs; the PRCC of output y comes from the inverse of the rank correlation
         matrix of the inputs and y (executor.partial_rank_correlation), NaN where that matrix holds a NaN or is
         singular.  Every output shares one set of complete worlds, those whose inputs and outputs are all finite: to
-        rank an output over only its own finite worlds, call it separately."""
-        inputs = [inputs] if isinstance(inputs, str) else list(inputs)
-        outputs = [outputs] if isinstance(outputs, str) else list(outputs)
-        if not inputs or not outputs or set(inputs) & set(outputs):
-            raise ValueError(f"outcome_sensitivity: inputs {inputs!r} and outputs {outputs!r}, non-empty and disjoint")
-        if len(inputs) + len(outputs) > _lib.MAX_OUTCOMES:
-            raise ValueError(f"outcome_sensitivity: {len(inputs) + len(outputs)} names, at most {_lib.MAX_OUTCOMES}")
-        names = inputs + outputs
-        planes = self._rank_planes("outcome_sensitivity", names, groups, 2)
+        rank an output over only its own finite worlds, call it separately.  A world-sharded Exec uses
+        sharding.outcome_sensitivity."""
+        inputs, outputs, planes = self._sensitivity_names(inputs, outputs, groups)
         t = self.backend.outcome_group_rank_correlation(planes) if groups else self.backend.outcome_rank_correlation(planes)
-        p, n_in = len(names), len(inputs)
-        R = t[..., 1:].reshape(*t.shape[:-1], p, p)
-        rho = np.ascontiguousarray(R[..., n_in:, :n_in])
-        prcc = np.empty_like(rho)
-        for y in range(len(outputs)):
-            sub = list(range(n_in)) + [n_in + y]
-            prcc[..., y, :] = partial_rank_correlation(R[..., sub, :][..., :, sub])
-        return {"count": np.array(t[..., 0]), "rho": rho, "prcc": prcc, "inputs": inputs, "outputs": outputs}
+        return _sensitivity_dict(inputs, outputs, t)
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)
@@ -1946,3 +1954,27 @@ class Exec:
                "real_time_factor": (batch_ms / tick) if tick > 0 else float("inf")}
         out.update({"backend": self.backend.timings()})
         return out
+
+
+def _ranks_dict(names: List[str], t: np.ndarray) -> Dict[str, np.ndarray]:
+    """Exec.outcome_ranks' dict of rank rows t [n_worlds, p]."""
+    return {n: np.ascontiguousarray(t[:, k]) for k, n in enumerate(names)}
+
+
+def _rank_correlation_dict(names: List[str], t: np.ndarray) -> Dict[str, object]:
+    """Exec.outcome_rank_correlation's dict of rank correlation records t [..., 1 + p*p]."""
+    p = len(names)
+    return {"count": np.array(t[..., 0]), "rho": t[..., 1:].reshape(*t.shape[:-1], p, p), "names": names}
+
+
+def _sensitivity_dict(inputs: List[str], outputs: List[str], t: np.ndarray) -> Dict[str, object]:
+    """Exec.outcome_sensitivity's dict of rank correlation records t [..., 1 + p*p] over inputs + outputs: rho, and the
+    PRCC of each output from the inputs' and its rows and columns."""
+    p, n_in = len(inputs) + len(outputs), len(inputs)
+    R = t[..., 1:].reshape(*t.shape[:-1], p, p)
+    rho = np.ascontiguousarray(R[..., n_in:, :n_in])
+    prcc = np.empty_like(rho)
+    for y in range(len(outputs)):
+        sub = list(range(n_in)) + [n_in + y]
+        prcc[..., y, :] = partial_rank_correlation(R[..., sub, :][..., :, sub])
+    return {"count": np.array(t[..., 0]), "rho": rho, "prcc": prcc, "inputs": inputs, "outputs": outputs}

@@ -804,6 +804,85 @@ int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *p
 /* average plane reads per task of the last rank call (0 for a null handle or before any call) */
 double b200_sixdof_rank_reads(const b200_sixdof *h);
 
+/* ---- world-sharded ranks: the midranks above (grouped or not) of a campaign whose worlds are split over several
+ * handles ("ranks"), over the union of their worlds, and the covariance record of each rank's rank planes.  A midrank is
+ * not a function of the ranks' local midranks, so the ranks exchange what the bucket pass counts, in rounds with the
+ * protocol of the sharded quantiles: each rank sends the u32 words of a round (`partial`), the host sums them
+ * elementwise over the ranks (SUM of unsigned 32-bit words, over any channel) and hands each rank the sums (`reduced`)
+ * in its next round call.  Afterwards the rank planes of every rank hold the campaign midranks of its own worlds: bit
+ * for bit the rows of b200_sixdof_outcome_[group_]ranks on one handle holding every rank's worlds in rank order, for any
+ * rank count >= 1 and any split (empty ranks and empty groups included).  The rank correlation of the campaign is then
+ * the rank correlation (b200_sixdof_outcome_rank_correlation's formula) of the covariance records of the ranks merged in
+ * rank order with b200_covariance_merge: with one rank the unsharded record's bits.
+ *   Exchanges.  Every (group, plane) task whose group holds a complete world on some rank takes the MSD bucket pass
+ *   (the shared-memory routes would see only local worlds), with an exchange before each step that needs the other
+ *   ranks' counts or keys:
+ *     sizes    once per call: every group's complete worlds and worlds, rank-slotted (G * n_ranks * 2 u32: rank r
+ *              writes slots (g * n_ranks + r) * 2 + {0, 1}, the others leave them 0), so every rank knows each group's
+ *              global count and every rank's share.  The tasks are cut into slices from these alike on every rank.
+ *     hist     at most 5 per slice: each task's counts of its ranges' 2^14 bins at one level (2^14 u32 per range).  Plan 0
+ *              starts from the whole key range (min and max do not add), so the levels are at shifts 50, 36, 22, 8 and
+ *              0 and every bin is one key wide after at most 5.  A bin one key wide, or of one world over every rank, is
+ *              a tie run ranked base + (count + 1) / 2 with no further exchange; one of at most 8192 worlds is a bucket;
+ *              a larger one refines at the next level.  A task of at most 8192 complete worlds is one bucket at once.
+ *              After the last level each rank puts its bucket worlds and their keys in a list of its own (the scatter,
+ *              the last read of the plane).
+ *     windows  the slice's buckets, in windows of their first key's place in the slice's key words: a window holds
+ *              W = min(4,186,111, 2^23 / n_ranks - 1) places, so both of its exchanges stay below 32 MiB:
+ *       offsets  each bucket's count on each rank, rank-slotted (W * n_ranks u32, at the bucket's first place).
+ *       keys     every key of the window's buckets as a u64 (two u32 words, W + 8192 at most), each rank writing its
+ *                own at the bucket's place plus its offset and leaving the other words 0.  Each rank then sorts the
+ *                window's buckets that hold its worlds in shared memory and writes its worlds' midranks from two
+ *                binary searches of the sorted keys; world indices never travel.
+ *   So one sizes exchange per call, then per slice at most 5 histogram exchanges and two per window of its keys (one
+ *   window unless the slice's buckets hold more than W worlds), fewer where the summed counts show no work.  Only the
+ *   histogram exchange can pass 32 MiB (the max_round_bytes begin reports, whatever the campaign's size); it is sent
+ *   in rounds of at most that many bytes.  Every key of every bucket reaches every rank, a window at a time: about 8
+ *   bytes per complete world and selected plane, as much as gathering the planes; what the rounds buy is device memory
+ *   per rank bounded by its own worlds and a window, never every rank's planes.  A task reads the rank's plane at most
+ *   6 times (5 histogram passes and the scatter; the completeness read not counted); b200_sixdof_rank_reads, set by the
+ *   end, averages them over every (group, plane) task of the call, a group with no complete world on any rank counting
+ *   none.
+ *   Memory.  The rank planes of the unsharded entries.  Device scratch of the call's own (not the staging buffer),
+ *   allocated as the call needs it and freed by its end (or by a discard, a failure or the next begin):
+ *     - per task of a slice, for its worlds on this rank: 48 bytes per complete world (its pieces, bucket list and
+ *       keys: only pieces that hold worlds of this rank are kept) and 4 per world, plus 32 bytes per 8193 complete
+ *       worlds over every rank (the ranges); the slices are cut so that this is at most 256 MiB on the rank holding
+ *       the most of each group, unless one task alone needs more;
+ *     - the histograms of two consecutive levels, 64 KiB per range that exists (a range holds more than 8192 worlds
+ *       over every rank; tens of ranges on continuous values);
+ *     - the exchange: at most 32 MiB, or one level's histograms if they are larger.
+ *   A cudaMalloc that fails ends the call with B200_ERR_OUT_OF_MEMORY and leaves the handle usable.
+ *   Preconditions (a C host checks them itself; sharding.gather_ranks does): every rank passes the same grouping,
+ *   planes, n_ranks and outcome count and a distinct rank, a rank's groups are the global groups cut to its worlds (the
+ *   same G on every rank; a group may be empty on a rank).  A group of more than 1,073,872,895 complete worlds over the
+ *   ranks (what a world state can index) fails the sizes round with B200_ERR_INVALID_ARGUMENT on every rank.
+ *   Between begin and end the handle's outcome planes must not change: a step, upload, invoke_batch,
+ *   trajectory_reset, set_channels, set_outcomes, set_world_groups, summary begin, start or add makes the next round or
+ *   end fail with B200_ERR_INVALID_ARGUMENT and discards the call.  Any call of an unsharded rank entry
+ *   (b200_sixdof_outcome_[group_]ranks or _rank_correlation) discards it too, since it rewrites the rank planes; any
+ *   other reduction may run between rounds. ---- */
+/* Checks what b200_sixdof_outcome_[group_]ranks checks, in the same order (the outcome set, the groups when grouped,
+ * the selection of 1 .. P planes), then the sticky status, then rank < n_ranks (B200_ERR_INVALID_ARGUMENT), after
+ * B200_ERR_INVALID_ARGUMENT for a null handle or a null max_round_bytes; discards a call still pending; writes the
+ * outcome planes of the summaries, fixes the grouping, planes, rank and n_ranks of the call and writes its largest round
+ * in bytes. */
+int b200_sixdof_sharded_ranks_begin(b200_sixdof *h, int grouped, const uint32_t *planes, uint32_t n_p, uint32_t rank,
+                                    uint32_t n_ranks, uint64_t *max_round_bytes);
+/* One round, with the contract of b200_sixdof_sharded_quantiles_round: `reduced` = the ranks' elementwise sum of this
+ * rank's previous partial (NULL, 0 on the first call), `partial` (partial_cap >= begin's max_round_bytes) receives the
+ * next round's words, *partial_bytes == 0: the rank planes are ready.  The same refusals, and
+ * B200_ERR_INVALID_ARGUMENT, discarding the call, for a group too large (above). */
+int b200_sixdof_sharded_ranks_round(b200_sixdof *h, const void *reduced, uint64_t reduced_bytes, void *partial,
+                                    uint64_t partial_cap, uint64_t *partial_bytes);
+/* ranks_dst (host or device, or NULL) = [n_worlds][n_p] f64: the campaign midranks of this rank's worlds; cov_dst (host
+ * or device, or NULL) = [G, or 1 ungrouped][1 + n_p + n_p^2] f64: the covariance record (b200_sixdof_outcome_covariance's
+ * layout and kernels) of the rank planes over this rank's complete worlds.  A destination's bytes must match exactly
+ * (else B200_ERR_VALUE_SIZE_MISMATCH).  B200_ERR_INVALID_ARGUMENT for an end without a begin, before the last round, or
+ * after the outcomes changed.  Ends the call. */
+int b200_sixdof_sharded_ranks_end(b200_sixdof *h, void *ranks_dst, uint64_t ranks_bytes, void *cov_dst,
+                                  uint64_t cov_bytes);
+
 /* plumbing */
 uint64_t b200_sixdof_tick_count(const b200_sixdof *h);
 /* Run the handle's work on a caller-owned cudaStream_t (`cuda_stream`, where NULL is
