@@ -80,6 +80,7 @@ SYMBOLS = [
     "b200_sixdof_outcome_rank_correlation", "b200_sixdof_outcome_group_rank_correlation", "b200_sixdof_rank_reads",
     "b200_sixdof_sharded_quantiles_begin", "b200_sixdof_sharded_quantiles_round", "b200_sixdof_sharded_quantiles_end",
     "b200_sixdof_sharded_ranks_begin", "b200_sixdof_sharded_ranks_round", "b200_sixdof_sharded_ranks_end",
+    "b200_sixdof_outcome_sobol", "b200_sixdof_outcome_group_sobol",
 ]
 STATS_FIELDS = 5  # count, mean, m2 = sum (x - mean)^2, min, max over the finite values of the worlds
 EXTREMA_FIELDS = 5  # min, max, min_tick, max_tick, first_nonfinite_tick over a world's rows
@@ -111,6 +112,8 @@ OUTCOME_DWELL = 4
 OUTCOME_COLUMN = 5
 OUTCOME_VALUES = 6
 MAX_TOP_WORLDS = 1024  # worlds per record of the worst-worlds entries (b200_sixdof_outcome_top_worlds)
+MAX_SOBOL_INPUTS = 23  # inputs d of a Sobol call: its d + 2 derived planes fit one covariance selection
+MAX_SOBOL_RESAMPLES = 10000  # bootstrap resamples of a Sobol call
 COMM_ID_BYTES = 128
 
 
@@ -360,6 +363,8 @@ def lib():
     for name in ("ranks", "group_ranks", "rank_correlation", "group_rank_correlation"):
         getattr(L, f"b200_sixdof_outcome_{name}").argtypes = [vp, C.POINTER(u32), u32, vp, u64]
     L.b200_sixdof_rank_reads.argtypes = [vp]
+    for name in ("sobol", "group_sobol"):
+        getattr(L, f"b200_sixdof_outcome_{name}").argtypes = [vp, C.POINTER(u32), u32, u32, u32, u64, vp, u64]
     L.b200_sixdof_rank_reads.restype = C.c_double
     L.b200_sixdof_sharded_ranks_begin.argtypes = [vp, C.c_int, C.POINTER(u32), u32, u32, u32, C.POINTER(u64)]
     L.b200_sixdof_sharded_ranks_round.argtypes = [vp, vp, u64, vp, u64, C.POINTER(u64)]

@@ -751,6 +751,7 @@ void b200_sixdof_destroy(b200_sixdof *h)
     if (h->sum_dwell) cudaFree(h->sum_dwell);
     if (h->out_planes) cudaFree(h->out_planes);
     if (h->rank_planes) cudaFree(h->rank_planes);
+    if (h->sobol_planes) cudaFree(h->sobol_planes);
     rank_shard_free(h->sr.Q);
     for (const auto *ts : {h->tables, h->out_tables})
         for (int g = 0; g < 2; ++g)
@@ -2463,6 +2464,9 @@ int b200_sixdof_set_outcomes(b200_sixdof *h, const b200_outcome *o, uint32_t n)
     if (h->rank_planes) CU(h, cudaFree(h->rank_planes));  // the next rank call allocates for the new set
     h->rank_planes = nullptr;
     h->rank_bytes = 0;
+    if (h->sobol_planes) CU(h, cudaFree(h->sobol_planes));
+    h->sobol_planes = nullptr;
+    h->sobol_bytes = 0;
     h->ld_o = ld_o;
     h->outcomes.assign(o, o + n);
     for (auto &x : h->outcomes) x.values = nullptr;
@@ -2598,19 +2602,20 @@ double b200_sixdof_top_worlds_reads(const b200_sixdof *h) { return h ? h->topk_r
 // `bytes`, then the handle's status.  The outcome planes are only read.
 // The checks of a rank call on the outcome set, groups and selection, in order (run_ranks); least: the fewest planes
 static int rank_selection(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t least,
-                          const char *what)
+                          const char *what, const char *noun = "rank")
 {
     int rc = reduction_ready(h, Rows::outcomes, grouped, what);
     if (rc) return rc;
     CU(h, cudaSetDevice(h->device));
     const uint32_t P = (uint32_t)h->outcomes.size();
-    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null rank planes");
-    if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u rank planes: %u to %u", n_p, least, P);
+    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null %s planes", noun);
+    if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u %s planes: %u to %u", n_p, noun, least, P);
     uint64_t seen = 0;
     for (uint32_t j = 0; j < n_p; ++j) {
         if (planes[j] >= P)
-            return fail(B200_ERR_INVALID_ARGUMENT, "rank plane %u is %u: the outcome has %u planes", j, planes[j], P);
-        if (seen & (1ull << planes[j])) return fail(B200_ERR_INVALID_ARGUMENT, "rank plane %u listed twice", planes[j]);
+            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u is %u: the outcome has %u planes", noun, j, planes[j], P);
+        if (seen & (1ull << planes[j]))
+            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u listed twice", noun, planes[j]);
         seen |= 1ull << planes[j];
     }
     return B200_OK;
@@ -2722,6 +2727,122 @@ int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *p
 }
 
 double b200_sixdof_rank_reads(const b200_sixdof *h) { return h ? h->rank_reads : 0.0; }
+
+// ---- Sobol indices (sobol_kernels.cu) ----
+
+// *ptr grown to need_bytes as grow_device, but a failed allocation is not sticky: it returns B200_ERR_OUT_OF_MEMORY and
+// leaves the handle usable (with *ptr freed)
+static int grow_device_soft(b200_sixdof *h, double **ptr, uint64_t *have_bytes, uint64_t need_bytes, const char *what)
+{
+    if (*have_bytes >= need_bytes) return B200_OK;
+    if (*ptr) CU(h, cudaFree(*ptr));
+    *ptr = nullptr;
+    *have_bytes = 0;
+    const cudaError_t e = cudaMalloc(ptr, need_bytes);
+    if (e == cudaErrorMemoryAllocation) {
+        (void)cudaGetLastError();
+        *ptr = nullptr;
+        return fail(B200_ERR_OUT_OF_MEMORY, "%s: out of device memory for %llu bytes", what, (unsigned long long)need_bytes);
+    }
+    CU(h, e);
+    *have_bytes = need_bytes;
+    return B200_OK;
+}
+
+// The Sobol records of the selected outcomes (include/b200_sixdof.h b200_sixdof_outcome_sobol): the derived planes into
+// the handle's Sobol buffer, their covariance on the sample axis (the covariance kernels, unchanged) at the front of the
+// scratch, then the bootstrap and the records.
+static int run_sobol(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
+                     uint64_t seed, void *dst, uint64_t bytes)
+{
+    int rc = rank_selection(h, grouped, planes, n_p, 1, "outcome sobol", "sobol");
+    if (rc) return rc;
+    if (d < 1 || d > B200_MAX_SOBOL_INPUTS)
+        return fail(B200_ERR_INVALID_ARGUMENT, "sobol: %u inputs, 1 to %u", d, B200_MAX_SOBOL_INPUTS);
+    const uint32_t q = d + 2;
+    const std::vector<uint64_t> sizes = reduction_groups(h, grouped);
+    std::vector<uint64_t> samples(sizes.size());
+    for (size_t g = 0; g < sizes.size(); ++g) {
+        if (sizes[g] % q && grouped)
+            return fail(B200_ERR_INVALID_ARGUMENT, "sobol: group %zu has %llu worlds, not a multiple of d + 2 = %u", g,
+                        (unsigned long long)sizes[g], q);
+        if (sizes[g] % q)
+            return fail(B200_ERR_INVALID_ARGUMENT, "sobol: the batch has %llu worlds, not a multiple of d + 2 = %u",
+                        (unsigned long long)sizes[g], q);
+        samples[g] = sizes[g] / q;
+        if (samples[g] >> 32)
+            return fail(B200_ERR_INVALID_ARGUMENT, "sobol: group %zu has %llu samples, at most 2^32 - 1", g,
+                        (unsigned long long)samples[g]);
+    }
+    if (n_boot > B200_MAX_SOBOL_RESAMPLES)
+        return fail(B200_ERR_INVALID_ARGUMENT, "sobol: %u resamples, at most %u", n_boot, B200_MAX_SOBOL_RESAMPLES);
+    const uint64_t G = sizes.size(), W = h->desc.n_worlds, N = W / q;
+    const uint64_t want = G * n_p * (3ull + 4ull * d) * 8ull;
+    if (bytes != want)
+        return fail(B200_ERR_VALUE_SIZE_MISMATCH, "outcome sobol records are %llu bytes, got %llu", (unsigned long long)want,
+                    (unsigned long long)bytes);
+    if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
+    if (bytes == 0) return B200_OK;
+    if (!dst) return fail(B200_ERR_INVALID_ARGUMENT, "null destination buffer");
+    SobolParams S{};
+    S.planes = h->out_planes;
+    S.ld_o = h->ld_o;
+    S.n_p = n_p;
+    for (uint32_t j = 0; j < n_p; ++j) S.plane[j] = planes[j];
+    S.d = d;
+    S.n_samples = N;
+    S.ld = round_up(std::max<uint64_t>(N, 1), 128);
+    const uint64_t plane_bytes = (uint64_t)n_p * q * S.ld * 8ull, list_bytes = (uint64_t)n_p * S.ld * 4ull;
+    if ((rc = grow_device_soft(h, &h->sobol_planes, &h->sobol_bytes, plane_bytes + list_bytes + n_p * S.ld, "sobol")))
+        return rc;
+    S.sp = h->sobol_planes;
+    S.list = (uint32_t *)((char *)h->sobol_planes + plane_bytes);
+    S.mask = (uint8_t *)((char *)h->sobol_planes + plane_bytes + list_bytes);
+    // the covariance of the derived planes: output k is sample k of a one-entity state of q planes, over the group
+    // table of the sample axis that b200_sixdof_set_world_groups would build for groups of N_g worlds
+    CovParams C{};
+    C.seg[0] = {h->sobol_planes, q, (uint64_t)q * S.ld};
+    C.n_segs = 1;
+    C.planes_per_sample = q;
+    C.n_planes = (uint64_t)n_p * q;
+    C.ld = S.ld;
+    C.n_worlds = N;
+    C.n_entities = 1;
+    C.n_p = q;
+    for (uint32_t j = 0; j < q; ++j) C.planes[j] = j;
+    const std::vector<WorldGroup> table = cov_group_table(samples.data(), G, 1);
+    const uint64_t cov_bytes = G * n_p * (1ull + q + (uint64_t)q * q) * 8ull, table_bytes = G * sizeof(WorldGroup);
+    const uint64_t front = cov_bytes + round_up(table_bytes, 8);
+    const uint64_t scratch = front + std::max(cov_scratch_bytes(C, table), sobol_scratch_bytes(S, G * n_p, n_boot));
+    // the staging buffer grown here, so that running out of memory leaves the handle usable
+    const uint64_t stage = std::max<uint64_t>(round_up(scratch, 8) + (device_destination(h, dst) ? 0 : bytes), 8);
+    if ((rc = grow_device_soft(h, &h->staging, &h->staging_bytes, stage, "sobol"))) return rc;
+    return run_world_reduction(h, Rows::outcomes, false, scratch, dst, bytes, [&](double *out, void *scr, int *n) {
+        double *cov = (double *)scr;
+        WorldGroup *groups = (WorldGroup *)((char *)scr + cov_bytes);
+        void *rest = (char *)scr + front;
+        cudaError_t e = cudaMemcpyAsync(groups, table.data(), table_bytes, cudaMemcpyHostToDevice, h->stream);
+        int a = 0, b = 0, c = 0;
+        if (e == cudaSuccess) e = launch_sobol_planes(S, &a, h->stream);
+        C.out = cov;
+        if (e == cudaSuccess) e = launch_covariance(C, groups, table, rest, &b, h->stream);
+        if (e == cudaSuccess) e = launch_sobol_indices(S, cov, groups, G, n_boot, seed, out, rest, &c, h->stream);
+        *n = a + b + c;
+        return e;
+    });
+}
+
+int b200_sixdof_outcome_sobol(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
+                              uint64_t seed, void *dst, uint64_t bytes)
+{
+    return run_sobol(h, false, planes, n_p, d, n_boot, seed, dst, bytes);
+}
+
+int b200_sixdof_outcome_group_sobol(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
+                                    uint64_t seed, void *dst, uint64_t bytes)
+{
+    return run_sobol(h, true, planes, n_p, d, n_boot, seed, dst, bytes);
+}
 
 // ---- world-sharded ranks (rank_kernels.cu: sharded_rank_round) ----
 

@@ -68,6 +68,11 @@ struct b200_sixdof {
     // first rank call, freed by set_outcomes and destroy
     double *rank_planes = nullptr;
     uint64_t rank_bytes = 0;
+    // the derived planes, complete-sample lists and completeness bytes of the last Sobol call (SobolParams): allocated
+    // by the first Sobol call, freed by set_outcomes and destroy; apart from the rank planes, which a sharded rank call
+    // owns between its rounds
+    double *sobol_planes = nullptr;
+    uint64_t sobol_bytes = 0;
     // a world-sharded quantile call (b200_sixdof_sharded_quantiles_*) between begin and end: its state, the write
     // generation of the rows at begin (rows_gen: bumped by every entry that changes what a reduction reads), and its own
     // device scratch (not the staging buffer, which the other reductions reuse between its rounds)

@@ -555,4 +555,31 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
                                cudaStream_t s);
 void rank_shard_free(RankShard &Q);
 
+// Sobol indices of the outcome planes of a Saltelli campaign (sobol_kernels.cu, include/b200_sixdof.h
+// b200_sixdof_outcome_sobol): sample j is the worlds [j (d + 2), (j + 1) (d + 2)), [A, AB^(1) .. AB^(d), B].
+struct SobolParams {
+    const double *planes;  // outcome plane 0; plane p at planes + p * ld_o, world w at [w]
+    uint64_t ld_o;
+    uint32_t n_p;          // selected outputs
+    uint32_t plane[B200_MAX_OUTCOMES];
+    uint32_t d;            // inputs
+    uint64_t n_samples;    // n_worlds / (d + 2)
+    uint64_t ld;           // n_samples rounded up to 128
+    double *sp;            // derived plane j (0: a, 1: b, 2 + i: D_i) of output k at sp + (k (d + 2) + j) ld
+    uint32_t *list;        // output k's complete samples at list + k ld, group g's from its first sample o
+    uint8_t *mask;         // output k's completeness bytes at mask + k ld
+};
+// The derived planes and completeness bytes of every selected output: one launch (*launches; none without samples).
+cudaError_t launch_sobol_planes(const SobolParams &S, int *launches, cudaStream_t s);
+// bytes of device scratch launch_sobol_indices needs over `tasks` (group, output) tasks: at most 256 MiB unless one
+// task alone needs more
+uint64_t sobol_scratch_bytes(const SobolParams &S, uint64_t tasks, uint32_t n_boot);
+// The records [G][n_p][3 + 4d] into out (device) from the covariance table `cov` of the derived planes ([n_p][G]
+// records of 1 + q + q^2, q = d + 2, sample axis = output) over the sample-axis group table `groups` (device, G groups;
+// only o and n are read).  Per slice of tasks: with n_boot > 0 the list launch and the bootstrap launch, then the finish
+// launch (*launches).
+cudaError_t launch_sobol_indices(const SobolParams &S, const double *cov, const WorldGroup *groups, uint64_t G,
+                                 uint32_t n_boot, uint64_t seed, double *out, void *scratch, int *launches,
+                                 cudaStream_t s);
+
 } // namespace b200

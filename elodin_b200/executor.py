@@ -631,6 +631,21 @@ class B200Exec:
         """Reads of the outcome planes the last rank call made, averaged over its (group, plane) tasks."""
         return float(self._L.b200_sixdof_rank_reads(self._h))
 
+    def outcome_sobol(self, planes, d: int, n_boot: int, seed: int) -> np.ndarray:
+        """[p, 3 + 4d]: per outcome of `planes` (distinct indices below P) of a Saltelli campaign of d inputs
+        (monte_carlo.saltelli: blocks of d + 2 worlds), the record [n, V, n_boot_ok, S1[d], ST[d], S1_sd[d], ST_sd[d]]:
+        the first-order and total Sobol indices and the standard deviations of n_boot bootstrap resamples drawn from
+        `seed` (include/b200_sixdof.h b200_sixdof_outcome_sobol)."""
+        sel = self._selection(planes)
+        args = sel + (int(d), int(n_boot), int(seed) % (1 << 64))
+        return self._reduce("sobol", "outcome", args, (sel[1], 3 + 4 * int(d)))
+
+    def outcome_group_sobol(self, planes, d: int, n_boot: int, seed: int) -> np.ndarray:
+        """[G, p, 3 + 4d]: outcome_sobol(planes, d, n_boot, seed) per group of set_world_groups."""
+        sel = self._selection(planes)
+        args = sel + (int(d), int(n_boot), int(seed) % (1 << 64))
+        return self._reduce("group_sobol", "outcome", args, (self.world_groups, sel[1], 3 + 4 * int(d)))
+
     # ---- world-sharded ranks: the midranks of the union of every rank's worlds, in rounds ----------------------------
     def sharded_ranks_begin(self, planes, groups: bool, rank: int, n_ranks: int) -> int:
         """Begin this rank's part of a world-sharded rank call (b200_sixdof_sharded_ranks_begin): the outcomes
@@ -852,6 +867,29 @@ def rank_correlation(cov: np.ndarray, p: int) -> np.ndarray:
     ok = (n[..., None] >= 2) & (d[..., :, None] > 0) & (d[..., None, :] > 0)
     rho = np.where(ok, rho, np.nan)
     return np.concatenate([n, rho.reshape(*cov.shape[:-1], p * p)], axis=-1)
+
+
+def sobol_indices(cov: np.ndarray, d: int) -> tuple:
+    """(n, V, S1 [..., d], ST [..., d]) of covariance records [..., 1 + q + q*q] (q = d + 2) of the derived planes
+    (a, b, D_1 .. D_d) of a Saltelli campaign, as the device computes them (include/b200_sixdof.h
+    b200_sixdof_outcome_sobol; each operation correctly rounded in the same order, so the same bits):
+    V = (M_aa + M_bb) / (2n) + ((m_a - m_b) * (m_a - m_b)) * 0.25, S1_i = (M_bDi / n + m_b m_Di) / V,
+    ST_i = (M_DiDi / n + m_Di m_Di) / (2V).  V is NaN where n < 2; S1 and ST are NaN where n < 2 or V is not > 0."""
+    cov = np.asarray(cov, dtype=np.float64)
+    q = d + 2
+    n = cov[..., 0]
+    m = cov[..., 1:1 + q]
+    M = cov[..., 1 + q:].reshape(*cov.shape[:-1], q, q)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        dab = m[..., 0] - m[..., 1]
+        V = (M[..., 0, 0] + M[..., 1, 1]) / (2.0 * n) + (dab * dab) * 0.25
+        Md = np.diagonal(M, axis1=-2, axis2=-1)[..., 2:]
+        EbD = M[..., 1, 2:] / n[..., None] + m[..., 1:2] * m[..., 2:]
+        EDD = Md / n[..., None] + m[..., 2:] * m[..., 2:]
+        S1 = EbD / V[..., None]
+        ST = EDD / (2.0 * V[..., None])
+    ok = ((n >= 2) & (V > 0))[..., None]
+    return n, np.where(n >= 2, V, np.nan), np.where(ok, S1, np.nan), np.where(ok, ST, np.nan)
 
 
 def partial_rank_correlation(R: np.ndarray) -> np.ndarray:

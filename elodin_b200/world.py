@@ -23,6 +23,7 @@ import os
 import sys
 import time
 import typing
+from statistics import NormalDist
 from typing import Callable, Dict, List, Optional, Sequence, Union
 
 import numpy as np
@@ -1935,6 +1936,52 @@ class Exec:
         inputs, outputs, planes = self._sensitivity_names(inputs, outputs, groups)
         t = self.backend.outcome_group_rank_correlation(planes) if groups else self.backend.outcome_rank_correlation(planes)
         return _sensitivity_dict(inputs, outputs, t)
+
+    def outcome_sobol(self, inputs: Sequence[str], outputs: Sequence[str], groups: bool = False, bootstrap: int = 100,
+                      level: float = 0.95, seed: int = 0) -> Dict[str, object]:
+        """Variance-based sensitivity of a Saltelli campaign (monte_carlo.saltelli, world k = plan row k), on the
+        device: {"count" [n_out], "var" [n_out], "S1" [n_out, d], "ST" [n_out, d], "S1_conf", "ST_conf" [n_out, d],
+        "inputs", "outputs"}, a group axis first with groups=True.  S1[y, i] is the share of output y's variance that
+        input i explains alone, ST[y, i] that share with all of i's interactions (Saltelli 2010 and Jansen
+        estimators); unlike rho and PRCC (outcome_sensitivity) they see non-monotone effects.  `inputs` is the
+        design's `inputs`: its length d fixes the block of d + 2 worlds, the names only label the result.  Each output
+        has its own count: the base samples whose d + 2 values of it are all finite.  The confidence half-widths are
+        z * sd over `bootstrap` resamples (0: NaN) drawn from `seed`, z = NormalDist().inv_cdf(0.5 + level / 2), as
+        SALib reports them.  A constant output, or fewer than 2 samples, gives NaN."""
+        accessor = "outcome_sobol"
+        inputs = [inputs] if isinstance(inputs, str) else list(inputs)
+        outputs = [outputs] if isinstance(outputs, str) else list(outputs)
+        if not 1 <= len(inputs) <= _lib.MAX_SOBOL_INPUTS or len(set(inputs)) != len(inputs):
+            raise ValueError(f"{accessor}: inputs {inputs!r}, 1 to {_lib.MAX_SOBOL_INPUTS} distinct names (the design's inputs)")
+        if not 1 <= len(outputs) <= _lib.MAX_OUTCOMES or len(set(outputs)) != len(outputs):
+            raise ValueError(f"{accessor}: outputs {outputs!r}, 1 to {_lib.MAX_OUTCOMES} distinct outcome names")
+        if isinstance(bootstrap, bool) or not isinstance(bootstrap, (int, np.integer)) or \
+                not 0 <= int(bootstrap) <= _lib.MAX_SOBOL_RESAMPLES:
+            raise ValueError(f"{accessor}: bootstrap = {bootstrap!r}, an int in [0, {_lib.MAX_SOBOL_RESAMPLES}]")
+        if isinstance(level, bool) or not isinstance(level, (int, float, np.floating)) or not 0.0 < float(level) < 1.0:
+            raise ValueError(f"{accessor}: level = {level!r}, a number in (0, 1)")
+        if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+            raise TypeError(f"{accessor}: seed = {seed!r}, an int")
+        self._outcome_ready(accessor, groups)
+        if self._pg is not None:
+            raise _lib.B200Error(_lib.ERR_UNSUPPORTED,
+                                 f"{accessor}: Sobol indices over the worlds of a world-sharded campaign are not "
+                                 "supported; build without process_group to analyse one handle's worlds")
+        d = len(inputs)
+        sizes = self.groups if groups else [self.n_worlds]
+        bad = [n for n in sizes if n % (d + 2)]
+        if bad:
+            raise ValueError(f"{accessor}: {d} inputs make blocks of {d + 2} worlds, but "
+                             f"{'a group has' if groups else 'the batch has'} {bad[0]} worlds (monte_carlo.saltelli "
+                             "gives N (d + 2) worlds per sweep point)")
+        planes = [self._outcome_plane(n) for n in outputs]
+        be = self.backend
+        t = (be.outcome_group_sobol(planes, d, int(bootstrap), int(seed)) if groups
+             else be.outcome_sobol(planes, d, int(bootstrap), int(seed)))
+        z = NormalDist().inv_cdf(0.5 + float(level) / 2)
+        part = lambda k: np.ascontiguousarray(t[..., 3 + k * d:3 + (k + 1) * d])
+        return {"count": np.ascontiguousarray(t[..., 0]), "var": np.ascontiguousarray(t[..., 1]), "S1": part(0),
+                "ST": part(1), "S1_conf": z * part(2), "ST_conf": z * part(3), "inputs": inputs, "outputs": outputs}
 
     def column_array(self, cid) -> np.ndarray:
         cid = component_id(cid) if isinstance(cid, str) else int(cid)

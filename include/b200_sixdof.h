@@ -804,6 +804,59 @@ int b200_sixdof_outcome_group_rank_correlation(b200_sixdof *h, const uint32_t *p
 /* average plane reads per task of the last rank call (0 for a null handle or before any call) */
 double b200_sixdof_rank_reads(const b200_sixdof *h);
 
+/* ---- variance-based sensitivity: first-order and total Sobol indices of chosen outcomes of a Saltelli campaign
+ * (monte_carlo.saltelli), with bootstrap spreads, computed on the device.  Unlike rank correlation they see
+ * non-monotone effects and interactions: S1_i is the share of an output's variance input i explains alone, ST_i that
+ * share with every interaction it takes part in.
+ *   Layout    sample j of a group is its worlds [j (d + 2), (j + 1) (d + 2)) in order: [A_j, AB_j^(1) .. AB_j^(d), B_j]
+ *             (AB^(i) = A with input i taken from B; SALib's layout without second-order rows).  Every group's world
+ *             count (n_worlds, ungrouped) must be a multiple of d + 2; N_g = its samples.
+ *   Task      (group g, selected outcome y).  Sample j is complete for y when its d + 2 values of y are finite and
+ *             every difference below is finite; listwise deletion is per output, so each output has its own n.
+ *   Planes    a complete sample gives a = f(A_j), b = f(B_j), D_i = f(AB_j^(i)) - f(A_j) (correctly rounded); an
+ *             incomplete one NaN in all d + 2.  The point record comes from the covariance record [n, m[d+2],
+ *             M[d+2][d+2]] of the planes (a, b, D_1 .. D_d) over the task's samples: the outcome covariance kernels,
+ *             chunking and merge on the group table of the sample axis (sizes N_g), so it equals the covariance of a
+ *             handle whose worlds are the samples.  With each operation correctly rounded, in this order:
+ *               V    = (M_aa + M_bb) / (2n) + ((m_a - m_b) * (m_a - m_b)) * 0.25     np.var(np.r_[fA, fB])
+ *               EbD  = M_bDi / n + m_b * m_Di                                      mean(fB (fABi - fA)), Saltelli 2010
+ *               EDD  = M_DiDi / n + m_Di * m_Di                                    mean((fA - fABi)^2), Jansen
+ *               S1_i = EbD / V;  ST_i = EDD / (2 V)
+ *             V is NaN where n < 2; S1 and ST are NaN where n < 2 or V is not > 0 (a constant output).
+ *   Bootstrap n_boot resamples (0: none, at most B200_MAX_SOBOL_RESAMPLES).  Draw t in [0, n) of resample r takes
+ *             complete sample c[umulhi64(x, n)], c = the task's complete samples in sample order, x = mix(seed +
+ *             0x9E3779B97F4A7C15 (r 2^32 + t + 1)) mod 2^64, mix = SplitMix64's output function (z ^= z >> 30;
+ *             z *= 0xBF58476D1CE4E5B9; z ^= z >> 27; z *= 0x94D049BB133111EB; z ^= z >> 31).  The stream depends on
+ *             neither the group nor the output.  With the draws shifted by the point record's means (a' = a - m_a, ..),
+ *             sums s_a, s_aa, s_b, s_bb and per input s_D, s_DD, s_bD, and e_x = s_x / n:
+ *               V(r)   = ((s_aa/n - e_a e_a) + (s_bb/n - e_b e_b)) * 0.5 + dm * dm * 0.25,  dm = (m_a + e_a) - (m_b + e_b)
+ *               EbD(r) = s_bD/n + m_b e_D + m_D e_b + m_b m_D;   EDD(r) = s_DD/n + 2 m_D e_D + m_D m_D
+ *             S1(r) and ST(r) as above, NaN where n < 2 or V(r) is not > 0.  The record carries the sample standard
+ *             deviation (ddof 1) of the finite S1(r) and ST(r) per input (NaN below 2) and the count of resamples with
+ *             V(r) > 0.  The summation order is fixed (no floating-point atomics): the same inputs give the same bits on
+ *             every call, stream and destination.
+ *   Record    per (group, output) 3 + 4d f64: [n, V, n_boot_ok, S1[d], ST[d], S1_sd[d], ST_sd[d]].
+ *   Memory    the derived planes, lists and completeness bytes, n_p ((d + 2) 8 + 5) ld bytes (ld = the sample count
+ *             rounded up to 128), are allocated by the first Sobol call (grown by a later, larger one) and freed by
+ *             set_outcomes and destroy; they are not the rank planes.  Device scratch (in the staging buffer): the
+ *             covariance table, the group table of the samples, and the covariance's or the bootstrap's scratch (at most
+ *             256 MiB; the bootstrap runs its tasks in slices, which changes no bits).  A failed allocation returns
+ *             B200_ERR_OUT_OF_MEMORY and leaves the handle usable.  The outcome planes are only read.
+ * Each entry checks, in this order: what every outcome entry checks (the outcome set; the groups for the grouped
+ * entry); null planes, n_p of 0 or above P, a plane >= P or listed twice; d of 0 or above B200_MAX_SOBOL_INPUTS; a world
+ * or group count that d + 2 does not divide, or a group of 2^32 samples or more; n_boot above B200_MAX_SOBOL_RESAMPLES
+ * (all B200_ERR_INVALID_ARGUMENT); then the byte count (B200_ERR_VALUE_SIZE_MISMATCH) and the sticky status.  Like
+ * every outcome entry it first writes the outcome planes of the summaries and columns, runs on the handle's stream,
+ * returns once dst (host or device) is filled and counts its launches in timings.kernel_launches. ---- */
+#define B200_MAX_SOBOL_INPUTS 23u         /* d + 2 derived planes fit one covariance selection */
+#define B200_MAX_SOBOL_RESAMPLES 10000u
+/* dst = [n_p][3 + 4d] f64 */
+int b200_sixdof_outcome_sobol(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
+                              uint64_t seed, void *dst, uint64_t bytes);
+/* dst = [G][n_p][3 + 4d] f64, per group of b200_sixdof_set_world_groups */
+int b200_sixdof_outcome_group_sobol(b200_sixdof *h, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
+                                    uint64_t seed, void *dst, uint64_t bytes);
+
 /* ---- world-sharded ranks: the midranks above (grouped or not) of a campaign whose worlds are split over several
  * handles ("ranks"), over the union of their worlds, and the covariance record of each rank's rank planes.  A midrank is
  * not a function of the ranks' local midranks, so the ranks exchange what the bucket pass counts, in rounds with the
