@@ -7,7 +7,8 @@
 // the bits of the ungrouped call on a batch of exactly its group's worlds whatever the other groups of the call.
 //
 // Values are ordered by the IEEE totalOrder key (key(-0) < key(+0); NaN and +-inf are dropped before).  Three routes,
-// chosen per world group from its size n alone (quantile_order lists the groups by route); one call can take all three:
+// chosen per world group from its size n alone (route_of in order_stats.cuh; quantile_order lists the groups by route);
+// one call can take all three:
 //  - small groups (n <= kSmallMax): a warp (n <= 256, empty groups included) or a block per triple loads the triple's
 //    finite keys into shared memory, sorts them (bitonic) and reads off the ranks.  One read of the planes, one launch
 //    per route that has groups, no scratch; the block route's shared memory is sized by its largest group.
@@ -32,16 +33,14 @@
 //    to the scratch ahead of the slice's launches) by binary search over the rows' first chunks.
 // Counts and keys are integers, so the order in which atomics land changes no result.
 #include <algorithm>
-#include <cfloat>
 #include <cub/block/block_scan.cuh>
 
+#include "order_stats.cuh"
 #include "sixdof_internal.h"
 
 namespace b200 {
 namespace {
 
-constexpr unsigned kSmallMax = 8192;   // largest n_worlds sorted in shared memory (64 KB of keys)
-constexpr unsigned kWarpMax = 256;     // up to this n_worlds a warp sorts a group, eight groups per block
 constexpr unsigned kBins = 1u << 14;   // histogram bins per group and pass (64 KB of u32, in shared memory when E = 1)
 constexpr unsigned kBinBits = 14;
 constexpr unsigned kBucketCap = 8192;  // a range of at most this many keys is compacted and sorted in shared memory
@@ -98,19 +97,6 @@ struct Layout {
     uint32_t *todo;
 };
 
-__device__ __forceinline__ unsigned long long order_key(double x)
-{
-    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ double key_value(unsigned long long k)
-{
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-
-__device__ __forceinline__ bool finite(double x) { return fabs(x) <= DBL_MAX; }
-
 __device__ __forceinline__ double *out_of(const QuantileParams &S, uint64_t g, uint64_t i, uint64_t e)
 {
     const uint64_t W = S.planes_per_sample;
@@ -154,11 +140,6 @@ __device__ void bitonic(unsigned long long *a, uint32_t P, uint32_t tid, uint32_
             sync();
         }
     }
-}
-
-__device__ __forceinline__ uint32_t pow2_at_least(uint32_t n)
-{
-    return n <= 1 ? 1 : 1u << (32 - __clz(n - 1));
 }
 
 // ---- small groups ---------------------------------------------------------------------------------------------------
@@ -258,18 +239,6 @@ inline PassShape pass_shape(uint64_t n_worlds, uint64_t E, uint64_t n_planes)
     s.Wc = per * s.J;
     s.C = (n_worlds + s.Wc - 1) / s.Wc;
     return s;
-}
-
-// the row of chunk k of a slice: the last of rows[0 .. nr) whose first chunk is at most k
-__device__ inline uint64_t row_of_chunk(const QRow *rows, uint64_t nr, uint64_t k)
-{
-    uint64_t lo = 0, hi = nr - 1;
-    while (lo < hi) {
-        const uint64_t mid = (lo + hi + 1) / 2;
-        if (rows[mid].k0 <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
 }
 
 // pass 0: finite count and min / max key per triple
@@ -383,8 +352,6 @@ __global__ void __launch_bounds__(kPassThreads) quantile_pass_kernel(QuantilePar
         }
     }
 }
-
-__device__ __forceinline__ uint32_t bit_len(unsigned long long x) { return 64 - __clzll(x); }
 
 // Plan after pass `level`: one block per group.  Moves each refined rank into its bin, then (thread 0) groups the ranks
 // into ranges and decides what the next pass does with each; clears the histogram for the next pass.
@@ -605,21 +572,6 @@ inline Slice slice_shape(uint64_t E)
     return Slice{0, 1, 0, kSliceGroups, 0, 0};
 }
 
-// the groups of each route: order[0 .. warp) warp, [warp, block) block, [block, size) radix
-struct Routes {
-    uint32_t warp, block;
-};
-
-inline Routes routes_of(const std::vector<WorldGroup> &table, const std::vector<uint32_t> &order)
-{
-    Routes r{0, 0};
-    for (uint32_t g : order) {
-        r.warp += table[g].n <= kWarpMax;
-        r.block += table[g].n <= kSmallMax;
-    }
-    return r;
-}
-
 // One slice of the radix sequence over the large groups large[0 .. n_large) of a table (slice_shape; row slices
 // outermost, then entity slices): its triples, row table, scratch layout and pass launch shape.
 struct SliceRun {
@@ -630,8 +582,6 @@ struct SliceRun {
     size_t hist_smem;
     std::vector<QRow> rows;
 };
-
-constexpr uint64_t kGridCap = 64ull * kNumSMs * 8;
 
 inline uint64_t slices_of(const QuantileParams &S, uint64_t n_large)
 {
@@ -707,10 +657,9 @@ void launch_finish(const QuantileParams &S, const SliceRun &r, cudaStream_t s)
 std::vector<uint32_t> quantile_order(const std::vector<WorldGroup> &table)
 {
     std::vector<uint32_t> order;
-    for (int route = 0; route < 3; ++route)
+    for (int route = kWarpRoute; route <= kRadixRoute; ++route)
         for (uint32_t g = 0; g < table.size(); ++g) {
-            const uint64_t n = table[g].n;
-            if ((n <= kWarpMax ? 0 : n <= kSmallMax ? 1 : 2) == route) order.push_back(g);
+            if (route_of(table[g].n) == route) order.push_back(g);
         }
     return order;
 }
@@ -718,7 +667,7 @@ std::vector<uint32_t> quantile_order(const std::vector<WorldGroup> &table)
 uint64_t quantile_scratch_bytes(const QuantileParams &S, const std::vector<WorldGroup> &table)
 {
     uint64_t large = 0;
-    for (const WorldGroup &wg : table) large += wg.n > kSmallMax;
+    for (const WorldGroup &wg : table) large += route_of(wg.n) == kRadixRoute;
     if (S.n_planes == 0 || S.n_entities == 0 || large == 0) return 0;
     const Slice sh = slice_shape(S.n_entities);
     return 256 + kRowBytes + std::min(sh.nr, large * S.n_planes) * sh.ne * kGroupBytes;
@@ -738,11 +687,7 @@ cudaError_t launch_quantiles(const QuantileParams &S, const std::vector<WorldGro
         *launches += 1;
     }
     if (rt.block > rt.warp) {
-        uint64_t n = 0;
-        for (uint32_t k = rt.warp; k < rt.block; ++k) n = std::max(n, table[order[k]].n);
-        uint32_t P = 1;
-        while (P < n) P <<= 1;
-        const size_t smem = P * 8ull;
+        const size_t smem = block_keys(table, order, rt) * 8ull;
         e = cudaFuncSetAttribute(quantile_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         quantile_block_kernel<<<(unsigned)std::min((rt.block - rt.warp) * PE, kGridCap), 512, smem, s>>>(S, rt.warp,
@@ -803,11 +748,6 @@ uint64_t sharded_quantile_round_bytes(const QuantileParams &S, uint64_t n_groups
 cudaError_t sharded_quantile_round(QuantileShard &Q, const void *reduced, void *partial, uint64_t *partial_bytes,
                                    int *launches, cudaStream_t s)
 {
-#define QTRY(call)                                   \
-    do {                                             \
-        const cudaError_t e_ = (call);               \
-        if (e_ != cudaSuccess) return e_;            \
-    } while (0)
     *partial_bytes = 0;
     *launches = 0;
     const QuantileParams &S = Q.S;
@@ -815,24 +755,24 @@ cudaError_t sharded_quantile_round(QuantileShard &Q, const void *reduced, void *
     const uint64_t n_slices = S.n_planes && S.n_entities ? slices_of(S, n_groups) : 0;
     std::vector<uint32_t> all(n_groups);
     for (uint32_t g = 0; g < n_groups; ++g) all[g] = g;
-    QTRY(radix_attributes());
+    CUDA_TRY(radix_attributes());
     if (Q.level >= 0) {  // the sums of the last round's words, then the plan of the pass they count
         const SliceRun r = slice_run(S, Q.table, all.data(), n_groups, Q.slice, Q.scratch, true);
         const uint64_t G = r.L.G;
-        QTRY(cudaMemcpyAsync(Q.level == 0 ? (void *)r.L.cnt : (void *)r.L.hist, reduced,
-                             Q.level == 0 ? G * 4 : G * kExchangeBytes, cudaMemcpyDefault, s));
-        QTRY(cudaMemsetAsync(r.L.todo, 0, 4, s));
+        CUDA_TRY(cudaMemcpyAsync(Q.level == 0 ? (void *)r.L.cnt : (void *)r.L.hist, reduced,
+                                 Q.level == 0 ? G * 4 : G * kExchangeBytes, cudaMemcpyDefault, s));
+        CUDA_TRY(cudaMemsetAsync(r.L.todo, 0, 4, s));
         launch_plan(S, r, Q.level, s);
         uint32_t todo = 0;
-        QTRY(cudaMemcpyAsync(&todo, r.L.todo, 4, cudaMemcpyDeviceToHost, s));
-        QTRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaMemcpyAsync(&todo, r.L.todo, 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         *launches += 1;
         if (todo && Q.level < kLevels) {
             launch_pass(S, r, s);
             ++Q.level;
             *launches += 1;
-            QTRY(cudaMemcpyAsync(partial, r.L.hist, G * kExchangeBytes, cudaMemcpyDefault, s));
-            QTRY(cudaStreamSynchronize(s));
+            CUDA_TRY(cudaMemcpyAsync(partial, r.L.hist, G * kExchangeBytes, cudaMemcpyDefault, s));
+            CUDA_TRY(cudaStreamSynchronize(s));
             *partial_bytes = G * kExchangeBytes;
             return cudaGetLastError();
         }
@@ -843,18 +783,18 @@ cudaError_t sharded_quantile_round(QuantileShard &Q, const void *reduced, void *
     }
     if (Q.slice < n_slices) {
         const SliceRun r = slice_run(S, Q.table, all.data(), n_groups, Q.slice, Q.scratch, true);
-        QTRY(launch_open(S, r, Q.slice == 0, 0, s));
+        CUDA_TRY(launch_open(S, r, Q.slice == 0, 0, s));
         *launches += r.grid ? 2 : 1;
         Q.level = 0;
-        QTRY(cudaMemcpyAsync(partial, r.L.cnt, r.L.G * 4, cudaMemcpyDefault, s));
-        QTRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaMemcpyAsync(partial, r.L.cnt, r.L.G * 4, cudaMemcpyDefault, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         *partial_bytes = r.L.G * 4;
         return cudaGetLastError();
     }
-    if (n_slices) QTRY(cudaMemcpyAsync(&Q.reads, layout_of(0, Q.scratch, true).reads, 8, cudaMemcpyDeviceToHost, s));
-    QTRY(cudaStreamSynchronize(s));
+    if (n_slices)
+        CUDA_TRY(cudaMemcpyAsync(&Q.reads, layout_of(0, Q.scratch, true).reads, 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     return cudaGetLastError();
-#undef QTRY
 }
 
 } // namespace b200

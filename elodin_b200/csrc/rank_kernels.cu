@@ -34,14 +34,11 @@
 // A world-sharded call (sharded_rank_round, below) runs the same bucket pass over every task, in rounds whose u32 words
 // the ranks sum: the plan sees the summed counts, so every rank resolves the same ranges, tie runs and buckets, and the
 // buckets' keys travel summed too (each rank writes its own, the others leave those words 0).
-//
-// The order helpers and bitonic_pairs are duplicated from topk_kernels.cu (the top-worlds kernels keep their registers
-// and this file's rank key differs at zero).
 #include <algorithm>
-#include <cfloat>
 #include <cooperative_groups.h>
 #include <cub/block/block_scan.cuh>
 
+#include "order_stats.cuh"
 #include "sixdof_internal.h"
 
 namespace b200 {
@@ -49,8 +46,6 @@ namespace {
 
 namespace cg = cooperative_groups;
 
-constexpr unsigned kSmallMax = 8192;  // largest group sorted in shared memory by the small routes
-constexpr unsigned kWarpMax = 256;    // up to this size a warp sorts a task, eight tasks per block
 constexpr unsigned kBins = 1u << 14;  // histogram bins per range and level
 constexpr unsigned kBinBits = 14;
 constexpr unsigned kCap = 8192;       // a bin of at most this many worlds is a bucket, sorted in shared memory
@@ -61,48 +56,8 @@ constexpr uint32_t kNone = 0xffffffffu;      // world state: not complete
 constexpr uint32_t kPiece = 0x80000000u;     // world state / bin code: the piece whose base is the low 31 bits
 constexpr unsigned long long kRun = 1ull << 63;  // piece word: a tie run (count in bits 32..62, bucket fill in 0..31)
 
-__device__ __forceinline__ unsigned long long order_key(double x)
-{
-    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ bool finite(double x) { return fabs(x) <= DBL_MAX; }
-
 // the key of a finite value: ascending keys are ascending values, equal keys equal values (-0 == +0)
 __device__ __forceinline__ unsigned long long rank_key(double x) { return order_key(x == 0.0 ? 0.0 : x); }
-
-__device__ __forceinline__ bool ck_less(unsigned long long a, uint32_t ai, unsigned long long b, uint32_t bi)
-{
-    return a < b || (a == b && ai < bi);
-}
-
-__device__ __forceinline__ uint32_t pow2_at_least(uint32_t n)
-{
-    return n <= 1 ? 1 : 1u << (32 - __clz(n - 1));
-}
-
-__device__ __forceinline__ uint32_t bit_len(unsigned long long x) { return 64 - __clzll(x); }
-
-// ascending bitonic sort of the pairs (a[], b[])[0, P) (P a power of two) by `team` threads; sync() is the team barrier
-template <class Sync>
-__device__ void bitonic_pairs(unsigned long long *a, uint32_t *b, uint32_t P, uint32_t tid, uint32_t team, Sync sync)
-{
-    for (uint32_t k = 2; k <= P; k <<= 1) {
-        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-            for (uint32_t t = tid; t < P / 2; t += team) {
-                const uint32_t i = 2 * j * (t / j) + t % j, l = i + j;
-                const unsigned long long x = a[i], y = a[l];
-                const uint32_t xi = b[i], yi = b[l];
-                if (ck_less(y, yi, x, xi) == ((i & k) == 0)) {
-                    a[i] = y; a[l] = x;
-                    b[i] = yi; b[l] = xi;
-                }
-            }
-            sync();
-        }
-    }
-}
 
 // the midrank, within the sorted keys a[0, n), of position i: its tie run [s, e) found by two binary searches
 __device__ __forceinline__ double midrank_at(const unsigned long long *a, uint32_t n, uint32_t i)
@@ -285,17 +240,6 @@ struct Layout {
     const TRow *rows;           // [T]
     void *base;                 // the tasks' areas, at rows[t].off
 };
-
-__device__ inline uint32_t row_of_chunk(const TRow *rows, uint64_t T, uint64_t k)
-{
-    uint64_t lo = 0, hi = T - 1;
-    while (lo < hi) {
-        const uint64_t mid = (lo + hi + 1) / 2;
-        if (rows[mid].k0 <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return (uint32_t)lo;
-}
 
 // zero every task's plan and both histograms
 __global__ void rank_init_kernel(Layout L, bool first, unsigned long long reads0)
@@ -688,24 +632,13 @@ __global__ void shard_plan0_kernel(SLayout L)
     L.st[ti] = s;
 }
 
-__device__ inline uint32_t srow_of_chunk(const SRow *rows, uint64_t T, uint64_t k)
-{
-    uint64_t lo = 0, hi = T - 1;
-    while (lo < hi) {
-        const uint64_t mid = (lo + hi + 1) / 2;
-        if (rows[mid].k0 <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return (uint32_t)lo;
-}
-
 // pass l >= 1, as rank_pass_kernel: the rank's worlds of a task with ranges at level l leave their level l - 1 bin (at
 // level 1, the task's one range) for a piece or a level l bin, counted in the level's pool
 __global__ void __launch_bounds__(kPassThreads) shard_pass_kernel(RankParams S, uint64_t K, SLayout L, int level)
 {
     const uint32_t t = threadIdx.x;
     for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
-        const uint32_t ti = srow_of_chunk(L.rows, L.T, c);
+        const uint32_t ti = row_of_chunk(L.rows, L.T, c);
         const SRow r = L.rows[ti];
         const SArea A = shard_area_of(L.base, r);
         const uint32_t w0 = (uint32_t)(c - r.k0) * r.Wc, w1 = min(w0 + r.Wc, r.n);
@@ -848,7 +781,7 @@ __global__ void __launch_bounds__(kPassThreads) shard_scatter_kernel(RankParams 
 {
     const uint32_t t = threadIdx.x;
     for (uint64_t c = blockIdx.x; c < K; c += gridDim.x) {
-        const uint32_t ti = srow_of_chunk(L.rows, L.T, c);
+        const uint32_t ti = row_of_chunk(L.rows, L.T, c);
         const SRow r = L.rows[ti];
         const SArea A = shard_area_of(L.base, r);
         const uint32_t level = L.st[ti].level;
@@ -953,19 +886,8 @@ __global__ void __launch_bounds__(kPlanThreads) shard_finish_kernel(RankParams S
 
 constexpr uint64_t kScratchCap = 256ull << 20;  // device scratch of a large-group call, unless one task needs more
 constexpr uint64_t kHeader = 256;               // the reads counter
-constexpr uint64_t kGridCap = 64ull * kNumSMs * 8;
 
 inline uint64_t ranges_of(uint64_t n) { return std::max<uint64_t>(1, n / (kCap + 1)); }
-
-// the world chunk of a task of n worlds in a slice of T tasks: about 8 blocks per SM over the slice, at least 16
-// worlds per thread
-inline uint32_t chunk_of(uint64_t n, uint64_t T)
-{
-    const uint64_t want = std::max<uint64_t>(1, 8ull * kNumSMs / std::max<uint64_t>(1, T));
-    uint64_t per = (n + want - 1) / want;
-    per = std::max<uint64_t>(per, 16ull * kPassThreads);
-    return (uint32_t)((per + kPassThreads - 1) / kPassThreads * kPassThreads);
-}
 
 // The large tasks (large groups of order[block ..] outermost, then the selected planes) cut into slices: each slice
 // the longest run of tasks whose rows and areas fit in kScratchCap, at least one task
@@ -993,25 +915,12 @@ std::vector<Slice> slices_of(const RankParams &S, const std::vector<WorldGroup> 
     return out;
 }
 
-uint32_t small_routes(const std::vector<WorldGroup> &table, const std::vector<uint32_t> &order, uint32_t *warp)
-{
-    uint32_t block = 0;
-    *warp = 0;
-    for (uint32_t g : order) {
-        *warp += table[g].n <= kWarpMax;
-        block += table[g].n <= kSmallMax;
-    }
-    return block;
-}
-
 } // namespace
 
 uint64_t rank_scratch_bytes(const RankParams &S, const std::vector<WorldGroup> &table, const std::vector<uint32_t> &order)
 {
-    uint32_t warp;
-    const uint32_t block = small_routes(table, order, &warp);
     uint64_t most = 0;
-    for (const Slice &s : slices_of(S, table, order, block)) most = std::max(most, s.bytes);
+    for (const Slice &s : slices_of(S, table, order, routes_of(table, order).block)) most = std::max(most, s.bytes);
     return most;
 }
 
@@ -1023,18 +932,15 @@ cudaError_t launch_ranks(const RankParams &S, uint64_t n_worlds, const std::vect
     if (n_worlds == 0) return cudaSuccess;
     rank_mask_kernel<<<(unsigned)std::min<uint64_t>((n_worlds + 255) / 256, kGridCap), 256, 0, s>>>(S, n_worlds);
     *launches += 1;
-    uint32_t warp;
-    const uint32_t block = small_routes(table, order, &warp);
+    const Routes rt = routes_of(table, order);
+    const uint32_t warp = rt.warp, block = rt.block;
     cudaError_t e = cudaSuccess;
     if (warp > 0) {
         rank_warp_kernel<<<(unsigned)std::min((warp * (uint64_t)S.n_p + 7) / 8, kGridCap), 256, 0, s>>>(S, 0, warp);
         *launches += 1;
     }
     if (block > warp) {
-        uint64_t n = 0;
-        for (uint32_t k = warp; k < block; ++k) n = std::max(n, table[order[k]].n);
-        uint32_t P = 1;
-        while (P < n) P <<= 1;
+        const uint32_t P = block_keys(table, order, rt);
         const size_t smem = P * 12ull;
         e = cudaFuncSetAttribute(rank_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -1055,7 +961,7 @@ cudaError_t launch_ranks(const RankParams &S, uint64_t n_worlds, const std::vect
         for (uint64_t i = 0; i < sl.T; ++i) {
             const uint64_t t = sl.t0 + i;
             const WorldGroup &wg = table[order[block + t / S.n_p]];
-            const uint32_t Wc = chunk_of(wg.n, sl.T), C = (uint32_t)((wg.n + Wc - 1) / Wc);
+            const uint32_t Wc = chunk_of(wg.n, sl.T, kPassThreads), C = (uint32_t)((wg.n + Wc - 1) / Wc);
             const uint64_t R = ranges_of(wg.n);
             rows[i] = TRow{off, (uint32_t)wg.o, (uint32_t)wg.n, Wc, C, (uint32_t)K, (uint32_t)(t % S.n_p), (uint32_t)R, 0};
             off += task_bytes(wg.n, R);
@@ -1177,7 +1083,7 @@ std::vector<SRow> slice_rows(const RankShard &Q, uint64_t k, uint64_t *bytes)
         const uint32_t g = (uint32_t)(Q.tasks[t0 + i] >> 32), j = (uint32_t)Q.tasks[t0 + i];
         const WorldGroup &wg = Q.table[g];
         const uint64_t N = Q.n_global[g], R = shard_ranges(N), lcn = Q.n_local[g];
-        const uint32_t Wc = chunk_of(wg.n, T), C = (uint32_t)((wg.n + Wc - 1) / Wc);
+        const uint32_t Wc = chunk_of(wg.n, T, kPassThreads), C = (uint32_t)((wg.n + Wc - 1) / Wc);
         rows[i] = SRow{off, (uint32_t)wg.o, (uint32_t)wg.n, Wc, C, (uint32_t)K, j, (uint32_t)R, (uint32_t)N,
                        (uint32_t)lcn, 0};
         off += align8(shard_area_bytes(R, lcn, wg.n));
@@ -1212,21 +1118,15 @@ SliceRun slice_run(const RankShard &Q)
     return r;
 }
 
-#define RTRY(call)                        \
-    do {                                  \
-        const cudaError_t e_ = (call);    \
-        if (e_ != cudaSuccess) return e_; \
-    } while (0)
-
 // a grow-only buffer of at least `need` bytes, once the stream is done with the old one
 cudaError_t grow(void **p, uint64_t *have, uint64_t need, cudaStream_t s)
 {
     if (*have >= need) return cudaSuccess;
-    RTRY(cudaStreamSynchronize(s));
-    if (*p) RTRY(cudaFree(*p));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (*p) CUDA_TRY(cudaFree(*p));
     *p = nullptr;
     *have = 0;
-    RTRY(cudaMalloc(p, need));
+    CUDA_TRY(cudaMalloc(p, need));
     *have = need;
     return cudaSuccess;
 }
@@ -1252,8 +1152,8 @@ cudaError_t start(RankShard &Q, int step, uint64_t bytes, void *partial, uint64_
     Q.xbytes = bytes;
     Q.xpos = 0;
     const uint64_t n = std::min(bytes, kRoundCap);
-    RTRY(cudaMemcpyAsync(partial, Q.x, n, cudaMemcpyDefault, s));
-    RTRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaMemcpyAsync(partial, Q.x, n, cudaMemcpyDefault, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     *partial_bytes = n;
     return cudaGetLastError();
 }
@@ -1262,7 +1162,7 @@ cudaError_t start(RankShard &Q, int step, uint64_t bytes, void *partial, uint64_
 cudaError_t read_states(RankShard &Q, const SliceRun &r, cudaStream_t s)
 {
     Q.st.resize(r.L.T);
-    RTRY(cudaMemcpyAsync(Q.st.data(), r.L.st, r.L.T * sizeof(TaskState), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(Q.st.data(), r.L.st, r.L.T * sizeof(TaskState), cudaMemcpyDeviceToHost, s));
     return cudaStreamSynchronize(s);
 }
 
@@ -1272,9 +1172,9 @@ cudaError_t open_window(RankShard &Q, void *partial, uint64_t *partial_bytes, in
     const uint64_t s0 = Q.window * Q.wkeys, s1 = std::min(s0 + Q.wkeys, Q.keys);
     const uint64_t bytes = (s1 - s0) * Q.n_ranks * 4;
     // room for the keys exchange too: it follows in the same words, without a sync in between
-    RTRY(grow((void **)&Q.x, &Q.x_bytes, std::max(bytes, (std::min(s1 + kCap, Q.keys) - s0) * 8), s));
+    CUDA_TRY(grow((void **)&Q.x, &Q.x_bytes, std::max(bytes, (std::min(s1 + kCap, Q.keys) - s0) * 8), s));
     SliceRun r = slice_run(Q);
-    RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+    CUDA_TRY(cudaMemsetAsync(Q.x, 0, bytes, s));
     shard_window_kernel<<<dim3(r.per_task, (unsigned)r.L.T), 256, 0, s>>>(r.L, s0, s1, 0);
     *launches += 1;
     return start(Q, kOffsets, bytes, partial, partial_bytes, s);
@@ -1285,7 +1185,7 @@ cudaError_t open_window(RankShard &Q, void *partial, uint64_t *partial_bytes, in
 cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial_bytes, int *launches, cudaStream_t s)
 {
     SliceRun r = slice_run(Q);
-    RTRY(read_states(Q, r, s));
+    CUDA_TRY(read_states(Q, r, s));
     const uint64_t T = r.L.T;
     const SliceHeader H = slice_header(T);
     std::vector<uint64_t> words(T);
@@ -1299,17 +1199,17 @@ cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial
         const int next = level + 1, p = next & 1;
         for (uint64_t t = 0; t < T; ++t) words[t] = (uint64_t)Q.st[t].nr[next] * kBins;
         const uint64_t total = set_offsets(Q, p ? H.hoff1 : H.hoff0, words, s, &e);
-        RTRY(e);
-        RTRY(grow((void **)&Q.pool[p], &Q.pool_bytes[p], total * 4, s));
-        RTRY(grow((void **)&Q.x, &Q.x_bytes, total * 4, s));
+        CUDA_TRY(e);
+        CUDA_TRY(grow((void **)&Q.pool[p], &Q.pool_bytes[p], total * 4, s));
+        CUDA_TRY(grow((void **)&Q.x, &Q.x_bytes, total * 4, s));
         r = slice_run(Q);
-        RTRY(cudaMemsetAsync(Q.pool[p], 0, total * 4, s));
+        CUDA_TRY(cudaMemsetAsync(Q.pool[p], 0, total * 4, s));
         Q.reads += refine;
         if (r.grid) {
             shard_pass_kernel<<<r.grid, kPassThreads, 0, s>>>(Q.S, r.K, r.L, next);
             *launches += 1;
         }
-        RTRY(cudaMemcpyAsync(Q.x, Q.pool[p], total * 4, cudaMemcpyDeviceToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(Q.x, Q.pool[p], total * 4, cudaMemcpyDeviceToDevice, s));
         Q.level = next;
         return start(Q, kHist, total * 4, partial, partial_bytes, s);
     }
@@ -1321,7 +1221,7 @@ cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial
     if (keys) {
         for (uint64_t t = 0; t < T; ++t) words[t] = Q.st[t].bucket_worlds;
         Q.keys = set_offsets(Q, H.xk, words, s, &e);
-        RTRY(e);
+        CUDA_TRY(e);
         // an offsets window of wkeys * n_ranks u32 and its keys (up to kCap past it) are both one round below the cap
         Q.wkeys = std::max<uint64_t>(1, std::min((kRoundCap - kCap * 8ull) / 8, kRoundCap / (4ull * Q.n_ranks)) - 1);
         Q.window = 0;
@@ -1334,7 +1234,7 @@ cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial
 cudaError_t open_slice(RankShard &Q, void *partial, uint64_t *partial_bytes, int *launches, cudaStream_t s)
 {
     const SliceRun r = slice_run(Q);
-    RTRY(cudaMemcpyAsync((void *)r.L.rows, r.rows.data(), r.rows.size() * sizeof(SRow), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync((void *)r.L.rows, r.rows.data(), r.rows.size() * sizeof(SRow), cudaMemcpyHostToDevice, s));
     shard_init_kernel<<<dim3(r.per_task, (unsigned)r.L.T), 256, 0, s>>>(r.L, Q.S.mask);
     shard_plan0_kernel<<<(unsigned)((r.L.T + 127) / 128), 128, 0, s>>>(r.L);
     *launches += 2;
@@ -1365,8 +1265,8 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
     const uint64_t G = Q.table.size();
     if (Q.step == kStart) {  // the completeness mask, then the sizes
         const uint64_t bytes = G * Q.n_ranks * 8;
-        RTRY(grow((void **)&Q.x, &Q.x_bytes, bytes, s));
-        RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+        CUDA_TRY(grow((void **)&Q.x, &Q.x_bytes, bytes, s));
+        CUDA_TRY(cudaMemsetAsync(Q.x, 0, bytes, s));
         uint64_t W = 0;
         for (const WorldGroup &wg : Q.table) W = std::max(W, wg.o + wg.n);
         if (W) {
@@ -1379,19 +1279,19 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
     if (Q.step == kDone) return cudaSuccess;
     // the sums of the round last sent
     const uint64_t n = std::min(Q.xbytes - Q.xpos, kRoundCap);
-    RTRY(cudaMemcpyAsync((char *)Q.x + Q.xpos, reduced, n, cudaMemcpyDefault, s));
+    CUDA_TRY(cudaMemcpyAsync((char *)Q.x + Q.xpos, reduced, n, cudaMemcpyDefault, s));
     Q.xpos += n;
     if (Q.xpos < Q.xbytes) {  // the exchange's next round
         const uint64_t m = std::min(Q.xbytes - Q.xpos, kRoundCap);
-        RTRY(cudaMemcpyAsync(partial, (char *)Q.x + Q.xpos, m, cudaMemcpyDefault, s));
-        RTRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaMemcpyAsync(partial, (char *)Q.x + Q.xpos, m, cudaMemcpyDefault, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         *partial_bytes = m;
         return cudaGetLastError();
     }
     if (Q.step == kSizes) {
         std::vector<uint32_t> words(G * Q.n_ranks * 2);
-        RTRY(cudaMemcpyAsync(words.data(), Q.x, words.size() * 4, cudaMemcpyDeviceToHost, s));
-        RTRY(cudaStreamSynchronize(s));
+        CUDA_TRY(cudaMemcpyAsync(words.data(), Q.x, words.size() * 4, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
         Q.n_global.assign(G, 0);
         Q.n_local.assign(G, 0);
         Q.l_most.assign(G, 0);
@@ -1417,7 +1317,7 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
             slice_rows(Q, Q.slice, &bytes);
             most = std::max(most, bytes);
         }
-        RTRY(grow(&Q.area, &Q.area_bytes, std::max<uint64_t>(most, 8), s));
+        CUDA_TRY(grow(&Q.area, &Q.area_bytes, std::max<uint64_t>(most, 8), s));
         Q.slice = 0;
         Q.step = kDone;
     } else {
@@ -1426,19 +1326,20 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
         if (Q.step == kHist) {
             shard_plan_kernel<<<dim3(1, (unsigned)T), kShardPlanThreads, 0, s>>>(r.L, Q.level);
             *launches += 1;
-            RTRY(after_plan(Q, Q.level, partial, partial_bytes, launches, s));
+            CUDA_TRY(after_plan(Q, Q.level, partial, partial_bytes, launches, s));
             if (Q.step != kDone) return cudaSuccess;
         } else {
             const uint64_t s0 = Q.window * Q.wkeys, s1 = std::min(s0 + Q.wkeys, Q.keys);
             if (Q.step == kOffsets) {  // the offsets applied, then this rank's keys of the window
                 const uint64_t bytes = (std::min(s1 + kCap, Q.keys) - s0) * 8;
                 shard_window_kernel<<<dim3(r.per_task, (unsigned)T), 256, 0, s>>>(r.L, s0, s1, 1);
-                RTRY(cudaMemsetAsync(Q.x, 0, bytes, s));
+                CUDA_TRY(cudaMemsetAsync(Q.x, 0, bytes, s));
                 shard_window_kernel<<<dim3(r.per_task, (unsigned)T), 256, 0, s>>>(r.L, s0, s1, 2);
                 *launches += 2;
                 return start(Q, kKeys, bytes, partial, partial_bytes, s);
             }
-            RTRY(cudaFuncSetAttribute(shard_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kCap * 12)));
+            CUDA_TRY(cudaFuncSetAttribute(shard_finish_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          (int)(kCap * 12)));
             shard_finish_kernel<<<dim3(r.per_task, (unsigned)T), kPlanThreads, kCap * 12, s>>>(Q.S, r.L, s0, s1);
             *launches += 1;
             if (s1 < Q.keys) {
@@ -1450,15 +1351,13 @@ cudaError_t sharded_rank_round(RankShard &Q, const void *reduced, void *partial,
     }
     // the slice just ended (or the sizes): open slices until one makes an exchange
     while (Q.slice + 1 < Q.slices.size()) {
-        RTRY(open_slice(Q, partial, partial_bytes, launches, s));
+        CUDA_TRY(open_slice(Q, partial, partial_bytes, launches, s));
         if (Q.step != kDone) return cudaSuccess;
         ++Q.slice;
     }
     Q.step = kDone;
-    RTRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaStreamSynchronize(s));
     return cudaGetLastError();
 }
-
-#undef RTRY
 
 } // namespace b200

@@ -2535,24 +2535,35 @@ int b200_sixdof_outcome_group_histograms(b200_sixdof *h, const b200_histogram *s
     return run_histograms(h, Rows::outcomes, true, specs, n_specs, dst, bytes, "outcome");
 }
 
+// The checks of a call over selected outcome planes (top worlds, ranks, sobol) on the outcome set, groups and
+// selection, in order; least: the fewest planes; noun names the planes in the messages
+static int outcome_selection(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t least,
+                             const char *what, const char *noun = "rank")
+{
+    int rc = reduction_ready(h, Rows::outcomes, grouped, what);
+    if (rc) return rc;
+    CU(h, cudaSetDevice(h->device));
+    const uint32_t P = (uint32_t)h->outcomes.size();
+    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null %s planes", noun);
+    if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u %s planes: %u to %u", n_p, noun, least, P);
+    uint64_t seen = 0;
+    for (uint32_t j = 0; j < n_p; ++j) {
+        if (planes[j] >= P)
+            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u is %u: the outcome has %u planes", noun, j, planes[j], P);
+        if (seen & (1ull << planes[j]))
+            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u listed twice", noun, planes[j]);
+        seen |= 1ull << planes[j];
+    }
+    return B200_OK;
+}
+
 // The k worst worlds of the selected outcome planes, per group when `grouped` (topk_kernels.cu), into dst: the outcome
 // set and groups checked, then the selection, k, largest and `bytes`; the handle's status in run_world_reduction.
 static int run_top_worlds(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t k, int largest,
                           void *dst, uint64_t bytes)
 {
-    int rc = reduction_ready(h, Rows::outcomes, grouped, "outcome top worlds");
+    int rc = outcome_selection(h, grouped, planes, n_p, 1, "outcome top worlds", "top-worlds");
     if (rc) return rc;
-    CU(h, cudaSetDevice(h->device));
-    const uint32_t P = (uint32_t)h->outcomes.size();
-    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null top-worlds planes");
-    if (n_p == 0 || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u top-worlds planes: 1 to %u", n_p, P);
-    uint64_t seen = 0;
-    for (uint32_t j = 0; j < n_p; ++j) {
-        if (planes[j] >= P)
-            return fail(B200_ERR_INVALID_ARGUMENT, "top-worlds plane %u is %u: the outcome has %u planes", j, planes[j], P);
-        if (seen & (1ull << planes[j])) return fail(B200_ERR_INVALID_ARGUMENT, "top-worlds plane %u listed twice", planes[j]);
-        seen |= 1ull << planes[j];
-    }
     if (k == 0 || k > B200_MAX_TOP_WORLDS)
         return fail(B200_ERR_INVALID_ARGUMENT, "top worlds k = %u: 1 to %u", k, B200_MAX_TOP_WORLDS);
     if (largest != 0 && largest != 1) return fail(B200_ERR_INVALID_ARGUMENT, "top worlds largest = %d: 0 or 1", largest);
@@ -2600,26 +2611,6 @@ double b200_sixdof_top_worlds_reads(const b200_sixdof *h) { return h ? h->topk_r
 // dst: as [n_worlds][n_p] rows, or (corr) as the rank correlation records, the covariance of the rank planes (the
 // covariance kernels, unchanged) turned into [n, rho].  The outcome set and groups checked, then the selection, then
 // `bytes`, then the handle's status.  The outcome planes are only read.
-// The checks of a rank call on the outcome set, groups and selection, in order (run_ranks); least: the fewest planes
-static int rank_selection(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t least,
-                          const char *what, const char *noun = "rank")
-{
-    int rc = reduction_ready(h, Rows::outcomes, grouped, what);
-    if (rc) return rc;
-    CU(h, cudaSetDevice(h->device));
-    const uint32_t P = (uint32_t)h->outcomes.size();
-    if (!planes) return fail(B200_ERR_INVALID_ARGUMENT, "null %s planes", noun);
-    if (n_p < least || n_p > P) return fail(B200_ERR_INVALID_ARGUMENT, "%u %s planes: %u to %u", n_p, noun, least, P);
-    uint64_t seen = 0;
-    for (uint32_t j = 0; j < n_p; ++j) {
-        if (planes[j] >= P)
-            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u is %u: the outcome has %u planes", noun, j, planes[j], P);
-        if (seen & (1ull << planes[j]))
-            return fail(B200_ERR_INVALID_ARGUMENT, "%s plane %u listed twice", noun, planes[j]);
-        seen |= 1ull << planes[j];
-    }
-    return B200_OK;
-}
 
 // The parameters of a rank call over the handle's rank planes (grown to n_p planes)
 static int rank_params(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, RankParams &S)
@@ -2663,7 +2654,7 @@ static int run_ranks(b200_sixdof *h, bool grouped, bool corr, const uint32_t *pl
         h->sr.active = false;
         rank_shard_free(h->sr.Q);
     }
-    int rc = rank_selection(h, grouped, planes, n_p, corr ? 2 : 1, corr ? "outcome rank correlation" : "outcome ranks");
+    int rc = outcome_selection(h, grouped, planes, n_p, corr ? 2 : 1, corr ? "outcome rank correlation" : "outcome ranks");
     if (rc) return rc;
     const uint64_t G = reduction_groups(h, grouped).size(), W = h->desc.n_worlds;
     const uint64_t want = corr ? G * (1ull + (uint64_t)n_p * n_p) * 8ull : W * n_p * 8ull;
@@ -2755,7 +2746,7 @@ static int grow_device_soft(b200_sixdof *h, double **ptr, uint64_t *have_bytes, 
 static int run_sobol(b200_sixdof *h, bool grouped, const uint32_t *planes, uint32_t n_p, uint32_t d, uint32_t n_boot,
                      uint64_t seed, void *dst, uint64_t bytes)
 {
-    int rc = rank_selection(h, grouped, planes, n_p, 1, "outcome sobol", "sobol");
+    int rc = outcome_selection(h, grouped, planes, n_p, 1, "outcome sobol", "sobol");
     if (rc) return rc;
     if (d < 1 || d > B200_MAX_SOBOL_INPUTS)
         return fail(B200_ERR_INVALID_ARGUMENT, "sobol: %u inputs, 1 to %u", d, B200_MAX_SOBOL_INPUTS);
@@ -2853,7 +2844,7 @@ int b200_sixdof_sharded_ranks_begin(b200_sixdof *h, int grouped, const uint32_t 
     if (!max_round_bytes) return fail(B200_ERR_INVALID_ARGUMENT, "null max_round_bytes");
     h->sr.active = false;  // a call still pending is discarded, and its scratch freed
     rank_shard_free(h->sr.Q);
-    int rc = rank_selection(h, grouped != 0, planes, n_p, 1, "sharded outcome ranks");
+    int rc = outcome_selection(h, grouped != 0, planes, n_p, 1, "sharded outcome ranks");
     if (rc) return rc;
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (rank >= n_ranks) return fail(B200_ERR_INVALID_ARGUMENT, "rank %u of %u ranks", rank, n_ranks);

@@ -244,8 +244,8 @@ struct QuantileParams : StatsParams {
     const uint32_t *order;     // quantile_order(table), in device memory
     uint64_t n_groups;
 };
-// the groups of a table listed by route, each route in table order: at most 256 worlds (the warp route, empty groups
-// included), then at most 8192 (the block route), then the rest (the radix select)
+// the groups of a table listed by route (route_of, order_stats.cuh), each route in table order: the warp route (empty
+// groups included), then the block route, then the rest (the radix select)
 std::vector<uint32_t> quantile_order(const std::vector<WorldGroup> &table);
 // bytes of device scratch the call over the groups of `table` needs: 0 without a group above 8192 worlds (one pass,
 // no scratch), else at most 256 MiB

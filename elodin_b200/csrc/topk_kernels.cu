@@ -6,7 +6,7 @@
 // index within the group, so the order is a total order of the data alone and no route, launch shape, slicing or
 // atomic order changes a record.
 //
-// Routes, chosen per group from its size n (the quantile kernels' order, quantile_order, lists the groups by route):
+// Routes, chosen per group from its size n (route_of in order_stats.cuh; quantile_order lists the groups by route):
 //  - small groups (n <= kSmallMax): a warp (n <= 256, empty groups included) or a block per task loads the task's
 //    finite (s, i) pairs into shared memory, sorts them (bitonic) and writes the first k.  One read of the plane, one
 //    launch per route that has groups, no scratch.
@@ -31,16 +31,14 @@
 //    the large tasks run in slices of at most kSliceTasks tasks, the same launch sequence per slice, so the scratch
 //    stays under kScratchCap = 256 MiB whatever G x p is.
 #include <algorithm>
-#include <cfloat>
 #include <cub/block/block_scan.cuh>
 
+#include "order_stats.cuh"
 #include "sixdof_internal.h"
 
 namespace b200 {
 namespace {
 
-constexpr unsigned kSmallMax = 8192;  // largest group sorted in shared memory by the small routes
-constexpr unsigned kWarpMax = 256;    // up to this size a warp sorts a task, eight tasks per block
 constexpr unsigned kBins = 1u << 14;  // histogram bins per task and pass
 constexpr unsigned kBinBits = 14;
 constexpr unsigned kCap = 8192;                      // a range of at most this many worlds is gathered and sorted
@@ -51,57 +49,11 @@ constexpr unsigned kPlanThreads = 1024;
 
 enum : uint32_t { kDone = 0, kRefine = 1, kGather = 2 };
 
-__device__ __forceinline__ unsigned long long order_key(double x)
-{
-    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ double key_value(unsigned long long k)
-{
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-
-__device__ __forceinline__ bool finite(double x) { return fabs(x) <= DBL_MAX; }
-
 // the sort key of x: ascending s is the task's order
 __device__ __forceinline__ unsigned long long sort_key(double x, int largest)
 {
     const unsigned long long k = order_key(x);
     return largest ? ~k : k;
-}
-
-// (a, ai) < (b, bi) in the composite order
-__device__ __forceinline__ bool ck_less(unsigned long long a, uint32_t ai, unsigned long long b, uint32_t bi)
-{
-    return a < b || (a == b && ai < bi);
-}
-
-__device__ __forceinline__ uint32_t pow2_at_least(uint32_t n)
-{
-    return n <= 1 ? 1 : 1u << (32 - __clz(n - 1));
-}
-
-__device__ __forceinline__ uint32_t bit_len(unsigned long long x) { return 64 - __clzll(x); }
-
-// ascending bitonic sort of the pairs (a[], b[])[0, P) (P a power of two) by `team` threads; sync() is the team barrier
-template <class Sync>
-__device__ void bitonic_pairs(unsigned long long *a, uint32_t *b, uint32_t P, uint32_t tid, uint32_t team, Sync sync)
-{
-    for (uint32_t k = 2; k <= P; k <<= 1) {
-        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
-            for (uint32_t t = tid; t < P / 2; t += team) {
-                const uint32_t i = 2 * j * (t / j) + t % j, l = i + j;
-                const unsigned long long x = a[i], y = a[l];
-                const uint32_t xi = b[i], yi = b[l];
-                if (ck_less(y, yi, x, xi) == ((i & k) == 0)) {
-                    a[i] = y; a[l] = x;
-                    b[i] = yi; b[l] = xi;
-                }
-            }
-            sync();
-        }
-    }
 }
 
 // the record of task (g, j): [count, value_0 .. value_{k-1}, world_0 .. world_{k-1}]
@@ -226,18 +178,6 @@ struct Layout {
     unsigned long long *bk, *rk;       // [T][kBelow], [T][kCap]: the areas' keys
     uint32_t *bi, *ri;                 // and indices
 };
-
-// the task of chunk k of a slice: the last of rows[0 .. T) whose first chunk is at most k
-__device__ inline uint32_t row_of_chunk(const TRow *rows, uint64_t T, uint64_t k)
-{
-    uint64_t lo = 0, hi = T - 1;
-    while (lo < hi) {
-        const uint64_t mid = (lo + hi + 1) / 2;
-        if (rows[mid].k0 <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return (uint32_t)lo;
-}
 
 // pass 0: finite count and min / max sort key per task; a block per chunk
 __global__ void __launch_bounds__(kPassThreads) topk_count_kernel(TopkParams S, uint64_t K, Layout L)
@@ -525,24 +465,12 @@ __global__ void topk_init_kernel(Layout L, bool first, unsigned long long reads0
         L.hist[i] = 0;
 }
 
-constexpr uint64_t kGridCap = 64ull * kNumSMs * 8;
-
-// the world chunk of a task of n worlds in a slice of T tasks: about 8 blocks per SM over the slice, at least 16
-// worlds per thread (a block's histogram clear and flush is amortised)
-inline uint32_t chunk_of(uint64_t n, uint64_t T)
-{
-    const uint64_t want = std::max<uint64_t>(1, 8ull * kNumSMs / std::max<uint64_t>(1, T));
-    uint64_t per = (n + want - 1) / want;
-    per = std::max<uint64_t>(per, 16ull * kPassThreads);
-    return (uint32_t)((per + kPassThreads - 1) / kPassThreads * kPassThreads);
-}
-
 } // namespace
 
 uint64_t topk_scratch_bytes(const TopkParams &S, const std::vector<WorldGroup> &table)
 {
     uint64_t large = 0;
-    for (const WorldGroup &wg : table) large += wg.n > kSmallMax;
+    for (const WorldGroup &wg : table) large += route_of(wg.n) == kRadixRoute;
     if (large == 0) return 0;
     return 256 + std::min<uint64_t>(kSliceTasks, large * S.n_p) * kTaskBytes;
 }
@@ -552,21 +480,15 @@ cudaError_t launch_top_worlds(const TopkParams &S, const std::vector<WorldGroup>
                               unsigned long long *reads, cudaStream_t s)
 {
     *launches = 0;
-    uint32_t warp = 0, block = 0;  // order[0 .. warp) warp route, [warp, block) block route, the rest radix
-    for (uint32_t g : order) {
-        warp += table[g].n <= kWarpMax;
-        block += table[g].n <= kSmallMax;
-    }
+    const Routes rt = routes_of(table, order);
+    const uint32_t warp = rt.warp, block = rt.block;
     cudaError_t e = cudaSuccess;
     if (warp > 0) {
         topk_warp_kernel<<<(unsigned)std::min((warp * (uint64_t)S.n_p + 7) / 8, kGridCap), 256, 0, s>>>(S, 0, warp);
         *launches += 1;
     }
     if (block > warp) {
-        uint64_t n = 0;
-        for (uint32_t k = warp; k < block; ++k) n = std::max(n, table[order[k]].n);
-        uint32_t P = 1;
-        while (P < n) P <<= 1;
+        const uint32_t P = block_keys(table, order, rt);
         const size_t smem = P * 12ull;
         e = cudaFuncSetAttribute(topk_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -589,7 +511,7 @@ cudaError_t launch_top_worlds(const TopkParams &S, const std::vector<WorldGroup>
         for (uint64_t i = 0; i < T; ++i) {
             const uint32_t g = order[block + (t0 + i) / S.n_p];
             const WorldGroup &wg = table[g];
-            const uint32_t Wc = chunk_of(wg.n, T), C = (uint32_t)((wg.n + Wc - 1) / Wc);
+            const uint32_t Wc = chunk_of(wg.n, T, kPassThreads), C = (uint32_t)((wg.n + Wc - 1) / Wc);
             rows[i] = TRow{(uint32_t)wg.o, (uint32_t)wg.n, Wc, C, (uint32_t)K, g, (uint32_t)((t0 + i) % S.n_p), 0};
             K += C;
         }

@@ -12,8 +12,9 @@ whole), phase-0 histograms of the value key with shift bit_len(hi - lo) - 14, th
 the switch to world indices [0, n - 1] once the range holds one key (phase 1), and the gather; its record must equal
 ref_top.  rank_geometry and topk_geometry restate the routes (quantile_order), the slices of the scratch (256 MiB;
 sizeof(TRow) = 32 and sizeof(TState) = 80 give 176,240 bytes per top-worlds task and 1523 tasks a slice), the world
-chunks (kNumSMs = 132) and the launch counts.  test_constants_match_the_sources reads every constant and struct the
-restatement uses from the sources, so an edit to a kernel that leaves it behind fails without a GPU.
+chunks (kNumSMs = 132) and the launch counts.  test_constants_match_the_sources_and_the_shared_header reads every
+constant and struct the restatement uses from the sources (each kernel file with order_stats.cuh, which holds the route
+split and chunk_of), so an edit to a kernel that leaves it behind fails without a GPU.
 
 Catalogue.  The planes are built from keys (key_value, the inverse of order_key), so that a case sits on the bin edge
 it names rather than hoping random data finds it: a bin of kCap and of kCap + 1 worlds at levels 1, 2 and 4, R ranges
@@ -795,8 +796,8 @@ def clean_outcome():
 # --------------------------------------------------------------------------- CPU
 
 
-def _constants(path):
-    src = re.sub(r"//[^\n]*", "", open(path).read())
+def _constants(*paths):
+    src = re.sub(r"//[^\n]*", "", "".join(open(p).read() for p in paths))
     out = {}
     for m in re.finditer(r"constexpr\s+[\w ]+?\s+(k\w+)\s*=\s*([^;]+);", src):
         expr = re.sub(r"\b(\d+)(ull|u)\b", r"\1", m.group(2))
@@ -818,9 +819,10 @@ def _struct_bytes(src, name, consts):
     return align8(size) if wide else size
 
 
-def test_constants_match_the_sources():
-    rsrc, rk = _constants(os.path.join(CSRC, "rank_kernels.cu"))
-    tsrc, tk = _constants(os.path.join(CSRC, "topk_kernels.cu"))
+def test_constants_match_the_sources_and_the_shared_header():
+    shared = os.path.join(CSRC, "order_stats.cuh")  # the route split, chunk_of and the order helpers of both files
+    rsrc, rk = _constants(os.path.join(CSRC, "rank_kernels.cu"), shared)
+    tsrc, tk = _constants(os.path.join(CSRC, "topk_kernels.cu"), shared)
     h = open(os.path.join(CSRC, "sixdof_internal.h")).read()
     assert int(re.search(r"constexpr unsigned kNumSMs = (\d+);", h).group(1)) == NUM_SMS
     common = dict(kCap=KCAP, kBins=KBINS, kBinBits=KBINBITS, kSmallMax=SMALL_MAX, kWarpMax=WARP_MAX,
@@ -844,7 +846,12 @@ def test_constants_match_the_sources():
         squash(tsrc)
     for src in (rsrc, tsrc):
         assert squash("want = std::max<uint64_t>(1, 8ull * kNumSMs / std::max<uint64_t>(1, T));") in squash(src)
-        assert squash("(per + kPassThreads - 1) / kPassThreads * kPassThreads") in squash(src)
+        assert squash("(per + threads - 1) / threads * threads") in squash(src)
+    for name in ("rank_kernels.cu", "topk_kernels.cu"):
+        src = open(os.path.join(CSRC, name)).read()
+        assert '#include "order_stats.cuh"' in src, name
+        calls = re.findall(r"\bchunk_of\(([^()]*)\)", src)  # every chunk in blocks of the file's kPassThreads
+        assert calls and all(squash(c).endswith(",kPassThreads") for c in calls), name
 
 
 def test_restatements_on_hand_cases():
