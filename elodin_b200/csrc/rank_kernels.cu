@@ -1013,8 +1013,8 @@ cudaError_t launch_rank_correlation(const double *cov, double *out, uint64_t G, 
 //             keys     each rank's keys (u64) at the bucket's place plus its offset, the other ranks leaving those words
 //                      0; in: every key of the window's buckets, then the finish
 // A step that finds no work skips the exchange.  Every rank plans from the same sums, numbers ranges and buckets in the
-// same order and so makes the same exchanges, each of the same size.  The histograms are sent in rounds of at most
-// kRoundCap bytes.
+// same order and so makes the same exchanges, each of the same size.  The sizes and the histograms are sent in rounds of
+// at most kRoundCap bytes.
 namespace {
 
 enum : int { kStart = 0, kSizes, kHist, kOffsets, kKeys, kDone };
@@ -1222,8 +1222,10 @@ cudaError_t after_plan(RankShard &Q, int level, void *partial, uint64_t *partial
         for (uint64_t t = 0; t < T; ++t) words[t] = Q.st[t].bucket_worlds;
         Q.keys = set_offsets(Q, H.xk, words, s, &e);
         CUDA_TRY(e);
-        // an offsets window of wkeys * n_ranks u32 and its keys (up to kCap past it) are both one round below the cap
-        Q.wkeys = std::max<uint64_t>(1, std::min((kRoundCap - kCap * 8ull) / 8, kRoundCap / (4ull * Q.n_ranks)) - 1);
+        // an offsets window of wkeys * n_ranks u32 and its keys (up to kCap past it) are both one round below the cap;
+        // at least one place (the begin refuses n_ranks >= kRoundCap / 4, where even one place reaches the cap), and
+        // the max before the - 1 so that a min of 0 cannot wrap
+        Q.wkeys = std::max<uint64_t>(2, std::min((kRoundCap - kCap * 8ull) / 8, kRoundCap / (4ull * Q.n_ranks))) - 1;
         Q.window = 0;
         return open_window(Q, partial, partial_bytes, launches, s);
     }

@@ -2848,6 +2848,10 @@ int b200_sixdof_sharded_ranks_begin(b200_sixdof *h, int grouped, const uint32_t 
     if (rc) return rc;
     if (h->status != B200_OK) return fail(h->status, "handle is in a failed state");
     if (rank >= n_ranks) return fail(B200_ERR_INVALID_ARGUMENT, "rank %u of %u ranks", rank, n_ranks);
+    // a window's offsets exchange is n_ranks u32 per place: from here on even one place is not below the round cap
+    if ((uint64_t)n_ranks * 4 >= sharded_rank_round_bytes())
+        return fail(B200_ERR_INVALID_ARGUMENT, "sharded ranks: %u ranks, at most %llu", n_ranks,
+                    (unsigned long long)(sharded_rank_round_bytes() / 4 - 1));
     RankParams S;
     if ((rc = write_outcomes(h)) || (rc = rank_params(h, grouped != 0, planes, n_p, S))) return rc;
     b200_sixdof::ShardedRanks &c = h->sr;

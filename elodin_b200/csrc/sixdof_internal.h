@@ -506,8 +506,8 @@ cudaError_t launch_rank_correlation(const double *cov, double *out, uint64_t G, 
 // A rank's part of a world-sharded rank call between its rounds (b200_sixdof_sharded_ranks_*): the MSD bucket pass over
 // every (group, plane) task, slice by slice, each exchange's u32 words summed over the ranks before the step that reads
 // them.  The exchanges, in order: the group sizes (once per call), then per slice at most 5 histograms, then per window
-// of the slice's buckets their local counts and their keys; none passes sharded_rank_round_bytes() but the histograms,
-// which are sent in rounds of at most that many bytes.
+// of the slice's buckets their local counts and their keys; none passes sharded_rank_round_bytes() but the sizes and the
+// histograms, which are sent in rounds of at most that many bytes.
 struct RankShard {
     // one per task of the slice, in device scratch, copied back after every plan
     struct TaskState {

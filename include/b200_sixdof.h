@@ -881,16 +881,18 @@ int b200_sixdof_outcome_group_sobol(b200_sixdof *h, const uint32_t *planes, uint
  *              After the last level each rank puts its bucket worlds and their keys in a list of its own (the scatter,
  *              the last read of the plane).
  *     windows  the slice's buckets, in windows of their first key's place in the slice's key words: a window holds
- *              W = min(4,186,111, 2^23 / n_ranks - 1) places, so both of its exchanges stay below 32 MiB:
+ *              W = max(1, min(4,186,111, floor(2^23 / n_ranks) - 1)) places, so both of its exchanges stay below
+ *              32 MiB (n_ranks < 2^23, so even a window of one place does):
  *       offsets  each bucket's count on each rank, rank-slotted (W * n_ranks u32, at the bucket's first place).
  *       keys     every key of the window's buckets as a u64 (two u32 words, W + 8192 at most), each rank writing its
  *                own at the bucket's place plus its offset and leaving the other words 0.  Each rank then sorts the
  *                window's buckets that hold its worlds in shared memory and writes its worlds' midranks from two
  *                binary searches of the sorted keys; world indices never travel.
  *   So one sizes exchange per call, then per slice at most 5 histogram exchanges and two per window of its keys (one
- *   window unless the slice's buckets hold more than W worlds), fewer where the summed counts show no work.  Only the
- *   histogram exchange can pass 32 MiB (the max_round_bytes begin reports, whatever the campaign's size); it is sent
- *   in rounds of at most that many bytes.  Every key of every bucket reaches every rank, a window at a time: about 8
+ *   window unless the slice's buckets hold more than W worlds), fewer where the summed counts show no work.  The
+ *   sizes exchange is G * n_ranks * 8 bytes and a histogram exchange 64 KiB per range; these two can pass 32 MiB (the
+ *   max_round_bytes begin reports, whatever the campaign's size) and are then sent in rounds of at most that many
+ *   bytes.  Every key of every bucket reaches every rank, a window at a time: about 8
  *   bytes per complete world and selected plane, as much as gathering the planes; what the rounds buy is device memory
  *   per rank bounded by its own worlds and a window, never every rank's planes.  A task reads the rank's plane at most
  *   6 times (5 histogram passes and the scatter; the completeness read not counted); b200_sixdof_rank_reads, set by the
@@ -904,8 +906,11 @@ int b200_sixdof_outcome_group_sobol(b200_sixdof *h, const uint32_t *planes, uint
  *       the most of each group, unless one task alone needs more;
  *     - the histograms of two consecutive levels, 64 KiB per range that exists (a range holds more than 8192 worlds
  *       over every rank; tens of ranges on continuous values);
- *     - the exchange: at most 32 MiB, or one level's histograms if they are larger.
+ *     - the exchange: at most 32 MiB, or one level's histograms or the sizes (G * n_ranks * 8 bytes) if they are
+ *       larger.  The sizes grow with the rank count: 8 KiB per rank at 1024 groups, about 64 GiB of device memory
+ *       (and as much host memory, which the sizes round reads back) near the limit of 2^23 - 1 ranks.
  *   A cudaMalloc that fails ends the call with B200_ERR_OUT_OF_MEMORY and leaves the handle usable.
+ *   At most 8,388,607 ranks (2^23 - 1): the begin refuses more with B200_ERR_INVALID_ARGUMENT.
  *   Preconditions (a C host checks them itself; sharding.gather_ranks does): every rank passes the same grouping,
  *   planes, n_ranks and outcome count and a distinct rank, a rank's groups are the global groups cut to its worlds (the
  *   same G on every rank; a group may be empty on a rank).  A group of more than 1,073,872,895 complete worlds over the
@@ -916,10 +921,10 @@ int b200_sixdof_outcome_group_sobol(b200_sixdof *h, const uint32_t *planes, uint
  *   (b200_sixdof_outcome_[group_]ranks or _rank_correlation) discards it too, since it rewrites the rank planes; any
  *   other reduction may run between rounds. ---- */
 /* Checks what b200_sixdof_outcome_[group_]ranks checks, in the same order (the outcome set, the groups when grouped,
- * the selection of 1 .. P planes), then the sticky status, then rank < n_ranks (B200_ERR_INVALID_ARGUMENT), after
- * B200_ERR_INVALID_ARGUMENT for a null handle or a null max_round_bytes; discards a call still pending; writes the
- * outcome planes of the summaries, fixes the grouping, planes, rank and n_ranks of the call and writes its largest round
- * in bytes. */
+ * the selection of 1 .. P planes), then the sticky status, then rank < n_ranks and n_ranks < 2^23
+ * (B200_ERR_INVALID_ARGUMENT), after B200_ERR_INVALID_ARGUMENT for a null handle or a null max_round_bytes; discards a
+ * call still pending; writes the outcome planes of the summaries, fixes the grouping, planes, rank and n_ranks of the
+ * call and writes its largest round in bytes. */
 int b200_sixdof_sharded_ranks_begin(b200_sixdof *h, int grouped, const uint32_t *planes, uint32_t n_p, uint32_t rank,
                                     uint32_t n_ranks, uint64_t *max_round_bytes);
 /* One round, with the contract of b200_sixdof_sharded_quantiles_round: `reduced` = the ranks' elementwise sum of this

@@ -7,8 +7,9 @@ world, bit for bit, for any rank count and split; rho is the merged covariance o
 The CPU tests check the bindings and prototypes, the refusals made before any backend call, and that an argument one
 rank cannot use raises on every rank over two gloo processes.  The GPU tests drive simulated ranks in lockstep in one
 process (the partials summed with numpy) over adversarial planes, group sizes at every route edge, several scratch
-slices and a split key exchange, and check the round and read bounds, the rho and PRCC contracts and the protocol's
-refusals; two gloo processes on one GPU then run a whole campaign through World.build(..., process_group=)."""
+slices and a split key exchange, and check the rounds and the reads against the restated protocol of
+test_sharded_rank_shapes (sharded_plan), the rho and PRCC contracts and the protocol's refusals; two gloo processes on
+one GPU then run a whole campaign through World.build(..., process_group=)."""
 
 import os
 import re
@@ -23,11 +24,10 @@ from elodin_b200 import _lib, sharding
 from elodin_b200.executor import merge_covariance, partial_rank_correlation, rank_correlation
 from tests.ensemble_util import need_gpu, run_gloo
 from tests.test_outcome_rank_correlation import _adversarial, _only_values, ref_ranks, same
+from tests.test_sharded_rank_shapes import Split, sharded_plan
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CAP = 32 << 20  # include/b200_sixdof.h: the largest round of a sharded rank call, in bytes
-EXCHANGES_PER_SLICE = 7  # at most 5 histogram exchanges, the offsets and the keys
-READ_BOUND = 6  # 5 histogram passes and the scatter
 
 
 # --------------------------------------------------------------------------- helpers
@@ -62,12 +62,6 @@ def drive(exs, planes, groups=False, between=None):
     return [ex.sharded_ranks_end() for ex in exs], sizes, bound[0]
 
 
-def exchanges(sizes):
-    """The exchanges of a call from its round sizes: every exchange ends on a round below the cap (an exchange of an
-    exact multiple of the cap is counted with the next one, which only lowers the count)."""
-    return sum(1 for n in sizes[:-1] if n < CAP)
-
-
 def sharded(values, bounds, planes, sizes=None):
     """The sharded ranks of values [M, p] over the ranks of `bounds` (grouped when `sizes` holds the global groups)."""
     M = values.shape[0]
@@ -88,47 +82,17 @@ def sharding_cut(sizes, a, b):
     return out
 
 
-SLICE_CAP, TASK_FIXED = 256 << 20, 144  # rank_kernels.cu: kScratchCap; a task's row, state and three offsets
+def restated(values, planes, spans, sizes=None):
+    """The restated protocol of the call over the ranks of `spans` (sharded_plan); its plans keep in bounds."""
+    P = sharded_plan(values, sizes, planes, Split(len(spans), dict(enumerate(spans))))
+    assert P["errors"] == [], P["errors"]
+    return P
 
 
-def slices_of(values, planes, spans, sizes=None):
-    """The slices of a sharded call, restated from rank_kernels.cu (cut_slices): the tasks of every group with complete
-    worlds, each sized for the rank holding the most of the group (its pieces, states, bucket list and keys: 48 bytes
-    per complete world and 4 per world, and the ranges), packed greedily into kScratchCap.  Returns each slice's
-    tasks' complete worlds over every rank."""
-    ok = np.all(np.isfinite(values[:, planes]), axis=1)
-    groups = [values.shape[0]] if sizes is None else list(sizes)
-    o = np.cumsum([0] + groups)
-    N, l_most, w_most = [], [], []
-    for g in range(len(groups)):
-        parts = [(max(a, o[g]), min(b, o[g + 1])) for a, b in spans]
-        per = [(int(ok[a:b].sum()), b - a) if b > a else (0, 0) for a, b in parts]
-        N.append(sum(c for c, _ in per))
-        l_most.append(max(c for c, _ in per))
-        w_most.append(max(w for _, w in per))
-
-    def task(g):
-        R = max(1, N[g] // 8193) if N[g] > 8192 else 0
-        a8 = lambda x: (x + 7) // 8 * 8
-        return TASK_FIXED + a8(2 * R * 16 + 32 * l_most[g] + a8(4 * w_most[g]) + a8(4 * l_most[g]) + 8 * l_most[g])
-
-    slices, used = [], None
-    for g in (g for g in range(len(groups)) if N[g] for _ in planes):
-        if used is None or used + task(g) > SLICE_CAP:
-            slices.append([])
-            used = 256 + task(g)
-        else:
-            used += task(g)
-        slices[-1].append(N[g])
-    return slices
-
-
-def exchange_bound(values, planes, spans, sizes=None):
-    """The most exchanges of a call: the sizes, then per slice 5 histogram levels and two per window of its keys (at
-    most its tasks' complete worlds; a window holds the first keys of (CAP - 8192 * 8) / 8 or CAP / (4 R) of them, less
-    one, so that every exchange is one round below the cap)."""
-    wkeys = max(1, min((CAP - 8192 * 8) // 8, CAP // (4 * len(spans))) - 1)
-    return 1 + sum(5 + 2 * max(1, -(-sum(sl) // wkeys)) for sl in slices_of(values, planes, spans, sizes))
+def check_reads(exs, P, sizes, p):
+    tasks = len(sizes or [0]) * p
+    for ex in exs:
+        assert round(ex.rank_reads() * tasks) == P["reads"] and ex.rank_reads() == P["reads"] / tasks
 
 
 def rho_of(covs, p):
@@ -228,8 +192,9 @@ def _check(values, bounds, planes, sizes=None, math="fast"):
     assert same(want, ref_ranks(values[:, planes], sizes))
     for (a, b), (r, _) in zip(spans, out):
         assert same(r, want[a:b]), (a, b)
-    for ex in exs:
-        assert ex.rank_reads() <= READ_BOUND
+    P = restated(values, planes, spans, sizes)
+    assert rounds == P["rounds"], rounds
+    check_reads(exs, P, sizes, len(planes))
     return exs, spans, out, rounds, one
 
 
@@ -277,14 +242,14 @@ def test_ranks_over_ranks_equal_one_handle(R):
     bounds = sorted(rng.choice(np.arange(1, M), R - 1, replace=False).tolist())
     planes = list(range(8))
     exs, spans, out, rounds, one = _check(values, bounds, planes)
-    assert len(slices_of(values, planes, spans)) == 1 and exchanges(rounds) <= 1 + EXCHANGES_PER_SLICE
     _check_rho(values, [0, 1, 3, 4, 6], *sharded(values, bounds, [0, 1, 3, 4, 6])[:3], one)
     for j in planes:  # each plane alone: its own finite worlds; the read bound on every plane
         e, _, o, r = sharded(values, bounds, [j])
         for (a, b), (rk, _) in zip(spans, o):
             assert same(rk, ref_ranks(values[:, [j]])[a:b]), j
-        assert max(x.rank_reads() for x in e) <= READ_BOUND, j
-        assert exchanges(r) <= 1 + EXCHANGES_PER_SLICE, (j, r)
+        P = restated(values, [j], spans)
+        assert r == P["rounds"], (j, r)
+        check_reads(e, P, None, 1)
 
 
 @pytest.mark.gpu
@@ -309,8 +274,7 @@ def test_grouped_route_edges_over_ranks():
     bounds = [int(o[4]) + 100, int(o[6]) + 5000, int(o[7]) + 4]
     planes = list(range(8))
     exs, spans, out, rounds, one = _check(values, bounds, planes, sizes)
-    assert len(slices_of(values, planes, spans, sizes)) >= 2  # the 2^20 + 5 group's 8 tasks do not fit in one slice
-    assert exchanges(rounds) <= exchange_bound(values, planes, spans, sizes)
+    assert len(restated(values, planes, spans, sizes)["slices"]) >= 2  # the 2^20 + 5 group's 8 tasks need two
     _check_rho(values, [0, 1, 2, 4, 6], *sharded(values, bounds, [0, 1, 2, 4, 6], sizes)[:3], one, sizes)
 
 
@@ -327,9 +291,8 @@ def test_several_scratch_slices():
     exs, spans, out, rounds, one = _check(values, [sum(sizes) // 3], order, sizes)
     # every group has at most 8192 complete worlds: one bucket per task, so each slice makes no histogram exchange and
     # the offsets and the keys of each window of its keys
-    sl = slices_of(values, order, spans, sizes)
-    wkeys = min((CAP - 8192 * 8) // 8, CAP // 8) - 1
-    assert len(sl) >= 2 and exchanges(rounds) == 1 + sum(2 * -(-sum(k) // wkeys) for k in sl), (len(sl), rounds)
+    P = restated(values, order, spans, sizes)
+    assert len(P["slices"]) >= 2 and P["hist"] == [] and len(rounds) == 1 + 2 * len(P["windows"]) + 1
 
 
 @pytest.mark.gpu
@@ -365,7 +328,9 @@ def test_a_split_key_exchange_and_the_scratch_bound():
     want = ref_ranks(values)
     for (a, b), (r, _) in zip(spans, out):
         assert same(r, want[a:b])
-    assert max(rounds) < CAP and exchanges(rounds) >= 1 + 1 + 2 * 2, rounds  # sizes, a level, two windows
+    P = restated(values, [0], spans)
+    assert rounds == P["rounds"] and max(rounds) < CAP and len(P["windows"]) >= 2, rounds  # a level, two windows
+    check_reads(exs, P, None, 1)
     used = base - least
     per_rank = CAP + (16 << 20) + 64 * (M // R)
     assert used <= R * per_rank, (used, R * per_rank)
